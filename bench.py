@@ -1,6 +1,6 @@
 """Benchmark of the hot path: seconds-of-audio per second separated (n_fft=2048, hop=1024).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 One "step" = the whole inference hot path (STFT -> sliding windows -> CascadedNet -> mask -> 2x inverse STFT,
@@ -10,7 +10,7 @@ one mask gather to rank 0 before the overlap-add).  Prints ONE JSON line (rank 0
 
   value      device-resident region: wave already in HBM -> both stems in HBM, CUDA-event timed, max over ranks
   e2e        same through the public host-buffer call (pinned host wave -> pinned host stems), copies inside
-  roofline   tcgen05 convolution kernel: algorithmic conv FLOPs / CUDA-event kernel time vs measured bf16 peak
+  roofline   wgmma convolution kernels: algorithmic conv FLOPs / CUDA-event kernel time vs the H100 SXM bf16 peak
   cpu_baseline  the CPU oracle port of the reference path (oracle/), all host threads, bounded sample
   parity     measured max-abs errors of this build on the 10 s golden fixture (tests/golden), before timing
   tta        the same track with --tta (BASELINE configs[3], 163 windows)
@@ -18,8 +18,11 @@ one mask gather to rank 0 before the overlap-add).  Prints ONE JSON line (rank 0
   cudnn_baseline  the reference's own GPU arithmetic: the oracle's functional restatement of the reference modules on
              cuda:0 through stock PyTorch / cuDNN (TF32 convolutions allowed, the torch default) + torch.stft/istft
   mgpu_check (N > 1) sharded vs single-GPU stems on a 31 s track, with and without --tta; the run fails above 1e-5
---impl reference runs only that CPU arm (the reference itself is Python over librosa and cannot travel to the
-GPU box; oracle/ is its restatement, validated against the unmodified reference in tests/).
+--impl reference runs only that CPU arm (the reference itself is Python over librosa; oracle/ is its restatement,
+validated against golden outputs of the unmodified reference in tests/).
+--dump-outputs DIR writes the stems of the last timed step as DIR/instruments.npy and DIR/vocals.npy (float32, shape
+(2, n)): every sample when the track has at most 2^21 of them, else a fixed seeded sample of 2^21 sample indices
+(sorted), so that two builds can be compared output for output on identical inputs.
 """
 import argparse
 import json
@@ -42,21 +45,10 @@ UNIT = 'audio-s/s'
 SR = 44100
 SECONDS_PER_GPU = 240.0
 CONV_FLOP_PER_WINDOW = 135.714e9   # SURVEY.md 8(d)
-# dram__bytes_read.sum + dram__bytes_write.sum summed over the tensor-core convolution launches of the round-2 ncu launch
-# list (profiles/r02_launches_bench.csv: 127.3 GB over the 141 windows that bench run pushes through the net; round 1
-# measured 0.879 GB with the LSTM channel still interleaved into the skip tensor, 1.225 GB before the decoder upsample
-# was fused); the un-fused minimum of SURVEY 8(d) is 1.142 GB/window.
-CONV_DRAM_BYTES_PER_WINDOW = 0.903e9
-GOLDEN = os.path.join(ROOT, 'tests', 'golden', 'ref_10s_default.npz')
-
-
-def measured_peaks():
-    path = os.path.join(ROOT, 'MEASURED_PEAKS.json')
-    if os.path.exists(path):
-        with open(path) as f:
-            d = json.load(f)
-        return d.get('bf16_tflops_sustained', 1430.1), d.get('hbm_gbs', 6566.1), 'measured (MEASURED_PEAKS.json, sustained)'
-    return 1590.0, 6650.0, 'fallback (B200_PROFILING.md)'
+GOLDEN_PREFIX = os.path.join(ROOT, 'tests', 'golden', 'ref_10s_default')
+# NVIDIA H100 SXM data sheet, dense BF16 tensor throughput at the 700 W power limit (not a measured rate)
+PEAK_BF16_TFLOPS = 989.0
+DUMP_SAMPLES = 1 << 21   # stem samples per channel written by --dump-outputs (2 stems x 2 channels x 8 MB)
 
 
 class ClockSampler(threading.Thread):
@@ -196,9 +188,14 @@ def parity_block(sp, dev):
     (tests/golden/ref_10s_default.npz, oracle/make_golden.py): mask, --tta mask, masked spectrogram in normalised units."""
     import inference
     from lib import spec_utils, synth
-    if not os.path.exists(GOLDEN):
+    import glob
+    paths = sorted(glob.glob(GOLDEN_PREFIX + '.part*.npz'))
+    if not paths:
         return None
-    g = np.load(GOLDEN)
+    g = {}
+    for path in paths:
+        with np.load(path) as part:
+            g.update({k: part[k] for k in part.files})
     wave = synth.sine_mix(10.0)
     X = spec_utils.wave_to_spectrogram(wave, 1024, 2048)
     d_spec = torch.from_numpy(X).to(dev)
@@ -281,6 +278,18 @@ def mgpu_check(sp, dev, world, rank):
     return out
 
 
+def dump_outputs(out_dir, inst, voc):
+    """The stems of one step as float32 .npy files: all samples, or a fixed seeded sample of DUMP_SAMPLES columns."""
+    os.makedirs(out_dir, exist_ok=True)
+    L = inst.shape[1]
+    if L > DUMP_SAMPLES:
+        cols = np.sort(np.random.default_rng(0).choice(L, DUMP_SAMPLES, replace=False))
+        idx = torch.from_numpy(cols).to(inst.device)
+        inst, voc = inst.index_select(1, idx), voc.index_select(1, idx)
+    for name, t in (('instruments', inst), ('vocals', voc)):
+        np.save(os.path.join(out_dir, name + '.npy'), t.float().cpu().numpy())
+
+
 def run_gpu(args):
     import torch.distributed as dist
     import inference
@@ -308,8 +317,12 @@ def run_gpu(args):
     h_wave = torch.from_numpy(wave).pin_memory()
     ctx = sp._ctx()
 
+    last = []   # stems of the most recent step_device() call (for --dump-outputs)
+
     def step_device():
-        return vr_dist.separate_wave(sp, d_wave, tta=False, world=world, rank=rank)
+        out = vr_dist.separate_wave(sp, d_wave, tta=False, world=world, rank=rank)
+        last[:] = [out]
+        return out
 
     def barrier():
         if world > 1:
@@ -352,6 +365,9 @@ def run_gpu(args):
     launches = ctx.launch_count() - launches0
     sampler.stop_flag = True
     sampler.join(timeout=2)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *last[0])
+    del last[:]
     ms_step = ms / args.steps
     value = seconds / (ms_step * 1e-3)
     ms_median = sorted(per_step)[len(per_step) // 2]
@@ -443,18 +459,14 @@ def run_gpu(args):
         h_inst = h_voc = None
         shared_host.close(world)
 
-    peak_tf, peak_hbm, peak_src = measured_peaks()
     tc_ms, tc_flops, tc_n, cc_ms, cc_flops, cc_n = [float(x) for x in prof]
     roof = None
     if tc_n > 0:
         ach = tc_flops / (tc_ms * 1e-3) / 1e12
-        roof = {'bound': 'tensor', 'kernel': 'conv_tc_rows_kernel + conv_tc_kernel (tcgen05 implicit-GEMM conv family, '
+        roof = {'bound': 'tensor', 'kernel': 'conv_tc_rows_kernel + conv_tc_kernel (wgmma implicit-GEMM conv family, '
                           'bf16x3 split precision)',
-                'achieved': ach, 'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': ach / peak_tf,
-                'traffic': CONV_DRAM_BYTES_PER_WINDOW * n_windows / world / max(1.0, tc_n),
-                'traffic_note': 'average DRAM bytes per convolution launch = 0.903 GB per window (ncu, '
-                                'profiles/r02_launches_bench.csv) x windows per rank / launches',
-                'peak_source': peak_src,
+                'achieved': ach, 'peak': PEAK_BF16_TFLOPS, 'unit': 'TFLOP/s', 'frac': ach / PEAK_BF16_TFLOPS,
+                'peak_source': 'H100 SXM data sheet, dense BF16 at 700 W',
                 'note': 'achieved = algorithmic conv FLOPs (real channel counts, 1x per product; the kernel issues 3 '
                         'bf16 MMA passes per product) of %d launches / their summed CUDA-event time %.2f ms on rank '
                         '0 over one profiled step of the same workload (%.1f ms, band streams serialised); kernel '
@@ -483,11 +495,11 @@ def run_gpu(args):
             'metric': METRIC, 'value': value, 'unit': UNIT, 'n_gpus': world, 'steps': args.steps, 'warmup': args.warmup,
             'ms_per_step': ms_step, 'ms_per_step_median': ms_median, 'value_at_median': seconds / (ms_median * 1e-3),
             'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
-            'dtype': 'bf16x3 (split-bf16 operands hi+lo, 3 tcgen05 passes, fp32 accumulate); fft/lstm fp32',
+            'dtype': 'bf16x3 (split-bf16 operands hi+lo, 3 wgmma passes, fp32 accumulate); fft/lstm fp32',
             'data': 'synthetic',
             'config': {'workload': workload_text(seconds, n_windows, args.batch),
                        'l2': 'no flush needed: per-step working set (spectrogram %.0f MB + activations > 1 GB) exceeds '
-                             'the 126 MB L2' % (2 * 1025 * T * 8 / 1e6),
+                             'the 50 MB L2' % (2 * 1025 * T * 8 / 1e6),
                        'parallelism': ('window-sharded x%d: STFT / net / inverse STFT per rank span, 4-byte max all-reduce, 8 KB '
                                        'halo mask frame, overlap-add kernel stores its span into rank 0 HBM over NVLink'
                                        % world) if world > 1 else 'single GPU'},
@@ -522,7 +534,7 @@ def run_gpu(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
-    ap.add_argument('--steps', type=int, default=5)
+    ap.add_argument('--steps', type=int, default=5, help='timed steps of the headline measurement (>= 1)')
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--impl', type=str, default='b200')
     ap.add_argument('--batch', type=int, default=27, help='windows per forward launch sequence (240 s = 81 windows = 3 x 27)')
@@ -533,7 +545,11 @@ def main():
     ap.add_argument('--no-strong', action='store_true', help='skip the 40-minute strong-scaling sub-record')
     ap.add_argument('--seconds-per-gpu', type=float, default=SECONDS_PER_GPU,
                     help='track length per GPU (default 240 s = BASELINE configs[2]; shorter only for profiling)')
+    ap.add_argument('--dump-outputs', type=str, default='', metavar='DIR',
+                    help='write the stems of the last timed step to DIR/instruments.npy and DIR/vocals.npy')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
     if args.impl == 'reference':
         run_reference(args)
     else:

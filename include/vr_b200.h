@@ -1,4 +1,4 @@
-/* vr_b200.h - C ABI of the B200-native vocal-remover inference hot path (libvr_b200.so).
+/* vr_b200.h - C ABI of the H100-native vocal-remover inference hot path (libvr_b200.so).
  *
  * The reference (tsurumeso/vocal-remover @ 99f92fe) is pure Python and has NO plugin / FFI interface;
  * the drop-in boundary is the Python call surface used by inference.py:130-176 and pseudo.py:32-67.
@@ -42,7 +42,7 @@ typedef struct vr_config {
   int32_t nout_lstm;   /* CascadedNet nout_lstm (128)                            (inference.py:130)      */
   int32_t cropsize;    /* --cropsize, multiple of 16, > 128                      (inference.py:116)      */
   int32_t max_batch;   /* windows per forward launch sequence (--batchsize)      (inference.py:115)      */
-  int32_t conv_mode;   /* 0 = tcgen05 tensor-core conv where the tile fits, 1 = CUDA-core conv only     */
+  int32_t conv_mode;   /* 0 = wgmma tensor-core conv where the tile fits,  1 = CUDA-core conv only     */
 } vr_config;
 
 /* nets.CascadedNet(n_fft, hop, nout, nout_lstm).to(device)                      (lib/nets.py:46-80)     */
@@ -159,7 +159,7 @@ VR_API int vr_profile_dump(vr_ctx* ctx, char* text, int64_t cap, int64_t* needed
 
 /* ---- validation hooks used by tests/ (not part of the reference surface) ---------------------------- */
 /* One Conv2DBNActiv-shaped layer (lib/layers.py:8-26; BN already folded into w/bias by the caller):
- * x [N][Cin][H][W] -> y [N][Cout][Ho][Wo]; use_tc selects the tcgen05 kernel (error if tile does not fit). */
+ * x [N][Cin][H][W] -> y [N][Cout][Ho][Wo]; use_tc selects the wgmma kernel (error if tile does not fit). */
 VR_API int vr_debug_conv(vr_ctx* ctx, const float* x, int32_t N, int32_t Cin, int32_t H, int32_t W, const float* w,
                   const float* bias, int32_t Cout, int32_t k, int32_t stride, int32_t dil_h, int32_t dil_w,
                   int32_t act, int32_t use_tc, float* y, void* stream);
@@ -169,13 +169,14 @@ VR_API int vr_debug_conv(vr_ctx* ctx, const float* x, int32_t N, int32_t Cin, in
 VR_API int vr_debug_decoder(vr_ctx* ctx, const float* low, int32_t N, int32_t Cl, int32_t h, int32_t w, const float* skip,
                      int32_t Cs, const float* wgt, const float* bias, int32_t Cout, int32_t act, int32_t fused, float* y,
                      void* stream);
-/* Process-wide debug knobs of the tensor-core kernels: key 0 = 1 sets the UMMA matrix-base-offset field in the
- * row-streaming kernel's shifted descriptors (wrong on B200, kept for tests/diag_rows.py), key 1 = 1 disables that kernel, key 2 = 64 makes it use 64-channel (SW128) chunks instead of 32 (set before vr_create), key 3 = 1 enables the experimental flat-halo kernel (before vr_create), key 5 = 1 fuses the decoder upsample into
- * the row-streaming kernel (before vr_create).                  */
+/* Process-wide debug knobs of the tensor-core kernels: key 0 = 1 makes CTA 0 of the row-streaming kernel record a
+ * timeline (builds with -DVR_TRACE), key 1 = 1 disables that kernel, key 2 = 1 makes vr_debug_conv use its 64-channel
+ * output tile, key 4 = k gives k of its operand slots to the interpolation warps, key 5 = 1 (default) fuses the decoder
+ * upsample into it (before vr_create), key 6 = 1 (default) skips channel groups whose weights are all zero.        */
 VR_API int vr_debug_set(int32_t key, int32_t value);
 /* Internal activation of the last forward as NCHW float32; dims receives [N,C,H,W].                       */
 /* timeline of CTA 0 of the last row-kernel launch made with vr_debug_set(0, 1): 3 roles x 2048 events x 3 clock64 stamps
- * (MMA issuer / TMA producer / interpolation warp 0), copied to HOST memory; returns the number of values or -1 */
+ * (unused / TMA producer / interpolation warp 0), copied to HOST memory; returns the number of values or -1 */
 VR_API int64_t vr_debug_trace(uint64_t* host_out, int64_t capacity);
 VR_API int vr_debug_read(vr_ctx* ctx, const char* what, float* out, int64_t capacity, int64_t* dims, void* stream);
 

@@ -4,16 +4,16 @@ TEST INFRASTRUCTURE.  ``lib/spec_utils.py:3,5`` imports ``librosa`` and ``soundf
 module top level; neither is installed here and there is no network.  ``install()`` registers
 stub modules whose ``stft`` / ``istft`` are the restatements in ``oracle/stft_oracle.py``
 (SURVEY.md App. A) so that ``lib.nets``, ``lib.layers``, ``lib.dataset`` and
-``inference.Separator`` import and run unmodified from /root/reference.  Used only by
-``oracle/make_golden.py`` and by tests that are skipped when /root/reference is absent
-(it does not exist on the GPU box).
+``inference.Separator`` import and run unmodified from a checkout of the reference (VR_REFERENCE_ROOT).
+Used only by ``oracle/make_golden.py``; the tests compare against the fixtures it writes.
 """
+import os
 import sys
 import types
 
 from . import stft_oracle
 
-REFERENCE_ROOT = '/root/reference'
+REFERENCE_ROOT = os.environ.get('VR_REFERENCE_ROOT', '')
 
 
 def install():
@@ -40,6 +40,8 @@ def install():
 
 def import_reference():
     """Returns (inference, nets, spec_utils, dataset) modules of the unmodified reference."""
+    if not os.path.isdir(REFERENCE_ROOT):
+        raise RuntimeError('set VR_REFERENCE_ROOT to a checkout of the reference vocal-remover')
     install()
     if REFERENCE_ROOT not in sys.path:
         sys.path.insert(0, REFERENCE_ROOT)

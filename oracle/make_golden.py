@@ -1,8 +1,10 @@
-"""Generates tests/golden/*.npz by running the UNMODIFIED reference (imported from /root/reference
-through oracle/librosa_shim.py) on the seeded synthetic input / checkpoint.  TEST INFRASTRUCTURE.
+"""Generates tests/golden/*.npz by running the UNMODIFIED reference (its checkout is given by
+VR_REFERENCE_ROOT, imported through oracle/librosa_shim.py) on the seeded synthetic input / checkpoint.
+TEST INFRASTRUCTURE.
 
-Run in the build container only (``python -m oracle.make_golden`` from the repo root); the
-fixtures are committed because /root/reference does not exist on the GPU box.
+Run where the reference checkout exists (``python -m oracle.make_golden`` from the repo root); the
+fixtures are committed so that the tests never need the reference itself.  Each fixture is written as
+``<name>.partN.npz`` files of at most ~1 MB (tests/conftest.py:load_golden merges them).
 
 What is pinned, per case:
   * reference ``inference.Separator.separate`` / ``separate_tta`` (inference.py:70-102) with the
@@ -117,9 +119,67 @@ def run_case(name, seconds, n_fft, hop, nout, nout_lstm, cropsize, batchsize, fs
             out['win1_' + k + '_sum'] = checksum(a)
         lg = acts['logit'][..., model.offset:-model.offset]
         print(name, 'win1 logit std', lg.std(), 'stages', {k: float(np.abs(a).max()) for k, a in acts.items()})
-    path = os.path.join(GOLDEN_DIR, name + '.npz')
-    np.savez_compressed(path, **out)
-    print('wrote', path, os.path.getsize(path) // 1024, 'KiB')
+    save_parts(name, out)
+
+
+PART_BYTES = 900 * 1024
+
+
+def save_parts(name, out):
+    """Writes `out` as <name>.part1.npz, <name>.part2.npz, ... each holding at most PART_BYTES of array data."""
+    parts, cur, size = [], {}, 0
+    for k, a in out.items():
+        a = np.asarray(a)
+        if cur and size + a.nbytes > PART_BYTES:
+            parts.append(cur)
+            cur, size = {}, 0
+        cur[k] = a
+        size += a.nbytes
+    parts.append(cur)
+    for i, part in enumerate(parts):
+        path = os.path.join(GOLDEN_DIR, '%s.part%d.npz' % (name, i + 1))
+        np.savez_compressed(path, **part)
+        print('wrote', path, os.path.getsize(path) // 1024, 'KiB')
+
+
+def merge_artifacts_trials():
+    """The masks the merge_artifacts comparison runs on (tests/test_host_logic.py): seeded, regenerated by the test."""
+    rng = np.random.default_rng(0)
+    trials = []
+    for trial in range(6):
+        m = rng.uniform(0.0, 0.04, size=(2, 33, 400)).astype(np.float32)
+        for s, e in ((0, 90), (150, 260), (275, 400))[:1 + trial % 3]:
+            m[:, :, s:e] = rng.uniform(0.06, 1.0, size=(2, 33, e - s))
+        trials.append(m)
+    return trials
+
+
+def first_window(seconds=10.0, n_fft=2048, hop=1024, cropsize=256):
+    """|normalised padded spectrogram| of the first window of the 10 s input (the oracle's own STFT)."""
+    from lib import synth
+    from oracle import separator_oracle, stft_oracle
+    X = stft_oracle.wave_to_spectrogram(synth.sine_mix(seconds), hop, n_fft)
+    pad_l, pad_r, roi = separator_oracle.make_padding(X.shape[2], cropsize, 64)
+    Xp = np.pad(X, ((0, 0), (0, 0), (pad_l, pad_r)))
+    Xp /= np.abs(X).max()
+    return np.abs(Xp[None, :, :, roi:roi + cropsize])
+
+
+def run_direct():
+    """Outputs of single reference functions: CascadedNet.predict_mask on the first 10 s window (default net, every
+    second frequency bin stored) and spec_utils.merge_artifacts on merge_artifacts_trials()."""
+    ref_inference, ref_nets, ref_spec_utils, ref_dataset = librosa_shim.import_reference()
+    from lib import synth
+    sd = synth.to_torch_state_dict(synth.make_state_dict())
+    m = ref_nets.CascadedNet(2048, 1024, 32, 128)
+    m.load_state_dict(sd)
+    m.eval()
+    with torch.no_grad():
+        pm = m.predict_mask(torch.from_numpy(first_window())).numpy()
+    out = {'predict_mask_sub': pm[:, :, ::2, :]}
+    for i, t in enumerate(merge_artifacts_trials()):
+        out['merge_artifacts_%d' % i] = ref_spec_utils.merge_artifacts(t.copy())
+    save_parts('ref_direct', out)
 
 
 class _Wrap(torch.nn.Module):
@@ -138,6 +198,7 @@ def main():
     run_case('ref_10s_default', 10.0, 2048, 1024, 32, 128, 256, 4, 8, 1, True, True)
     # a small configuration exercising the n_fft / cropsize / nout flags
     run_case('ref_3s_small', 3.0, 512, 256, 16, 32, 192, 2, 2, 1, False, False)
+    run_direct()
 
 
 if __name__ == '__main__':

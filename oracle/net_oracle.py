@@ -13,7 +13,7 @@ checkpoint's ``state_dict`` keys) of the reference model:
 
 The oracle is pinned in tests/test_oracle_net.py against golden tensors produced by the
 UNMODIFIED reference modules (oracle/make_golden.py, run in the build container where
-/root/reference exists) and, when the reference is importable, against it directly.
+a reference checkout is given) and, when the reference is importable, against it directly.
 """
 import torch
 import torch.nn.functional as F

@@ -5,7 +5,7 @@ inference.py:136-138, pseudo.py:47-50), i.e. ``resampy.resample(y, orig_sr, sr, 
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py): the product path is vocal-remover_b200/csrc/resample.cu.
 
 PARITY UNPINNED.  resampy (requirements.txt: ``resampy~=0.4.0``) is a third-party dependency that is neither under
-/root/reference nor installed offline, and the reference holds no golden vectors for this step.  What is restated here
+the reference checkout nor installed offline, and the reference holds no golden vectors for this step.  What is restated here
 is resampy 0.4's published algorithm:
 
 * ``resampy.filters.sinc_window``: half of a Kaiser-windowed sinc, ``num_zeros`` zero crossings, ``2**precision`` table

@@ -4,7 +4,7 @@ The reference calls ``librosa.stft(wave[c], n_fft=n_fft, hop_length=hop_length)`
 (lib/spec_utils.py:27-28) and ``librosa.istft(spec[c], hop_length=hop_length)``
 (lib/spec_utils.py:159-162).  librosa (pinned ``librosa~=0.10.0``,
 requirements.txt:4) is a third-party dependency that is NOT vendored under
-/root/reference and is not installable offline, so this file restates the
+the reference checkout and is not installable offline, so this file restates the
 published librosa 0.10 algorithm (defaults: window='hann' periodic, center=True,
 pad_mode='constant', win_length=n_fft) as summarised in SURVEY.md App. A.
 

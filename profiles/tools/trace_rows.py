@@ -1,5 +1,5 @@
-"""Timeline of CTA 0 of the row-streaming convolution (vr_debug_set(0, 1) + vr_debug_trace): which of the MMA issuer,
-the TMA producer and the interpolation warps waits for which.  Runs one layer through the debug entry points.
+"""Timeline of CTA 0 of the row-streaming convolution (vr_debug_set(0, 1) + vr_debug_trace): how long the TMA producer
+and the interpolation warps wait for operand slots (role 0, the consumers, is not recorded).  Runs one layer through the debug entry points.
 
 Needs a library built with the timeline compiled in:
     VR_BUILD_TAG=trace VR_BUILD_FLAGS=-DVR_TRACE python vocal-remover_b200/build.py
@@ -57,8 +57,8 @@ def main():
     mma, tma, itp = t[0], t[1], t[2]
     nm = int((mma[:, 2] > 0).sum())
     mma = mma[:nm]
-    print('MMA issuer: %d rows' % nm)
     if nm > 20:
+        print('consumers: %d rows' % nm)
         per_row = np.diff(mma[:, 2])
         wait = mma[:, 1] - mma[:, 0]
         print('  cycles between consecutive rows (issue end to issue end): median %d  mean %.0f  p10 %d  p90 %d' % (

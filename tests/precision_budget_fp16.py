@@ -1,7 +1,7 @@
 """fp16 instead of bf16 operand pairs (CPU emulation; not a pytest module; companion of precision_budget.py).
 
 x = hi + lo with both parts rounded to IEEE half (11-bit significands) instead of bf16 (8-bit): mask error of the whole net
-for the three-product scheme and for the cheaper ones.  Measured (profiles/r02_precision_budget_fp16.txt): 3pass 9.9e-6
+for the three-product scheme and for the cheaper ones.  Emulated: 3pass 9.9e-6
 (bf16: 1.2e-4), two products 4.7e-3 / 6.0e-3, one product 8.3e-3 - with halves too every layer needs all three products
 at the 1e-3 gate; the three-product error itself is 12x lower than with bf16 at the same tensor-core rate.
 Usage: python tests/precision_budget_fp16.py"""

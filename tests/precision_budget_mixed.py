@@ -2,11 +2,11 @@
 
 Main product in IEEE half (x_hi16 * w_hi16, fp32 accumulate) and the two correction products with BOTH operands in fp8
 (per-tensor power-of-two scale): x_lo * w_hi + x_hi * w_lo.  With a half hi part the lo part is 2^-12 of the value instead
-of bf16's 2^-9, so the fp8 rounding of the corrections weighs 8x less than in precision_budget_fp8.py.  On tcgen05 the
-half product runs at the bf16 rate and the two kind::f8f6f4 products at twice that rate: 1 + 1/2 + 1/2 = 2 units of tensor
+of bf16's 2^-9, so the fp8 rounding of the corrections weighs 8x less than in precision_budget_fp8.py.  With wgmma the
+half product runs at the bf16 rate and the two fp8 products at twice that rate: 1 + 1/2 + 1/2 = 2 units of tensor
 time per product instead of 3, i.e. the roofline bound moves from 0.33 to 0.50, and an activation still costs 4 bytes
-(half hi + fp8 lo + fp8 copy of hi).  Measured, every layer at once (profiles/r02_precision_budget_mixed.txt):
-corrections in half 9.9e-6, in e4m3 2.7e-4 (gate 1e-3), in e5m2 5.5e-4, in block-scaled fp4 (a 1.5-unit scheme) 1.4e-3 - too coarse.
+(half hi + fp8 lo + fp8 copy of hi).  Emulated, every layer at once: corrections in half 9.9e-6, in e4m3 2.7e-4
+(gate 1e-3), in e5m2 5.5e-4, in block-scaled fp4 1.4e-3 - too coarse (and the H100 has no fp4 tensor-core path).
 Usage: python tests/precision_budget_mixed.py"""
 import os, sys, numpy as np, torch, torch.nn.functional as F
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))

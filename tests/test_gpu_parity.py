@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): the CUDA path, called through the C ABI / the reference-shaped
+"""GPU parity tests (run on an H100): the CUDA path, called through the C ABI / the reference-shaped
 Python surface, against the CPU oracle (oracle/) and the golden fixtures produced by the unmodified
 reference (tests/golden, oracle/make_golden.py).
 

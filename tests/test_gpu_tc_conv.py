@@ -1,4 +1,4 @@
-"""tcgen05 implicit-GEMM convolution (csrc/conv_tc.cu) against a float64 torch reference of the same op,
+"""wgmma implicit-GEMM convolution (csrc/conv_tc.cu) against a float64 torch reference of the same op,
 layer class by layer class (3x3, strided, dilated, 1x1, ragged batch, multi-N-tile), called through the C ABI."""
 import pytest
 import torch
@@ -47,7 +47,7 @@ def test_conv_tcgen05_vs_torch(case):
     y = _run_debug_conv(ctx, x, w, b, k, stride, dil, act, 1)
     ref = _ref_conv(x, w, b, k, stride, dil, act)
     err = (y - ref).abs().max().item()
-    record_parity('conv_tcgen05_%s' % '_'.join(str(v) for v in case).replace(' ', ''), err / max(1.0, ref.abs().max().item()), 2e-4)
+    record_parity('conv_tc_%s' % '_'.join(str(v) for v in case).replace(' ', ''), err / max(1.0, ref.abs().max().item()), 2e-4)
     assert err < 2e-4 * max(1.0, ref.abs().max().item()), err
     # and the CUDA-core kernel agrees with it even more closely (same split-bf16 storage)
     y2 = _run_debug_conv(ctx, x, w, b, k, stride, dil, act, 0)
@@ -111,5 +111,5 @@ def test_row_kernel_64_wide_tile_on_plain_convolution():
     finally:
         ctx.lib.vr_debug_set(2, 0)
     err = (y - ref).abs().max().item()
-    record_parity('conv_tcgen05_rows64_%s' % '_'.join(str(v) for v in case).replace(' ', ''), err / max(1.0, ref.abs().max().item()), 2e-4)
+    record_parity('conv_tc_rows64_%s' % '_'.join(str(v) for v in case).replace(' ', ''), err / max(1.0, ref.abs().max().item()), 2e-4)
     assert err < 2e-4 * max(1.0, ref.abs().max().item()), err

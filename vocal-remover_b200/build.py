@@ -1,4 +1,4 @@
-"""Builds libvr_b200.so (the C-ABI CUDA library, sm_100a only) in-tree with nvcc.
+"""Builds libvr_b200.so (the C-ABI CUDA library, sm_90a only) in-tree with nvcc.
 
 ``python build.py`` from this directory, or ``__graft_entry__.build()`` from the repo root.  nvcc
 cross-compiles without a GPU.  Objects are rebuilt only when their sources are newer.
@@ -14,7 +14,7 @@ OBJ = os.path.join(HERE, 'build')
 LIB = os.path.join(HERE, 'libvr_b200.so')
 SOURCES = ['api.cu', 'engine.cu', 'conv_simt.cu', 'conv_tc.cu', 'conv_tc_rows.cu', 'elementwise.cu', 'lstm.cu', 'fft.cu', 'resample.cu']
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
          '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden', '--expt-relaxed-constexpr']
 
 
@@ -56,7 +56,7 @@ def build(verbose=False, force=False):
             print(lg)
     objs = [os.path.join(OBJ, s.replace('.cu', '.o')) for s in SOURCES]
     if jobs or not os.path.exists(LIB):
-        cmd = [NVCC, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a']
+        cmd = [NVCC, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a']
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError('link failed:\n%s\n%s' % (r.stdout, r.stderr))

@@ -1,10 +1,10 @@
-// Shared device/host definitions for the vocal-remover B200 hot path (sm_100a only).
+// Shared device/host definitions for the vocal-remover H100 hot path (sm_90a only).
 //
 // Activation storage ("split-bf16"): every activation tensor of the CascadedNet forward
 // (reference lib/nets.py:82-117) lives in HBM as TWO NHWC bf16 planes, hi = bf16(x) and
-// lo = bf16(x - hi).  hi+lo carries a 16-bit significand, which is what lets the tcgen05
-// kind::f16 tensor-core convolution (conv_tc.cu) reach the 1e-3 mask parity gate with three
-// bf16 passes (hi*hi + lo*hi + hi*lo, fp32 accumulate in TMEM); a single bf16/fp16 pass fails it
+// lo = bf16(x - hi).  hi+lo carries a 16-bit significand, which is what lets the wgmma
+// bf16 tensor-core convolution (conv_tc.cu) reach the 1e-3 mask parity gate with three
+// bf16 passes (hi*hi + lo*hi + hi*lo, fp32 accumulate in registers); a single bf16/fp16 pass fails it
 // (DESIGN.md "Precision").  The planes cost the same 4 B/element as fp32 and are directly
 // TMA-loadable as tensor-core operands.
 #pragma once
@@ -99,11 +99,10 @@ __device__ __forceinline__ void split8(const float* x, bf16x8& h, bf16x8& l) {
   l = make_uint4(ul[0], ul[1], ul[2], ul[3]);
 }
 
-// 32-byte (16-channel) store: one full sector per lane (STG.E.256 on sm_100a)
+// 32-byte (16-channel) store: one full sector per lane, as two 16-byte stores (sm_90 has no 256-bit store)
 __device__ __forceinline__ void st256(bf16* p, const bf16x8& a, const bf16x8& b) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(a.x), "r"(a.y), "r"(a.z),
-               "r"(a.w), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w)
-               : "memory");
+  st128(p, a);
+  st128(p + 8, b);
 }
 
 // Store `cnt` consecutive channels (fp32 values) of one pixel as split-bf16.

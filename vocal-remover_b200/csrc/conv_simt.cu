@@ -3,8 +3,8 @@
 // Replaces one reference Conv2DBNActiv (lib/layers.py:8-26: Conv2d(bias=False) -> BatchNorm2d(eval)
 // -> ReLU | LeakyReLU) for ANY geometry on the path: 3x3 / 1x1, stride 1 / 2, dilation (dh, dw),
 // arbitrary channel counts and channel-sliced inputs / outputs (concats are written in place).
-// It is (a) the on-device numerical yardstick the tcgen05 kernel (conv_tc.cu) is validated against
-// and (b) the kernel used for the geometries that do not map onto a 128-row UMMA tile
+// It is (a) the on-device numerical yardstick the wgmma kernel (conv_tc.cu) is validated against
+// and (b) the kernel used for the geometries that do not map onto a 128-row wgmma tile
 // (tiny feature maps, Cout in {1,2}).  Math is exact fp32 FMA over the 16-bit-significand
 // split-bf16 activations.
 #include "common.cuh"

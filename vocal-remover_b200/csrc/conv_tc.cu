@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / TMA implicit-GEMM convolution for sm_100a with fused folded-BN bias + activation.
+// wgmma / TMA implicit-GEMM convolution for sm_90a with fused folded-BN bias + activation.
 //
 // Replaces the reference's Conv2DBNActiv (lib/layers.py:8-26) for the dense 3x3 / 1x1 / strided / dilated
 // layers that carry 99.8 % of the FLOPs (SURVEY App. B).  GEMM view per CTA tile:
@@ -6,15 +6,16 @@
 //   * A is never materialised: for every (tap, 64/32/16-channel chunk) ONE TMA tiled load fetches the
 //     shifted (dilated / strided, zero-filled out of bounds = conv padding) pixel box of the NHWC
 //     split-bf16 activation, both planes (hi, lo) in one instruction, straight into the 128B/64B/32B
-//     swizzled K-major layout tcgen05 consumes.
+//     swizzled K-major layout wgmma consumes.
 //   * B (BN-folded weights, split into bf16 hi/lo once at load time) arrives by TMA the same way.
-//   * One elected thread issues tcgen05.mma.cta_group::1.kind::f16 (bf16 x bf16 -> fp32 in TMEM).
-//     Three passes per k-step, hi*hi + lo*hi + hi*lo, give a ~2^-16 relative product error - the
-//     precision the 1e-3 mask gate needs (single-pass bf16/fp16 measurably fails it, DESIGN.md).
-//   * Warp-specialised persistent kernel: warp 0 TMA producer, warp 1 MMA issuer (+TMEM alloc),
-//     warps 2-5 epilogue (tcgen05.ld -> bias -> ReLU/LeakyReLU -> split to bf16 hi/lo -> channel slice of
-//     the destination NHWC buffer, which is how concats are written in place).  smem ring of 3-6 stages,
-//     two TMEM accumulators so the epilogue of tile i overlaps the MMAs of tile i+1.
+//   * Two consumer warpgroups (pixels [0,64) and [64,128) of the tile) issue wgmma.mma_async m64nBNk16
+//     (bf16 x bf16 -> fp32 in registers).  Three passes per k-step, hi*hi + lo*hi + hi*lo, give a ~2^-16
+//     relative product error - the precision the 1e-3 mask gate needs (single-pass bf16/fp16 measurably
+//     fails it, DESIGN.md).
+//   * Warp-specialised persistent kernel: warp 8 is the TMA producer; the consumer warpgroups release a stage
+//     as soon as the wgmma group that read it has completed, then run the epilogue (bias -> ReLU/LeakyReLU ->
+//     split to bf16 hi/lo -> channel slice of the destination NHWC buffer, which is how concats are written in
+//     place) from registers while the producer already fills the ring for the next tile.
 #include <cuda.h>
 #include <stdio.h>
 
@@ -28,80 +29,59 @@
 namespace vr {
 
 static constexpr int kMaxStages = 8;
-static constexpr int kThreads = 192;
+static constexpr int kConsumerWarps = 8;                 // two warpgroups
+static constexpr int kThreads = 32 * kConsumerWarps + 32;   // + the TMA producer warp
 
 struct TcParams {
   int N, Ho, Wo, Wt, Ht, Nt, tiles_w, tiles_h, m_tiles, n_tiles;
   int stride, pad_h, pad_w, dil_h, dil_w, KW;
-  int KB, cchunks, SUBS, total_sub, CinPadTC, BN, Cout, act, stages;
-  int a_sub_bytes, b_sub_bytes, a_plane_bytes, b_plane_bytes;
-  uint32_t idesc;    // N = BN
-  uint32_t idesc2;   // N = 2*BN: one MMA against the stacked [B_hi ; B_lo] planes
-  uint32_t sbo_bytes, layout_type;
+  int cchunks, total_sub, CinPadTC, Cout, act, stages;
   bf16* out_hi;
   bf16* out_lo;
   int64_t osn, osh;
   int osw;
   const float* bias;
-  int tmem_cols;
 };
 
 // ------------------------------------------------------------------------------------------------
 // KB: channels per operand sub-tile (64 / 32 / 16 = SWIZZLE_128B / 64B / 32B); a pipeline stage holds 64 / KB sub-tiles.
-// The producer and the MMA issuer are single elected lanes running their whole loop nests with compile-time operand
-// strides (see conv_tc_rows.cu: the tensor pipe queues only a few MMAs, so scalar work between the last MMA of a stage
-// and the first of the next one is a bubble; ~500 cycles per stage were measured with the per-stage election and
-// run-time strides of the first version).
-template <int KB>
+// BN: output channels per tile (the wgmma N), a multiple of 16 up to 128.
+template <int KB, int BN>
 __global__ void __launch_bounds__(kThreads, 1)
     conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p) {
   constexpr int SUBS = 64 / KB;
   constexpr int kSteps = KB / 16;
   constexpr uint32_t kAPlane = 128 * KB * 2;     // one plane of an A sub-tile (128 pixels x KB channels)
   constexpr uint32_t kASub = 2 * kAPlane;        // hi + lo
+  constexpr uint32_t kBPlane = BN * KB * 2;
+  constexpr uint32_t kBSub = 2 * kBPlane;
+  constexpr uint32_t kStageBytes = SUBS * (kASub + kBSub);
+  constexpr uint32_t kBRegion = SUBS * kASub;    // B sub-tiles follow the A sub-tiles inside a stage
+  constexpr uint32_t kLayout = KB == 64 ? 1u : KB == 32 ? 2u : 3u;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_full[kMaxStages];
   __shared__ __align__(8) uint64_t bar_empty[kMaxStages];
-  __shared__ __align__(8) uint64_t bar_tfull[2];
-  __shared__ __align__(8) uint64_t bar_tempty[2];
-  __shared__ uint32_t tmem_slot;
   __shared__ float bias_s[256];   // folded-BN bias of every N tile, staged once (a global load per use stalled the epilogue)
 
-  const int warp = threadIdx.x >> 5;
+  const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);   // provably warp-uniform: keeps wgmma unserialised
   const int lane = threadIdx.x & 31;
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t b_sub_bytes = (uint32_t)p.b_sub_bytes;
-  const uint32_t stage_bytes = (uint32_t)SUBS * (kASub + b_sub_bytes);
-  constexpr uint32_t b_region = (uint32_t)SUBS * kASub;   // B sub-tiles follow the A sub-tiles inside a stage
   const int total_tiles = p.m_tiles * p.n_tiles;
   const int num_iters = (p.total_sub + SUBS - 1) / SUBS;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kConsumerWarps && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(smem_u32(&bar_tfull[a]), 1);
-      mbar_init(smem_u32(&bar_tempty[a]), 4);
+      mbar_init(smem_u32(&bar_empty[s]), kConsumerWarps);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)),
-                 "r"((uint32_t)p.tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  for (int i = threadIdx.x; i < p.n_tiles * p.BN; i += blockDim.x) bias_s[i] = __ldg(p.bias + i);
-  tc_fence_before();
+  for (int i = threadIdx.x; i < p.n_tiles * BN; i += blockDim.x) bias_s[i] = __ldg(p.bias + i);
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
 
-  if (warp == 0) {
+  if (warp == kConsumerWarps) {
     // ===================== TMA producer (one elected lane runs the whole loop nest) =====================
     if (elect_one_sync()) {
       int stage = 0;
@@ -114,19 +94,19 @@ __global__ void __launch_bounds__(kThreads, 1)
         const int h0 = ((mt / p.tiles_w) % p.tiles_h) * p.Ht;
         const int n0 = (mt / (p.tiles_w * p.tiles_h)) * p.Nt;
         const int wbase = w0 * p.stride - p.pad_w, hbase = h0 * p.stride - p.pad_h;
-        const int nrow = nt * p.BN;
+        const int nrow = nt * BN;
         int cc = 0, kw = 0, kh = 0, sub = 0;   // (tap, channel chunk) of the next sub-tile, advanced without divisions
         for (int it = 0; it < num_iters; ++it) {
           mbar_wait(empty0 + (uint32_t)stage * 8u, phase ^ 1u);
           const int nsub = min(SUBS, p.total_sub - sub);
           const uint32_t full = full0 + (uint32_t)stage * 8u;
-          const uint32_t sbase = smem_base + (uint32_t)stage * stage_bytes;
-          mbar_expect_tx(full, (uint32_t)nsub * (kASub + b_sub_bytes));
+          const uint32_t sbase = smem_base + (uint32_t)stage * kStageBytes;
+          mbar_expect_tx(full, (uint32_t)nsub * (kASub + kBSub));
 #pragma unroll
           for (int j = 0; j < SUBS; ++j) {
             if (j < nsub) {
               tma_load_5d(sbase + (uint32_t)j * kASub, &tmA, cc * KB, wbase + kw * p.dil_w, hbase + kh * p.dil_h, n0, 0, full);
-              tma_load_3d(sbase + b_region + (uint32_t)j * b_sub_bytes, &tmB, (kh * p.KW + kw) * p.CinPadTC + cc * KB, nrow, 0,
+              tma_load_3d(sbase + kBRegion + (uint32_t)j * kBSub, &tmB, (kh * p.KW + kw) * p.CinPadTC + cc * KB, nrow, 0,
                           full);
               ++sub;
               if (++cc == p.cchunks) {
@@ -146,123 +126,78 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer (one elected lane runs the whole loop nest) =====================
-    if (elect_one_sync()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      const uint32_t dhi = desc_hi(p.sbo_bytes, p.layout_type);
-      const uint32_t full0 = smem_u32(&bar_full[0]), empty0 = smem_u32(&bar_empty[0]);
-      const uint32_t b_sub16 = b_sub_bytes >> 4;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        mbar_wait(smem_u32(&bar_tempty[acc]), acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * 2 * p.BN);   // [D1 | D2], see the issue loop
+  } else {
+    // ===================== consumer warpgroups: wgmma into registers, then the epilogue =====================
+    const int wg = warp >> 2;   // pixels [64 wg, 64 wg + 64) of the tile
+    const float slope = p.act == ACT_RELU ? 0.f : p.act == ACT_LEAKY ? 0.01f : 1.f;
+    const uint32_t dhi = desc_hi(8 * KB * 2, kLayout);
+    const uint32_t full0 = smem_u32(&bar_full[0]), empty0 = smem_u32(&bar_empty[0]);
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int it = 0; it < num_iters; ++it) {
+        const int nsub = min(SUBS, p.total_sub - it * SUBS);
         mbar_wait(full0 + (uint32_t)stage * 8u, phase);
-        int sub = 0;
-        for (int it = 0; it < num_iters; ++it) {
-          const int nsub = min(SUBS, p.total_sub - sub);
-          sub += nsub;
-          const uint32_t sdesc = desc_lo(smem_base + (uint32_t)stage * stage_bytes);
-          const uint32_t empty = empty0 + (uint32_t)stage * 8u;
-          if (++stage == p.stages) {
-            stage = 0;
-            phase ^= 1u;
-          }
-          // The hi and lo weight planes are adjacent in the stage ([BN rows hi][BN rows lo], same pitch), so A_hi meets
-          // both in ONE N = 2*BN instruction: D1 += A_hi*B_hi, D2 += A_hi*B_lo.  A second N = BN instruction adds
-          // A_lo*B_hi to D1.  Two instructions and one shared-memory pass over A_hi per k-step instead of three; the
-          // epilogue adds D1 + D2.  The wait for the NEXT stage is issued before the last pair of this one, so that it
-          // overlaps the products still queued in the tensor pipe.
+        const uint32_t sdesc = desc_lo(smem_base + (uint32_t)stage * kStageBytes);
+        wg_fence();
 #pragma unroll
-          for (int j = 0; j < SUBS; ++j) {
-            if (j < nsub) {
-              const uint32_t a_hi = sdesc + (uint32_t)((j * kASub) >> 4);
-              const uint32_t a_lo = a_hi + (kAPlane >> 4);
-              const uint32_t b_hi = sdesc + (b_region >> 4) + (uint32_t)j * b_sub16;
+        for (int j = 0; j < SUBS; ++j) {
+          if (j < nsub) {
+            const uint32_t a_hi = sdesc + ((j * kASub + (uint32_t)wg * (kAPlane / 2)) >> 4);
+            const uint32_t a_lo = a_hi + (kAPlane >> 4);
+            const uint32_t b_hi = sdesc + ((kBRegion + j * kBSub) >> 4);
+            const uint32_t b_lo = b_hi + (kBPlane >> 4);
 #pragma unroll
-              for (int k = 0; k < kSteps; ++k) {
-                if (j == nsub - 1 && k == kSteps - 1 && it + 1 < num_iters) mbar_wait(full0 + (uint32_t)stage * 8u, phase);
-                const uint32_t acc_flag = (it | j | k) ? 1u : 0u;
-                umma_bf16_w(d_tmem, a_hi + 2u * k, b_hi + 2u * k, dhi, p.idesc2, acc_flag);
-                umma_bf16_w(d_tmem, a_lo + 2u * k, b_hi + 2u * k, dhi, p.idesc, 1u);
-              }
-            }
+            for (int k = 0; k < kSteps; ++k)
+              wgmma_split3<BN>(acc, a_hi + 2u * k, a_lo + 2u * k, b_hi + 2u * k, b_lo + 2u * k, dhi);
           }
-          umma_commit(empty);   // frees the slot once the MMAs have read it
         }
-        umma_commit(smem_u32(&bar_tfull[acc]));       // accumulator complete -> epilogue
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1u;
+        wg_commit();
+        wg_wait<1>();   // the group of the previous stage has read its operands: hand that slot back
+        if (prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty0 + (uint32_t)prev * 8u);
+        }
+        prev = stage;
+        if (++stage == p.stages) {
+          stage = 0;
+          phase ^= 1u;
         }
       }
-    }
-    __syncwarp();
-  } else {
-    // ===================== epilogue (warps 2..5 <-> TMEM lane quarters 2,3,0,1) =====================
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const float slope = p.act == ACT_RELU ? 0.f : p.act == ACT_LEAKY ? 0.01f : 1.f;
-    const int dw = row % p.Wt;
-    const int dh = (row / p.Wt) % p.Ht;
-    const int dn = row / (p.Wt * p.Ht);
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      wg_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty0 + (uint32_t)prev * 8u);
+
       const int nt = tile % p.n_tiles;
       const int mt = tile / p.n_tiles;
       const int w0 = (mt % p.tiles_w) * p.Wt;
       const int h0 = ((mt / p.tiles_w) % p.tiles_h) * p.Ht;
       const int n0 = (mt / (p.tiles_w * p.tiles_h)) * p.Nt;
-      const int n = n0 + dn;
-      const bool valid = n < p.N;
-      const int64_t obase = (int64_t)n * p.osn + (int64_t)(h0 + dh) * p.osh + (int64_t)(w0 + dw) * p.osw;
-      mbar_wait(smem_u32(&bar_tfull[acc]), acc_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (uint32_t)(acc * 2 * p.BN) + ((uint32_t)(q * 32) << 16);
-      int c0 = 0;
-      for (; c0 + 32 <= p.BN; c0 += 32) {
-        float v[32], v2[32];
-        tmem_ld32(t_row + (uint32_t)c0, v);
-        tmem_ld32(t_row + (uint32_t)(p.BN + c0), v2);
+      const int c_lane = nt * BN + 2 * (lane & 3);
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] += v2[i];
-        if (c0 + 32 >= p.BN) {   // all of this warp's TMEM reads are done: hand the accumulator back
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(&bar_tempty[acc]));
-        }
-        if (valid) epilogue_store<2>(v, bias_s, nt * p.BN + c0, p.Cout, slope, p.out_hi + obase, p.out_lo + obase);
-      }
-      if (c0 < p.BN) {   // BN is a multiple of 16: one trailing 16-column group
-        float v[16], v2[16];
-        tmem_ld16(t_row + (uint32_t)c0, v);
-        tmem_ld16(t_row + (uint32_t)(p.BN + c0), v2);
+      for (int hr = 0; hr < 2; ++hr) {
+        const int row = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
+        const int dw = row % p.Wt;
+        const int dh = (row / p.Wt) % p.Ht;
+        const int n = n0 + row / (p.Wt * p.Ht);
+        if (n >= p.N) continue;
+        const int64_t obase = (int64_t)n * p.osn + (int64_t)(h0 + dh) * p.osh + (int64_t)(w0 + dw) * p.osw;
 #pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] += v2[i];
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&bar_tempty[acc]));
-        if (valid) epilogue_store<1>(v, bias_s, nt * p.BN + c0, p.Cout, slope, p.out_hi + obase, p.out_lo + obase);
-      }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1u;
+        for (int j = 0; j < BN / 8; ++j)
+          epilogue_pair(acc[4 * j + 2 * hr], acc[4 * j + 2 * hr + 1], bias_s, c_lane + 8 * j, p.Cout, slope,
+                        p.out_hi + obase, p.out_lo + obase);
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols)
-                 : "memory");
-  }
 }
+
+// every (KB, BN) instantiation the host can launch
+#define VR_TC_FOR_BN(X, KB) X(KB, 16) X(KB, 32) X(KB, 48) X(KB, 64) X(KB, 80) X(KB, 96) X(KB, 112) X(KB, 128)
+#define VR_TC_FOR_ALL(X) VR_TC_FOR_BN(X, 64) VR_TC_FOR_BN(X, 32) VR_TC_FOR_BN(X, 16)
 
 // ------------------------------------------------------------------------------------------------
 // host side
@@ -279,9 +214,10 @@ const TcDevice& tc_device() {
     if (cudaDeviceGetAttribute(&d.max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&d.num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
       return none;
-    cudaFuncSetAttribute(conv_tc_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem - 2048);
-    cudaFuncSetAttribute(conv_tc_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem - 2048);
-    cudaFuncSetAttribute(conv_tc_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem - 2048);
+#define VR_TC_SET_SMEM(KB, BN) \
+  cudaFuncSetAttribute(conv_tc_kernel<KB, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem - 2048);
+    VR_TC_FOR_ALL(VR_TC_SET_SMEM)
+#undef VR_TC_SET_SMEM
     tc_rows_set_attributes(d.max_smem);
     d.ok = true;
   }
@@ -461,13 +397,9 @@ cudaError_t tc_launch(ConvLayer& L, const ActView& in, const ActView& out, cudaS
   p.stride = L.stride; p.dil_h = L.dil_h; p.dil_w = L.dil_w;
   p.pad_h = L.dil_h * (L.k / 2); p.pad_w = L.dil_w * (L.k / 2);
   p.KW = L.k;
-  p.KB = tc.KB; p.cchunks = tc.cchunks; p.SUBS = tc.SUBS; p.total_sub = tc.taps * tc.cchunks;
-  p.CinPadTC = tc.CinPadTC; p.BN = tc.BN; p.Cout = L.Cout; p.act = L.act;
-  p.a_plane_bytes = 128 * tc.KB * 2;
-  p.b_plane_bytes = tc.BN * tc.KB * 2;
-  p.a_sub_bytes = 2 * p.a_plane_bytes;
-  p.b_sub_bytes = 2 * p.b_plane_bytes;
-  const int stage_bytes = tc.SUBS * (p.a_sub_bytes + p.b_sub_bytes);
+  p.cchunks = tc.cchunks; p.total_sub = tc.taps * tc.cchunks;
+  p.CinPadTC = tc.CinPadTC; p.Cout = L.Cout; p.act = L.act;
+  const int stage_bytes = tc.SUBS * (2 * 128 * tc.KB * 2 + 2 * tc.BN * tc.KB * 2);
   const TcDevice& dv = tc_device();
   if (!dv.ok) {
     err = "tc_launch: cannot query the current device";
@@ -480,27 +412,20 @@ cudaError_t tc_launch(ConvLayer& L, const ActView& in, const ActView& out, cudaS
     err = "tc_launch: shared memory too small for two pipeline stages";
     return cudaErrorInvalidValue;
   }
-  // instruction descriptor (cute::UMMA::InstrDescriptor): D=f32 [4,6)=1, A=bf16 [7,10)=1, B=bf16 [10,13)=1,
-  // K-major A and B (bits 15,16 = 0), N>>3 at [17,23), M>>4 at [24,29)
-  p.idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(tc.BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  p.idesc2 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)((2 * tc.BN) >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  p.sbo_bytes = (uint32_t)(8 * tc.KB * 2);
-  p.layout_type = tc.KB == 64 ? 2u : tc.KB == 32 ? 4u : 6u;
   p.out_hi = out.hi; p.out_lo = out.lo;
   p.osn = out.sn; p.osh = out.sh; p.osw = out.sw;
   p.bias = tc.bias;
-  int cols = 32;
-  while (cols < 4 * tc.BN) cols <<= 1;   // two accumulators x [D1 | D2]
-  p.tmem_cols = cols;
   const int total_tiles = p.m_tiles * p.n_tiles;
   const int grid = total_tiles < dv.num_sms ? total_tiles : dv.num_sms;
-  if (tc.KB == 64)
-    conv_tc_kernel<64><<<grid, kThreads, dyn, s>>>(it->second, tc.map_b, p);
-  else if (tc.KB == 32)
-    conv_tc_kernel<32><<<grid, kThreads, dyn, s>>>(it->second, tc.map_b, p);
-  else
-    conv_tc_kernel<16><<<grid, kThreads, dyn, s>>>(it->second, tc.map_b, p);
-  return cudaGetLastError();
+#define VR_TC_LAUNCH(KB_, BN_)                                                           \
+  if (tc.KB == KB_ && tc.BN == BN_) {                                                    \
+    conv_tc_kernel<KB_, BN_><<<grid, kThreads, dyn, s>>>(it->second, tc.map_b, p);     \
+    return cudaGetLastError();                                                           \
+  }
+  VR_TC_FOR_ALL(VR_TC_LAUNCH)
+#undef VR_TC_LAUNCH
+  err = "tc_launch: no kernel instantiation for this channel tile";
+  return cudaErrorInvalidValue;
 }
 
 }  // namespace vr

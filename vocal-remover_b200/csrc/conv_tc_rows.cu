@@ -1,35 +1,28 @@
-// Row-streaming tcgen05 convolution: 3x3, stride 1, dilation 1, output width a multiple of 128.
+// Row-streaming wgmma convolution: 3x3, stride 1, dilation 1, output width a multiple of 128.
 //
 // The generic kernel (conv_tc.cu) re-fetches every input pixel from L2 once per tap (9x) and is bound
-// by L2->SM bandwidth on the wide, shallow layers (enc1, enc2.conv2, dec2, dec1 of every BaseNet:
-// 69 % of the convolution time in profiles/r01_launches_bench30s_v1_direct.csv).  Here one CTA owns a
-// block of R=8 output rows x 128 pixels x BN couts with R accumulators resident in TMEM, and streams
-// the R+2 input rows it needs through shared memory ONCE per 32-channel chunk:
-//   * each input row (130 pixels incl. the +-1 halo, 32 channels, hi and lo plane) is one pair of TMA
-//     loads; out-of-image rows / columns are zero-filled by TMA = the conv padding;
+// by L2->SM bandwidth on the wide, shallow layers (enc1, enc2.conv2, dec2, dec1 of every BaseNet).
+// Here one CTA owns a block of R output rows x 128 pixels x BN couts with R accumulators resident in
+// registers, and streams the R+2 input rows it needs through shared memory ONCE per 32-channel chunk:
+//   * each input row (130 pixels incl. the +-1 halo, 32 channels, hi and lo plane) is one TMA load of
+//     a two-plane box; out-of-image rows / columns are zero-filled by TMA = the conv padding;
 //   * a row feeds up to three output rows (kh = 0,1,2) and, for each, the three kw taps are the SAME
-//     shared-memory tile read through UMMA descriptors whose start address is shifted by kw pixels
-//     (+ kw * 64 B) - no data movement per tap.  Measured on B200: the swizzle is applied to the absolute
-//     shared-memory address, so the shifted start needs NO matrix-base-offset (setting the field to
-//     (addr>>7)&7 produces garbage);
+//     shared-memory tile read through GMMA descriptors whose start address is shifted by kw pixels
+//     (+ kw * 64 B) - no data movement per tap.  The swizzle is a function of the absolute shared-memory
+//     address, so the shifted start needs no matrix-base-offset;
 //   * the weights of the three kh taps are STACKED along the MMA N dimension ([kh=2 | kh=1 | kh=0] x BN couts)
-//     and the R accumulators sit in adjacent TMEM columns, so ONE tcgen05.mma of N = 3*BN adds an input
-//     row's contribution to output rows r-2, r-1 and r at once;
+//     and the R accumulators of a thread are adjacent column blocks of one register fragment, so ONE
+//     wgmma of N = 3*BN adds an input row's contribution to output rows r-2, r-1 and r at once;
 //   * the 9-tap weight slab of the chunk (3 kw x [3*BN] x 32, hi+lo) is double-buffered in shared memory.
-// L2->SM traffic per output pixel drops from 9 to (R+2)/R = 1.25 operand fetches.
+// L2->SM traffic per output pixel drops from 9 to (R+2)/R operand fetches.
 //
-// MMA issue (round 2): everything the issuer adds to a descriptor inside a row is a compile-time constant (the
-// kernel is a template on BN; chunk width, slot and slab strides are constexpr).  With run-time strides ptxas kept
-// the descriptor arithmetic in vector registers and moved the operands of every UTCHMMA through R2UR: the row
-// kernel issued one MMA per 85-98 cycles whatever its N (profiles/r02_layers_before.tsv), i.e. the issuing thread
-// was the limit.  The micro-benchmark profiles/ubench/umma_issue.cu measures the same 18-MMA row with constant
-// offsets at 44 cycles per N=48 MMA and 56 per N=96 MMA - the shared-memory operand fetch of the tensor pipe,
-// (4096 + 32 N) bytes at 128 B/cycle, which is the next bound (N >= 128 is needed for N/2 cycles).
+// Two consumer warpgroups (warps 0-7) each own 64 of the 128 pixels; warp 8 is the TMA producer.  R is chosen per
+// (BN, fused upsample) so that the R * BN / 2 accumulator registers of a thread fit the register budget of the block.
 //
 // Fused decoder upsample (optional, Decoder of lib/layers.py:51-64): the leading `up_chunks` channel chunks of the
 // input are F.interpolate(x2, bilinear, align_corners=True) of a tensor at half resolution.  Instead of reading a
-// materialised up-sampled copy (4x the bytes, and the decoder layers are HBM-bound), nine producer warps
-// interpolate each 130-pixel row from TMA-staged half-resolution rows into the swizzled operand slot
+// materialised up-sampled copy (4x the bytes, and the decoder layers are HBM-bound), ten producer warps
+// interpolate each 130-pixel row from half-resolution rows into the swizzled operand slot
 // (generic-proxy stores + fence.proxy.async + mbarrier arrive), bit-identical to upsample2x_kernel up to the
 // order of the two blends.
 #include <stdio.h>
@@ -41,9 +34,17 @@
 namespace vr {
 
 static constexpr int kInterpWarps = 10;             // each covers 7 staged source pixels (+1 neighbour): 70 >= kSrcPx
-static constexpr int kInterpThreads = 32 * kInterpWarps;
-static constexpr int kRowsThreads = 192 + kInterpThreads;   // TMA, MMA, 4 epilogue warps + the interpolation warps
-static constexpr int kMaxR = 8;                    // output rows per CTA tile
+static constexpr int kConsumerWarps = 8;            // two warpgroups: pixels [0,64) and [64,128) of the tile
+static constexpr int kTmaWarp = kConsumerWarps;
+static constexpr int kInterpWarp0 = kConsumerWarps + 1;
+static constexpr int kMaxR = 8;                     // largest number of output rows per CTA tile (H must be a multiple)
+// output rows per tile: R * BN / 2 accumulator registers per consumer thread.  The warps of a block are spread over the
+// four SM sub-partitions, each with a quarter of the register file: 9 warps (3 per sub-partition) get 168 registers
+// per thread, 19 warps (with the ten interpolation warps, 5 per sub-partition) get 96.
+__host__ __device__ constexpr int rows_per_tile(int BN, bool up) {
+  return up ? (BN == 16 ? 4 : 2) : (BN == 64 ? 2 : BN == 32 ? 4 : 8);
+}
+__host__ __device__ constexpr int rows_threads(bool up) { return 32 * (kConsumerWarps + 1 + (up ? kInterpWarps : 0)); }
 static constexpr int kRowPx = 130;                 // 128 + 2 halo pixels
 static constexpr int kBoxPx = 136;                 // pixels per TMA row box: makes one plane 17 x 512 B, so that the lo plane
                                                    // of the two-plane box starts on the SWIZZLE_64B repeat (8 rows x 64 B)
@@ -55,9 +56,9 @@ static constexpr uint32_t kAPlane = kBoxPx * kRowB; // 8704: hi plane, then lo p
 static constexpr uint32_t kASlot = 2 * kAPlane;     // 17408 = 17 KiB
 
 // Optional timeline of CTA 0 (builds with -DVR_TRACE only: vr_debug_set(0, 1), read back with vr_debug_trace): clock64 stamps of the three producer /
-// consumer loops, to see which of them the others wait for.  [role][event index][3] : role 0 = MMA issuer (before the
-// operand wait, after it, after the row's last MMA was issued), role 1 = TMA producer (before the slot wait, after the
-// load was issued, 0), role 2 = interpolation warp 0 (row start, after the slot wait, after the arrive).
+// consumer loops, to see which of them the others wait for.  [role][event index][3] : role 0 is not recorded, role 1 =
+// TMA producer (before the slot wait, after the load was issued, 0), role 2 = interpolation warp 0 (row start, after the
+// slot wait, after the arrive).
 static constexpr int kTraceEvents = 2048;
 __device__ unsigned long long g_rows_trace[3 * kTraceEvents * 3];
 
@@ -104,154 +105,108 @@ __device__ __forceinline__ uint32_t chunk_groups(unsigned long long kmask, int c
   return sh + 4 <= 64 ? (uint32_t)(kmask >> sh) & 0xFu : 0xFu;
 }
 
-// tcgen05.mma with the accumulate flag as a compile-time constant (UPT / !UPT in SASS)
-template <int ACC>
-__device__ __forceinline__ void umma_c(uint32_t d_tmem, uint32_t a_lo32, uint32_t b_lo32, uint32_t hi32, uint32_t idesc) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b64 da, db;\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "mov.b64 da, {%1, %3};\n\t"
-      "mov.b64 db, {%2, %3};\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t"
-      "}" ::"r"(d_tmem),
-      "r"(a_lo32), "r"(b_lo32), "r"(hi32), "r"(idesc), "n"(ACC)
-      : "memory");
-}
-
-// The three split-precision products of one 16-channel k-step: hi*hi + lo*hi + hi*lo
-template <int BN, int ACC0>
-__device__ __forceinline__ void umma_triple(uint32_t d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t dhi,
-                                            uint32_t idesc) {
-  umma_c<ACC0>(d, a_hi, b_hi, dhi, idesc);
-  umma_c<1>(d, a_lo, b_hi, dhi, idesc);
-  umma_c<1>(d, a_hi, b_hi + (RowsGeom<BN>::kBPlane >> 4), dhi, idesc);
-}
-
-// The MMAs of one input row of one chunk, in two parts so that the issuer can wait for the NEXT row's operands while the
-// tensor pipe still has this row's last products queued: PART 0 = everything but the last k-step triple, PART 1 = that
-// triple.  KSM: k-steps (16 channels) of the chunk that carry weights (bit 0 / 1).  a_hi: descriptor low word of the
-// slot's hi plane; b_row: low word of the weight rows of the first accumulator fed.
-template <int BN, int KSM, int PART>
-__device__ __forceinline__ void issue_row(uint32_t d, uint32_t a_hi, uint32_t b_row, uint32_t dhi, uint32_t idesc) {
+// The wgmmas of input row r of one chunk: N = cnt * BN into the accumulators of output rows o_lo..o_hi (adjacent column
+// blocks of the fragment).  ksm: k-steps (16 channels) of the chunk that carry weights (bit 0 / 1).  a_hi: descriptor low
+// word of this warpgroup's 64 pixels in the slot's hi plane; bsrc: low word of the chunk's weight buffer.
+template <int BN, int R, int r>
+__device__ __forceinline__ void issue_row(float* acc, uint32_t a_hi, uint32_t bsrc, uint32_t dhi, uint32_t ksm) {
+  constexpr int o_lo = r - 2 < 0 ? 0 : r - 2;
+  constexpr int o_hi = r > R - 1 ? R - 1 : r;
+  constexpr int cnt = o_hi - o_lo + 1;
   const uint32_t a_lo = a_hi + (kAPlane >> 4);
-  constexpr int kLastKs = (KSM & 2) ? 1 : 0;
+  const uint32_t b_row = bsrc + (((uint32_t)((2 - (r - o_lo)) * BN) * kRowB) >> 4);
 #pragma unroll
   for (int kw = 0; kw < 3; ++kw) {
 #pragma unroll
     for (int ks = 0; ks < 2; ++ks) {
-      if (!((KSM >> ks) & 1)) continue;
-      const bool last = kw == 2 && ks == kLastKs;
-      if ((PART == 0) == last) continue;
+      if (!((ksm >> ks) & 1u)) continue;
       const uint32_t ao = (uint32_t)(kw * kRowB + ks * 32) >> 4;
       const uint32_t bo = (uint32_t)(kw * RowsGeom<BN>::kBKw + ks * 32) >> 4;
-      umma_triple<BN, 1>(d, a_hi + ao, a_lo + ao, b_row + bo, dhi, idesc);
+      wgmma_split3<cnt * BN>(acc + o_lo * (BN / 2), a_hi + ao, a_lo + ao, b_row + bo,
+                             b_row + bo + (RowsGeom<BN>::kBPlane >> 4), dhi);
     }
   }
 }
 
-// Same for a row that is the FIRST contribution to its newest accumulator (chunk 0, r < R): k-step 0 of tap kw = 0
-// overwrites that accumulator (accumulate = 0) and accumulates into the `cnt - 1` older ones; the rest is issue_row
-// minus that k-step.
-template <int BN, int KSM>
-__device__ __forceinline__ void issue_row_fresh_head(uint32_t d, uint32_t a_hi, uint32_t b_row, uint32_t dhi, uint32_t idesc0,
-                                                     int cnt) {
-  const uint32_t a_lo = a_hi + (kAPlane >> 4);
-  const uint32_t n_old = (uint32_t)((cnt - 1) * BN);
-  const uint32_t idesc_new = idesc0 | ((uint32_t)(BN >> 3) << 17);
-  const uint32_t idesc_all = idesc0 | ((uint32_t)((cnt * BN) >> 3) << 17);
-  constexpr int kLastKs = (KSM & 2) ? 1 : 0;
-  if (cnt > 1) {
-    const uint32_t idesc_old = idesc0 | ((n_old >> 3) << 17);
-    umma_triple<BN, 1>(d, a_hi, a_lo, b_row, dhi, idesc_old);
+// Consumer state across the rows of a tile: the A ring position of each producer's ring, the B buffer, and the slots
+// whose wgmma group is still in flight (released once the NEXT group has been committed and the older one waited for).
+struct RowsConsumer {
+  int as_t, as_u, bs, as, pend_a, pend_b;
+  uint32_t aph_t, aph_u, bph, aph;
+  int ring_lo, ring_hi;
+};
+
+template <int BN, int R, int r>
+__device__ __forceinline__ void consume_rows(RowsConsumer& st, float* acc, uint32_t a_desc0, uint32_t bsrc, uint32_t dhi,
+                                             uint32_t ksm, uint32_t afull0, uint32_t aempty0, uint32_t bempty0,
+                                             int lane) {
+  mbar_wait(afull0 + (uint32_t)st.as * 8u, st.aph);
+  wg_fence();
+  issue_row<BN, R, r>(acc, a_desc0 + (uint32_t)st.as * (kASlot >> 4), bsrc, dhi, ksm);
+  wg_commit();
+  wg_wait<1>();   // every group but this one is complete: the slots it read can be refilled
+  __syncwarp();
+  if (lane == 0) {
+    if (st.pend_a >= 0) mbar_arrive(aempty0 + (uint32_t)st.pend_a * 8u);
+    if (st.pend_b >= 0) mbar_arrive(bempty0 + (uint32_t)st.pend_b * 8u);
   }
-  umma_triple<BN, 0>(d + n_old, a_hi, a_lo, b_row + ((n_old * kRowB) >> 4), dhi, idesc_new);
-#pragma unroll
-  for (int kw = 0; kw < 3; ++kw) {
-#pragma unroll
-    for (int ks = 0; ks < 2; ++ks) {
-      if ((kw == 0 && ks == 0) || !((KSM >> ks) & 1) || (kw == 2 && ks == kLastKs)) continue;
-      const uint32_t ao = (uint32_t)(kw * kRowB + ks * 32) >> 4;
-      const uint32_t bo = (uint32_t)(kw * RowsGeom<BN>::kBKw + ks * 32) >> 4;
-      umma_triple<BN, 1>(d, a_hi + ao, a_lo + ao, b_row + bo, dhi, idesc_all);
-    }
+  st.pend_a = st.as;
+  st.pend_b = -1;
+  if (++st.as == st.ring_hi) {
+    st.as = st.ring_lo;
+    st.aph ^= 1u;
   }
+  if constexpr (r + 1 < R + 2) consume_rows<BN, R, r + 1>(st, acc, a_desc0, bsrc, dhi, ksm, afull0, aempty0, bempty0, lane);
 }
 
-// sum_i w[co + i] * act(v[i] + bias[co + i]) over CNT accumulator columns: the fused single-channel 1x1 convolution on
-// the fp32 activations of this tile (weights past Cout are zero)
-template <int CNT>
-__device__ __forceinline__ float dot_activated(const float* v, const float* bias_s, const float* dot_s, int co, float slope) {
-  float d0 = 0.f, d1 = 0.f;
-#pragma unroll
-  for (int i = 0; i < CNT; i += 2) {
-    const float t0 = v[i] + bias_s[co + i], t1 = v[i + 1] + bias_s[co + i + 1];
-    d0 = fmaf(fmaxf(t0, 0.f) + slope * fminf(t0, 0.f), dot_s[co + i], d0);
-    d1 = fmaf(fmaxf(t1, 0.f) + slope * fminf(t1, 0.f), dot_s[co + i + 1], d1);
-  }
-  return d0 + d1;
+// w[c] * act(v0 + bias[c]) + w[c + 1] * act(v1 + bias[c + 1]): this thread's share of the fused single-channel 1x1
+// convolution on the fp32 activations of one pixel (weights past Cout are zero)
+__device__ __forceinline__ float dot_pair(float v0, float v1, const float* bias_s, const float* dot_s, int c, float slope) {
+  const float t0 = v0 + bias_s[c], t1 = v1 + bias_s[c + 1];
+  return fmaf(fmaxf(t0, 0.f) + slope * fminf(t0, 0.f), dot_s[c], (fmaxf(t1, 0.f) + slope * fminf(t1, 0.f)) * dot_s[c + 1]);
 }
 
-template <int BN>
-__global__ void __launch_bounds__(kRowsThreads, 1)
+template <int BN, bool UP>
+__global__ void __launch_bounds__(rows_threads(UP), 1)
     conv_tc_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                         const __grid_constant__ CUtensorMap tmL, const RowsParams p) {
   typedef RowsGeom<BN> G;
-  constexpr int R = kMaxR;
+  constexpr int R = rows_per_tile(BN, UP);
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_afull[kMaxASlots];
   __shared__ __align__(8) uint64_t bar_aempty[kMaxASlots];
   __shared__ __align__(8) uint64_t bar_bfull[2];
   __shared__ __align__(8) uint64_t bar_bempty[2];
-  __shared__ __align__(8) uint64_t bar_tfull[2];
-  __shared__ __align__(8) uint64_t bar_tempty[2];
-  __shared__ uint32_t tmem_slot;
   __shared__ float bias_s[256];   // folded-BN bias of every N tile, staged once (a global load per use stalled the epilogue)
   __shared__ float dot_s[256];    // weights of the fused single-channel 1x1 convolution (zeros past Cout)
 
-  const int warp = threadIdx.x >> 5;
+  const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);   // provably warp-uniform: keeps wgmma unserialised
   const int lane = threadIdx.x & 31;
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_base = smem_base;
   const uint32_t b_base = smem_base + (uint32_t)p.n_aslots * kASlot;
-  // accumulators: R rows x BN columns per set; two sets (the epilogue of tile i overlaps the MMAs of tile i+1) when
-  // they fit the 512 TMEM columns, one set for BN = 64
-  constexpr int kAccSets = 2 * R * BN <= 512 ? 2 : 1;
-  constexpr uint32_t kTmemCols = kAccSets * R * BN;   // 512 (BN=64, 32) or 256 (BN=16): powers of two
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kTmaWarp && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     for (int s = 0; s < p.n_aslots; ++s) {
       // slots of the interpolation ring are filled by kInterpWarps producers (one arrive each), the others by one TMA box
       mbar_init(smem_u32(&bar_afull[s]), s < p.n_uslots ? (uint32_t)kInterpWarps : 1u);
-      mbar_init(smem_u32(&bar_aempty[s]), 1);
+      mbar_init(smem_u32(&bar_aempty[s]), kConsumerWarps);
     }
     for (int s = 0; s < 2; ++s) {
       mbar_init(smem_u32(&bar_bfull[s]), 1);
-      mbar_init(smem_u32(&bar_bempty[s]), 1);
-      mbar_init(smem_u32(&bar_tfull[s]), 1);
-      mbar_init(smem_u32(&bar_tempty[s]), 4);
+      mbar_init(smem_u32(&bar_bempty[s]), kConsumerWarps);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)),
-                 "r"(kTmemCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   for (int i = threadIdx.x; i < p.n_tiles * BN; i += blockDim.x) {
     bias_s[i] = __ldg(p.bias + i);
     dot_s[i] = p.dot_out && i < p.Cout ? __ldg(p.dot_w + i) : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
 
-  if (warp == 0) {
+  if (warp == kTmaWarp) {
     // ===================== TMA producer: one elected lane runs the whole loop nest =====================
     if (elect_one_sync()) {
       int as = p.n_uslots, bs = 0;
@@ -306,118 +261,86 @@ __global__ void __launch_bounds__(kRowsThreads, 1)
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer: ONE elected lane runs the whole loop nest =====================
-    // The tensor pipe queues only a few MMAs, so every cycle the issuing thread spends between the last MMA of a row
-    // and the first MMA of the next one is a bubble in the pipe (measured: ~490 cycles of per-row scalar code made a
-    // 920-cycle row take 1440).  Hence: the row loop is fully unrolled (accumulator offsets, weight-row offsets and the
-    // N field of the instruction descriptor are immediates), per-chunk quantities are hoisted, the lane election
-    // happens once per kernel, and the wait for the next row's operands is issued BEFORE the last k-step of the
-    // current row so that it overlaps the products still queued.
-    if (elect_one_sync()) {
-      int as_t = p.n_uslots, as_u = 0, bs = 0, acc = 0;
-      uint32_t aph_t = 0, aph_u = 0, bph = 0, acc_phase = 0;
-      const uint32_t dhi = desc_hi(8 * kRowB, 4u);   // SWIZZLE_64B, 8-row groups of 64-byte rows
-      // instruction descriptor without the N field: D=f32, A=B=bf16, K-major, M=128
-      constexpr uint32_t idesc0 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(128 >> 4) << 24);
-      const uint32_t afull0 = smem_u32(&bar_afull[0]), aempty0 = smem_u32(&bar_aempty[0]);
-      const uint32_t a_lo0 = desc_lo(a_base);
-#ifdef VR_TRACE
-      const bool tr = p.trace && blockIdx.x == 0;
-#else
-      constexpr bool tr = false;
-#endif
-      int tn = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        mbar_wait(smem_u32(&bar_tempty[acc]), acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_set = tmem_base + (uint32_t)(acc * R * BN);
-        for (int cc = 0; cc < p.chunks; ++cc) {
-          mbar_wait(smem_u32(&bar_bfull[bs]), bph);
-          const uint32_t bsrc = desc_lo(b_base + (uint32_t)bs * G::kBBuf);
-          const bool up = cc < p.up_chunks;
-          // k-steps (16 channels = two groups) whose weights are all zero are not issued: exact, since the products
-          // would be 0 (lstm / pad channel groups of the concat layouts); chunk 0 always keeps k-step 0 (accumulator init)
-          const uint32_t gm = chunk_groups(p.kmask, cc);
-          const uint32_t ksm = ((gm & 0x3u) ? 1u : 0u) | ((gm & 0xCu) ? 2u : 0u);
-          // this chunk's ring of A slots: the interpolation ring [0, n_uslots) or the TMA ring [n_uslots, n_aslots)
-          int as = up ? as_u : as_t;
-          uint32_t aph = up ? aph_u : aph_t;
-          const int ring_lo = up ? 0 : p.n_uslots, ring_hi = up ? p.n_uslots : p.n_aslots;
-          unsigned long long t_w0 = tr ? clock64() : 0ull;
-          mbar_wait(afull0 + (uint32_t)as * 8u, aph);
-          unsigned long long t_w1 = tr ? clock64() : 0ull;
-          // fully unrolled: measured 1080 cycles per steady N=96 row against 1235 with a rolled loop (timeline of CTA 0,
-          // profiles/tools/trace_rows.py); the rows of chunk 0 cost ~1700 either way - they overlap the previous tile's
-          // epilogue, whose tcgen05.ld traffic competes with the accumulator read-modify-write of the MMAs
+  } else if (warp < kConsumerWarps) {
+    // ===================== consumer warpgroups: wgmma into registers, then the epilogue =====================
+    const int wg = warp >> 2;   // pixels [64 wg, 64 wg + 64) of the tile
+    const float slope = p.act == ACT_RELU ? 0.f : p.act == ACT_LEAKY ? 0.01f : 1.f;
+    const uint32_t dhi = desc_hi(8 * kRowB, 2u);   // SWIZZLE_64B, 8-row groups of 64-byte rows
+    const uint32_t afull0 = smem_u32(&bar_afull[0]), aempty0 = smem_u32(&bar_aempty[0]);
+    const uint32_t bempty0 = smem_u32(&bar_bempty[0]);
+    const uint32_t a_desc0 = desc_lo(a_base) + ((uint32_t)(64 * wg) * kRowB >> 4);
+    RowsConsumer st;
+    st.as_t = p.n_uslots; st.as_u = 0; st.bs = 0; st.pend_a = -1; st.pend_b = -1;
+    st.aph_t = 0; st.aph_u = 0; st.bph = 0;
+    float acc[R * BN / 2];
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
 #pragma unroll
-          for (int r = 0; r < R + 2; ++r) {
-            // input row r feeds output rows o = r-kh; accumulators o_lo..o_hi are adjacent TMEM column blocks; the
-            // weight rows are stacked [kh=2 | kh=1 | kh=0], the block of accumulator o_lo is kh = r - o_lo
-            constexpr int kR = R;
-            const int o_lo = r - 2 < 0 ? 0 : r - 2;
-            const int o_hi = r > kR - 1 ? kR - 1 : r;
-            const int cnt = o_hi - o_lo + 1;
-            const uint32_t d_tmem = d_set + (uint32_t)(o_lo * BN);
-            const uint32_t b_row = bsrc + (((uint32_t)((2 - (r - o_lo)) * BN) * kRowB) >> 4);
-            const uint32_t idesc_all = idesc0 | ((uint32_t)((cnt * BN) >> 3) << 17);
-            const uint32_t a_hi = a_lo0 + (uint32_t)as * (kASlot >> 4);
-            const uint32_t aempty = aempty0 + (uint32_t)as * 8u;
-            if (cc == 0 && r <= kR - 1) {   // accumulator r receives its first product now
-              if (ksm == 3u) issue_row_fresh_head<BN, 3>(d_tmem, a_hi, b_row, dhi, idesc0, cnt);
-              else issue_row_fresh_head<BN, 1>(d_tmem, a_hi, b_row, dhi, idesc0, cnt);
-            } else if (ksm == 3u) {
-              issue_row<BN, 3, 0>(d_tmem, a_hi, b_row, dhi, idesc_all);
-            } else if (ksm == 1u) {
-              issue_row<BN, 1, 0>(d_tmem, a_hi, b_row, dhi, idesc_all);
-            } else if (ksm == 2u) {
-              issue_row<BN, 2, 0>(d_tmem, a_hi, b_row, dhi, idesc_all);
-            }
-            if (++as == ring_hi) {
-              as = ring_lo;
-              aph ^= 1u;
-            }
-            unsigned long long t_n0 = 0ull, t_n1 = 0ull;
-            if (r < R + 1) {   // next row of this chunk, while MMAs are queued
-              if (tr) t_n0 = clock64();
-              mbar_wait(afull0 + (uint32_t)as * 8u, aph);
-              if (tr) t_n1 = clock64();
-            }
-            if (ksm == 3u) issue_row<BN, 3, 1>(d_tmem, a_hi, b_row, dhi, idesc_all);
-            else if (ksm == 1u) issue_row<BN, 1, 1>(d_tmem, a_hi, b_row, dhi, idesc_all);
-            else if (ksm == 2u) issue_row<BN, 2, 1>(d_tmem, a_hi, b_row, dhi, idesc_all);
-            umma_commit(aempty);
-            if (tr && tn < kTraceEvents) {
-              g_rows_trace[(0 * kTraceEvents + tn) * 3 + 0] = t_w0;
-              g_rows_trace[(0 * kTraceEvents + tn) * 3 + 1] = t_w1;
-              g_rows_trace[(0 * kTraceEvents + tn) * 3 + 2] = clock64();
-              ++tn;
-            }
-            t_w0 = t_n0;
-            t_w1 = t_n1;
-          }
-          if (up) {
-            as_u = as;
-            aph_u = aph;
-          } else {
-            as_t = as;
-            aph_t = aph;
-          }
-          umma_commit(smem_u32(&bar_bempty[bs]));
-          if (++bs == 2) {
-            bs = 0;
-            bph ^= 1u;
-          }
+      for (int i = 0; i < R * BN / 2; ++i) acc[i] = 0.f;
+      for (int cc = 0; cc < p.chunks; ++cc) {
+        mbar_wait(smem_u32(&bar_bfull[st.bs]), st.bph);
+        const uint32_t bsrc = desc_lo(b_base + (uint32_t)st.bs * G::kBBuf);
+        const bool up = cc < p.up_chunks;
+        // k-steps (16 channels = two groups) whose weights are all zero are not issued: exact, since the products
+        // would be 0 (lstm / pad channel groups of the concat layouts)
+        const uint32_t gm = chunk_groups(p.kmask, cc);
+        const uint32_t ksm = ((gm & 0x3u) ? 1u : 0u) | ((gm & 0xCu) ? 2u : 0u);
+        // this chunk's ring of A slots: the interpolation ring [0, n_uslots) or the TMA ring [n_uslots, n_aslots)
+        st.as = up ? st.as_u : st.as_t;
+        st.aph = up ? st.aph_u : st.aph_t;
+        st.ring_lo = up ? 0 : p.n_uslots;
+        st.ring_hi = up ? p.n_uslots : p.n_aslots;
+        consume_rows<BN, R, 0>(st, acc, a_desc0, bsrc, dhi, ksm, afull0, aempty0, bempty0, lane);
+        if (up) {
+          st.as_u = st.as;
+          st.aph_u = st.aph;
+        } else {
+          st.as_t = st.as;
+          st.aph_t = st.aph;
         }
-        umma_commit(smem_u32(&bar_tfull[acc]));
-        if (++acc == kAccSets) {
-          acc = 0;
-          acc_phase ^= 1u;
+        st.pend_b = st.bs;   // released with the last row's slot, once the next group has been committed
+        if (++st.bs == 2) {
+          st.bs = 0;
+          st.bph ^= 1u;
+        }
+      }
+      wg_wait<0>();
+      __syncwarp();
+      if (lane == 0) {
+        if (st.pend_a >= 0) mbar_arrive(aempty0 + (uint32_t)st.pend_a * 8u);
+        if (st.pend_b >= 0) mbar_arrive(bempty0 + (uint32_t)st.pend_b * 8u);
+      }
+      st.pend_a = st.pend_b = -1;
+
+      const int nt = tile % p.n_tiles;
+      int mt = tile / p.n_tiles;
+      const int w0 = (mt % p.tiles_w) * 128;
+      mt /= p.tiles_w;
+      const int h0 = (mt % p.tiles_h) * R;
+      const int n = mt / p.tiles_h;
+      const int c_lane = nt * BN + 2 * (lane & 3);
+#pragma unroll
+      for (int orow = 0; orow < R; ++orow) {
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int px = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
+          const float* v = acc + orow * (BN / 2) + 2 * hr;
+          if (p.dot_out) {
+            float d = 0.f;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) d += dot_pair(v[4 * j], v[4 * j + 1], bias_s, dot_s, c_lane + 8 * j, slope);
+            d += __shfl_xor_sync(0xffffffffu, d, 1);
+            d += __shfl_xor_sync(0xffffffffu, d, 2);
+            if ((lane & 3) == 0) atomicAdd(p.dot_out + ((int64_t)n * p.H + (h0 + orow)) * p.W + (w0 + px), d);
+          }
+          const int64_t obase = (int64_t)n * p.osn + (int64_t)(h0 + orow) * p.osh + (int64_t)(w0 + px) * p.osw;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j)
+            epilogue_pair(v[4 * j], v[4 * j + 1], bias_s, c_lane + 8 * j, p.Cout, slope, p.out_hi + obase,
+                          p.out_lo + obase);
         }
       }
     }
-    __syncwarp();
-  } else if (warp >= 6) {
+  } else if (UP && warp >= kInterpWarp0) {
     // ===================== bilinear x2 producer (kInterpWarps autonomous warps) =====================
     // align_corners=True bilinear x2 (ATen upsample_bilinear2d / upsample2x_kernel weights; the vertical blend is done
     // first here).  Warp k owns the source pixels xs + [7k, 7k+7) of the row (+ pixel 7k+7 as right neighbour): lane =
@@ -427,9 +350,9 @@ __global__ void __launch_bounds__(kRowsThreads, 1)
     // split to hi/lo, straight into the SWIZZLE_64B slot.  Which output pixels those are (and their horizontal weights
     // and slot offsets) depends only on the tile: computed once per tile.  No block-wide barrier and no shared-memory
     // staging (the tensor pipe already uses the full shared-memory bandwidth for its operands): every warp waits for
-    // the slot (MMA commit) itself and arrives on the slot's mbarrier (count = kInterpWarps).
+    // the slot (released by the consumer warps) itself and arrives on the slot's mbarrier (count = kInterpWarps).
     if (p.up_chunks > 0) {
-      const int wk = warp - 6;
+      const int wk = warp - kInterpWarp0;
       const int xi = lane >> 2, j = lane & 3;
       const int sx = 7 * wk + xi;              // source pixel of this lane, relative to xs
       const bool emit = xi < 7 && sx < kSrcPx; // xi == 7 only provides the neighbour of xi == 6
@@ -516,7 +439,7 @@ __global__ void __launch_bounds__(kRowsThreads, 1)
             const float fx = p.up_sw * (float)w;
             if (w < 0 || w >= p.W || (int)fx != X || w < w0 - 1 || w > w0 + 128) continue;
             const int q = w - (w0 - 1);
-            // SWIZZLE_64B (same pattern TMA writes and UMMA reads): 16-byte chunk j of 64-byte row q sits at chunk
+            // SWIZZLE_64B (same pattern TMA writes and wgmma reads): 16-byte chunk j of 64-byte row q sits at chunk
             // j ^ ((q >> 1) & 3) because the XOR takes address bits [7,9) and the planes are 512-byte aligned
             const int off = q * 64 + ((j ^ ((q >> 1) & 3)) << 4);
             const float lx = fx - (float)X;
@@ -575,7 +498,7 @@ __global__ void __launch_bounds__(kRowsThreads, 1)
               *reinterpret_cast<uint4*>(slot + z_off) = make_uint4(0, 0, 0, 0);
               *reinterpret_cast<uint4*>(slot + kAPlane + z_off) = make_uint4(0, 0, 0, 0);
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> async proxy (UMMA)
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> async proxy (wgmma)
             __syncwarp();
             if (lane == 0) mbar_arrive(afull0 + (uint32_t)as * 8u);
             fetch();   // row k+2 (after the fence, see above); past the last row it only shifts the pipeline
@@ -593,70 +516,6 @@ __global__ void __launch_bounds__(kRowsThreads, 1)
         }
       }
     }
-  } else {
-    // ===================== epilogue =====================
-    const int q = warp & 3;
-    const int px = q * 32 + lane;
-    const float slope = p.act == ACT_RELU ? 0.f : p.act == ACT_LEAKY ? 0.01f : 1.f;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const int nt = tile % p.n_tiles;
-      int mt = tile / p.n_tiles;
-      const int w0 = (mt % p.tiles_w) * 128;
-      mt /= p.tiles_w;
-      const int h0 = (mt % p.tiles_h) * R;
-      const int n = mt / p.tiles_h;
-      mbar_wait(smem_u32(&bar_tfull[acc]), acc_phase);
-      tc_fence_after();
-      const uint32_t t_set = tmem_base + (uint32_t)(acc * R * BN) + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-      for (int orow = 0; orow < R; ++orow) {
-        const int64_t obase = (int64_t)n * p.osn + (int64_t)(h0 + orow) * p.osh + (int64_t)(w0 + px) * p.osw;
-        const bool last_row = orow == R - 1;
-        if (BN == 64) {
-          float v[32], v2[32];
-          tmem_ld32(t_set + (uint32_t)(orow * BN), v);
-          tmem_ld32(t_set + (uint32_t)(orow * BN + 32), v2);
-          if (last_row) {   // all of this warp's TMEM reads are done: hand the accumulator set back
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&bar_tempty[acc]));
-          }
-          if (p.dot_out) {
-            const float d = dot_activated<32>(v, bias_s, dot_s, nt * BN, slope) +
-                            dot_activated<32>(v2, bias_s, dot_s, nt * BN + 32, slope);
-            atomicAdd(p.dot_out + ((int64_t)n * p.H + (h0 + orow)) * p.W + (w0 + px), d);
-          }
-          epilogue_store<2>(v, bias_s, nt * BN, p.Cout, slope, p.out_hi + obase, p.out_lo + obase);
-          epilogue_store<2>(v2, bias_s, nt * BN + 32, p.Cout, slope, p.out_hi + obase, p.out_lo + obase);
-        } else {
-          float v[BN];
-          if (BN == 32) tmem_ld32(t_set + (uint32_t)(orow * BN), v);
-          else tmem_ld16(t_set + (uint32_t)(orow * BN), v);
-          if (last_row) {
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&bar_tempty[acc]));
-          }
-          if (p.dot_out)
-            atomicAdd(p.dot_out + ((int64_t)n * p.H + (h0 + orow)) * p.W + (w0 + px),
-                      dot_activated<BN>(v, bias_s, dot_s, nt * BN, slope));
-          epilogue_store<(BN >= 32 ? 2 : 1)>(v, bias_s, nt * BN, p.Cout, slope, p.out_hi + obase, p.out_lo + obase);
-        }
-      }
-      if (++acc == kAccSets) {
-        acc = 0;
-        acc_phase ^= 1u;
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols) : "memory");
   }
 }
 
@@ -798,7 +657,8 @@ cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   }
   RowsParams p;
   p.N = out.N; p.H = out.H; p.W = out.W;
-  p.tiles_w = out.W / 128; p.tiles_h = out.H / kMaxR; p.n_tiles = R.n_tiles;
+  const bool up = up_src != nullptr;
+  p.tiles_w = out.W / 128; p.tiles_h = out.H / rows_per_tile(R.BN, up); p.n_tiles = R.n_tiles;
   p.total_tiles = p.tiles_w * p.tiles_h * out.N * R.n_tiles;
   p.chunks = R.chunks; p.CinPadR = R.CinPadR; p.Cout = L.Cout; p.act = L.act;
   p.out_hi = out.hi; p.out_lo = out.lo;
@@ -845,13 +705,21 @@ cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   if (p.up_chunks > 0 && g_tc_debug[4] >= 1 && g_tc_debug[4] <= p.n_aslots - 2) p.n_uslots = g_tc_debug[4];
   const int dyn = p.n_aslots * (int)kASlot + b_bytes + 1024;
   const int grid = p.total_tiles < dv.num_sms ? p.total_tiles : dv.num_sms;   // persistent: one CTA per SM
-  if (R.BN == 16)
-    conv_tc_rows_kernel<16><<<grid, kRowsThreads, dyn, s>>>(it->second, R.map_b, itl->second, p);
-  else if (R.BN == 32)
-    conv_tc_rows_kernel<32><<<grid, kRowsThreads, dyn, s>>>(it->second, R.map_b, itl->second, p);
-  else
-    conv_tc_rows_kernel<64><<<grid, kRowsThreads, dyn, s>>>(it->second, R.map_b, itl->second, p);
-  return cudaGetLastError();
+  const int threads = rows_threads(up);
+#define VR_ROWS_LAUNCH(BN_)                                                                            \
+  if (R.BN == BN_) {                                                                                   \
+    if (up)                                                                                            \
+      conv_tc_rows_kernel<BN_, true><<<grid, threads, dyn, s>>>(it->second, R.map_b, itl->second, p);  \
+    else                                                                                               \
+      conv_tc_rows_kernel<BN_, false><<<grid, threads, dyn, s>>>(it->second, R.map_b, itl->second, p); \
+    return cudaGetLastError();                                                                         \
+  }
+  VR_ROWS_LAUNCH(16)
+  VR_ROWS_LAUNCH(32)
+  VR_ROWS_LAUNCH(64)
+#undef VR_ROWS_LAUNCH
+  err = "tc_rows_launch: no kernel instantiation for this channel tile";
+  return cudaErrorInvalidValue;
 }
 
 // copies the timeline of the last traced launch (vr_debug_set(0, 1)) to the host: 3 roles x kTraceEvents x 3 stamps
@@ -864,12 +732,13 @@ int tc_rows_read_trace(unsigned long long* out, long long capacity) {
 
 // cudaFuncSetAttribute is per device: called by tc_device() the first time a device is used (conv_tc.cu)
 void tc_rows_set_attributes(int max_smem) {
-  cudaFuncSetAttribute(conv_tc_rows_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem - 3072);
-  cudaFuncSetAttribute(conv_tc_rows_kernel<16>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-  cudaFuncSetAttribute(conv_tc_rows_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem - 3072);
-  cudaFuncSetAttribute(conv_tc_rows_kernel<32>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-  cudaFuncSetAttribute(conv_tc_rows_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem - 3072);
-  cudaFuncSetAttribute(conv_tc_rows_kernel<64>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+#define VR_ROWS_SET(BN_, UP_)                                                                                     \
+  cudaFuncSetAttribute(conv_tc_rows_kernel<BN_, UP_>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem - 3072); \
+  cudaFuncSetAttribute(conv_tc_rows_kernel<BN_, UP_>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+  VR_ROWS_SET(16, false) VR_ROWS_SET(16, true)
+  VR_ROWS_SET(32, false) VR_ROWS_SET(32, true)
+  VR_ROWS_SET(64, false) VR_ROWS_SET(64, true)
+#undef VR_ROWS_SET
 }
 
 }  // namespace vr

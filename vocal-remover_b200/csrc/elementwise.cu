@@ -345,7 +345,7 @@ cudaError_t launch_absmax(const float2* spec, int64_t n, float* out_absmax, cuda
   cudaError_t e = cudaMemsetAsync(out_absmax, 0, sizeof(float), stream);
   if (e != cudaSuccess) return e;
   if (n == 0) return cudaSuccess;
-  int grid = (int)(((n + 255) / 256) < 148 * 8 ? ((n + 255) / 256) : 148 * 8);
+  int grid = (int)(((n + 255) / 256) < 132 * 8 ? ((n + 255) / 256) : 132 * 8);
   absmax_kernel<<<grid, 256, 0, stream>>>(spec, n, out_absmax);
   return cudaGetLastError();
 }
@@ -370,7 +370,7 @@ cudaError_t launch_absmax_range(const float2* spec, int nrows, int64_t T, int64_
   if (e != cudaSuccess) return e;
   const int64_t n = (int64_t)nrows * (t1 - t0);
   if (n <= 0) return cudaSuccess;
-  int grid = (int)(((n + 255) / 256) < 148 * 8 ? ((n + 255) / 256) : 148 * 8);
+  int grid = (int)(((n + 255) / 256) < 132 * 8 ? ((n + 255) / 256) : 132 * 8);
   absmax_range_kernel<<<grid, 256, 0, stream>>>(spec, nrows, T, t0, t1, out_absmax);
   return cudaGetLastError();
 }
@@ -415,7 +415,7 @@ cudaError_t launch_lexmax_abs(const float2* spec, int64_t n, unsigned long long*
   cudaError_t e = cudaMemsetAsync(scratch, 0, sizeof(unsigned long long), stream);
   if (e != cudaSuccess) return e;
   if (n > 0) {
-    int grid = (int)(((n + 255) / 256) < 148 * 8 ? ((n + 255) / 256) : 148 * 8);
+    int grid = (int)(((n + 255) / 256) < 132 * 8 ? ((n + 255) / 256) : 132 * 8);
     lexmax_kernel<<<grid, 256, 0, stream>>>(spec, n, scratch);
   }
   lexmax_finish_kernel<<<1, 1, 0, stream>>>(scratch, out_norm);

@@ -481,7 +481,7 @@ bool Engine::run_conv(ConvLayer& L, const ActView& in, const ActView& out, cudaS
   ++launches;
   const bool use_tc = L.tc && cfg_.conv_mode == 0 && tc_supported(L, in, out);
   if (!use_tc && cfg_.conv_mode == 0 && L.Cout >= 4 && !warned_simt_) {
-    // loud, once per context: this geometry does not tile for the tcgen05 kernels (e.g. a cropsize whose feature-map
+    // loud, once per context: this geometry does not tile for the wgmma kernels (e.g. a cropsize whose feature-map
     // widths are not powers of two / multiples of 128) and runs on the fp32 CUDA-core kernel, an order of magnitude slower
     warned_simt_ = true;
     fprintf(stderr,
@@ -965,7 +965,7 @@ bool Engine::debug_conv(const float* x_nchw, int N, int Cin, int H, int W, const
   if (ok && use_tc) {
     ok = tc_prepare(L, err, allocs_);
     if (ok && !(L.tc && tc_supported(L, bin.all(N), bout.view(N, 0, Ho, 0, Cout)))) {
-      err = "debug_conv: geometry not supported by the tcgen05 kernel";
+      err = "debug_conv: geometry not supported by the wgmma kernel";
       ok = false;
     }
     cfg_.conv_mode = 0;

@@ -39,7 +39,7 @@ struct Buffer {   // a whole NHWC split-bf16 allocation
   ActView all(int n) const { return view(n, 0, H, 0, C); }
 };
 
-struct TcConv;   // tcgen05 plan (conv_tc.cu)
+struct TcConv;   // tensor-core plan (conv_tc.cu)
 
 struct ConvLayer {
   std::string name;
@@ -96,7 +96,7 @@ struct Config {
   int device = 0;
   int n_fft = 2048, hop = 1024, nout = 32, nout_lstm = 128, cropsize = 256, max_batch = 4;
   int offset = 64;
-  int conv_mode = 0;   // 0: tcgen05 where eligible, 1: CUDA-core kernel everywhere (validation)
+  int conv_mode = 0;   // 0: wgmma where eligible, 1: CUDA-core kernel everywhere (validation)
 };
 
 class Engine {

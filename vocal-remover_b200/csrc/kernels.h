@@ -1,4 +1,4 @@
-// Host-side launch prototypes for the hand-written sm_100a kernels of the hot path.
+// Host-side launch prototypes for the hand-written sm_90a kernels of the hot path.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

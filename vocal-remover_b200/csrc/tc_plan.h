@@ -1,4 +1,4 @@
-// Host-side plan of one convolution layer for the tcgen05 kernels (conv_tc.cu, conv_tc_rows.cu).
+// Host-side plan of one convolution layer for the wgmma kernels (conv_tc.cu, conv_tc_rows.cu).
 #pragma once
 #include <cuda.h>
 

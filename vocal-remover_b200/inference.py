@@ -1,9 +1,9 @@
-"""B200-native drop-in for the reference's inference.py (Separator + CLI).
+"""H100-native drop-in for the reference's inference.py (Separator + CLI).
 
 Same command line (12 flags, inference.py:109-120), same output files and stage banners, same
 ``Separator(model, device, batchsize, cropsize, postprocess).separate / separate_tta`` contract
 (numpy complex64 (2, bins, T) in, (y_spec, v_spec) out), but the sliding-window STFT -> CascadedNet ->
-mask -> inverse-STFT path runs in hand-written sm_100a CUDA (libvr_b200.so, include/vr_b200.h).
+mask -> inverse-STFT path runs in hand-written sm_90a CUDA (libvr_b200.so, include/vr_b200.h).
 ``Separator.separate_wave`` is the fused device-resident form of the same path used by ``main``.
 """
 import argparse
@@ -172,9 +172,9 @@ def main():
 
     # unsupported surfaces fail before any heavy work (model load, audio decode, output directory)
     if args.output_image:
-        raise NotImplementedError('--output_image (debug JPGs, lib/utils.py) is outside the B200 hot path')
+        raise NotImplementedError('--output_image (debug JPGs, lib/utils.py) is outside the H100 hot path')
     if not torch.cuda.is_available():
-        raise RuntimeError('no CUDA device: the B200 build of vocal-remover has no CPU path')
+        raise RuntimeError('no CUDA device: the H100 build of vocal-remover has no CPU path')
     if args.gpu < 0:
         # the reference's default (--gpu -1) means CPU; this build has no CPU path
         print('note: --gpu {} selects the CPU in the reference; this build has no CPU path and uses cuda:0'.format(args.gpu))

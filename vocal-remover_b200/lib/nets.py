@@ -1,9 +1,9 @@
-"""B200-native mirror of the reference's lib/nets.py model-load API.
+"""H100-native mirror of the reference's lib/nets.py model-load API.
 
 ``CascadedNet(n_fft, hop_length, nout=32, nout_lstm=128)`` keeps the constructor, attributes
 (``offset``, ``n_fft``, ``hop_length``, ``max_bin``, ``output_bin``), the 689-key ``state_dict`` format
 and the ``predict_mask`` / ``predict`` / ``forward`` calls of lib/nets.py:44-141, but holds no
-torch layers: the forward runs in libvr_b200.so (hand-written sm_100a kernels) on a CUDA device.
+torch layers: the forward runs in libvr_b200.so (hand-written sm_90a kernels) on a CUDA device.
 There is no CPU execution path; calling the model before ``.to(cuda)`` raises.
 """
 import os
@@ -23,7 +23,7 @@ class CascadedNet(nn.Module):
         super(CascadedNet, self).__init__()
         if is_complex:
             # never enabled by any reference caller (inference.py:130, train.py:208, pseudo.py:32)
-            raise NotImplementedError('is_complex=True is outside the B200 inference hot path')
+            raise NotImplementedError('is_complex=True is outside the H100 inference hot path')
         self.n_fft = n_fft
         self.hop_length = hop_length
         self.is_complex = False
@@ -41,7 +41,7 @@ class CascadedNet(nn.Module):
             for k, s, kind in self._spec)
         self._device = torch.device('cpu')
         self._ctxs = {}
-        # 0: tcgen05 tensor-core convolutions where the tile fits (default); 1: CUDA-core kernel everywhere.
+        # 0: wgmma tensor-core convolutions where the tile fits (default); 1: CUDA-core kernel everywhere.
         # VR_CONV_MODE=1 is a validation switch (same device, same library), not a backend.
         self.conv_mode = int(os.environ.get('VR_CONV_MODE', '0'))
 
@@ -100,7 +100,7 @@ class CascadedNet(nn.Module):
     def native_context(self, cropsize, max_batch):
         """The vr_ctx for (cropsize, max_batch) on this model's CUDA device, with weights loaded."""
         if self._device.type != 'cuda':
-            raise RuntimeError('CascadedNet (B200) has no CPU execution path: call model.to(torch.device("cuda:N")) '
+            raise RuntimeError('CascadedNet (H100) has no CPU execution path: call model.to(torch.device("cuda:N")) '
                                'first (the reference default --gpu -1 is not available here)')
         key = (int(cropsize), int(max_batch), int(self.conv_mode))
         ctx = self._ctxs.get(key)
@@ -119,7 +119,7 @@ class CascadedNet(nn.Module):
         if x.dim() != 4 or x.size(1) != 2 or x.size(2) != self.output_bin:
             raise ValueError('expected input of shape (N, 2, {}, W), got {}'.format(self.output_bin, tuple(x.shape)))
         if x.device.type != 'cuda':
-            raise RuntimeError('CascadedNet (B200) input must be a CUDA tensor; there is no CPU path')
+            raise RuntimeError('CascadedNet (H100) input must be a CUDA tensor; there is no CPU path')
         N, W = x.size(0), x.size(3)
         out_w = W - 2 * self.offset if cropped else W
         assert out_w > 0   # lib/nets.py:129

@@ -1,4 +1,4 @@
-"""B200-native mirror of the reference's lib/spec_utils.py for the inference path.
+"""H100-native mirror of the reference's lib/spec_utils.py for the inference path.
 
 wave_to_spectrogram / spectrogram_to_wave keep the reference signatures and numpy in / numpy out
 contract (lib/spec_utils.py:26-31, 157-165) but run the framed FFT / inverse FFT + overlap-add on the

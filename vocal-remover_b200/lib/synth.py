@@ -3,7 +3,7 @@
 No pretrained ``baseline.pth`` ships with the reference (models/.gitkeep only;
 inference.py:104-105 expects a GitHub-release download) and there is no network, so
 every parity / timing run uses the seeded recipes below.  Both the unmodified reference
-(oracle side) and the B200 path load the same ``state_dict``.
+(oracle side) and the H100 path load the same ``state_dict``.
 
 * ``sine_mix``            - SURVEY.md section 8(d) synthetic 44.1 kHz stereo sine mix + 1 % noise.
 * ``state_dict_spec``     - (key, shape, kind) for every entry of ``CascadedNet.state_dict()``

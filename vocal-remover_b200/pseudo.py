@@ -1,4 +1,4 @@
-"""B200-native drop-in for the reference's pseudo.py (pseudo-label generation over a directory of track pairs), the
+"""H100-native drop-in for the reference's pseudo.py (pseudo-label generation over a directory of track pairs), the
 second caller of ``Separator.separate_tta`` (pseudo.py:56-74) and the many-file front-end of the hot path.
 
 Same command line (pseudo.py:17-28) and the same outputs (``pseudo/{basename}_PseudoInstruments.npy`` + the empty
@@ -74,7 +74,7 @@ def main():
     args = p.parse_args()
 
     if not torch.cuda.is_available():
-        raise RuntimeError('no CUDA device: the B200 build of vocal-remover has no CPU path')
+        raise RuntimeError('no CUDA device: the H100 build of vocal-remover has no CPU path')
     world = int(os.environ.get('WORLD_SIZE', '1'))
     rank = int(os.environ.get('RANK', '0'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
