@@ -10,9 +10,9 @@
 //     shared-memory tile read through GMMA descriptors whose start address is shifted by kw pixels
 //     (+ kw * 64 B) - no data movement per tap.  The swizzle is a function of the absolute shared-memory
 //     address, so the shifted start needs no matrix-base-offset;
-//   * the weights of the three kh taps are STACKED along the MMA N dimension ([kh=2 | kh=1 | kh=0] x BN couts)
-//     and the R accumulators of a thread are adjacent column blocks of one register fragment, so ONE
-//     wgmma of N = 3*BN adds an input row's contribution to output rows r-2, r-1 and r at once;
+//   * the weights of the three kh taps are stacked ([kh=2 | kh=1 | kh=0] x BN couts) and each of the R output rows
+//     has its own BN-column block of the accumulator fragment; input row r issues one N = BN wgmma per output row
+//     r-2, r-1, r it feeds, all in one commit group (see issue_row for why they are not one N = 3*BN wgmma);
 //   * the 9-tap weight slab of the chunk (3 kw x [3*BN] x 32, hi+lo) is double-buffered in shared memory.
 // L2->SM traffic per output pixel drops from 9 to (R+2)/R operand fetches.
 //
@@ -105,16 +105,18 @@ __device__ __forceinline__ uint32_t chunk_groups(unsigned long long kmask, int c
   return sh + 4 <= 64 ? (uint32_t)(kmask >> sh) & 0xFu : 0xFu;
 }
 
-// The wgmmas of input row r of one chunk: N = cnt * BN into the accumulators of output rows o_lo..o_hi (adjacent column
-// blocks of the fragment).  ksm: k-steps (16 channels) of the chunk that carry weights (bit 0 / 1).  a_hi: descriptor low
-// word of this warpgroup's 64 pixels in the slot's hi plane; bsrc: low word of the chunk's weight buffer.
+// The wgmmas of input row r of one chunk: one N = BN product per output row o_lo..o_hi it feeds, each into that row's
+// own column block of the fragment.  The kh taps are not merged into one N = cnt * BN wgmma: ptxas keeps the wgmma
+// pipeline only if every accumulator register sits at the same position in every wgmma that writes it, and the
+// windows [r-2, r] of consecutive rows overlap at different offsets (ptxas C7511: it then waits for every wgmma to
+// complete before the next; tests/test_sass_wgmma_pipeline.py).  Each output row's sum keeps its order.
+// ksm: k-steps (16 channels) of the chunk that carry weights (bit 0 / 1).  a_hi: descriptor low word of this
+// warpgroup's 64 pixels in the slot's hi plane; bsrc: low word of the chunk's weight buffer.
 template <int BN, int R, int r>
 __device__ __forceinline__ void issue_row(float* acc, uint32_t a_hi, uint32_t bsrc, uint32_t dhi, uint32_t ksm) {
   constexpr int o_lo = r - 2 < 0 ? 0 : r - 2;
   constexpr int o_hi = r > R - 1 ? R - 1 : r;
-  constexpr int cnt = o_hi - o_lo + 1;
   const uint32_t a_lo = a_hi + (kAPlane >> 4);
-  const uint32_t b_row = bsrc + (((uint32_t)((2 - (r - o_lo)) * BN) * kRowB) >> 4);
 #pragma unroll
   for (int kw = 0; kw < 3; ++kw) {
 #pragma unroll
@@ -122,8 +124,11 @@ __device__ __forceinline__ void issue_row(float* acc, uint32_t a_hi, uint32_t bs
       if (!((ksm >> ks) & 1u)) continue;
       const uint32_t ao = (uint32_t)(kw * kRowB + ks * 32) >> 4;
       const uint32_t bo = (uint32_t)(kw * RowsGeom<BN>::kBKw + ks * 32) >> 4;
-      wgmma_split3<cnt * BN>(acc + o_lo * (BN / 2), a_hi + ao, a_lo + ao, b_row + bo,
-                             b_row + bo + (RowsGeom<BN>::kBPlane >> 4), dhi);
+#pragma unroll
+      for (int o = o_lo; o <= o_hi; ++o) {
+        const uint32_t b_row = bsrc + (((uint32_t)((2 - (r - o)) * BN) * kRowB) >> 4) + bo;   // tap kh = r - o
+        wgmma_split3<BN>(acc + o * (BN / 2), a_hi + ao, a_lo + ao, b_row, b_row + (RowsGeom<BN>::kBPlane >> 4), dhi);
+      }
     }
   }
 }
@@ -525,9 +530,9 @@ bool tc_rows_prepare(ConvLayer& L, TcConv& tc, std::string& err, std::vector<voi
   R.ok = false;
   if (L.k != 3 || L.stride != 1 || L.dil_h != 1 || L.dil_w != 1) return true;
   const int cout16 = round_up(L.Cout, 16);
-  // 64 output channels per tile for the decoder layers with a fused upsample: one N = 192 MMA per product instead of two
-  // N = 96 ones (tensor-bound instead of shared-memory-bound) and every input row is interpolated once instead of once per
-  // N tile (dec2: 3.6 -> 2.8 ms).  Plain TMA layers stay at 32: the 64-wide tile has a single accumulator set (no
+  // 64 output channels per tile for the decoder layers with a fused upsample: one N = 64 MMA per product and output row
+  // instead of two N = 32 ones (half the A-operand reads from shared memory) and every input row is interpolated once
+  // instead of once per N tile.  Plain TMA layers stay at 32: the 64-wide tile has a single accumulator set (no
   // epilogue overlap) and only four operand slots next to its 147 KB of weights, and measured slower there.
   R.BN = cout16 == 16 ? 16 : (L.rows_wide && cout16 % 64 == 0 ? 64 : 32);
   R.n_tiles = ceil_div(cout16, R.BN);
