@@ -7,23 +7,22 @@
 //   * each input row (130 pixels incl. the +-1 halo, 32 channels, hi and lo plane) is one TMA load of
 //     a two-plane box; out-of-image rows / columns are zero-filled by TMA = the conv padding;
 //   * a row feeds up to three output rows (kh = 0,1,2) and, for each, the three kw taps are the SAME
-//     shared-memory tile read through GMMA descriptors whose start address is shifted by kw pixels
-//     (+ kw * 64 B) - no data movement per tap.  The swizzle is a function of the absolute shared-memory
-//     address, so the shifted start needs no matrix-base-offset;
+//     shared-memory tile read with ldmatrix at rows shifted by kw pixels - no data movement per tap.  Each A
+//     fragment is loaded into registers once per (row, kw, k-step) and serves every wgmma of the row;
 //   * the weights of the three kh taps are stacked ([kh=2 | kh=1 | kh=0] x BN couts) and each of the R output rows
 //     has its own BN-column block of the accumulator fragment; input row r issues one N = BN wgmma per output row
-//     r-2, r-1, r it feeds, all in one commit group (see issue_row for why they are not one N = 3*BN wgmma);
+//     r-2, r-1, r it feeds (see consume_rows for why they are not one N = 3*BN wgmma);
 //   * the 9-tap weight slab of the chunk (3 kw x [3*BN] x 32, hi+lo) is double-buffered in shared memory.
 // L2->SM traffic per output pixel drops from 9 to (R+2)/R operand fetches.
 //
-// Two consumer warpgroups (warps 0-7) each own 64 of the 128 pixels; warp 8 is the TMA producer.  R is chosen per
-// (BN, fused upsample) so that the R * BN / 2 accumulator registers of a thread fit the register budget of the block.
+// Two consumer warpgroups (warps 0-7) each own 64 of the 128 pixels; warp 8 is the TMA producer.  R is chosen per BN
+// so that the R * BN / 2 accumulator registers of a thread fit the consumers' register budget.
 //
 // Fused decoder upsample (optional, Decoder of lib/layers.py:51-64): the leading `up_chunks` channel chunks of the
 // input are F.interpolate(x2, bilinear, align_corners=True) of a tensor at half resolution.  Instead of reading a
 // materialised up-sampled copy (4x the bytes, and the decoder layers are HBM-bound), ten producer warps
 // interpolate each 130-pixel row from half-resolution rows into the swizzled operand slot
-// (generic-proxy stores + fence.proxy.async + mbarrier arrive), bit-identical to upsample2x_kernel up to the
+// (plain stores + mbarrier arrive; the consumers read the slot with ldmatrix), bit-identical to upsample2x_kernel up to the
 // order of the two blends.
 #include <stdio.h>
 
@@ -38,13 +37,22 @@ static constexpr int kConsumerWarps = 8;            // two warpgroups: pixels [0
 static constexpr int kTmaWarp = kConsumerWarps;
 static constexpr int kInterpWarp0 = kConsumerWarps + 1;
 static constexpr int kMaxR = 8;                     // largest number of output rows per CTA tile (H must be a multiple)
-// output rows per tile: R * BN / 2 accumulator registers per consumer thread.  The warps of a block are spread over the
-// four SM sub-partitions, each with a quarter of the register file: 9 warps (3 per sub-partition) get 168 registers
-// per thread, 19 warps (with the ten interpolation warps, 5 per sub-partition) get 96.
-__host__ __device__ constexpr int rows_per_tile(int BN, bool up) {
-  return up ? (BN == 16 ? 4 : 2) : (BN == 64 ? 2 : BN == 32 ? 4 : 8);
-}
-__host__ __device__ constexpr int rows_threads(bool up) { return 32 * (kConsumerWarps + 1 + (up ? kInterpWarps : 0)); }
+// output rows per tile: R * BN / 2 accumulator registers per consumer thread, next to 32 registers of A fragments.
+// The warps of a block are spread over the four SM sub-partitions, each with 512 registers per lane.  Without the
+// fused upsample the block is 9 warps (3 per sub-partition: 168 registers per thread).  With it the block is five
+// warpgroups (the TMA warp, the ten interpolation warps and one idle warp make three producer warpgroups; 5 warps
+// per sub-partition, 96 registers at launch), and setmaxnreg moves registers from the producer warpgroups to the
+// consumers.  setmaxnreg.inc waits until the block's pool, which holds what the block was launched with, can grant
+// the request: the budgets must add up to no more than 20 warps x 96 registers.
+__host__ __device__ constexpr int rows_per_tile(int BN) { return BN == 64 ? 2 : BN == 32 ? 4 : 8; }
+static constexpr int kUpProducerWarps = 12;
+static constexpr int kUpConsumerRegs = 128;
+static constexpr int kUpProducerRegs = 72;
+static constexpr int kUpLaunchRegs = 96;   // 65536 / 640 threads, rounded down to a multiple of 8
+static_assert(kConsumerWarps * kUpConsumerRegs + kUpProducerWarps * kUpProducerRegs <=
+                  (kConsumerWarps + kUpProducerWarps) * kUpLaunchRegs,
+              "setmaxnreg.inc would wait forever for registers the block does not own");
+__host__ __device__ constexpr int rows_threads(bool up) { return 32 * (kConsumerWarps + (up ? kUpProducerWarps : 1)); }
 static constexpr int kRowPx = 130;                 // 128 + 2 halo pixels
 static constexpr int kBoxPx = 136;                 // pixels per TMA row box: makes one plane 17 x 512 B, so that the lo plane
                                                    // of the two-plane box starts on the SWIZZLE_64B repeat (8 rows x 64 B)
@@ -105,63 +113,76 @@ __device__ __forceinline__ uint32_t chunk_groups(unsigned long long kmask, int c
   return sh + 4 <= 64 ? (uint32_t)(kmask >> sh) & 0xFu : 0xFu;
 }
 
-// The wgmmas of input row r of one chunk: one N = BN product per output row o_lo..o_hi it feeds, each into that row's
-// own column block of the fragment.  The kh taps are not merged into one N = cnt * BN wgmma: ptxas keeps the wgmma
-// pipeline only if every accumulator register sits at the same position in every wgmma that writes it, and the
-// windows [r-2, r] of consecutive rows overlap at different offsets (ptxas C7511: it then waits for every wgmma to
-// complete before the next; tests/test_sass_wgmma_pipeline.py).  Each output row's sum keeps its order.
-// ksm: k-steps (16 channels) of the chunk that carry weights (bit 0 / 1).  a_hi: descriptor low word of this
-// warpgroup's 64 pixels in the slot's hi plane; bsrc: low word of the chunk's weight buffer.
-template <int BN, int R, int r>
-__device__ __forceinline__ void issue_row(float* acc, uint32_t a_hi, uint32_t bsrc, uint32_t dhi, uint32_t ksm) {
-  constexpr int o_lo = r - 2 < 0 ? 0 : r - 2;
-  constexpr int o_hi = r > R - 1 ? R - 1 : r;
-  const uint32_t a_lo = a_hi + (kAPlane >> 4);
-#pragma unroll
-  for (int kw = 0; kw < 3; ++kw) {
-#pragma unroll
-    for (int ks = 0; ks < 2; ++ks) {
-      if (!((ksm >> ks) & 1u)) continue;
-      const uint32_t ao = (uint32_t)(kw * kRowB + ks * 32) >> 4;
-      const uint32_t bo = (uint32_t)(kw * RowsGeom<BN>::kBKw + ks * 32) >> 4;
-#pragma unroll
-      for (int o = o_lo; o <= o_hi; ++o) {
-        const uint32_t b_row = bsrc + (((uint32_t)((2 - (r - o)) * BN) * kRowB) >> 4) + bo;   // tap kh = r - o
-        wgmma_split3<BN>(acc + o * (BN / 2), a_hi + ao, a_lo + ao, b_row, b_row + (RowsGeom<BN>::kBPlane >> 4), dhi);
-      }
-    }
-  }
-}
-
-// Consumer state across the rows of a tile: the A ring position of each producer's ring, the B buffer, and the slots
-// whose wgmma group is still in flight (released once the NEXT group has been committed and the older one waited for).
+// Consumer state across the rows of a tile: the A ring position of each producer's ring, the B buffer, and the weight
+// buffer whose last wgmma group may still be in flight (released once the NEXT group has been committed and the older
+// one waited for).
 struct RowsConsumer {
-  int as_t, as_u, bs, as, pend_a, pend_b;
+  int as_t, as_u, bs, as, pend_b;
   uint32_t aph_t, aph_u, bph, aph;
   int ring_lo, ring_hi;
 };
 
+// Input row r of one chunk.  For each kw tap the warp loads its 16 x 16 A fragments (hi and lo plane, both k-steps) of
+// the slot once with ldmatrix, rows shifted by kw pixels, and every wgmma that needs them reads them from registers:
+// one N = BN product per output row o_lo..o_hi the row feeds, each into that row's own column block of the accumulator
+// fragment (merging the kh taps into one N = cnt * BN wgmma would make the accumulator windows of consecutive rows
+// overlap at different offsets, and ptxas then serialises every wgmma, C7511).  Each kw tap is one commit group; the
+// fragments of two consecutive groups live in the two halves of fr, so a group's fragments are overwritten only after
+// `wait_group 1` has retired it.  The wgmma read only weights from shared memory: the A slot is free once the last
+// ldmatrix of the row has returned.  Every accumulator receives its products in the order chunk, row, kw, k-step,
+// hi*hi, lo*hi, hi*lo.
+// ksm: k-steps (16 channels) of the chunk that carry weights (bit 0 / 1).  lrow: shared-memory address of this lane's
+// ldmatrix row (pixel 64 wg + 16 (warp % 4) + lane % 16) in slot 0; bsrc: descriptor low word of the weight buffer.
 template <int BN, int R, int r>
-__device__ __forceinline__ void consume_rows(RowsConsumer& st, float* acc, uint32_t a_desc0, uint32_t bsrc, uint32_t dhi,
-                                             uint32_t ksm, uint32_t afull0, uint32_t aempty0, uint32_t bempty0,
-                                             int lane) {
+__device__ __forceinline__ void consume_rows(RowsConsumer& st, float* acc, uint32_t (&fr)[2][16], uint32_t lrow,
+                                             uint32_t bsrc, uint32_t dhi, uint32_t ksm, uint32_t afull0,
+                                             uint32_t aempty0, uint32_t bempty0, int lane) {
+  constexpr int o_lo = r - 2 < 0 ? 0 : r - 2;
+  constexpr int o_hi = r > R - 1 ? R - 1 : r;
   mbar_wait(afull0 + (uint32_t)st.as * 8u, st.aph);
-  wg_fence();
-  issue_row<BN, R, r>(acc, a_desc0 + (uint32_t)st.as * (kASlot >> 4), bsrc, dhi, ksm);
-  wg_commit();
-  wg_wait<1>();   // every group but this one is complete: the slots it read can be refilled
-  __syncwarp();
-  if (lane == 0) {
-    if (st.pend_a >= 0) mbar_arrive(aempty0 + (uint32_t)st.pend_a * 8u);
-    if (st.pend_b >= 0) mbar_arrive(bempty0 + (uint32_t)st.pend_b * 8u);
+  const uint32_t row = lrow + (uint32_t)st.as * kASlot;
+#pragma unroll
+  for (int kw = 0; kw < 3; ++kw) {
+    uint32_t* f = fr[(3 * r + kw) & 1];
+    // SWIZZLE_64B: 16-byte chunk j of 64-byte row q sits at chunk j ^ ((q >> 1) & 3) (planes are 512-byte aligned)
+    const uint32_t q = (row >> 6) + (uint32_t)kw;
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {
+      if (!((ksm >> ks) & 1u)) continue;
+      const uint32_t a = (q << 6) + ((((uint32_t)(2 * ks) + ((uint32_t)lane >> 4)) ^ ((q >> 1) & 3u)) << 4);
+      ldsm_x4(f + 8 * ks, a);
+      ldsm_x4(f + 8 * ks + 4, a + kAPlane);
+    }
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {
+      if (!((ksm >> ks) & 1u)) continue;
+      const uint32_t bo = (uint32_t)(kw * RowsGeom<BN>::kBKw + ks * 32) >> 4;
+#pragma unroll
+      for (int o = o_lo; o <= o_hi; ++o) {
+        const uint32_t b_row = bsrc + (((uint32_t)((2 - (r - o)) * BN) * kRowB) >> 4) + bo;   // tap kh = r - o
+        wgmma_split3_rs<BN>(acc + o * (BN / 2), f + 8 * ks, f + 8 * ks + 4, b_row,
+                            b_row + (RowsGeom<BN>::kBPlane >> 4), dhi);
+      }
+    }
+    wg_commit();
+    if (kw == 2) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(aempty0 + (uint32_t)st.as * 8u);
+    }
+    wg_wait<1>();   // every group but this one is complete: its fragments and the weights it read can be reused
+    if (st.pend_b >= 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bempty0 + (uint32_t)st.pend_b * 8u);
+      st.pend_b = -1;
+    }
   }
-  st.pend_a = st.as;
-  st.pend_b = -1;
   if (++st.as == st.ring_hi) {
     st.as = st.ring_lo;
     st.aph ^= 1u;
   }
-  if constexpr (r + 1 < R + 2) consume_rows<BN, R, r + 1>(st, acc, a_desc0, bsrc, dhi, ksm, afull0, aempty0, bempty0, lane);
+  if constexpr (r + 1 < R + 2)
+    consume_rows<BN, R, r + 1>(st, acc, fr, lrow, bsrc, dhi, ksm, afull0, aempty0, bempty0, lane);
 }
 
 // w[c] * act(v0 + bias[c]) + w[c + 1] * act(v1 + bias[c + 1]): this thread's share of the fused single-channel 1x1
@@ -176,7 +197,7 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
     conv_tc_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                         const __grid_constant__ CUtensorMap tmL, const RowsParams p) {
   typedef RowsGeom<BN> G;
-  constexpr int R = rows_per_tile(BN, UP);
+  constexpr int R = rows_per_tile(BN);
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_afull[kMaxASlots];
   __shared__ __align__(8) uint64_t bar_aempty[kMaxASlots];
@@ -210,74 +231,24 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
     dot_s[i] = p.dot_out && i < p.Cout ? __ldg(p.dot_w + i) : 0.f;
   }
   __syncthreads();
-
-  if (warp == kTmaWarp) {
-    // ===================== TMA producer: one elected lane runs the whole loop nest =====================
-    if (elect_one_sync()) {
-      int as = p.n_uslots, bs = 0;
-      uint32_t aph = 0, bph = 0;
-      const uint32_t afull0 = smem_u32(&bar_afull[0]), aempty0 = smem_u32(&bar_aempty[0]);
-#ifdef VR_TRACE
-      const bool tr = p.trace && blockIdx.x == 0;
-#else
-      constexpr bool tr = false;
-#endif
-      int tn = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        const int nt = tile % p.n_tiles;
-        int mt = tile / p.n_tiles;
-        const int w0 = (mt % p.tiles_w) * 128;
-        mt /= p.tiles_w;
-        const int h0 = (mt % p.tiles_h) * R;
-        const int n = mt / p.tiles_h;
-        for (int cc = 0; cc < p.chunks; ++cc) {
-          mbar_wait(smem_u32(&bar_bempty[bs]), bph ^ 1u);
-          const uint32_t bfull = smem_u32(&bar_bfull[bs]);
-          const uint32_t bdst = b_base + (uint32_t)bs * G::kBBuf;
-          mbar_expect_tx(bfull, G::kBBuf);
-#pragma unroll
-          for (int kw = 0; kw < 3; ++kw)
-            tma_load_3d(bdst + (uint32_t)kw * G::kBKw, &tmB, kw * p.CinPadR + cc * (int)kKB, nt * 3 * BN, 0, bfull);
-          if (++bs == 2) {
-            bs = 0;
-            bph ^= 1u;
-          }
-          if (cc < p.up_chunks) continue;   // rows of this chunk are produced by the interpolation warps
-          const bool from_l = cc == p.l_chunk;
-          const int c0 = from_l ? 0 : cc * (int)kKB + p.a_c_off;
-          for (int r = 0; r < R + 2; ++r) {
-            const unsigned long long t0 = tr ? clock64() : 0ull;
-            mbar_wait(aempty0 + (uint32_t)as * 8u, aph ^ 1u);
-            const uint32_t afull = afull0 + (uint32_t)as * 8u;
-            mbar_expect_tx(afull, kASlot);
-            tma_load_5d(a_base + (uint32_t)as * kASlot, from_l ? &tmL : &tmA, c0, w0 - 1, h0 - 1 + r, n, 0, afull);
-            if (tr && tn < kTraceEvents) {
-              g_rows_trace[(1 * kTraceEvents + tn) * 3 + 0] = t0;
-              g_rows_trace[(1 * kTraceEvents + tn) * 3 + 1] = clock64();
-              g_rows_trace[(1 * kTraceEvents + tn) * 3 + 2] = 0ull;
-              ++tn;
-            }
-            if (++as == p.n_aslots) {
-              as = p.n_uslots;
-              aph ^= 1u;
-            }
-          }
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp < kConsumerWarps) {
+  // Consumers and producers split first: each producer warpgroup (with UP: the TMA warp with interpolation warps 0-2,
+  // interpolation warps 3-6, interpolation warps 7-9 with the idle warp) executes the one setmaxnreg.dec below, as
+  // setmaxnreg requires of all threads of a warpgroup, and ptxas allocates the consumer code for kUpConsumerRegs
+  // because no producer path reaches it.
+  if (warp < kConsumerWarps) {
     // ===================== consumer warpgroups: wgmma into registers, then the epilogue =====================
+    if constexpr (UP) setmaxnreg_inc<kUpConsumerRegs>();
     const int wg = warp >> 2;   // pixels [64 wg, 64 wg + 64) of the tile
     const float slope = p.act == ACT_RELU ? 0.f : p.act == ACT_LEAKY ? 0.01f : 1.f;
     const uint32_t dhi = desc_hi(8 * kRowB, 2u);   // SWIZZLE_64B, 8-row groups of 64-byte rows
     const uint32_t afull0 = smem_u32(&bar_afull[0]), aempty0 = smem_u32(&bar_aempty[0]);
     const uint32_t bempty0 = smem_u32(&bar_bempty[0]);
-    const uint32_t a_desc0 = desc_lo(a_base) + ((uint32_t)(64 * wg) * kRowB >> 4);
+    const uint32_t lrow = a_base + (uint32_t)(64 * wg + 16 * (warp & 3) + (lane & 15)) * kRowB;
     RowsConsumer st;
-    st.as_t = p.n_uslots; st.as_u = 0; st.bs = 0; st.pend_a = -1; st.pend_b = -1;
+    st.as_t = p.n_uslots; st.as_u = 0; st.bs = 0; st.pend_b = -1;
     st.aph_t = 0; st.aph_u = 0; st.bph = 0;
     float acc[R * BN / 2];
+    uint32_t fr[2][16];
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
 #pragma unroll
       for (int i = 0; i < R * BN / 2; ++i) acc[i] = 0.f;
@@ -294,7 +265,7 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
         st.aph = up ? st.aph_u : st.aph_t;
         st.ring_lo = up ? 0 : p.n_uslots;
         st.ring_hi = up ? p.n_uslots : p.n_aslots;
-        consume_rows<BN, R, 0>(st, acc, a_desc0, bsrc, dhi, ksm, afull0, aempty0, bempty0, lane);
+        consume_rows<BN, R, 0>(st, acc, fr, lrow, bsrc, dhi, ksm, afull0, aempty0, bempty0, lane);
         if (up) {
           st.as_u = st.as;
           st.aph_u = st.aph;
@@ -310,11 +281,8 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
       }
       wg_wait<0>();
       __syncwarp();
-      if (lane == 0) {
-        if (st.pend_a >= 0) mbar_arrive(aempty0 + (uint32_t)st.pend_a * 8u);
-        if (st.pend_b >= 0) mbar_arrive(bempty0 + (uint32_t)st.pend_b * 8u);
-      }
-      st.pend_a = st.pend_b = -1;
+      if (lane == 0 && st.pend_b >= 0) mbar_arrive(bempty0 + (uint32_t)st.pend_b * 8u);
+      st.pend_b = -1;
 
       const int nt = tile % p.n_tiles;
       int mt = tile / p.n_tiles;
@@ -345,182 +313,238 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
         }
       }
     }
-  } else if (UP && warp >= kInterpWarp0) {
-    // ===================== bilinear x2 producer (kInterpWarps autonomous warps) =====================
-    // align_corners=True bilinear x2 (ATen upsample_bilinear2d / upsample2x_kernel weights; the vertical blend is done
-    // first here).  Warp k owns the source pixels xs + [7k, 7k+7) of the row (+ pixel 7k+7 as right neighbour): lane =
-    // (source pixel, 8-channel group) reads its two source rows (hi and lo plane: four 16-byte global loads, issued one
-    // row AHEAD so that their latency overlaps the previous row's arithmetic), blends them vertically in registers,
-    // fetches the right neighbour's blend by shuffle and emits the 2-3 output pixels whose left source pixel it is,
-    // split to hi/lo, straight into the SWIZZLE_64B slot.  Which output pixels those are (and their horizontal weights
-    // and slot offsets) depends only on the tile: computed once per tile.  No block-wide barrier and no shared-memory
-    // staging (the tensor pipe already uses the full shared-memory bandwidth for its operands): every warp waits for
-    // the slot (released by the consumer warps) itself and arrives on the slot's mbarrier (count = kInterpWarps).
-    if (p.up_chunks > 0) {
-      const int wk = warp - kInterpWarp0;
-      const int xi = lane >> 2, j = lane & 3;
-      const int sx = 7 * wk + xi;              // source pixel of this lane, relative to xs
-      const bool emit = xi < 7 && sx < kSrcPx; // xi == 7 only provides the neighbour of xi == 6
-      int as = 0;
-      uint32_t aph = 0;
-      const uint32_t afull0 = smem_u32(&bar_afull[0]), aempty0 = smem_u32(&bar_aempty[0]);
-      const float inv_sw = p.up_sw > 0.f ? 1.f / p.up_sw : 0.f;
+  } else {
+    if constexpr (UP) setmaxnreg_dec<kUpProducerRegs>();
+    if (warp == kTmaWarp) {
+      // ===================== TMA producer: one elected lane runs the whole loop nest =====================
+      if (elect_one_sync()) {
+        int as = p.n_uslots, bs = 0;
+        uint32_t aph = 0, bph = 0;
+        const uint32_t afull0 = smem_u32(&bar_afull[0]), aempty0 = smem_u32(&bar_aempty[0]);
 #ifdef VR_TRACE
-      const bool tr = p.trace && blockIdx.x == 0 && wk == 0;
+        const bool tr = p.trace && blockIdx.x == 0;
 #else
-      constexpr bool tr = false;
+        constexpr bool tr = false;
 #endif
-      int tn = 0;
-      const int my_tiles = (p.total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-      const int fills = my_tiles * p.up_chunks * (R + 2);
-      // iteration state of the NEXT row to fetch (one ahead of the row being written); the tile decomposition
-      // (divisions) is redone only when the fetch moves on to another tile
-      int f_tile = blockIdx.x, f_cc = 0, f_r = 0, f_h0 = 0, f_X = 0;
-      int64_t f_base = 0;
-      bool f_px = false;
-      auto fetch_tile = [&]() {
-        int mt = f_tile / p.n_tiles;
-        const int w0 = (mt % p.tiles_w) * 128;
-        mt /= p.tiles_w;
-        f_h0 = (mt % p.tiles_h) * R - 1;
-        f_X = (int)(p.up_sw * (w0 > 0 ? w0 - 1 : 0)) + sx;
-        f_px = sx < kSrcPx && f_X < p.xW;
-        f_base = (int64_t)(mt / p.tiles_h) * p.xsn + (int64_t)f_X * p.xsw + j * 8;
-      };
-      fetch_tile();
-      // Two rows are in flight: the loads of row k+2 are issued right after the proxy fence of row k (fence.proxy.async
-      // compiles to MEMBAR.ALL.CTA + FENCE.VIEW.ASYNC and the MEMBAR waits for every global load still in flight), so that
-      // they have the whole of row k+1 to land before the next fence.  q* = row k+1, n* = row k+2.
-      bf16x8 qah, qch, qal, qcl, nah, nch, nal, ncl;   // rows y0 / y1 of the hi plane, rows y0 / y1 of the lo plane
-      float q_ly = 0.f, n_ly = 0.f;
-      bool q_ok = false, n_ok = false;
-      qah = qch = qal = qcl = nah = nch = nal = ncl = make_uint4(0, 0, 0, 0);
-      auto fetch = [&]() {
-        qah = nah; qch = nch; qal = nal; qcl = ncl;
-        q_ly = n_ly;
-        q_ok = n_ok;
-        const int h = f_h0 + f_r;
-        const bool grp = (chunk_groups(p.kmask, f_cc) >> j) & 1u;   // channel group without weights: zeros are written
-        n_ok = f_tile < p.total_tiles && h >= 0 && h < p.H && grp && f_px;
-        if (n_ok) {
-          const float fy = p.up_sh * h;
-          const int y0 = (int)fy;
-          n_ly = fy - (float)y0;
-          const int64_t o0 = f_base + (int64_t)y0 * p.xsh + f_cc * 32;
-          const int64_t o1 = o0 + (y0 < p.xH - 1 ? p.xsh : 0);
-          nah = ld128(p.x_hi + o0);
-          nch = ld128(p.x_hi + o1);
-          nal = ld128(p.x_lo + o0);
-          ncl = ld128(p.x_lo + o1);
-        }
-        if (++f_r == R + 2) {
-          f_r = 0;
-          if (++f_cc == p.up_chunks) {
-            f_cc = 0;
-            f_tile += gridDim.x;
-            if (f_tile < p.total_tiles) fetch_tile();
-          }
-        }
-      };
-      if (fills > 0) {
-        fetch();   // row 0
-        fetch();   // row 1 (row 0 moves to q*)
-      }
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        int mt = tile / p.n_tiles;
-        const int w0 = (mt % p.tiles_w) * 128;
-        const int X = (int)(p.up_sw * (w0 > 0 ? w0 - 1 : 0)) + sx;   // absolute source pixel
-        // the output pixels w with (int)(up_sw * w) == X lie in [wc - 1, wc + 3] and there are at most 3 of them
-        int e_off[3];
-        float e_lx[3];
+        int tn = 0;
+        for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+          const int nt = tile % p.n_tiles;
+          int mt = tile / p.n_tiles;
+          const int w0 = (mt % p.tiles_w) * 128;
+          mt /= p.tiles_w;
+          const int h0 = (mt % p.tiles_h) * R;
+          const int n = mt / p.tiles_h;
+          for (int cc = 0; cc < p.chunks; ++cc) {
+            mbar_wait(smem_u32(&bar_bempty[bs]), bph ^ 1u);
+            const uint32_t bfull = smem_u32(&bar_bfull[bs]);
+            const uint32_t bdst = b_base + (uint32_t)bs * G::kBBuf;
+            mbar_expect_tx(bfull, G::kBBuf);
 #pragma unroll
-        for (int k = 0; k < 3; ++k) e_off[k] = -1;
-        if (emit) {
-          const int wc = (int)((float)X * inv_sw);
-          int cnt = 0;
-#pragma unroll
-          for (int dw = -1; dw <= 3; ++dw) {
-            const int w = wc + dw;
-            const float fx = p.up_sw * (float)w;
-            if (w < 0 || w >= p.W || (int)fx != X || w < w0 - 1 || w > w0 + 128) continue;
-            const int q = w - (w0 - 1);
-            // SWIZZLE_64B (same pattern TMA writes and wgmma reads): 16-byte chunk j of 64-byte row q sits at chunk
-            // j ^ ((q >> 1) & 3) because the XOR takes address bits [7,9) and the planes are 512-byte aligned
-            const int off = q * 64 + ((j ^ ((q >> 1) & 3)) << 4);
-            const float lx = fx - (float)X;
-            if (cnt == 0) { e_off[0] = off; e_lx[0] = lx; }
-            else if (cnt == 1) { e_off[1] = off; e_lx[1] = lx; }
-            else if (cnt == 2) { e_off[2] = off; e_lx[2] = lx; }
-            ++cnt;
-          }
-        }
-        // conv padding columns of the row: slot pixel 0 at the left image border, slot pixel 129 at the right one
-        int z_off = -1;
-        if (wk == 0 && lane < 8) {
-          const int q = lane < 4 ? 0 : kRowPx - 1;
-          const int w = w0 - 1 + q;
-          if (w < 0 || w >= p.W) z_off = q * 64 + ((j ^ ((q >> 1) & 3)) << 4);
-        }
-        const bool last_px = X >= p.xW - 1;   // x1 = x0 on the last source pixel (upsample2x_kernel)
-        for (int cc = 0; cc < p.up_chunks; ++cc) {
-          for (int r = 0; r < R + 2; ++r) {
-            const unsigned long long t0 = tr ? clock64() : 0ull;
-            float v[8];
-            if (q_ok) {
-              float a[8], c[8];
-              unpack8(qah, qal, a);
-              unpack8(qch, qcl, c);
-              const float ly = q_ly, hy = 1.f - q_ly;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) v[i] = hy * a[i] + ly * c[i];
-            } else {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) v[i] = 0.f;
+            for (int kw = 0; kw < 3; ++kw)
+              tma_load_3d(bdst + (uint32_t)kw * G::kBKw, &tmB, kw * p.CinPadR + cc * (int)kKB, nt * 3 * BN, 0, bfull);
+            if (++bs == 2) {
+              bs = 0;
+              bph ^= 1u;
             }
-            float nv[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float t = __shfl_down_sync(0xffffffffu, v[i], 4);
-              nv[i] = last_px ? v[i] : t;
-            }
-            const unsigned long long t1 = tr ? clock64() : 0ull;
-            mbar_wait(aempty0 + (uint32_t)as * 8u, aph ^ 1u);
-            const unsigned long long t2 = tr ? clock64() : 0ull;
-            uint8_t* slot = smem_raw + (a_base - smem_u32(smem_raw)) + (size_t)as * kASlot;
-#pragma unroll
-            for (int k = 0; k < 3; ++k) {
-              if (e_off[k] < 0) continue;
-              const float lx = e_lx[k], hx = 1.f - lx;
-              float y[8];
-#pragma unroll
-              for (int i = 0; i < 8; ++i) y[i] = hx * v[i] + lx * nv[i];
-              bf16x8 oh, ol;
-              split8(y, oh, ol);
-              *reinterpret_cast<uint4*>(slot + e_off[k]) = oh;
-              *reinterpret_cast<uint4*>(slot + kAPlane + e_off[k]) = ol;
-            }
-            if (z_off >= 0) {
-              *reinterpret_cast<uint4*>(slot + z_off) = make_uint4(0, 0, 0, 0);
-              *reinterpret_cast<uint4*>(slot + kAPlane + z_off) = make_uint4(0, 0, 0, 0);
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> async proxy (wgmma)
-            __syncwarp();
-            if (lane == 0) mbar_arrive(afull0 + (uint32_t)as * 8u);
-            fetch();   // row k+2 (after the fence, see above); past the last row it only shifts the pipeline
-            if (tr && lane == 0 && tn < kTraceEvents) {
-              g_rows_trace[(2 * kTraceEvents + tn) * 3 + 0] = t0;
-              g_rows_trace[(2 * kTraceEvents + tn) * 3 + 1] = t2 - t1;   // cycles spent waiting for the slot
-              g_rows_trace[(2 * kTraceEvents + tn) * 3 + 2] = clock64();
-            }
-            ++tn;
-            if (++as == p.n_uslots) {
-              as = 0;
-              aph ^= 1u;
+            if (cc < p.up_chunks) continue;   // rows of this chunk are produced by the interpolation warps
+            const bool from_l = cc == p.l_chunk;
+            const int c0 = from_l ? 0 : cc * (int)kKB + p.a_c_off;
+            for (int r = 0; r < R + 2; ++r) {
+              const unsigned long long t0 = tr ? clock64() : 0ull;
+              mbar_wait(aempty0 + (uint32_t)as * 8u, aph ^ 1u);
+              const uint32_t afull = afull0 + (uint32_t)as * 8u;
+              mbar_expect_tx(afull, kASlot);
+              tma_load_5d(a_base + (uint32_t)as * kASlot, from_l ? &tmL : &tmA, c0, w0 - 1, h0 - 1 + r, n, 0, afull);
+              if (tr && tn < kTraceEvents) {
+                g_rows_trace[(1 * kTraceEvents + tn) * 3 + 0] = t0;
+                g_rows_trace[(1 * kTraceEvents + tn) * 3 + 1] = clock64();
+                g_rows_trace[(1 * kTraceEvents + tn) * 3 + 2] = 0ull;
+                ++tn;
+              }
+              if (++as == p.n_aslots) {
+                as = p.n_uslots;
+                aph ^= 1u;
+              }
             }
           }
         }
       }
-    }
+      __syncwarp();
+    } else if (UP && warp < kInterpWarp0 + kInterpWarps) {
+      // ===================== bilinear x2 producer (kInterpWarps autonomous warps) =====================
+      // align_corners=True bilinear x2 (ATen upsample_bilinear2d / upsample2x_kernel weights; the vertical blend is done
+      // first here).  Warp k owns the source pixels xs + [7k, 7k+7) of the row (+ pixel 7k+7 as right neighbour): lane =
+      // (source pixel, 8-channel group) reads its two source rows (hi and lo plane: four 16-byte global loads, issued one
+      // row AHEAD so that their latency overlaps the previous row's arithmetic), blends them vertically in registers,
+      // fetches the right neighbour's blend by shuffle and emits the 2-3 output pixels whose left source pixel it is,
+      // split to hi/lo, straight into the SWIZZLE_64B slot.  Which output pixels those are (and their horizontal weights
+      // and slot offsets) depends only on the tile: computed once per tile.  No block-wide barrier and no shared-memory
+      // staging (it would add shared-memory traffic next to the consumers' operand reads): every warp waits for
+      // the slot (released by the consumer warps) itself and arrives on the slot's mbarrier (count = kInterpWarps).
+      if (p.up_chunks > 0) {
+        const int wk = warp - kInterpWarp0;
+        const int xi = lane >> 2, j = lane & 3;
+        const int sx = 7 * wk + xi;              // source pixel of this lane, relative to xs
+        const bool emit = xi < 7 && sx < kSrcPx; // xi == 7 only provides the neighbour of xi == 6
+        int as = 0;
+        uint32_t aph = 0;
+        const uint32_t afull0 = smem_u32(&bar_afull[0]), aempty0 = smem_u32(&bar_aempty[0]);
+        const float inv_sw = p.up_sw > 0.f ? 1.f / p.up_sw : 0.f;
+#ifdef VR_TRACE
+        const bool tr = p.trace && blockIdx.x == 0 && wk == 0;
+#else
+        constexpr bool tr = false;
+#endif
+        int tn = 0;
+        const int my_tiles = (p.total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+        const int fills = my_tiles * p.up_chunks * (R + 2);
+        // iteration state of the NEXT row to fetch (one ahead of the row being written); the tile decomposition
+        // (divisions) is redone only when the fetch moves on to another tile
+        int f_tile = blockIdx.x, f_cc = 0, f_r = 0, f_h0 = 0, f_X = 0;
+        int64_t f_base = 0;
+        bool f_px = false;
+        auto fetch_tile = [&]() {
+          int mt = f_tile / p.n_tiles;
+          const int w0 = (mt % p.tiles_w) * 128;
+          mt /= p.tiles_w;
+          f_h0 = (mt % p.tiles_h) * R - 1;
+          f_X = (int)(p.up_sw * (w0 > 0 ? w0 - 1 : 0)) + sx;
+          f_px = sx < kSrcPx && f_X < p.xW;
+          f_base = (int64_t)(mt / p.tiles_h) * p.xsn + (int64_t)f_X * p.xsw + j * 8;
+        };
+        fetch_tile();
+        // Two rows are in flight: the loads of row k+2 are issued right after row k has been stored and announced, so
+        // that they have the whole of row k+1 to land.  q* = row k+1, n* = row k+2.
+        bf16x8 qah, qch, qal, qcl, nah, nch, nal, ncl;   // rows y0 / y1 of the hi plane, rows y0 / y1 of the lo plane
+        float q_ly = 0.f, n_ly = 0.f;
+        qah = qch = qal = qcl = nah = nch = nal = ncl = make_uint4(0, 0, 0, 0);
+        auto fetch = [&]() {
+          qah = nah; qch = nch; qal = nal; qcl = ncl;
+          q_ly = n_ly;
+          const int h = f_h0 + f_r;
+          const bool grp = (chunk_groups(p.kmask, f_cc) >> j) & 1u;   // channel group without weights: zeros are written
+          // a row without source data (image border, past the last tile, no weights) keeps all-zero registers, which
+          // blend to +0 exactly: no flag has to travel with the row
+          if (f_tile < p.total_tiles && h >= 0 && h < p.H && grp && f_px) {
+            const float fy = p.up_sh * h;
+            const int y0 = (int)fy;
+            n_ly = fy - (float)y0;
+            const int64_t o0 = f_base + (int64_t)y0 * p.xsh + f_cc * 32;
+            const int64_t o1 = o0 + (y0 < p.xH - 1 ? p.xsh : 0);
+            nah = ld128(p.x_hi + o0);
+            nch = ld128(p.x_hi + o1);
+            nal = ld128(p.x_lo + o0);
+            ncl = ld128(p.x_lo + o1);
+          } else {
+            nah = nch = nal = ncl = make_uint4(0, 0, 0, 0);
+          }
+          if (++f_r == R + 2) {
+            f_r = 0;
+            if (++f_cc == p.up_chunks) {
+              f_cc = 0;
+              f_tile += gridDim.x;
+              if (f_tile < p.total_tiles) fetch_tile();
+            }
+          }
+        };
+        if (fills > 0) {
+          fetch();   // row 0
+          fetch();   // row 1 (row 0 moves to q*)
+        }
+        for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+          int mt = tile / p.n_tiles;
+          const int w0 = (mt % p.tiles_w) * 128;
+          const int X = (int)(p.up_sw * (w0 > 0 ? w0 - 1 : 0)) + sx;   // absolute source pixel
+          // the output pixels w with (int)(up_sw * w) == X lie in [wc - 1, wc + 3] and there are at most 3 of them
+          int e_off[3];
+          float e_lx[3];
+#pragma unroll
+          for (int k = 0; k < 3; ++k) e_off[k] = -1;
+          if (emit) {
+            const int wc = (int)((float)X * inv_sw);
+            int cnt = 0;
+#pragma unroll
+            for (int dw = -1; dw <= 3; ++dw) {
+              const int w = wc + dw;
+              const float fx = p.up_sw * (float)w;
+              if (w < 0 || w >= p.W || (int)fx != X || w < w0 - 1 || w > w0 + 128) continue;
+              const int q = w - (w0 - 1);
+              // SWIZZLE_64B (same pattern TMA writes and the consumers' ldmatrix reads): 16-byte chunk j of 64-byte row q sits at chunk
+              // j ^ ((q >> 1) & 3) because the XOR takes address bits [7,9) and the planes are 512-byte aligned
+              const int off = q * 64 + ((j ^ ((q >> 1) & 3)) << 4);
+              const float lx = fx - (float)X;
+              if (cnt == 0) { e_off[0] = off; e_lx[0] = lx; }
+              else if (cnt == 1) { e_off[1] = off; e_lx[1] = lx; }
+              else if (cnt == 2) { e_off[2] = off; e_lx[2] = lx; }
+              ++cnt;
+            }
+          }
+          // conv padding columns of the row: slot pixel 0 at the left image border, slot pixel 129 at the right one
+          int z_off = -1;
+          if (wk == 0 && lane < 8) {
+            const int q = lane < 4 ? 0 : kRowPx - 1;
+            const int w = w0 - 1 + q;
+            if (w < 0 || w >= p.W) z_off = q * 64 + ((j ^ ((q >> 1) & 3)) << 4);
+          }
+          const bool last_px = X >= p.xW - 1;   // x1 = x0 on the last source pixel (upsample2x_kernel)
+          for (int cc = 0; cc < p.up_chunks; ++cc) {
+            for (int r = 0; r < R + 2; ++r) {
+              const unsigned long long t0 = tr ? clock64() : 0ull;
+              float v[8];
+              {
+                float a[8], c[8];
+                unpack8(qah, qal, a);
+                unpack8(qch, qcl, c);
+                const float ly = q_ly, hy = 1.f - q_ly;
+#pragma unroll
+                for (int i = 0; i < 8; ++i) v[i] = hy * a[i] + ly * c[i];
+              }
+              float nv[8];
+#pragma unroll
+              for (int i = 0; i < 8; ++i) {
+                const float t = __shfl_down_sync(0xffffffffu, v[i], 4);
+                nv[i] = last_px ? v[i] : t;
+              }
+              const unsigned long long t1 = tr ? clock64() : 0ull;
+              mbar_wait(aempty0 + (uint32_t)as * 8u, aph ^ 1u);
+              const unsigned long long t2 = tr ? clock64() : 0ull;
+              uint8_t* slot = smem_raw + (a_base - smem_u32(smem_raw)) + (size_t)as * kASlot;
+#pragma unroll
+              for (int k = 0; k < 3; ++k) {
+                if (e_off[k] < 0) continue;
+                const float lx = e_lx[k], hx = 1.f - lx;
+                float y[8];
+#pragma unroll
+                for (int i = 0; i < 8; ++i) y[i] = hx * v[i] + lx * nv[i];
+                bf16x8 oh, ol;
+                split8(y, oh, ol);
+                *reinterpret_cast<uint4*>(slot + e_off[k]) = oh;
+                *reinterpret_cast<uint4*>(slot + kAPlane + e_off[k]) = ol;
+              }
+              if (z_off >= 0) {
+                *reinterpret_cast<uint4*>(slot + z_off) = make_uint4(0, 0, 0, 0);
+                *reinterpret_cast<uint4*>(slot + kAPlane + z_off) = make_uint4(0, 0, 0, 0);
+              }
+              // no fence.proxy.async: the slot is read by the consumers' ldmatrix (generic proxy), never by wgmma or TMA;
+              // the arrive's release and the consumers' acquiring wait order the stores before those reads
+              __syncwarp();
+              if (lane == 0) mbar_arrive(afull0 + (uint32_t)as * 8u);
+              fetch();   // row k+2 (after the arrive, see above); past the last row it only shifts the pipeline
+              if (tr && lane == 0 && tn < kTraceEvents) {
+                g_rows_trace[(2 * kTraceEvents + tn) * 3 + 0] = t0;
+                g_rows_trace[(2 * kTraceEvents + tn) * 3 + 1] = t2 - t1;   // cycles spent waiting for the slot
+                g_rows_trace[(2 * kTraceEvents + tn) * 3 + 2] = clock64();
+              }
+              ++tn;
+              if (++as == p.n_uslots) {
+                as = 0;
+                aph ^= 1u;
+              }
+            }
+          }
+        }
+      }
+      }
   }
 }
 
@@ -663,7 +687,7 @@ cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   RowsParams p;
   p.N = out.N; p.H = out.H; p.W = out.W;
   const bool up = up_src != nullptr;
-  p.tiles_w = out.W / 128; p.tiles_h = out.H / rows_per_tile(R.BN, up); p.n_tiles = R.n_tiles;
+  p.tiles_w = out.W / 128; p.tiles_h = out.H / rows_per_tile(R.BN); p.n_tiles = R.n_tiles;
   p.total_tiles = p.tiles_w * p.tiles_h * out.N * R.n_tiles;
   p.chunks = R.chunks; p.CinPadR = R.CinPadR; p.Cout = L.Cout; p.act = L.act;
   p.out_hi = out.hi; p.out_lo = out.lo;

@@ -196,6 +196,67 @@ __device__ __forceinline__ void wgmma_split3(float* d, uint32_t a_hi, uint32_t a
   Wgmma<N>::mma(d, desc64(a_hi, dhi), desc64(b_lo, dhi));
 }
 
+// D[64][N] += A[64][16] * B[N][16]^T with A from registers: a[4] is the m16n8k16-style fragment of the warp's 16 rows
+// (rows m, m + 8 at channels 2*(t%4) + {0,1} and + 8), as ldmatrix.x4 of the 16 x 16 tile returns it; B as above.
+template <int N>
+struct WgmmaRS;
+template <>
+struct WgmmaRS<16> {
+  static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t b) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, 1, 1, 1, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b)
+        : "memory");
+  }
+};
+template <>
+struct WgmmaRS<32> {
+  static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t b) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, 1, 1, 1, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b)
+        : "memory");
+  }
+};
+template <>
+struct WgmmaRS<64> {
+  static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t b) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, 1, 1, 1, 0;"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b)
+        : "memory");
+  }
+};
+// The same three products with the A operands held in registers (a_hi[4], a_lo[4])
+template <int N>
+__device__ __forceinline__ void wgmma_split3_rs(float* d, const uint32_t* a_hi, const uint32_t* a_lo, uint32_t b_hi,
+                                                uint32_t b_lo, uint32_t dhi) {
+  WgmmaRS<N>::mma(d, a_hi, desc64(b_hi, dhi));
+  WgmmaRS<N>::mma(d, a_lo, desc64(b_hi, dhi));
+  WgmmaRS<N>::mma(d, a_hi, desc64(b_lo, dhi));
+}
+
+// four 8x8 bf16 matrices from shared memory: lane l supplies the address of row l % 8 of matrix l / 8
+__device__ __forceinline__ void ldsm_x4(uint32_t* r, uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+
+// per-thread register budget of the executing warpgroup (every thread of the warpgroup executes it)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+
 // bias + activation + split-bf16 store of the two adjacent channels (c, c + 1) a thread holds of one pixel.
 // slope: 0 = ReLU, 0.01 = LeakyReLU, 1 = identity  (y = max(v,0) + slope*min(v,0), branch-free)
 __device__ __forceinline__ void epilogue_pair(float v0, float v1, const float* bias_s, int c, int Cout, float slope,
