@@ -219,6 +219,7 @@ const TcDevice& tc_device() {
     VR_TC_FOR_ALL(VR_TC_SET_SMEM)
 #undef VR_TC_SET_SMEM
     tc_rows_set_attributes(d.max_smem);
+    tc_halo_set_attributes(d.max_smem);
     d.ok = true;
   }
   return d;
@@ -352,6 +353,7 @@ bool tc_prepare(ConvLayer& L, std::string& err, std::vector<void*>& allocs) {
     return false;
   }
   if (!tc_rows_prepare(L, *tc, err, allocs)) return false;
+  if (!tc_halo_prepare(L, *tc, err, allocs)) return false;
   L.tc = tc;
   return true;
 }
@@ -364,6 +366,7 @@ cudaError_t tc_launch(ConvLayer& L, const ActView& in, const ActView& out, cudaS
     err = "tc_launch: fused upsample is only implemented in the row-streaming kernel";
     return cudaErrorInvalidValue;
   }
+  if (tc_halo_supported(L, tc, in, out)) return tc_halo_launch(L, tc, in, out, s, err);
   const TileGeom g = tile_geom(out.H, out.W);
   auto key = std::make_tuple((const void*)in.hi, (const void*)in.lo, in.N, in.H, in.W, in.C);
   auto it = tc.map_a.find(key);

@@ -107,12 +107,6 @@ struct RowsParams {
   float* dot_out;
 };
 
-// 8-channel groups of chunk cc that carry any non-zero weight (4 bits per 32-channel chunk)
-__device__ __forceinline__ uint32_t chunk_groups(unsigned long long kmask, int cc) {
-  const int sh = cc * 4;
-  return sh + 4 <= 64 ? (uint32_t)(kmask >> sh) & 0xFu : 0xFu;
-}
-
 // Consumer state across the rows of a tile: the A ring position of each producer's ring, the B buffer, and the weight
 // buffer whose last wgmma group may still be in flight (released once the NEXT group has been committed and the older
 // one waited for).
