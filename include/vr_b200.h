@@ -124,6 +124,20 @@ VR_API int vr_separate_wave(vr_ctx* ctx, const float* wave, int64_t L, int32_t t
 VR_API int vr_separate_wave_host(vr_ctx* ctx, const float* wave_host, int64_t L, int32_t tta, float* inst_host,
                           float* voc_host, void* stream);
 
+/* vr_separate_wave_host plus the --output_image spectrogram images of both stems (inference.py:180-185), built on
+ * the device from the final spectrogram and mask: img_inst_host / img_voc_host are HOST uint8 [bins][T][3] buffers,
+ * or NULL for none (both NULL = vr_separate_wave_host).  The stems are the same as vr_separate_wave_host's.      */
+VR_API int vr_separate_wave_host_images(vr_ctx* ctx, const float* wave_host, int64_t L, int32_t tta, float* inst_host,
+                                        float* voc_host, uint8_t* img_inst_host, uint8_t* img_voc_host, void* stream);
+
+/* spec_utils.spectrogram_to_image(spec) in magnitude mode (lib/spec_utils.py:34-57) for spec [2][bins][T]:
+ * img [bins][T][3] uint8 = {max(L, R), L, R} of trunc(255 * (l - min l) / (max l - min l)), l = log10(|s|^2 + 1e-8),
+ * min / max over the whole array.  mask != NULL: img_a = image of mask * spec (y_spec of inference.py:32-36) and
+ * img_b = image of (1 - mask) * spec (v_spec); mask == NULL: img_a = image of spec, img_b unused.  A constant
+ * array (max == min, e.g. a silent track) gives an all-zero image (the reference's cast then sees NaN).          */
+VR_API int vr_spec_image(vr_ctx* ctx, const void* spec, const float* mask, int64_t T, uint8_t* img_a, uint8_t* img_b,
+                         void* stream);
+
 /* The sample-rate conversion inside librosa.load(path, sr=args.sr, res_type='kaiser_fast') (inference.py:136-138,
  * pseudo.py:47-50) = resampy.resample(y, orig_sr, sr, filter='kaiser_fast'): x [channels][n_in] -> y [channels][n_out],
  * n_out = (int64)(n_in * sample_ratio), sample_ratio = sr / orig_sr.  win / delta: DEVICE float64 arrays of nwin entries -

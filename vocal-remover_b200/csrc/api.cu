@@ -191,6 +191,19 @@ int vr_separate_wave_host(vr_ctx* ctx, const float* wave_host, int64_t L, int32_
   return done(ctx, ctx->eng->separate_wave_host(wave_host, L, tta, inst_host, voc_host, (cudaStream_t)stream));
 }
 
+int vr_separate_wave_host_images(vr_ctx* ctx, const float* wave_host, int64_t L, int32_t tta, float* inst_host,
+                                 float* voc_host, uint8_t* img_inst_host, uint8_t* img_voc_host, void* stream) {
+  CHECK_CTX(ctx);
+  return done(ctx, ctx->eng->separate_wave_host(wave_host, L, tta, inst_host, voc_host, (cudaStream_t)stream,
+                                                img_inst_host, img_voc_host));
+}
+
+int vr_spec_image(vr_ctx* ctx, const void* spec, const float* mask, int64_t T, uint8_t* img_a, uint8_t* img_b,
+                  void* stream) {
+  CHECK_CTX(ctx);
+  return done(ctx, ctx->eng->spec_image((const float2*)spec, mask, T, img_a, img_b, (cudaStream_t)stream));
+}
+
 int vr_resample(vr_ctx* ctx, const float* x, int32_t channels, int64_t n_in, float* y, int64_t n_out, double sample_ratio,
                 const double* win, const double* delta, int32_t nwin, int32_t table_per_crossing, void* stream) {
   // ctx may be NULL (audio is usually loaded before a model context exists): the call then runs on the calling

@@ -472,6 +472,118 @@ cudaError_t launch_apply_mask(const float2* spec, const float* mask, int64_t n, 
   return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------------------------
+// --output_image (reference spectrogram_to_image, magnitude mode): log10(a^2 + 1e-8) per (channel, bin, frame) with
+// a = m|X| (instruments), (1-m)|X| (vocals) or |X| (no mask), scaled to [0, 255] by the min / max over the whole stem.
+// Every step is a separately rounded fp32 operation (no fma contraction), as numpy's float32 arithmetic is; |X| and
+// log10 are evaluated in fp64 and rounded once, which gives the correctly rounded fp32 results of the host's hypotf /
+// log10f where CUDA's fp32 versions may be 1-2 ulp off and move a pixel across a truncation boundary.
+__device__ __forceinline__ float log_level(float a) {
+  return (float)log10((double)__fadd_rn(__fmul_rn(a, a), 1e-8f));
+}
+
+__device__ __forceinline__ void image_levels(float2 x, const float* mask, int64_t i, float& la, float& lb) {
+  const float mag = (float)sqrt(fma((double)x.x, (double)x.x, (double)x.y * (double)x.y));
+  float a = mag, b = 0.f;
+  if (mask) {
+    const float m = mask[i];
+    a = __fmul_rn(m, mag);
+    b = __fmul_rn(__fsub_rn(1.f, m), mag);
+  }
+  la = log_level(a);
+  lb = log_level(b);
+}
+
+// range[0..3] = {~key(min a), key(max a), ~key(min b), key(max b)} (order_key above, zero-initialised): atomicMax only,
+// which is order-independent, so the result does not depend on scheduling.  NaN levels do not take part.
+__global__ void image_range_kernel(const float2* __restrict__ spec, const float* __restrict__ mask, int64_t n,
+                                   unsigned int* range) {
+  unsigned int k[4] = {0u, 0u, 0u, 0u};
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float la, lb;
+    image_levels(spec[i], mask, i, la, lb);
+    if (la == la) {
+      k[0] = max(k[0], ~order_key(la));
+      k[1] = max(k[1], order_key(la));
+    }
+    if (lb == lb) {
+      k[2] = max(k[2], ~order_key(lb));
+      k[3] = max(k[3], order_key(lb));
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    for (int o = 16; o > 0; o >>= 1) k[j] = max(k[j], __shfl_xor_sync(0xffffffffu, k[j], o));
+  }
+  if ((threadIdx.x & 31) == 0) {
+    atomicMax(range + 0, k[0]);
+    atomicMax(range + 1, k[1]);
+    if (mask) {
+      atomicMax(range + 2, k[2]);
+      atomicMax(range + 3, k[3]);
+    }
+  }
+}
+
+// q = (L - min) * (255 / (max - min)) truncated; a constant stem (max == min), where the reference's uint8 cast sees
+// 0 * inf = NaN, and any NaN level give 0
+__device__ __forceinline__ unsigned char image_pixel(float l, float lo, float s) {
+  const float q = __fmul_rn(__fsub_rn(l, lo), s);
+  if (!(q > 0.f)) return 0;
+  return q >= 255.f ? 255 : (unsigned char)q;
+}
+
+__device__ __forceinline__ void image_scale(const unsigned int* range, float& lo, float& s) {
+  if (range[1] == 0u) {   // no finite level at all
+    lo = 0.f;
+    s = 0.f;
+    return;
+  }
+  lo = order_unkey(~range[0]);
+  const float span = __fsub_rn(order_unkey(range[1]), lo);
+  s = span > 0.f && span <= 3.0e38f ? __fdiv_rn(255.f, span) : 0.f;
+}
+
+// one thread per (bin, frame): img[bin][t][3] = {max(qL, qR), qL, qR}
+__global__ void image_pixels_kernel(const float2* __restrict__ spec, const float* __restrict__ mask, int64_t plane,
+                                    const unsigned int* __restrict__ range, unsigned char* __restrict__ img_a,
+                                    unsigned char* __restrict__ img_b) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= plane) return;
+  float lo_a, s_a, lo_b = 0.f, s_b = 0.f;
+  image_scale(range, lo_a, s_a);
+  if (mask) image_scale(range + 2, lo_b, s_b);
+  float la0, lb0, la1, lb1;
+  image_levels(spec[i], mask, i, la0, lb0);
+  image_levels(spec[plane + i], mask, plane + i, la1, lb1);
+  unsigned char l = image_pixel(la0, lo_a, s_a), r = image_pixel(la1, lo_a, s_a);
+  unsigned char* p = img_a + 3 * i;
+  p[0] = l > r ? l : r;
+  p[1] = l;
+  p[2] = r;
+  if (mask) {
+    l = image_pixel(lb0, lo_b, s_b);
+    r = image_pixel(lb1, lo_b, s_b);
+    p = img_b + 3 * i;
+    p[0] = l > r ? l : r;
+    p[1] = l;
+    p[2] = r;
+  }
+}
+
+cudaError_t launch_spec_image(const float2* spec, const float* mask, int64_t plane, unsigned int* range,
+                              unsigned char* img_a, unsigned char* img_b, cudaStream_t stream) {
+  cudaError_t e = cudaMemsetAsync(range, 0, 4 * sizeof(unsigned int), stream);
+  if (e != cudaSuccess || plane == 0) return e;
+  const int64_t n = 2 * plane;
+  const int grid = (int)(((n + 255) / 256) < 132 * 8 ? ((n + 255) / 256) : 132 * 8);
+  image_range_kernel<<<grid, 256, 0, stream>>>(spec, mask, n, range);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  image_pixels_kernel<<<(unsigned)((plane + 255) / 256), 256, 0, stream>>>(spec, mask, plane, range, img_a, img_b);
+  return cudaGetLastError();
+}
+
 }  // namespace vr
 
 // ------------------------------------------------------------------------------------------------

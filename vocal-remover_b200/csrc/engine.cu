@@ -82,6 +82,7 @@ Engine::~Engine() {
   if (ws_mask_) cudaFree(ws_mask_);
   if (ws_frames_) cudaFree(ws_frames_);
   if (ws_wave_) cudaFree(ws_wave_);
+  if (ws_img_) cudaFree(ws_img_);
   profile_enable(false);
   if (s_hi_) cudaStreamDestroy(s_hi_);
   if (s_copy_) cudaStreamDestroy(s_copy_);
@@ -768,6 +769,21 @@ bool Engine::apply_mask(const float2* spec, const float* mask, int64_t T, float2
   return ck(launch_apply_mask(spec, mask, (int64_t)2 * bins() * T, y, v, s), "apply_mask");
 }
 
+bool Engine::spec_image(const float2* spec, const float* mask, int64_t T, unsigned char* img_a, unsigned char* img_b,
+                        cudaStream_t s) {
+  cudaSetDevice(cfg_.device);
+  if (T < 0 || !spec || !img_a || (mask && !img_b)) {
+    err = "spec_image: needs spec, img_a, T >= 0 and, with a mask, img_b";
+    return false;
+  }
+  // allocated on first use, once per context
+  if (!ws_img_range_ && !(ws_img_range_ = (unsigned int*)dalloc(sizeof(unsigned int) * 4))) return false;
+  launches += 2;
+  return timed("spec_image", 1, bins(), (int)T, s, [&] {
+    return ck(launch_spec_image(spec, mask, (int64_t)bins() * T, ws_img_range_, img_a, img_b, s), "spec_image");
+  });
+}
+
 bool Engine::stft(const float* wave, int64_t L, float2* spec, int64_t T, float* absmax, cudaStream_t s) {
   if (!stft_range(wave, L, spec, T, 0, T, s)) return false;
   if (absmax) return normaliser(spec, T, 0, absmax, s);
@@ -873,7 +889,8 @@ bool Engine::separate_wave(const float* wave, int64_t L, int tta, float* inst, f
 }
 
 // Host-buffer entry (the end-to-end call): H2D of the wave, the whole path, D2H of both stems.
-bool Engine::separate_wave_host(const float* wave, int64_t L, int tta, float* inst, float* voc, cudaStream_t s) {
+bool Engine::separate_wave_host(const float* wave, int64_t L, int tta, float* inst, float* voc, cudaStream_t s,
+                                unsigned char* img_inst, unsigned char* img_voc) {
   cudaSetDevice(cfg_.device);
   const int64_t T = 1 + L / cfg_.hop;
   const int64_t Lo = (int64_t)cfg_.hop * (T - 1);
@@ -883,6 +900,13 @@ bool Engine::separate_wave_host(const float* wave, int64_t L, int tta, float* in
     ws_wave_ = nullptr;
     if (!ck(cudaMalloc(&ws_wave_, sizeof(float) * need_f), "workspace wave")) return false;
     ws_wave_cap_ = need_f;
+  }
+  const int64_t img_bytes = (int64_t)3 * bins() * T;
+  if ((img_inst || img_voc) && 2 * img_bytes > ws_img_cap_) {
+    if (ws_img_) cudaFree(ws_img_);
+    ws_img_ = nullptr;
+    if (!ck(cudaMalloc(&ws_img_, 2 * img_bytes), "workspace images")) return false;
+    ws_img_cap_ = 2 * img_bytes;
   }
   float* d_in = ws_wave_;
   float* d_inst = ws_wave_ + 2 * L;
@@ -917,6 +941,14 @@ bool Engine::separate_wave_host(const float* wave, int64_t L, int tta, float* in
   ok = separate(ws_spec_, T, tta, ws_mask_, s);
   on_frames_final_ = nullptr;
   if (ok) ok = flush(T);
+  if (ok && (img_inst || img_voc)) {
+    // after the last span: the images of the final mask, copied back behind the stems on the copy stream
+    ok = spec_image(ws_spec_, ws_mask_, T, ws_img_, ws_img_ + img_bytes, s) &&
+         ck(cudaEventRecord(ev_span_, s), "image event") && ck(cudaStreamWaitEvent(s_copy_, ev_span_, 0), "image wait") &&
+         (!img_inst || ck(cudaMemcpyAsync(img_inst, ws_img_, img_bytes, cudaMemcpyDeviceToHost, s_copy_), "D2H image")) &&
+         (!img_voc || ck(cudaMemcpyAsync(img_voc, ws_img_ + img_bytes, img_bytes, cudaMemcpyDeviceToHost, s_copy_),
+                         "D2H image"));
+  }
   if (!ok) {
     cudaStreamSynchronize(s);
     cudaStreamSynchronize(s_copy_);

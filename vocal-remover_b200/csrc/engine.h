@@ -125,7 +125,12 @@ class Engine {
   bool separate(const float2* spec, int64_t T, int tta, float* mask, cudaStream_t s);
   bool apply_mask(const float2* spec, const float* mask, int64_t T, float2* y, float2* v, cudaStream_t s);
   bool separate_wave(const float* wave, int64_t L, int tta, float* inst, float* voc, cudaStream_t s);
-  bool separate_wave_host(const float* wave, int64_t L, int tta, float* inst, float* voc, cudaStream_t s);
+  // img_inst / img_voc: HOST [bins][T][3] uint8 spectrogram images of the two stems, or nullptr for none
+  bool separate_wave_host(const float* wave, int64_t L, int tta, float* inst, float* voc, cudaStream_t s,
+                          unsigned char* img_inst = nullptr, unsigned char* img_voc = nullptr);
+  // spectrogram images of mask * spec and (1 - mask) * spec (mask == nullptr: of spec itself, img_b unused)
+  bool spec_image(const float2* spec, const float* mask, int64_t T, unsigned char* img_a, unsigned char* img_b,
+                  cudaStream_t s);
   bool normaliser(const float2* spec, int64_t T, int mode, float* out, cudaStream_t s);
 
   // debug / tests: run one reference Conv2DBNActiv-shaped layer through a chosen kernel
@@ -177,6 +182,8 @@ class Engine {
   float* ws_wave_ = nullptr; int64_t ws_wave_cap_ = 0;   // [2][L] in + 2 x [2][Lo] out (host-buffer entry)
   float* ws_norm_ = nullptr;            // [4] floats: absmax, lexmax-abs
   unsigned long long* ws_lex_ = nullptr;
+  unsigned int* ws_img_range_ = nullptr;   // [4] min / max keys of the spectrogram image pass (first use)
+  unsigned char* ws_img_ = nullptr; int64_t ws_img_cap_ = 0;   // two [bins][T][3] images (host-buffer entry)
 
   // the high-band BaseNets of stages 1-2 run on their own stream next to the low-band chain (independent until
   // stage 3, lib/nets.py:88-99); disabled while per-kernel profiling is on so event timings stay per-kernel

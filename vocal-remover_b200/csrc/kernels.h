@@ -49,6 +49,11 @@ cudaError_t launch_mask_frame_min(const float* mask, int rows, int64_t T, float*
 cudaError_t launch_mask_apply_weight(float* mask, int rows, int64_t T, const float* weight, cudaStream_t stream);
 cudaError_t launch_apply_mask(const float2* spec, const float* mask, int64_t n, float2* y, float2* v,
                               cudaStream_t stream);
+// spectrogram images (reference spec_utils.spectrogram_to_image): spec / mask [2][plane] with plane = bins * T ->
+// img_a / img_b [plane][3] uint8 (instruments / vocals; mask == nullptr: img_a = image of spec, img_b unused);
+// range: 4 unsigned ints of scratch
+cudaError_t launch_spec_image(const float2* spec, const float* mask, int64_t plane, unsigned int* range,
+                              unsigned char* img_a, unsigned char* img_b, cudaStream_t stream);
 
 // ---- LSTM branch (lstm.cu), reference lib/layers.py:108-133 ------------------------------------
 // 1x1 conv (C -> 1), pre-activation sums as an fp32 plane l0[n][bin][t] (the row kernel's epilogue accumulates the same

@@ -17,6 +17,7 @@ from lib import audio_io
 from lib import dataset
 from lib import nets
 from lib import spec_utils
+from lib import utils
 
 
 class Separator(object):
@@ -100,38 +101,26 @@ class Separator(object):
         return self._run(X_spec, tta=True)
 
     # ---- fused device-resident path -----------------------------------------------------------------
-    def separate_wave(self, wave, tta=False):
+    def separate_wave(self, wave, tta=False, images=False):
         """float32 (2, L) wave -> (instruments, vocals) float32 (2, hop*(T-1)) waves.
 
         Equivalent to wave_to_spectrogram -> separate[_tta] -> 2x spectrogram_to_wave
         (inference.py:147,158-161,171,176) without leaving the GPU in between.  ``wave`` may be a numpy
-        array (host; copied in and out) or a CUDA tensor (returns CUDA tensors).
+        array (host; copied in and out) or a CUDA tensor (returns CUDA tensors).  ``images=True`` also returns the
+        --output_image spectrogram images of both stems (spectrogram_to_image of y_spec / v_spec, inference.py:180-185)
+        as uint8 (bins, T, 3): (inst, voc, img_inst, img_voc); the stems are the same as with ``images=False``.
         """
         ctx = self._ctx()
         if self.postprocess:
             # staged on the device: STFT -> mask (+ postprocess) -> masked inverse STFT
-            dev = self._dev()
-            hop, n_fft = self.model.hop_length, self.model.n_fft
-            with torch.cuda.device(dev):
-                host = not (torch.is_tensor(wave) and wave.is_cuda)
-                w = (torch.from_numpy(np.ascontiguousarray(np.asarray(wave, dtype=np.float32))).to(dev) if host
-                     else wave.contiguous().float())
-                L = w.shape[1]
-                T = 1 + L // hop
-                d_spec = torch.empty((2, n_fft // 2 + 1, T), dtype=torch.complex64, device=dev)
-                ctx.check(ctx.lib.vr_stft(ctx.handle, _native.ptr(w), L, _native.ptr(d_spec), T, None,
-                                          _native.stream_ptr()), 'vr_stft')
-                d_mask = self._mask_device(d_spec, tta)
-                inst = torch.empty((2, hop * (T - 1)), dtype=torch.float32, device=dev)
-                voc = torch.empty_like(inst)
-                ctx.check(ctx.lib.vr_apply_mask_istft(ctx.handle, _native.ptr(d_spec), _native.ptr(d_mask), T,
-                                                      _native.ptr(inst), _native.ptr(voc), _native.stream_ptr()),
-                          'vr_apply_mask_istft')
-                return (inst.cpu().numpy(), voc.cpu().numpy()) if host else (inst, voc)
+            return self._separate_wave_staged(wave, tta, images)
         dev = self._dev()
         hop = self.model.hop_length
         with torch.cuda.device(dev):
             if torch.is_tensor(wave) and wave.is_cuda:
+                if images:
+                    # the engine calls vr_separate_wave makes, with the spectrogram and mask kept for the images
+                    return self._separate_wave_staged(wave, tta, images)
                 w = wave.contiguous().float()
                 L = w.shape[1]
                 Lo = hop * (L // hop)
@@ -145,13 +134,52 @@ class Separator(object):
             Lo = hop * (L // hop)
             inst = np.empty((2, Lo), dtype=np.float32)
             voc = np.empty((2, Lo), dtype=np.float32)
+            if images:
+                shape = (self.model.n_fft // 2 + 1, 1 + L // hop, 3)
+                img_inst = np.empty(shape, dtype=np.uint8)
+                img_voc = np.empty(shape, dtype=np.uint8)
+                ctx.check(ctx.lib.vr_separate_wave_host_images(ctx.handle, w.ctypes.data, L, 1 if tta else 0,
+                                                               inst.ctypes.data, voc.ctypes.data, img_inst.ctypes.data,
+                                                               img_voc.ctypes.data, _native.stream_ptr()),
+                          'vr_separate_wave_host_images')
+                return inst, voc, img_inst, img_voc
             ctx.check(ctx.lib.vr_separate_wave_host(ctx.handle, w.ctypes.data, L, 1 if tta else 0, inst.ctypes.data,
                                                     voc.ctypes.data, _native.stream_ptr()), 'vr_separate_wave_host')
             return inst, voc
 
+    def _separate_wave_staged(self, wave, tta, images):
+        ctx = self._ctx()
+        dev = self._dev()
+        hop, n_fft = self.model.hop_length, self.model.n_fft
+        with torch.cuda.device(dev):
+            host = not (torch.is_tensor(wave) and wave.is_cuda)
+            w = (torch.from_numpy(np.ascontiguousarray(np.asarray(wave, dtype=np.float32))).to(dev) if host
+                 else wave.contiguous().float())
+            L = w.shape[1]
+            T = 1 + L // hop
+            d_spec = torch.empty((2, n_fft // 2 + 1, T), dtype=torch.complex64, device=dev)
+            ctx.check(ctx.lib.vr_stft(ctx.handle, _native.ptr(w), L, _native.ptr(d_spec), T, None,
+                                      _native.stream_ptr()), 'vr_stft')
+            d_mask = self._mask_device(d_spec, tta)
+            inst = torch.empty((2, hop * (T - 1)), dtype=torch.float32, device=dev)
+            voc = torch.empty_like(inst)
+            ctx.check(ctx.lib.vr_apply_mask_istft(ctx.handle, _native.ptr(d_spec), _native.ptr(d_mask), T,
+                                                  _native.ptr(inst), _native.ptr(voc), _native.stream_ptr()),
+                      'vr_apply_mask_istft')
+            out = [inst, voc]
+            if images:
+                img_inst = torch.empty((n_fft // 2 + 1, T, 3), dtype=torch.uint8, device=dev)
+                img_voc = torch.empty_like(img_inst)
+                ctx.check(ctx.lib.vr_spec_image(ctx.handle, _native.ptr(d_spec), _native.ptr(d_mask), T,
+                                                _native.ptr(img_inst), _native.ptr(img_voc), _native.stream_ptr()),
+                          'vr_spec_image')
+                out += [img_inst, img_voc]
+            return tuple(t.cpu().numpy() for t in out) if host else tuple(out)
+
 
 MODEL_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'models')
 DEFAULT_MODEL_PATH = os.path.join(MODEL_DIR, 'baseline.pth')
+JPEG_MAX_WIDTH = 65500   # widest image the JPEG encoder accepts; one pixel per STFT frame
 
 
 def main():
@@ -170,9 +198,12 @@ def main():
     p.add_argument('--output_dir', '-o', type=str, default="")
     args = p.parse_args()
 
-    # unsupported surfaces fail before any heavy work (model load, audio decode, output directory)
+    # missing requirements fail before any heavy work (model load, audio decode, output directory)
     if args.output_image:
-        raise NotImplementedError('--output_image (debug JPGs, lib/utils.py) is outside the H100 hot path')
+        try:
+            import cv2  # noqa: F401  (the JPEG encoder of lib/utils.imwrite)
+        except ImportError as e:
+            raise ImportError('--output_image needs OpenCV (the cv2 module) to encode the JPGs: %s' % e) from e
     if not torch.cuda.is_available():
         raise RuntimeError('no CUDA device: the H100 build of vocal-remover has no CPU path')
     if args.gpu < 0:
@@ -211,12 +242,24 @@ def main():
         os.makedirs(output_dir, exist_ok=True)
     print('done')
 
+    images = args.output_image
+    n_frames = 1 + X.shape[1] // args.hop_length
+    if images and n_frames > JPEG_MAX_WIDTH:
+        # the reference's cv2.imencode refuses the image and imwrite returns False: no JPG, the WAVs are still written
+        print('skipping {0}_Instruments.jpg and {0}_Vocals.jpg: {1} frames exceed the {2}-pixel width limit of '
+              'JPEG'.format(basename, n_frames, JPEG_MAX_WIDTH))
+        images = False
+
     print('stft of wave source, separation, inverse stft of instruments and vocals...', end=' ')
-    wave_inst, wave_voc = sp.separate_wave(X, tta=args.tta)
+    out = sp.separate_wave(X, tta=args.tta, images=images)
+    wave_inst, wave_voc = out[:2]
     print('done')
-    writer = audio_io.AsyncWriter()   # the two stems are encoded and written concurrently
+    writer = audio_io.AsyncWriter()   # the two stems (and images) are encoded and written concurrently
     writer.write('{}{}_Instruments.wav'.format(output_dir, basename), wave_inst.T, sr)
     writer.write('{}{}_Vocals.wav'.format(output_dir, basename), wave_voc.T, sr)
+    if images:
+        writer.run(utils.imwrite, '{}{}_Instruments.jpg'.format(output_dir, basename), out[2])
+        writer.run(utils.imwrite, '{}{}_Vocals.jpg'.format(output_dir, basename), out[3])
     writer.join()
 
 

@@ -43,6 +43,8 @@ SIGNATURES = {
     'vr_apply_mask_istft_range': (c_i32, [c_vp, c_vp, c_fp, c_i64, c_i64, c_i64, c_fp, c_fp, c_vp]),
     'vr_separate_wave': (c_i32, [c_vp, c_fp, c_i64, c_i32, c_fp, c_fp, c_vp]),
     'vr_separate_wave_host': (c_i32, [c_vp, c_fp, c_i64, c_i32, c_fp, c_fp, c_vp]),
+    'vr_separate_wave_host_images': (c_i32, [c_vp, c_fp, c_i64, c_i32, c_fp, c_fp, c_vp, c_vp, c_vp]),
+    'vr_spec_image': (c_i32, [c_vp, c_vp, c_fp, c_i64, c_vp, c_vp, c_vp]),
     'vr_shared_alloc': (c_i32, [c_vp, c_i64, ctypes.POINTER(c_vp), ctypes.c_char_p]),
     'vr_shared_open': (c_i32, [c_vp, ctypes.c_char_p, ctypes.POINTER(c_vp)]),
     'vr_shared_close': (c_i32, [c_vp, c_vp, c_i32]),

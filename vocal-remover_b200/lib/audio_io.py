@@ -136,11 +136,15 @@ class AsyncWriter(object):
         self._jobs = []
 
     def write(self, path, data, sr):
+        self.run(write, path, data, sr)
+
+    def run(self, fn, *args):
+        """Runs ``fn(*args)`` on a worker thread (e.g. lib.utils.imwrite of the --output_image JPGs)."""
         box = {}
 
         def run():
             try:
-                write(path, data, sr)
+                fn(*args)
             except BaseException as exc:   # handed to join()
                 box['exc'] = exc
 

@@ -2,7 +2,8 @@
 
 wave_to_spectrogram / spectrogram_to_wave keep the reference signatures and numpy in / numpy out
 contract (lib/spec_utils.py:26-31, 157-165) but run the framed FFT / inverse FFT + overlap-add on the
-GPU through libvr_b200.so (csrc/fft.cu) instead of librosa on the host.
+GPU through libvr_b200.so (csrc/fft.cu) instead of librosa on the host.  spectrogram_to_image (--output_image) builds
+its uint8 image on the GPU as well (csrc/elementwise.cu).
 """
 import numpy as np
 import torch
@@ -77,6 +78,37 @@ def spectrogram_to_wave(spec, hop_length=1024):
                                    _native.stream_ptr()), 'vr_istft')
         out = d_wave.cpu().numpy()
     return out[0] if mono else out
+
+
+def spectrogram_to_image(spec, mode='magnitude'):
+    """complex (2, bins, T) -> uint8 (bins, T, 3) image {max(L, R), L, R} of the log power   (lib/spec_utils.py:34-57).
+
+    Built on the GPU (vr_spec_image).  A numpy array gives a numpy image, a CUDA complex64 tensor a CUDA uint8 tensor.
+    A constant spectrogram (e.g. silence) gives an all-zero image where the reference's uint8 cast sees NaN.
+    """
+    if mode != 'magnitude':
+        raise NotImplementedError("spectrogram_to_image: only mode='magnitude' (the --output_image path) is supported")
+    on_device = torch.is_tensor(spec)
+    if not on_device:
+        spec = np.asarray(spec)
+    if not (spec.is_complex() if on_device else np.iscomplexobj(spec)):
+        raise NotImplementedError('spectrogram_to_image: only complex spectrograms (the --output_image path)')
+    if spec.ndim != 3 or spec.shape[0] != 2:
+        raise NotImplementedError('spectrogram_to_image: only (2, bins, T) stereo spectrograms (the --output_image path)')
+    bins, T = spec.shape[1], spec.shape[2]
+    ctx = _spectral_ctx(2 * (bins - 1), bins - 1)
+    dev = torch.device('cuda', ctx.device_index)
+    with torch.cuda.device(dev):
+        if on_device:
+            if spec.device != dev:
+                raise ValueError('spectrogram_to_image: spec is on %s, the spectral functions use %s' % (spec.device, dev))
+            d_spec = spec.to(torch.complex64).contiguous()
+        else:
+            d_spec = torch.from_numpy(np.ascontiguousarray(np.asarray(spec, dtype=np.complex64))).to(dev)
+        img = torch.empty((bins, T, 3), dtype=torch.uint8, device=dev)
+        ctx.check(ctx.lib.vr_spec_image(ctx.handle, _native.ptr(d_spec), None, T, _native.ptr(img), None,
+                                        _native.stream_ptr()), 'vr_spec_image')
+        return img if on_device else img.cpu().numpy()
 
 
 def artifact_weights(frame_min, thres=0.05, min_range=64, fade_size=32):
