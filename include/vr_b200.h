@@ -138,6 +138,16 @@ VR_API int vr_separate_wave_host_images(vr_ctx* ctx, const float* wave_host, int
 VR_API int vr_spec_image(vr_ctx* ctx, const void* spec, const float* mask, int64_t T, uint8_t* img_a, uint8_t* img_b,
                          void* stream);
 
+/* train.py:108-134 validate_epoch over lib/dataset.py:220-248 make_validation_set, one track pair:
+ * window_sums[j], j < ceil(T/roi), = sum over (2, bins, roi) of |mask*|X|/coef - |y|/coef| for patch j,
+ * coef = max(max|X|, max|y|) written to *coef_out (device float, may be NULL).
+ * spec_x / spec_y: device complex64 [2][bins][T] (mixture / instruments); window_sums: device double[ceil(T/roi)].
+ * mask is the net's mask of patch j (X/coef padded by make_padding, the 1025th bin replicating the 1024th), frames
+ * past T count as zero.  Each patch's loss is window_sums[j] / (2 * bins * roi); the sums are bit-identical from
+ * call to call.  A zero or non-finite coef gives inv = 0 (all sums 0): the caller must reject such a pair.       */
+VR_API int vr_validation_loss(vr_ctx* ctx, const void* spec_x, const void* spec_y, int64_t T,
+                              float* coef_out, double* window_sums, void* stream);
+
 /* The sample-rate conversion inside librosa.load(path, sr=args.sr, res_type='kaiser_fast') (inference.py:136-138,
  * pseudo.py:47-50) = resampy.resample(y, orig_sr, sr, filter='kaiser_fast'): x [channels][n_in] -> y [channels][n_out],
  * n_out = (int64)(n_in * sample_ratio), sample_ratio = sr / orig_sr.  win / delta: DEVICE float64 arrays of nwin entries -

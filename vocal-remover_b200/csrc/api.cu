@@ -204,6 +204,13 @@ int vr_spec_image(vr_ctx* ctx, const void* spec, const float* mask, int64_t T, u
   return done(ctx, ctx->eng->spec_image((const float2*)spec, mask, T, img_a, img_b, (cudaStream_t)stream));
 }
 
+int vr_validation_loss(vr_ctx* ctx, const void* spec_x, const void* spec_y, int64_t T, float* coef_out,
+                       double* window_sums, void* stream) {
+  CHECK_CTX(ctx);
+  return done(ctx, ctx->eng->validation_loss((const float2*)spec_x, (const float2*)spec_y, T, coef_out, window_sums,
+                                             (cudaStream_t)stream));
+}
+
 int vr_resample(vr_ctx* ctx, const float* x, int32_t channels, int64_t n_in, float* y, int64_t n_out, double sample_ratio,
                 const double* win, const double* delta, int32_t nwin, int32_t table_per_crossing, void* stream) {
   // ctx may be NULL (audio is usually loaded before a model context exists): the call then runs on the calling

@@ -6,6 +6,7 @@
 //   mask_out        lib/nets.py:79,109-115,127-129  1x1 conv -> sigmoid -> replicate Nyquist row -> crop offset
 //   absmax / lexmax inference.py:74 / inference.py:87,94 global normalisers
 //   apply_mask      inference.py:32-36
+//   validation_l1   train.py:108-134 validate_epoch: per-window L1 sums of the masked mixture against the instruments
 #include "common.cuh"
 #include "kernels.h"
 
@@ -341,9 +342,11 @@ __global__ void absmax_kernel(const float2* __restrict__ spec, int64_t n, float*
   }
 }
 
-cudaError_t launch_absmax(const float2* spec, int64_t n, float* out_absmax, cudaStream_t stream) {
-  cudaError_t e = cudaMemsetAsync(out_absmax, 0, sizeof(float), stream);
-  if (e != cudaSuccess) return e;
+cudaError_t launch_absmax(const float2* spec, int64_t n, float* out_absmax, cudaStream_t stream, bool accumulate) {
+  if (!accumulate) {
+    cudaError_t e = cudaMemsetAsync(out_absmax, 0, sizeof(float), stream);
+    if (e != cudaSuccess) return e;
+  }
   if (n == 0) return cudaSuccess;
   int grid = (int)(((n + 255) / 256) < 132 * 8 ? ((n + 255) / 256) : 132 * 8);
   absmax_kernel<<<grid, 256, 0, stream>>>(spec, n, out_absmax);
@@ -581,6 +584,75 @@ cudaError_t launch_spec_image(const float2* spec, const float* mask, int64_t pla
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   image_pixels_kernel<<<(unsigned)((plane + 255) / 256), 256, 0, stream>>>(spec, mask, plane, range, img_a, img_b);
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------
+// Validation loss (reference train.py:108-134 over lib/dataset.py:220-248): per window j, the sum over (channel, bin,
+// roi frames t in [j*roi, (j+1)*roi)) of |m*|X|*inv - |y|*inv|, inv = 1/coef, zero for t >= T.  The terms are fp32
+// with the pack kernel's hypotf-and-reciprocal arithmetic and accumulate in fp64.  Every window is cut into
+// VAL_SLICES fixed slices; a slice's block reduces its threads' partials in a fixed tree, and a second kernel adds
+// the slices of a window in order - no float atomics, so the same input gives the same sums bit for bit.
+constexpr int VAL_SLICES = 16;
+constexpr int VAL_THREADS = 256;
+
+__global__ void __launch_bounds__(VAL_THREADS) validation_l1_kernel(const float2* __restrict__ spec_x,
+                                                                    const float2* __restrict__ spec_y,
+                                                                    const float* __restrict__ mask, int bins, int64_t T,
+                                                                    int roi, int64_t mask_T,
+                                                                    const float* __restrict__ coef,
+                                                                    double* __restrict__ partial) {
+  const int64_t j = blockIdx.x;
+  const int64_t per_window = (int64_t)2 * bins * roi;
+  const float cv = *coef;
+  const float inv = (cv > 0.f && cv <= 3.0e38f) ? 1.0f / cv : 0.f;   // as pack_mag_from_spec_kernel
+  double acc = 0.0;
+  for (int64_t e = (int64_t)blockIdx.y * VAL_THREADS + threadIdx.x; e < per_window;
+       e += (int64_t)VAL_SLICES * VAL_THREADS) {
+    const int64_t row = e / roi;   // channel * bins + bin
+    const int64_t t = j * roi + (e - row * roi);
+    if (t >= T) continue;   // the zero padding: both sides are 0
+    const float2 a = spec_x[row * T + t];
+    const float2 b = spec_y[row * T + t];
+    float mx = hypotf(a.x, a.y) * inv;
+    float my = hypotf(b.x, b.y) * inv;
+    if (!(mx <= 3.0e38f)) mx = 0.f;   // also catches NaN
+    if (!(my <= 3.0e38f)) my = 0.f;
+    acc += (double)fabsf(__fsub_rn(__fmul_rn(mask[row * mask_T + t], mx), my));
+  }
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  __shared__ double warp_sum[VAL_THREADS / 32];
+  if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+#pragma unroll
+    for (int w = 0; w < VAL_THREADS / 32; ++w) s += warp_sum[w];
+    partial[j * VAL_SLICES + blockIdx.y] = s;
+  }
+}
+
+__global__ void validation_sum_slices_kernel(const double* __restrict__ partial, int n, double* __restrict__ sums) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  double s = 0.0;
+#pragma unroll
+  for (int k = 0; k < VAL_SLICES; ++k) s += partial[(int64_t)j * VAL_SLICES + k];
+  sums[j] = s;
+}
+
+int64_t validation_l1_scratch(int n_windows) { return (int64_t)n_windows * VAL_SLICES; }
+
+cudaError_t launch_validation_l1(const float2* spec_x, const float2* spec_y, const float* mask, int bins, int64_t T,
+                                 int roi, int n_windows, const float* coef, double* partial, double* window_sums,
+                                 cudaStream_t stream) {
+  if (n_windows <= 0) return cudaSuccess;
+  validation_l1_kernel<<<dim3((unsigned)n_windows, VAL_SLICES), VAL_THREADS, 0, stream>>>(
+      spec_x, spec_y, mask, bins, T, roi, (int64_t)n_windows * roi, coef, partial);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  validation_sum_slices_kernel<<<(unsigned)((n_windows + 127) / 128), 128, 0, stream>>>(partial, n_windows,
+                                                                                       window_sums);
   return cudaGetLastError();
 }
 

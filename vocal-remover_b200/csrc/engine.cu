@@ -83,6 +83,7 @@ Engine::~Engine() {
   if (ws_frames_) cudaFree(ws_frames_);
   if (ws_wave_) cudaFree(ws_wave_);
   if (ws_img_) cudaFree(ws_img_);
+  if (ws_val_) cudaFree(ws_val_);
   profile_enable(false);
   if (s_hi_) cudaStreamDestroy(s_hi_);
   if (s_copy_) cudaStreamDestroy(s_copy_);
@@ -781,6 +782,62 @@ bool Engine::spec_image(const float2* spec, const float* mask, int64_t T, unsign
   launches += 2;
   return timed("spec_image", 1, bins(), (int)T, s, [&] {
     return ck(launch_spec_image(spec, mask, (int64_t)bins() * T, ws_img_range_, img_a, img_b, s), "spec_image");
+  });
+}
+
+// train.py:108-134 validate_epoch over lib/dataset.py:220-248 make_validation_set, one pair: coef = max(max|X|, max|y|),
+// ceil(T / roi) windows of X / coef padded by make_padding (left = offset) through the net, then the L1 sums of the
+// kept mask frames.  Only the mask workspace is needed (no inverse STFT, so not ensure_ws's frame workspace).
+bool Engine::validation_loss(const float2* spec_x, const float2* spec_y, int64_t T, float* coef_out,
+                             double* window_sums, cudaStream_t s) {
+  if (!finalized_) {
+    err = "weights not finalized";
+    return false;
+  }
+  cudaSetDevice(cfg_.device);
+  if (T < 1 || !spec_x || !spec_y || !window_sums) {
+    err = "validation_loss: needs spec_x, spec_y, window_sums and T >= 1";
+    return false;
+  }
+  if (cfg_.cropsize <= 2 * cfg_.offset) {
+    err = "validation_loss: cropsize must exceed 2 * offset (the reference's predict keeps no frame otherwise)";
+    return false;
+  }
+  const int r = roi();
+  const int64_t n64 = (T + r - 1) / r;   // lib/dataset.py:236, not Separator's (W_pad - 2*offset) // roi
+  if (n64 > (int64_t)INT32_MAX / 2) {
+    err = "validation_loss: track too long";
+    return false;
+  }
+  const int n = (int)n64;
+  const int64_t mask_T = n64 * r;
+  const int64_t nmask = (int64_t)2 * bins() * mask_T;
+  if (nmask > ws_mask_cap_) {
+    if (ws_mask_) cudaFree(ws_mask_);
+    ws_mask_ = nullptr;
+    if (!ck(cudaMalloc(&ws_mask_, sizeof(float) * nmask), "workspace mask")) return false;
+    ws_mask_cap_ = nmask;
+  }
+  const int64_t nval = validation_l1_scratch(n);
+  if (nval > ws_val_cap_) {
+    if (ws_val_) cudaFree(ws_val_);
+    ws_val_ = nullptr;
+    if (!ck(cudaMalloc(&ws_val_, sizeof(double) * nval), "workspace validation")) return false;
+    ws_val_cap_ = nval;
+  }
+  float* coef = coef_out ? coef_out : ws_norm_;
+  const int64_t nspec = (int64_t)2 * bins() * T;
+  launches += 2;
+  if (!timed("normaliser.absmax", 1, bins(), (int)T, s, [&] {
+        return ck(launch_absmax(spec_x, nspec, coef, s), "absmax X") &&
+               ck(launch_absmax(spec_y, nspec, coef, s, true), "absmax y");
+      }))
+    return false;
+  if (!separate_windows(spec_x, T, coef, cfg_.offset, 0, n, ws_mask_, mask_T, 0, 0, s)) return false;
+  launches += 2;
+  return timed("validation_l1", n, bins(), r, s, [&] {
+    return ck(launch_validation_l1(spec_x, spec_y, ws_mask_, bins(), T, r, n, coef, ws_val_, window_sums, s),
+              "validation_l1");
   });
 }
 

@@ -132,6 +132,9 @@ class Engine {
   bool spec_image(const float2* spec, const float* mask, int64_t T, unsigned char* img_a, unsigned char* img_b,
                   cudaStream_t s);
   bool normaliser(const float2* spec, int64_t T, int mode, float* out, cudaStream_t s);
+  // validation loss of one (mixture, instruments) pair; see vr_validation_loss in include/vr_b200.h
+  bool validation_loss(const float2* spec_x, const float2* spec_y, int64_t T, float* coef_out, double* window_sums,
+                       cudaStream_t s);
 
   // debug / tests: run one reference Conv2DBNActiv-shaped layer through a chosen kernel
   bool debug_conv(const float* x_nchw, int N, int Cin, int H, int W, const float* w, const float* bias, int Cout,
@@ -184,6 +187,7 @@ class Engine {
   unsigned long long* ws_lex_ = nullptr;
   unsigned int* ws_img_range_ = nullptr;   // [4] min / max keys of the spectrogram image pass (first use)
   unsigned char* ws_img_ = nullptr; int64_t ws_img_cap_ = 0;   // two [bins][T][3] images (host-buffer entry)
+  double* ws_val_ = nullptr; int64_t ws_val_cap_ = 0;   // per-slice partial sums of the validation loss
 
   // the high-band BaseNets of stages 1-2 run on their own stream next to the low-band chain (independent until
   // stage 3, lib/nets.py:88-99); disabled while per-kernel profiling is on so event timings stay per-kernel

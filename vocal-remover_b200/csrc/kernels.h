@@ -39,7 +39,9 @@ struct MaskOutParams {
 };
 cudaError_t launch_mask_out(const MaskOutParams& p, cudaStream_t stream);
 
-cudaError_t launch_absmax(const float2* spec, int64_t n, float* out_absmax, cudaStream_t stream);
+// accumulate: max with what *out_absmax holds (a non-negative float) instead of starting from 0
+cudaError_t launch_absmax(const float2* spec, int64_t n, float* out_absmax, cudaStream_t stream,
+                          bool accumulate = false);
 // max |spec[r][t]| over rows r < nrows and frames t in [t0, t1) of a [nrows][T] array
 cudaError_t launch_absmax_range(const float2* spec, int nrows, int64_t T, int64_t t0, int64_t t1, float* out_absmax,
                                 cudaStream_t stream);
@@ -54,6 +56,13 @@ cudaError_t launch_apply_mask(const float2* spec, const float* mask, int64_t n, 
 // range: 4 unsigned ints of scratch
 cudaError_t launch_spec_image(const float2* spec, const float* mask, int64_t plane, unsigned int* range,
                               unsigned char* img_a, unsigned char* img_b, cudaStream_t stream);
+// validation loss (reference train.py:108-134): window_sums[j] = sum over (channel, bin, frames [j*roi, (j+1)*roi) of
+// the track) of |mask * |X| / coef - |y| / coef|, spec_x / spec_y [2][bins][T], mask [2][bins][n_windows * roi],
+// *coef on the device; partial: validation_l1_scratch(n_windows) doubles of scratch
+int64_t validation_l1_scratch(int n_windows);
+cudaError_t launch_validation_l1(const float2* spec_x, const float2* spec_y, const float* mask, int bins, int64_t T,
+                                 int roi, int n_windows, const float* coef, double* partial, double* window_sums,
+                                 cudaStream_t stream);
 
 // ---- LSTM branch (lstm.cu), reference lib/layers.py:108-133 ------------------------------------
 // 1x1 conv (C -> 1), pre-activation sums as an fp32 plane l0[n][bin][t] (the row kernel's epilogue accumulates the same
