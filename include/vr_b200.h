@@ -194,9 +194,10 @@ VR_API int vr_debug_decoder(vr_ctx* ctx, const float* low, int32_t N, int32_t Cl
                      int32_t Cs, const float* wgt, const float* bias, int32_t Cout, int32_t act, int32_t fused, float* y,
                      void* stream);
 /* Process-wide debug knobs of the tensor-core kernels: key 0 = 1 makes CTA 0 of the row-streaming kernel record a
- * timeline (builds with -DVR_TRACE), key 1 = 1 disables that kernel, key 2 = 1 makes vr_debug_conv use its 64-channel
- * output tile, key 4 = k gives k of its operand slots to the interpolation warps, key 5 = 1 (default) fuses the decoder
- * upsample into it (before vr_create), key 6 = 1 (default) skips channel groups whose weights are all zero.        */
+ * timeline (builds with -DVR_TRACE), key 2 = 1 makes vr_debug_conv use its 64-channel output tile, key 3 = 1 sends the
+ * layers prepared afterwards (every vr_debug_conv call prepares its layer) from the halo-tile kernel to the generic
+ * one, key 3 = 2 / 3 makes the halo-tile kernel use MB = 1 / 2, key 6 = 1 (default) skips channel groups whose weights
+ * are all zero.  Returns -1 for any other key.                                                                      */
 VR_API int vr_debug_set(int32_t key, int32_t value);
 /* Internal activation of the last forward as NCHW float32; dims receives [N,C,H,W].                       */
 /* timeline of CTA 0 of the last row-kernel launch made with vr_debug_set(0, 1): 3 roles x 2048 events x 3 clock64 stamps

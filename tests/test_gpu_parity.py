@@ -380,7 +380,7 @@ def test_postprocess_device_matches_host_merge_artifacts(default_model):
 
 
 def test_zero_group_skipping_is_exact(default_model, wave10):
-    """g_tc_debug[6] (VR_KSKIP, on by default): the row kernel does not issue MMAs / interpolation for 8-channel
+    """vr_debug_set key 6 (VR_KSKIP, on by default): the row kernel does not issue MMAs / interpolation for 8-channel
     input groups whose weights are all zero (lstm and pad groups of the concat layouts) - the skipped products are
     exact zeros, so switching it off may not change the mask by a single bit."""
     import inference

@@ -1,5 +1,7 @@
-"""wgmma implicit-GEMM convolution (csrc/conv_tc.cu) against a float64 torch reference of the same op,
-layer class by layer class (3x3, strided, dilated, 1x1, ragged batch, multi-N-tile), called through the C ABI."""
+"""wgmma implicit-GEMM convolutions (csrc/conv_tc*.cu) against a float64 torch reference of the same op,
+layer class by layer class (3x3, strided, dilated, 1x1, ragged batch, multi-N-tile), called through the C ABI.  Each
+case runs on the kernel tc_choose picks for its geometry: the row kernel (3x3 stride 1, W % 128 == 0, H % 8 == 0), else
+the halo kernel (3x3 stride 1, W = 16 / 32 / 64, whole tiles of 128 / W rows), else the generic one."""
 import pytest
 import torch
 
@@ -10,24 +12,24 @@ pytestmark = pytest.mark.gpu
 
 TC_CASES = [
     # N, Cin, H, W, Cout, k, stride, (dh, dw), act
-    (1, 64, 8, 128, 64, 3, 1, (1, 1), 1),      # KB=64 (SW128), Wt=128
-    (1, 32, 16, 64, 32, 3, 1, (1, 1), 1),      # KB=32 (SW64), 2 rows per tile
-    (2, 16, 16, 16, 16, 3, 1, (1, 1), 2),      # KB=16 (SW32), 8 rows per tile
-    (1, 2, 8, 256, 16, 3, 1, (1, 1), 1),       # first layer shape class: Cin=2 padded to 16, W=256
-    (1, 64, 32, 32, 128, 3, 2, (1, 1), 2),     # stride 2 (TMA element strides)
+    (1, 64, 8, 128, 64, 3, 1, (1, 1), 1),      # row kernel, two N tiles of 32
+    (1, 32, 16, 64, 32, 3, 1, (1, 1), 1),      # halo kernel, 2 rows per 128-pixel tile
+    (2, 16, 16, 16, 16, 3, 1, (1, 1), 2),      # halo kernel, 8 rows per 128-pixel tile
+    (1, 2, 8, 256, 16, 3, 1, (1, 1), 1),       # first layer shape class (row kernel): Cin=2 padded to 32, W=256
+    (1, 64, 32, 32, 128, 3, 2, (1, 1), 2),     # generic, KB=64 (SW128): stride 2 (TMA element strides)
     (1, 32, 16, 256, 64, 3, 2, (1, 1), 2),     # stride 2, wide
     (1, 64, 32, 16, 64, 3, 1, (4, 2), 1),      # dilated ASPP
     (1, 64, 32, 16, 64, 3, 1, (12, 6), 1),
     (1, 320, 8, 16, 256, 1, 1, (1, 1), 1),     # 1x1 bottleneck, two N tiles of 128
-    (3, 64, 2, 16, 32, 3, 1, (1, 1), 1),       # 4 images per tile, ragged batch
-    (1, 128, 8, 32, 192, 3, 1, (1, 1), 1),     # BN=96 x 2
-    (1, 97, 4, 128, 32, 3, 1, (1, 1), 1),      # dec1 shape class: Cin=97 -> 112, KB=16
-    (2, 448, 8, 32, 192, 3, 1, (1, 1), 1),     # dec4 shape class, deep K
+    (3, 64, 2, 16, 32, 3, 1, (1, 1), 1),       # generic (H=2 is no halo tile): 4 images per tile, ragged batch
+    (1, 128, 8, 32, 192, 3, 1, (1, 1), 1),     # halo kernel, BN=96 x 2
+    (1, 97, 4, 128, 32, 3, 1, (1, 1), 1),      # generic (H=4 is no row tile): dec1 shape class, Cin=97 -> 112, KB=16
+    (2, 448, 8, 32, 192, 3, 1, (1, 1), 1),     # halo kernel: dec4 shape class, deep K
     (5, 256, 1, 16, 256, 1, 1, (1, 1), 1),     # ASPP pooled branch: H=1, 8 images per tile, ragged
-    (1, 16, 16, 64, 8, 3, 1, (1, 1), 0),       # Cout=8 -> N=16, no activation
+    (1, 16, 16, 64, 8, 3, 1, (1, 1), 0),       # halo kernel: Cout=8 -> N=16, no activation
     # row-streaming kernel (3x3, stride 1, W % 128 == 0, H % 8 == 0)
     (1, 64, 8, 128, 32, 3, 1, (1, 1), 1),
-    (1, 16, 8, 128, 16, 3, 1, (1, 1), 1),      # one 64-channel chunk, mostly TMA zero fill
+    (1, 16, 8, 128, 16, 3, 1, (1, 1), 1),      # one 32-channel chunk, half of it TMA zero fill
     (1, 32, 16, 256, 32, 3, 1, (1, 1), 2),     # two 128-pixel tiles per row
     (2, 97, 8, 128, 32, 3, 1, (1, 1), 1),      # dec1 class: 97 -> 112 channels, two chunks
     (1, 192, 16, 128, 64, 3, 1, (1, 1), 1),    # dec2 class: three chunks, two N tiles

@@ -314,8 +314,10 @@ int vr_debug_decoder(vr_ctx* ctx, const float* low, int32_t N, int32_t Cl, int32
 }
 
 int vr_debug_set(int32_t key, int32_t value) {
-  if (key < 0 || key >= 8) return -1;
-  vr::g_tc_debug[key] = value;
+  int* knob = key == 0 ? &vr::g_debug.trace : key == 2 ? &vr::g_debug.rows_wide : key == 3 ? &vr::g_debug.halo
+            : key == 6 ? &vr::g_debug.kskip : nullptr;
+  if (!knob) return -1;
+  *knob = value;
   return 0;
 }
 

@@ -199,9 +199,10 @@ __global__ void __launch_bounds__(kThreads, 1)
 #define VR_TC_FOR_BN(X, KB) X(KB, 16) X(KB, 32) X(KB, 48) X(KB, 64) X(KB, 80) X(KB, 96) X(KB, 112) X(KB, 128)
 #define VR_TC_FOR_ALL(X) VR_TC_FOR_BN(X, 64) VR_TC_FOR_BN(X, 32) VR_TC_FOR_BN(X, 16)
 
+
 // ------------------------------------------------------------------------------------------------
 // host side
-int g_tc_debug[8] = {0, 0, 0, 0, 0, 1, 1, 0};   // [5] fused decoder upsample, [6] zero-weight group skipping: on
+TcDebug g_debug;
 
 static constexpr int kMaxDevices = 64;
 const TcDevice& tc_device() {
@@ -225,7 +226,10 @@ const TcDevice& tc_device() {
   return d;
 }
 
-EncodeTiledFn tc_encode_fn() {
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+static EncodeTiledFn tc_encode_fn() {
   static EncodeTiledFn fn = nullptr;
   if (!fn) {
     void* p = nullptr;
@@ -241,14 +245,14 @@ static CUtensorMapSwizzle swizzle_for(int KB) {
   return KB == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : KB == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
 }
 
-uint16_t tc_f2bf(float f) {   // round-to-nearest-even, same as __float2bfloat16_rn for finite values
+static uint16_t tc_f2bf(float f) {   // round-to-nearest-even, same as __float2bfloat16_rn for finite values
   uint32_t u;
   memcpy(&u, &f, 4);
   if ((u & 0x7fffffffu) > 0x7f800000u) return (uint16_t)((u >> 16) | 0x40);
   uint32_t r = 0x7fffu + ((u >> 16) & 1u);
   return (uint16_t)((u + r) >> 16);
 }
-float tc_bf2f(uint16_t h) {
+static float tc_bf2f(uint16_t h) {
   uint32_t u = (uint32_t)h << 16;
   float f;
   memcpy(&f, &u, 4);
@@ -277,51 +281,150 @@ static TileGeom tile_geom(int Ho, int Wo) {
   return g;
 }
 
-bool tc_supported(const ConvLayer& L, const ActView& in, const ActView& out) {
-  if (!L.tc) return false;
-  if (!(L.k == 1 || L.k == 3) || !(L.stride == 1 || L.stride == 2)) return false;
-  TileGeom g = tile_geom(out.H, out.W);
-  if (!g.ok) return false;
-  if (g.Wt * L.stride > 256 || g.Ht * L.stride > 256) return false;
-  if (in.sw % 8 || in.sh % 8 || in.sn % 8) return false;
-  if ((reinterpret_cast<uintptr_t>(in.hi) | reinterpret_cast<uintptr_t>(in.lo)) & 15) return false;
-  if (in.C <= 0 || in.N <= 0) return false;
-  if ((in.H - 1) / L.stride + 1 != out.H || (in.W - 1) / L.stride + 1 != out.W) return false;
-  return tc_encode_fn() != nullptr;
+// output-channel tiles of the row kernel (rows) or of the generic and halo kernels
+struct NTiling {
+  int BN, n_tiles;
+};
+static NTiling n_tiling(const ConvLayer& L, bool rows) {
+  const int cout16 = round_up(L.Cout, 16);
+  if (rows) {
+    // 64 output channels per tile for the decoder layers with a fused upsample: one N = 64 MMA per product and output
+    // row instead of two N = 32 ones (half the A-operand reads from shared memory) and every input row is interpolated
+    // once instead of once per N tile.  Plain TMA layers stay at 32: the 64-wide tile has a single accumulator set (no
+    // epilogue overlap) and only four operand slots next to its 147 KB of weights, and measured slower there.
+    const int BN = cout16 == 16 ? 16 : (L.rows_wide && cout16 % 64 == 0 ? 64 : 32);
+    return {BN, ceil_div(cout16, BN)};
+  }
+  const int n_tiles = ceil_div(cout16, 128);
+  return {round_up(ceil_div(cout16, n_tiles), 16), n_tiles};
 }
 
-bool tc_can_fuse_upsample(const ConvLayer& L, const ActView& in, const ActView& out, const ActView& up_src) {
-  if (!L.tc || g_tc_debug[5] != 1) return false;
-  const TcConv& tc = *L.tc;
-  if (!tc_rows_supported(L, tc, in, out)) return false;
-  return up_src.C % 32 == 0 && up_src.C <= tc.rows.CinPadR && up_src.H * 2 == in.H && up_src.W * 2 == in.W &&
-         up_src.sw % 8 == 0;
+// the BN values conv_tc_halo.cu instantiates
+static bool halo_has_bn(int BN) { return BN == 16 || BN == 32 || BN == 48 || BN == 64 || BN == 96 || BN == 128; }
+
+// The kernel of a layer whose output maps are H x W: the row kernel where it applies, else the halo kernel, else the
+// generic one.  The row and halo kernels stage the bias of every N tile in 256 floats of shared memory.
+TcKind tc_choose(const ConvLayer& L, int H, int W) {
+  if (!(L.k == 1 || L.k == 3) || !(L.stride == 1 || L.stride == 2) || L.Cout < 4) return TC_NONE;
+  const TileGeom g = tile_geom(H, W);
+  if (!g.ok || g.Wt * L.stride > 256 || g.Ht * L.stride > 256) return TC_NONE;
+  const bool k3s1 = L.k == 3 && L.stride == 1 && L.dil_h == 1 && L.dil_w == 1;
+  const NTiling r = n_tiling(L, true), t = n_tiling(L, false);
+  // whole 128-pixel row tiles of 2, 4 or 8 rows (rows_per_tile, conv_tc_rows.cu)
+  if (k3s1 && W % 128 == 0 && H % 8 == 0 && r.n_tiles * r.BN <= 256) return TC_ROWS;
+  // whole tiles of 128 / W rows (MB = 1)
+  if (k3s1 && (W == 16 || W == 32 || W == 64) && H % (128 / W) == 0 && halo_has_bn(t.BN) &&
+      t.n_tiles * t.BN <= 256 && g_debug.halo != 1)
+    return TC_HALO;
+  return TC_GENERIC;
 }
 
-bool tc_prepare(ConvLayer& L, std::string& err, std::vector<void*>& allocs) {
-  if (!(L.k == 1 || L.k == 3) || L.Cout < 4) return true;   // stays on the CUDA-core kernel
-  auto tc = std::make_shared<TcConv>();
-  tc->taps = L.k * L.k;
-  tc->CinPadTC = round_up(L.CinPad, 16);
-  tc->KB = tc->CinPadTC % 64 == 0 ? 64 : tc->CinPadTC % 32 == 0 ? 32 : 16;
-  tc->cchunks = tc->CinPadTC / tc->KB;
-  tc->SUBS = 64 / tc->KB;
-  tc->Ktot = tc->taps * tc->CinPadTC;
-  tc->CoutPadN = round_up(L.Cout, 16);
-  tc->n_tiles = ceil_div(tc->CoutPadN, 128);
-  tc->BN = round_up(ceil_div(tc->CoutPadN, tc->n_tiles), 16);
-  const int rows = tc->n_tiles * tc->BN;
-  std::vector<uint16_t> planes((size_t)2 * rows * tc->Ktot, 0);
+// The folded fp32 weights split into bf16 hi / lo planes of rows x K; at(co, tap, ci) = row * K + k of one weight.
+template <class At>
+static std::vector<uint16_t> split_bf16(const ConvLayer& L, int rows, int K, At at) {
+  std::vector<uint16_t> planes((size_t)2 * rows * K, 0);
+  const size_t lo = (size_t)rows * K;
   for (int co = 0; co < L.Cout; ++co)
-    for (int t = 0; t < tc->taps; ++t)
+    for (int t = 0; t < L.k * L.k; ++t)
       for (int ci = 0; ci < L.CinPad; ++ci) {
         const float w = L.w_host[((size_t)t * L.CinPad + ci) * L.CoutPad + co];
         const uint16_t hi = tc_f2bf(w);
-        const uint16_t lo = tc_f2bf(w - tc_bf2f(hi));
-        const size_t k = (size_t)t * tc->CinPadTC + ci;
-        planes[(size_t)co * tc->Ktot + k] = hi;
-        planes[((size_t)rows + co) * tc->Ktot + k] = lo;
+        const size_t i = at(co, t, ci);
+        planes[i] = hi;
+        planes[lo + i] = tc_f2bf(w - tc_bf2f(hi));
       }
+  return planes;
+}
+
+// which 8-channel input groups carry any weight at all (the lstm / pad groups of the concat layouts do not)
+static unsigned long long weight_group_mask(const ConvLayer& L, int CinPad) {
+  if (CinPad / 8 > 64) return ~0ull;
+  unsigned long long m = 0x3ull;   // k-step 0 of chunk 0 initialises the accumulators: never skipped
+  for (int ci = 0; ci < L.CinPad; ++ci) {
+    bool any = false;
+    for (int t = 0; t < L.k * L.k && !any; ++t)
+      for (int co = 0; co < L.Cout && !any; ++co) any = L.w_host[((size_t)t * L.CinPad + ci) * L.CoutPad + co] != 0.f;
+    if (any) m |= 1ull << (ci / 8);
+  }
+  return m;
+}
+
+// TMA map of the packed weights [2][rows][K]: boxes of KB channels x box_rows rows, both planes
+static bool encode_weight_map(TcConv& tc, int rows, int K, int box_rows, std::string& err, const std::string& name) {
+  cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)rows, 2};
+  cuuint64_t strides[2] = {(cuuint64_t)K * 2, (cuuint64_t)rows * K * 2};
+  cuuint32_t box[3] = {(cuuint32_t)tc.KB, (cuuint32_t)box_rows, 2};
+  cuuint32_t es[3] = {1, 1, 1};
+  CUresult r = tc_encode_fn()(&tc.map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, tc.w_planes, dims, strides, box, es,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(tc.KB), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    err = "cuTensorMapEncodeTiled(weights) failed for " + name + " code " + std::to_string((int)r);
+    return false;
+  }
+  return true;
+}
+
+const CUtensorMap* tc_activation_map(TcConv& tc, const ActView& v, int bw, int bh, int bn, int es, std::string& err,
+                                     const std::string& name) {
+  const ViewKey key = std::make_tuple((const void*)v.hi, (const void*)v.lo, v.N, v.H, v.W, v.C, bw, bh, bn);
+  auto it = tc.map_a.find(key);
+  if (it != tc.map_a.end()) return &it->second;
+  // TMA reads 16-byte aligned rows; the lo plane is the box's outermost dimension
+  const int64_t plane = (const char*)v.lo - (const char*)v.hi;
+  if (v.sw % 8 || v.sh % 8 || v.sn % 8 || (reinterpret_cast<uintptr_t>(v.hi) & 15) || plane <= 0 || plane % 16) {
+    err = "internal: the input of " + name + " is not 16-byte aligned or its lo plane does not follow its hi plane";
+    return nullptr;
+  }
+  cuuint64_t dims[5] = {(cuuint64_t)v.C, (cuuint64_t)v.W, (cuuint64_t)v.H, (cuuint64_t)v.N, 2};
+  cuuint64_t strides[4] = {(cuuint64_t)v.sw * 2, (cuuint64_t)v.sh * 2, (cuuint64_t)v.sn * 2, (cuuint64_t)plane};
+  cuuint32_t box[5] = {(cuuint32_t)tc.KB, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bn, 2};
+  cuuint32_t estr[5] = {1, (cuuint32_t)es, (cuuint32_t)es, 1, 1};
+  CUtensorMap m;
+  CUresult r = tc_encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)v.hi, dims, strides, box, estr,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(tc.KB), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    err = "cuTensorMapEncodeTiled(activations) failed for " + name + " code " + std::to_string((int)r);
+    return nullptr;
+  }
+  return &tc.map_a.emplace(key, m).first->second;
+}
+
+bool tc_prepare(ConvLayer& L, int H, int W, std::string& err, std::vector<void*>& allocs) {
+  const TcKind kind = tc_choose(L, H, W);
+  if (kind == TC_NONE) return true;   // stays on the CUDA-core kernel
+  if (!tc_encode_fn()) {
+    err = "cuTensorMapEncodeTiled is not available from the driver";
+    return false;
+  }
+  auto tc = std::make_shared<TcConv>();
+  tc->kind = kind;
+  tc->H = H; tc->W = W;
+  const NTiling nt = n_tiling(L, kind == TC_ROWS);
+  const int BN = nt.BN, cin16 = round_up(L.CinPad, 16);
+  tc->BN = BN; tc->n_tiles = nt.n_tiles;
+  tc->KB = kind != TC_GENERIC ? 32 : cin16 % 64 == 0 ? 64 : cin16 % 32 == 0 ? 32 : 16;
+  const int CinPad = round_up(L.CinPad, tc->KB);
+  tc->CinPad = CinPad;
+  tc->chunks = CinPad / tc->KB;
+  tc->kmask = weight_group_mask(L, CinPad);
+  const int rows = nt.n_tiles * BN;
+  std::vector<uint16_t> planes;
+  int brows, K;
+  if (kind == TC_ROWS) {
+    // B[plane][nt*3*BN + (2-kh)*BN + co][kw*CinPad + ci]: the three kh taps stacked along the MMA N dimension
+    brows = 3 * rows;
+    K = 3 * CinPad;
+    planes = split_bf16(L, brows, K, [&](int co, int t, int ci) {
+      return (size_t)(co / BN * 3 * BN + (2 - t / 3) * BN + co % BN) * K + (size_t)(t % 3) * CinPad + ci;
+    });
+  } else {
+    // B[plane][co][tap*CinPad + ci]: every tap padded to whole chunks, so no chunk reads another tap's weights
+    brows = rows;
+    K = L.k * L.k * CinPad;
+    planes = split_bf16(L, brows, K, [&](int co, int t, int ci) { return (size_t)co * K + (size_t)t * CinPad + ci; });
+  }
   std::vector<float> bias((size_t)rows, 0.f);
   for (int co = 0; co < L.Cout; ++co) bias[(size_t)co] = L.bias_host[(size_t)co];
   void* dw = nullptr;
@@ -336,24 +439,7 @@ bool tc_prepare(ConvLayer& L, std::string& err, std::vector<void*>& allocs) {
   cudaMemcpy(db, bias.data(), bias.size() * 4, cudaMemcpyHostToDevice);
   tc->w_planes = (bf16*)dw;
   tc->bias = (float*)db;
-  EncodeTiledFn enc = tc_encode_fn();
-  if (!enc) {
-    err = "cuTensorMapEncodeTiled is not available from the driver";
-    return false;
-  }
-  cuuint64_t dims[3] = {(cuuint64_t)tc->Ktot, (cuuint64_t)rows, 2};
-  cuuint64_t strides[2] = {(cuuint64_t)tc->Ktot * 2, (cuuint64_t)rows * tc->Ktot * 2};
-  cuuint32_t box[3] = {(cuuint32_t)tc->KB, (cuuint32_t)tc->BN, 2};
-  cuuint32_t es[3] = {1, 1, 1};
-  CUresult r = enc(&tc->map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, dw, dims, strides, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(tc->KB), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    err = "cuTensorMapEncodeTiled(weights) failed for " + L.name + " code " + std::to_string((int)r);
-    return false;
-  }
-  if (!tc_rows_prepare(L, *tc, err, allocs)) return false;
-  if (!tc_halo_prepare(L, *tc, err, allocs)) return false;
+  if (!encode_weight_map(*tc, brows, K, kind == TC_ROWS ? 3 * BN : BN, err, L.name)) return false;
   L.tc = tc;
   return true;
 }
@@ -361,36 +447,20 @@ bool tc_prepare(ConvLayer& L, std::string& err, std::vector<void*>& allocs) {
 cudaError_t tc_launch(ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, std::string& err,
                       const ActView* up_src, const ActView* extra) {
   TcConv& tc = *L.tc;
-  if (tc_rows_supported(L, tc, in, out)) return tc_rows_launch(L, tc, in, out, s, err, up_src, extra);
+  if (out.H != tc.H || out.W != tc.W || (in.H - 1) / L.stride + 1 != out.H || (in.W - 1) / L.stride + 1 != out.W) {
+    err = "internal: " + L.name + " is launched on maps of another size than it was prepared for";
+    return cudaErrorInvalidValue;
+  }
+  if (tc.kind == TC_ROWS) return tc_rows_launch(L, tc, in, out, s, err, up_src, extra);
   if (up_src || extra) {
     err = "tc_launch: fused upsample is only implemented in the row-streaming kernel";
     return cudaErrorInvalidValue;
   }
-  if (tc_halo_supported(L, tc, in, out)) return tc_halo_launch(L, tc, in, out, s, err);
+  if (tc.kind == TC_HALO) return tc_halo_launch(L, tc, in, out, s, err);
   const TileGeom g = tile_geom(out.H, out.W);
-  auto key = std::make_tuple((const void*)in.hi, (const void*)in.lo, in.N, in.H, in.W, in.C);
-  auto it = tc.map_a.find(key);
-  if (it == tc.map_a.end()) {
-    CUtensorMap m;
-    cuuint64_t dims[5] = {(cuuint64_t)in.C, (cuuint64_t)in.W, (cuuint64_t)in.H, (cuuint64_t)in.N, 2};
-    const int64_t plane = (const char*)in.lo - (const char*)in.hi;
-    if (plane <= 0 || plane % 16) {
-      err = "tc_launch: hi/lo planes must be 16-byte aligned with lo after hi";
-      return cudaErrorInvalidValue;
-    }
-    cuuint64_t strides[4] = {(cuuint64_t)in.sw * 2, (cuuint64_t)in.sh * 2, (cuuint64_t)in.sn * 2, (cuuint64_t)plane};
-    cuuint32_t box[5] = {(cuuint32_t)tc.KB, (cuuint32_t)(g.Wt * L.stride), (cuuint32_t)(g.Ht * L.stride),
-                         (cuuint32_t)g.Nt, 2};
-    cuuint32_t es[5] = {1, (cuuint32_t)L.stride, (cuuint32_t)L.stride, 1, 1};
-    CUresult r = tc_encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)in.hi, dims, strides, box, es,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(tc.KB), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      err = "cuTensorMapEncodeTiled(activations) failed for " + L.name + " code " + std::to_string((int)r);
-      return cudaErrorInvalidValue;
-    }
-    it = tc.map_a.emplace(key, m).first;
-  }
+  const CUtensorMap* map_a = tc_activation_map(tc, in, g.Wt * L.stride, g.Ht * L.stride, g.Nt, L.stride, err, L.name);
+  if (!map_a) return cudaErrorInvalidValue;
+  const int SUBS = 64 / tc.KB;
   TcParams p;
   p.N = out.N; p.Ho = out.H; p.Wo = out.W;
   p.Wt = g.Wt; p.Ht = g.Ht; p.Nt = g.Nt;
@@ -400,9 +470,9 @@ cudaError_t tc_launch(ConvLayer& L, const ActView& in, const ActView& out, cudaS
   p.stride = L.stride; p.dil_h = L.dil_h; p.dil_w = L.dil_w;
   p.pad_h = L.dil_h * (L.k / 2); p.pad_w = L.dil_w * (L.k / 2);
   p.KW = L.k;
-  p.cchunks = tc.cchunks; p.total_sub = tc.taps * tc.cchunks;
-  p.CinPadTC = tc.CinPadTC; p.Cout = L.Cout; p.act = L.act;
-  const int stage_bytes = tc.SUBS * (2 * 128 * tc.KB * 2 + 2 * tc.BN * tc.KB * 2);
+  p.cchunks = tc.chunks; p.total_sub = L.k * L.k * tc.chunks;
+  p.CinPadTC = tc.CinPad; p.Cout = L.Cout; p.act = L.act;
+  const int stage_bytes = SUBS * (2 * 128 * tc.KB * 2 + 2 * tc.BN * tc.KB * 2);
   const TcDevice& dv = tc_device();
   if (!dv.ok) {
     err = "tc_launch: cannot query the current device";
@@ -420,10 +490,10 @@ cudaError_t tc_launch(ConvLayer& L, const ActView& in, const ActView& out, cudaS
   p.bias = tc.bias;
   const int total_tiles = p.m_tiles * p.n_tiles;
   const int grid = total_tiles < dv.num_sms ? total_tiles : dv.num_sms;
-#define VR_TC_LAUNCH(KB_, BN_)                                                           \
-  if (tc.KB == KB_ && tc.BN == BN_) {                                                    \
-    conv_tc_kernel<KB_, BN_><<<grid, kThreads, dyn, s>>>(it->second, tc.map_b, p);     \
-    return cudaGetLastError();                                                           \
+#define VR_TC_LAUNCH(KB_, BN_)                                                       \
+  if (tc.KB == KB_ && tc.BN == BN_) {                                                \
+    conv_tc_kernel<KB_, BN_><<<grid, kThreads, dyn, s>>>(*map_a, tc.map_b, p);       \
+    return cudaGetLastError();                                                       \
   }
   VR_TC_FOR_ALL(VR_TC_LAUNCH)
 #undef VR_TC_LAUNCH

@@ -253,84 +253,15 @@ __global__ void __launch_bounds__(kThreads, 1)
   }
 }
 
-// every (BN, MB) instantiation the host can launch: the BN values tc_prepare picks for these layers
+// every (BN, MB) instantiation the host can launch: the BN values tc_choose accepts for these layers (halo_has_bn)
 #define VR_HALO_FOR_MB(X, BN) X(BN, 1) X(BN, 2)
 #define VR_HALO_FOR_ALL(X) \
   VR_HALO_FOR_MB(X, 16) VR_HALO_FOR_MB(X, 32) VR_HALO_FOR_MB(X, 48) VR_HALO_FOR_MB(X, 64) VR_HALO_FOR_MB(X, 96) \
   VR_HALO_FOR_MB(X, 128)
 
-static bool halo_has_bn(int BN) { return BN == 16 || BN == 32 || BN == 48 || BN == 64 || BN == 96 || BN == 128; }
-
 // ------------------------------------------------------------------------------------------------
-bool tc_halo_prepare(ConvLayer& L, TcConv& tc, std::string& err, std::vector<void*>& allocs) {
-  TcHaloPlan& Hp = tc.halo;
-  Hp.ok = false;
-  if (L.k != 3 || L.stride != 1 || L.dil_h != 1 || L.dil_w != 1 || !halo_has_bn(tc.BN)) return true;
-  if (tc.n_tiles * tc.BN > 256) return true;   // bias staging area of the kernel
-  Hp.CinPadH = round_up(L.CinPad, (int)kKB);
-  Hp.chunks = Hp.CinPadH / (int)kKB;
-  // B[plane][nt*BN + co][tap*CinPadH + ci]: every tap padded to whole 32-channel chunks, so no chunk reads another
-  // tap's weights
-  const int rows = tc.n_tiles * tc.BN;
-  const int Ktot = 9 * Hp.CinPadH;
-  std::vector<uint16_t> planes((size_t)2 * rows * Ktot, 0);
-  for (int co = 0; co < L.Cout; ++co)
-    for (int t = 0; t < 9; ++t)
-      for (int ci = 0; ci < L.CinPad; ++ci) {
-        const float w = L.w_host[((size_t)t * L.CinPad + ci) * L.CoutPad + co];
-        const uint16_t hi = tc_f2bf(w);
-        const uint16_t lo = tc_f2bf(w - tc_bf2f(hi));
-        const size_t k = (size_t)t * Hp.CinPadH + ci;
-        planes[(size_t)co * Ktot + k] = hi;
-        planes[((size_t)rows + co) * Ktot + k] = lo;
-      }
-  // which 8-channel input groups carry any weight at all (the lstm / pad groups of the concat layouts do not)
-  Hp.kmask = ~0ull;
-  if (Hp.CinPadH / 8 <= 64) {
-    Hp.kmask = 0x3ull;   // k-step 0 of chunk 0 is never skipped: every tile issues at least one chunk
-    for (int ci = 0; ci < L.CinPad; ++ci) {
-      bool any = false;
-      for (int t = 0; t < 9 && !any; ++t)
-        for (int co = 0; co < L.Cout && !any; ++co) any = L.w_host[((size_t)t * L.CinPad + ci) * L.CoutPad + co] != 0.f;
-      if (any) Hp.kmask |= 1ull << (ci / 8);
-    }
-  }
-  void* dw = nullptr;
-  if (cudaMalloc(&dw, planes.size() * 2) != cudaSuccess) {
-    err = "cudaMalloc failed while packing halo-kernel weights for " + L.name;
-    return false;
-  }
-  allocs.push_back(dw);
-  cudaMemcpy(dw, planes.data(), planes.size() * 2, cudaMemcpyHostToDevice);
-  Hp.w_planes = (bf16*)dw;
-  cuuint64_t dims[3] = {(cuuint64_t)Ktot, (cuuint64_t)rows, 2};
-  cuuint64_t strides[2] = {(cuuint64_t)Ktot * 2, (cuuint64_t)rows * Ktot * 2};
-  cuuint32_t box[3] = {kKB, (cuuint32_t)tc.BN, 2};
-  cuuint32_t es[3] = {1, 1, 1};
-  CUresult r = tc_encode_fn()(&Hp.map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, dw, dims, strides, box, es,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
-                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    err = "cuTensorMapEncodeTiled(halo-kernel weights) failed for " + L.name + " code " + std::to_string((int)r);
-    return false;
-  }
-  Hp.ok = true;
-  return true;
-}
-
-bool tc_halo_supported(const ConvLayer& L, const TcConv& tc, const ActView& in, const ActView& out) {
-  if (!tc.halo.ok || g_tc_debug[3] == 1) return false;
-  if (L.k != 3 || L.stride != 1 || L.dil_h != 1 || L.dil_w != 1) return false;
-  if (!(out.W == 16 || out.W == 32 || out.W == 64) || in.H != out.H || in.W != out.W) return false;
-  if (out.H % (128 / out.W)) return false;   // whole tiles of Ht = 128 / W rows (MB = 1)
-  if (in.sw % 8 || in.sh % 8 || in.sn % 8) return false;
-  if ((reinterpret_cast<uintptr_t>(in.hi) | reinterpret_cast<uintptr_t>(in.lo)) & 15) return false;
-  return in.C > 0 && in.N > 0;
-}
-
 cudaError_t tc_halo_launch(ConvLayer& L, TcConv& tc, const ActView& in, const ActView& out, cudaStream_t s,
                            std::string& err) {
-  TcHaloPlan& Hp = tc.halo;
   const TcDevice& dv = tc_device();
   if (!dv.ok) {
     err = "tc_halo_launch: cannot query the current device";
@@ -338,14 +269,14 @@ cudaError_t tc_halo_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   }
   // MB = 2 halves the weight traffic per pixel but also the number of tiles, so the last wave of the persistent grid
   // weighs twice as much.  A 256-pixel tile takes about 1.9x a 128-pixel one (H100, per-layer times of both): MB = 2
-  // where 1.9 x its waves are no more than MB = 1's (g_tc_debug[3] = 2 / 3 pins MB = 1 / 2).
+  // where 1.9 x its waves are no more than MB = 1's (vr_debug_set(3, 2 / 3) pins MB = 1 / 2).
   const int ht1 = 128 / out.W;
   const bool mb2_tiles = out.H % (2 * ht1) == 0;
   const int tiles1 = out.N * (out.H / ht1) * tc.n_tiles;
   const int waves1 = ceil_div(tiles1, dv.num_sms), waves2 = ceil_div(tiles1 / 2, dv.num_sms);
   int MB = mb2_tiles && 19 * waves2 <= 10 * waves1 ? 2 : 1;
-  if (g_tc_debug[3] == 2) MB = 1;
-  if (g_tc_debug[3] == 3 && mb2_tiles) MB = 2;
+  if (g_debug.halo == 2) MB = 1;
+  if (g_debug.halo == 3 && mb2_tiles) MB = 2;
   HaloParams p;
   p.N = out.N; p.H = out.H; p.W = out.W;
   p.lw = out.W == 16 ? 4 : out.W == 32 ? 5 : 6;
@@ -354,35 +285,16 @@ cudaError_t tc_halo_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   p.tiles_h = out.H / p.Ht;
   p.n_tiles = tc.n_tiles;
   p.total_tiles = out.N * p.tiles_h * p.n_tiles;
-  p.chunks = Hp.chunks; p.CinPadH = Hp.CinPadH; p.Cout = L.Cout; p.act = L.act;
+  p.chunks = tc.chunks; p.CinPadH = tc.CinPad; p.Cout = L.Cout; p.act = L.act;
   p.hplane = (uint32_t)((p.Ht + 2) * p.Wb) * kRowB;
   p.hslot = 2 * p.hplane;
-  p.kmask = g_tc_debug[6] == 1 ? Hp.kmask : ~0ull;
+  p.kmask = g_debug.kskip == 1 ? tc.kmask : ~0ull;
   p.out_hi = out.hi; p.out_lo = out.lo;
   p.osn = out.sn; p.osh = out.sh; p.osw = out.sw;
   p.bias = tc.bias;
-  ViewKey key = std::make_tuple((const void*)in.hi, (const void*)in.lo, in.N, in.H, in.W, in.C);
-  auto it = Hp.map_a[MB - 1].find(key);
-  if (it == Hp.map_a[MB - 1].end()) {
-    CUtensorMap m;
-    const int64_t plane = (const char*)in.lo - (const char*)in.hi;
-    if (plane <= 0 || plane % 16) {
-      err = "tc_halo_launch: hi/lo planes must be 16-byte aligned with lo after hi";
-      return cudaErrorInvalidValue;
-    }
-    cuuint64_t dims[5] = {(cuuint64_t)in.C, (cuuint64_t)in.W, (cuuint64_t)in.H, (cuuint64_t)in.N, 2};
-    cuuint64_t strides[4] = {(cuuint64_t)in.sw * 2, (cuuint64_t)in.sh * 2, (cuuint64_t)in.sn * 2, (cuuint64_t)plane};
-    cuuint32_t box[5] = {kKB, (cuuint32_t)p.Wb, (cuuint32_t)(p.Ht + 2), 1, 2};   // the halo tile, both planes
-    cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    CUresult r = tc_encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)in.hi, dims, strides, box, es,
-                                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
-                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      err = "cuTensorMapEncodeTiled(halo-kernel activations) failed for " + L.name + " code " + std::to_string((int)r);
-      return cudaErrorInvalidValue;
-    }
-    it = Hp.map_a[MB - 1].emplace(key, m).first;
-  }
+  // the halo tile, both planes
+  const CUtensorMap* map_a = tc_activation_map(tc, in, p.Wb, p.Ht + 2, 1, 1, err, L.name);
+  if (!map_a) return cudaErrorInvalidValue;
   // shared memory: up to kMaxHSlots halo slots next to one chunk's nine weight stages, the rest to weight stages
   const int w_stage = tc.BN * 2 * (int)kRowB;
   const int dyn = dv.max_smem - 2048;   // static barriers + staged bias live in the remaining 2 KiB
@@ -397,16 +309,17 @@ cudaError_t tc_halo_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
     return cudaErrorInvalidValue;
   }
   const int grid = p.total_tiles < dv.num_sms ? p.total_tiles : dv.num_sms;   // persistent: one CTA per SM
-#define VR_HALO_LAUNCH(BN_, MB_)                                                           \
-  if (tc.BN == BN_ && MB == MB_) {                                                         \
-    conv_tc_halo_kernel<BN_, MB_><<<grid, kThreads, dyn, s>>>(it->second, Hp.map_b, p);   \
-    return cudaGetLastError();                                                             \
+#define VR_HALO_LAUNCH(BN_, MB_)                                                        \
+  if (tc.BN == BN_ && MB == MB_) {                                                      \
+    conv_tc_halo_kernel<BN_, MB_><<<grid, kThreads, dyn, s>>>(*map_a, tc.map_b, p);     \
+    return cudaGetLastError();                                                          \
   }
   VR_HALO_FOR_ALL(VR_HALO_LAUNCH)
 #undef VR_HALO_LAUNCH
   err = "tc_halo_launch: no kernel instantiation for this channel tile";
   return cudaErrorInvalidValue;
 }
+
 
 // cudaFuncSetAttribute is per device: called by tc_device() the first time a device is used (conv_tc.cu)
 void tc_halo_set_attributes(int max_smem) {

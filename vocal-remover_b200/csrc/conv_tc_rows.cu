@@ -36,7 +36,6 @@ static constexpr int kInterpWarps = 10;             // each covers 7 staged sour
 static constexpr int kConsumerWarps = 8;            // two warpgroups: pixels [0,64) and [64,128) of the tile
 static constexpr int kTmaWarp = kConsumerWarps;
 static constexpr int kInterpWarp0 = kConsumerWarps + 1;
-static constexpr int kMaxR = 8;                     // largest number of output rows per CTA tile (H must be a multiple)
 // output rows per tile: R * BN / 2 accumulator registers per consumer thread, next to 32 registers of A fragments.
 // The warps of a block are spread over the four SM sub-partitions, each with 512 registers per lane.  Without the
 // fused upsample the block is 9 warps (3 per sub-partition: 168 registers per thread).  With it the block is five
@@ -543,162 +542,44 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
 }
 
 // ------------------------------------------------------------------------------------------------
-bool tc_rows_prepare(ConvLayer& L, TcConv& tc, std::string& err, std::vector<void*>& allocs) {
-  TcRowsPlan& R = tc.rows;
-  R.ok = false;
-  if (L.k != 3 || L.stride != 1 || L.dil_h != 1 || L.dil_w != 1) return true;
-  const int cout16 = round_up(L.Cout, 16);
-  // 64 output channels per tile for the decoder layers with a fused upsample: one N = 64 MMA per product and output row
-  // instead of two N = 32 ones (half the A-operand reads from shared memory) and every input row is interpolated once
-  // instead of once per N tile.  Plain TMA layers stay at 32: the 64-wide tile has a single accumulator set (no
-  // epilogue overlap) and only four operand slots next to its 147 KB of weights, and measured slower there.
-  R.BN = cout16 == 16 ? 16 : (L.rows_wide && cout16 % 64 == 0 ? 64 : 32);
-  R.n_tiles = ceil_div(cout16, R.BN);
-  if (R.n_tiles * R.BN > 256) return true;   // bias staging area of the kernel
-  R.KB = (int)kKB;
-  R.CinPadR = round_up(L.CinPad, R.KB);
-  R.chunks = R.CinPadR / R.KB;
-  // B[plane][nt*3*BN + (2-kh)*BN + co][kw*CinPadR + ci]: the three kh taps stacked along the MMA N dimension
-  const int rows = R.n_tiles * R.BN;
-  const int brows = 3 * rows;
-  const int Ktot = 3 * R.CinPadR;
-  std::vector<uint16_t> planes((size_t)2 * brows * Ktot, 0);
-  for (int co = 0; co < L.Cout; ++co) {
-    const int nt = co / R.BN, col = co % R.BN;
-    for (int kh = 0; kh < 3; ++kh)
-      for (int kw = 0; kw < 3; ++kw)
-        for (int ci = 0; ci < L.CinPad; ++ci) {
-          const float w = L.w_host[((size_t)(kh * 3 + kw) * L.CinPad + ci) * L.CoutPad + co];
-          const uint16_t hi = tc_f2bf(w);
-          const uint16_t lo = tc_f2bf(w - tc_bf2f(hi));
-          const size_t row = (size_t)nt * 3 * R.BN + (size_t)(2 - kh) * R.BN + col;
-          const size_t k = (size_t)kw * R.CinPadR + ci;
-          planes[row * Ktot + k] = hi;
-          planes[((size_t)brows + row) * Ktot + k] = lo;
-        }
-  }
-  // which 8-channel input groups carry any weight at all (the lstm / pad groups of the concat layouts do not)
-  R.kmask = ~0ull;
-  if (R.CinPadR / 8 <= 64) {
-    R.kmask = 0x3ull;   // k-step 0 of chunk 0 initialises the accumulators: never skipped
-    for (int ci = 0; ci < L.CinPad; ++ci) {
-      bool any = false;
-      for (int t = 0; t < 9 && !any; ++t)
-        for (int co = 0; co < L.Cout && !any; ++co) any = L.w_host[((size_t)t * L.CinPad + ci) * L.CoutPad + co] != 0.f;
-      if (any) R.kmask |= 1ull << (ci / 8);
-    }
-  }
-  std::vector<float> bias((size_t)rows, 0.f);
-  for (int co = 0; co < L.Cout; ++co) bias[(size_t)co] = L.bias_host[(size_t)co];
-  void* dw = nullptr;
-  void* db = nullptr;
-  if (cudaMalloc(&dw, planes.size() * 2) != cudaSuccess || cudaMalloc(&db, bias.size() * 4) != cudaSuccess) {
-    err = "cudaMalloc failed while packing row-kernel weights for " + L.name;
-    return false;
-  }
-  allocs.push_back(dw);
-  allocs.push_back(db);
-  cudaMemcpy(dw, planes.data(), planes.size() * 2, cudaMemcpyHostToDevice);
-  cudaMemcpy(db, bias.data(), bias.size() * 4, cudaMemcpyHostToDevice);
-  R.w_planes = (bf16*)dw;
-  R.bias = (float*)db;
-  cuuint64_t dims[3] = {(cuuint64_t)Ktot, (cuuint64_t)brows, 2};
-  cuuint64_t strides[2] = {(cuuint64_t)Ktot * 2, (cuuint64_t)brows * Ktot * 2};
-  cuuint32_t box[3] = {(cuuint32_t)R.KB, (cuuint32_t)(3 * R.BN), 2};
-  cuuint32_t es[3] = {1, 1, 1};
-  CUresult r = tc_encode_fn()(&R.map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, dw, dims, strides, box, es,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
-                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    err = "cuTensorMapEncodeTiled(row-kernel weights) failed for " + L.name + " code " + std::to_string((int)r);
-    return false;
-  }
-  R.ok = true;
-  return true;
-}
-
-bool tc_rows_supported(const ConvLayer& L, const TcConv& tc, const ActView& in, const ActView& out) {
-  if (!tc.rows.ok || g_tc_debug[1]) return false;
-  if (L.k != 3 || L.stride != 1 || L.dil_h != 1 || L.dil_w != 1) return false;
-  if (out.W % 128 || out.H % kMaxR || in.H != out.H || in.W != out.W) return false;
-  if (in.sw % 8 || in.sh % 8 || in.sn % 8) return false;
-  if ((reinterpret_cast<uintptr_t>(in.hi) | reinterpret_cast<uintptr_t>(in.lo)) & 15) return false;
-  return true;
-}
-
 // up_src != nullptr: the first up_src->C channels of `in` are NOT read; they are produced inside the kernel as the
-// bilinear x2 upsample of *up_src (half resolution).  Needs up_src->C % 32 == 0.
-static bool rows_activation_map(const ActView& v, CUtensorMap* m, std::string& err, const std::string& name) {
-  cuuint64_t dims[5] = {(cuuint64_t)v.C, (cuuint64_t)v.W, (cuuint64_t)v.H, (cuuint64_t)v.N, 2};
-  const int64_t plane = (const char*)v.lo - (const char*)v.hi;
-  if (plane <= 0 || plane % 16) {
-    err = "tc_rows_launch: hi/lo planes must be 16-byte aligned with lo after hi";
-    return false;
-  }
-  cuuint64_t strides[4] = {(cuuint64_t)v.sw * 2, (cuuint64_t)v.sh * 2, (cuuint64_t)v.sn * 2, (cuuint64_t)plane};
-  cuuint32_t box[5] = {kKB, (cuuint32_t)kBoxPx, 1, 1, 2};   // both planes of one row in one box
-  cuuint32_t es[5] = {1, 1, 1, 1, 1};
-  CUresult r = tc_encode_fn()(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)v.hi, dims, strides, box, es,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
-                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    err = "cuTensorMapEncodeTiled(row-kernel activations) failed for " + name + " code " + std::to_string((int)r);
-    return false;
-  }
-  return true;
-}
-
+// bilinear x2 upsample of *up_src (half resolution, tc.fuses_upsample(up_src->C)).
 // extra != nullptr: the LAST channel chunk is read from *extra (channels [0, extra->C), zero-filled up to the chunk).
 cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const ActView& out, cudaStream_t s,
                            std::string& err, const ActView* up_src, const ActView* extra) {
-  TcRowsPlan& R = tc.rows;
-  if (up_src && (up_src->C % 32 || up_src->H * 2 != in.H || up_src->W * 2 != in.W || up_src->sw % 8 ||
-                 up_src->C > R.CinPadR)) {
+  if (up_src && (!tc.fuses_upsample(up_src->C) || up_src->H * 2 != in.H || up_src->W * 2 != in.W || up_src->sw % 8)) {
     err = "tc_rows_launch: fused upsample needs a half-resolution source of 32k channels";
     return cudaErrorInvalidValue;
   }
-  ViewKey key = std::make_tuple((const void*)in.hi, (const void*)in.lo, in.N, in.H, in.W, in.C);
-  auto it = R.map_a.find(key);
-  if (it == R.map_a.end()) {
-    CUtensorMap m;
-    if (!rows_activation_map(in, &m, err, L.name)) return cudaErrorInvalidValue;
-    it = R.map_a.emplace(key, m).first;
+  if (extra && (extra->H != in.H || extra->W != in.W || extra->N != in.N || extra->C > tc.KB)) {
+    err = "tc_rows_launch: the extra last-chunk tensor must match the input geometry and fit one chunk";
+    return cudaErrorInvalidValue;
   }
-  auto itl = it;
-  if (extra) {
-    if (extra->H != in.H || extra->W != in.W || extra->N != in.N || extra->C > R.KB || extra->sw % 8) {
-      err = "tc_rows_launch: the extra last-chunk tensor must match the input geometry and fit one chunk";
-      return cudaErrorInvalidValue;
-    }
-    ViewKey kl = std::make_tuple((const void*)extra->hi, (const void*)extra->lo, extra->N, extra->H, extra->W, extra->C);
-    itl = R.map_l.find(kl);
-    if (itl == R.map_l.end()) {
-      CUtensorMap m;
-      if (!rows_activation_map(*extra, &m, err, L.name)) return cudaErrorInvalidValue;
-      itl = R.map_l.emplace(kl, m).first;
-    }
-  }
+  // both planes of one row in one box
+  const CUtensorMap* map_a = tc_activation_map(tc, in, kBoxPx, 1, 1, 1, err, L.name);
+  const CUtensorMap* map_l = extra ? tc_activation_map(tc, *extra, kBoxPx, 1, 1, 1, err, L.name) : map_a;
+  if (!map_a || !map_l) return cudaErrorInvalidValue;
   RowsParams p;
   p.N = out.N; p.H = out.H; p.W = out.W;
   const bool up = up_src != nullptr;
-  p.tiles_w = out.W / 128; p.tiles_h = out.H / rows_per_tile(R.BN); p.n_tiles = R.n_tiles;
-  p.total_tiles = p.tiles_w * p.tiles_h * out.N * R.n_tiles;
-  p.chunks = R.chunks; p.CinPadR = R.CinPadR; p.Cout = L.Cout; p.act = L.act;
+  p.tiles_w = out.W / 128; p.tiles_h = out.H / rows_per_tile(tc.BN); p.n_tiles = tc.n_tiles;
+  p.total_tiles = p.tiles_w * p.tiles_h * out.N * tc.n_tiles;
+  p.chunks = tc.chunks; p.CinPadR = tc.CinPad; p.Cout = L.Cout; p.act = L.act;
   p.out_hi = out.hi; p.out_lo = out.lo;
   p.osn = out.sn; p.osh = out.sh; p.osw = out.sw;
-  p.bias = R.bias;
+  p.bias = tc.bias;
   p.up_chunks = 0; p.xH = p.xW = 0;
   p.x_hi = p.x_lo = nullptr; p.xsn = p.xsh = 0; p.xsw = 0;
-  p.trace = g_tc_debug[0] == 1 ? 1 : 0;
+  p.trace = g_debug.trace == 1 ? 1 : 0;
   p.up_sh = p.up_sw = 0.f;
   p.dot_w = L.dot_w; p.dot_out = L.dot_w ? L.dot_out : nullptr;
   p.a_c_off = 0;
-  p.l_chunk = extra ? R.chunks - 1 : -1;
-  p.kmask = g_tc_debug[6] == 1 ? R.kmask : ~0ull;   // VR_KSKIP=0 issues the all-zero-weight channel groups too
+  p.l_chunk = extra ? tc.chunks - 1 : -1;
+  p.kmask = g_debug.kskip == 1 ? tc.kmask : ~0ull;   // VR_KSKIP=0 issues the all-zero-weight channel groups too
   if (up_src) {
     // `in` is either the whole concat buffer (its first up_src->C channels are then never read) or only the skip
     // tensor, which starts at reduction index up_src->C
-    if (in.C + up_src->C + (extra ? R.KB : 0) <= R.CinPadR) p.a_c_off = -up_src->C;
+    if (in.C + up_src->C + (extra ? tc.KB : 0) <= tc.CinPad) p.a_c_off = -up_src->C;
     p.up_chunks = up_src->C / 32;
     p.xH = up_src->H; p.xW = up_src->W;
     p.x_hi = up_src->hi; p.x_lo = up_src->lo;
@@ -715,7 +596,7 @@ cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
     err = "tc_rows_launch: cannot query the current device";
     return cudaErrorInvalidValue;
   }
-  const int b_bytes = R.BN == 16 ? (int)(2 * RowsGeom<16>::kBBuf) : R.BN == 32 ? (int)(2 * RowsGeom<32>::kBBuf) : (int)(2 * RowsGeom<64>::kBBuf);
+  const int b_bytes = tc.BN == 16 ? (int)(2 * RowsGeom<16>::kBBuf) : tc.BN == 32 ? (int)(2 * RowsGeom<32>::kBBuf) : (int)(2 * RowsGeom<64>::kBBuf);
   p.n_aslots = (dv.max_smem - 3072 - 1024 - b_bytes) / (int)kASlot;
   if (p.n_aslots > kMaxASlots) p.n_aslots = kMaxASlots;
   if (p.n_aslots < (p.up_chunks > 0 ? 4 : 2)) {
@@ -725,17 +606,16 @@ cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   // the interpolation ring gets the larger share: most chunks of the decoder layers are up-sampled
   p.n_uslots = p.up_chunks > 0 ? p.n_aslots - p.n_aslots / 2 : 0;
   if (p.up_chunks > 0 && p.n_aslots - p.n_uslots < 2) p.n_uslots = p.n_aslots - 2;
-  if (p.up_chunks > 0 && g_tc_debug[4] >= 1 && g_tc_debug[4] <= p.n_aslots - 2) p.n_uslots = g_tc_debug[4];
   const int dyn = p.n_aslots * (int)kASlot + b_bytes + 1024;
   const int grid = p.total_tiles < dv.num_sms ? p.total_tiles : dv.num_sms;   // persistent: one CTA per SM
   const int threads = rows_threads(up);
-#define VR_ROWS_LAUNCH(BN_)                                                                            \
-  if (R.BN == BN_) {                                                                                   \
-    if (up)                                                                                            \
-      conv_tc_rows_kernel<BN_, true><<<grid, threads, dyn, s>>>(it->second, R.map_b, itl->second, p);  \
-    else                                                                                               \
-      conv_tc_rows_kernel<BN_, false><<<grid, threads, dyn, s>>>(it->second, R.map_b, itl->second, p); \
-    return cudaGetLastError();                                                                         \
+#define VR_ROWS_LAUNCH(BN_)                                                                      \
+  if (tc.BN == BN_) {                                                                            \
+    if (up)                                                                                      \
+      conv_tc_rows_kernel<BN_, true><<<grid, threads, dyn, s>>>(*map_a, tc.map_b, *map_l, p);    \
+    else                                                                                         \
+      conv_tc_rows_kernel<BN_, false><<<grid, threads, dyn, s>>>(*map_a, tc.map_b, *map_l, p);   \
+    return cudaGetLastError();                                                                   \
   }
   VR_ROWS_LAUNCH(16)
   VR_ROWS_LAUNCH(32)
@@ -744,6 +624,7 @@ cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   err = "tc_rows_launch: no kernel instantiation for this channel tile";
   return cudaErrorInvalidValue;
 }
+
 
 // copies the timeline of the last traced launch (vr_debug_set(0, 1)) to the host: 3 roles x kTraceEvents x 3 stamps
 int tc_rows_read_trace(unsigned long long* out, long long capacity) {

@@ -137,7 +137,7 @@ bool Engine::need(const std::string& key, std::initializer_list<int64_t> shape, 
 // Fold BatchNorm2d(eval) into the bias-free conv and pack to [tap][CinPad][CoutPad] (lib/layers.py:12-23).
 // perm[packed_ci] = original input channel, or -1 for a zero (padding) channel.
 bool Engine::make_conv(ConvLayer& L, const std::string& prefix, const std::vector<int>& perm, int cin_pad, int k,
-                       int stride, int dh, int dw, int act) {
+                       int stride, int dh, int dw, int act, int H, int W) {
   L.name = prefix;
   L.k = k; L.stride = stride; L.dil_h = dh; L.dil_w = dw; L.act = act;
   auto itw = sd_.find(prefix + ".conv.0.weight");
@@ -182,10 +182,7 @@ bool Engine::make_conv(ConvLayer& L, const std::string& prefix, const std::vecto
   if (!L.w || !L.bias) return false;
   cudaMemcpy(L.w, L.w_host.data(), L.w_host.size() * sizeof(float), cudaMemcpyHostToDevice);
   cudaMemcpy(L.bias, L.bias_host.data(), L.bias_host.size() * sizeof(float), cudaMemcpyHostToDevice);
-  if (cfg_.conv_mode == 0) {
-    if (!tc_prepare(L, err, allocs_)) return false;
-  }
-  return true;
+  return cfg_.conv_mode != 0 || tc_prepare(L, H, W, err, allocs_);
 }
 
 static std::vector<int> identity_perm(int c, int pad) {
@@ -204,9 +201,12 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
     return false;
   }
   // Layouts of the dec1 input (see BaseNetPlan::skip_only in engine.h).  The fused layout needs the row kernel with
-  // dec1's up-sampled half (h, 2n channels) in whole 32-channel chunks.
-  P.skip_only = cfg_.conv_mode == 0 && g_tc_debug[5] == 1 && g_tc_debug[1] == 0 &&
-                (2 * n) % 32 == 0 && W % 128 == 0 && H % 8 == 0;
+  // dec1's up-sampled half (h, 2n channels) in whole 32-channel chunks.  dec1 is a 3x3 convolution to n channels at
+  // H x W; its weights are packed below, once the layout is known.
+  ConvLayer dec1;
+  dec1.k = 3;
+  dec1.Cout = n;
+  P.skip_only = cfg_.conv_mode == 0 && (2 * n) % 32 == 0 && tc_choose(dec1, H, W) == TC_ROWS;
   const int lg = 16;   // the lstm channel + 15 zeros keep every slice 32-byte aligned (full-sector 256-bit stores)
   P.lstm_own = P.skip_only && n % 32 == 0;
   const int c1 = P.skip_only ? 2 * n + round_up(n, 32) + (P.lstm_own ? lg : 0) : round_up(3 * n + lg, 16);
@@ -232,32 +232,39 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
   P.d2 = make_buffer(Nb, H / 2, W / 2, P.skip_only ? 2 * n : 2 * n + lg);
   if (!P.d2.hi || !P.cat1.hi) return false;
 
-  if (!make_conv(P.enc1, prefix + ".enc1", in_perm, cin_pad, 3, 1, 1, 1, ACT_RELU)) return false;
+  if (!make_conv(P.enc1, prefix + ".enc1", in_perm, cin_pad, 3, 1, 1, 1, ACT_RELU, H, W)) return false;
   const int mult[5] = {1, 2, 4, 6, 8};
   for (int i = 0; i < 4; ++i) {
-    const int cin = n * mult[i], cout = n * mult[i + 1];
+    const int cin = n * mult[i], cout = n * mult[i + 1], Ho = H >> (i + 1), Wo = W >> (i + 1);
     const std::string e = prefix + ".enc" + std::to_string(i + 2);
     if (!make_conv(P.enc_a[i], e + ".conv1", identity_perm(cin, round_up(cin, 8)), round_up(cin, 8), 3, 2, 1, 1,
-                   ACT_LEAKY))
+                   ACT_LEAKY, Ho, Wo))
       return false;
-    if (!make_conv(P.enc_b[i], e + ".conv2", identity_perm(cout, cout), cout, 3, 1, 1, 1, ACT_LEAKY)) return false;
+    if (!make_conv(P.enc_b[i], e + ".conv2", identity_perm(cout, cout), cout, 3, 1, 1, 1, ACT_LEAKY, Ho, Wo))
+      return false;
   }
-  const int c8 = 8 * n;
-  if (!make_conv(P.aspp1, prefix + ".aspp.conv1.1", identity_perm(c8, c8), c8, 1, 1, 1, 1, ACT_RELU)) return false;
-  if (!make_conv(P.aspp2, prefix + ".aspp.conv2", identity_perm(c8, c8), c8, 1, 1, 1, 1, ACT_RELU)) return false;
+  const int c8 = 8 * n, h16 = H / 16, w16 = W / 16;
+  if (!make_conv(P.aspp1, prefix + ".aspp.conv1.1", identity_perm(c8, c8), c8, 1, 1, 1, 1, ACT_RELU, 1, w16))
+    return false;
+  if (!make_conv(P.aspp2, prefix + ".aspp.conv2", identity_perm(c8, c8), c8, 1, 1, 1, 1, ACT_RELU, h16, w16))
+    return false;
   const int dil[3][2] = {{4, 2}, {8, 4}, {12, 6}};   // lib/nets.py:10
   for (int i = 0; i < 3; ++i)
     if (!make_conv(P.aspp_d[i], prefix + ".aspp.conv" + std::to_string(i + 3), identity_perm(c8, c8), c8, 3, 1,
-                   dil[i][0], dil[i][1], ACT_RELU))
+                   dil[i][0], dil[i][1], ACT_RELU, h16, w16))
       return false;
-  if (!make_conv(P.bott, prefix + ".aspp.bottleneck", identity_perm(5 * c8, 5 * c8), 5 * c8, 1, 1, 1, 1, ACT_RELU))
+  if (!make_conv(P.bott, prefix + ".aspp.bottleneck", identity_perm(5 * c8, 5 * c8), 5 * c8, 1, 1, 1, 1, ACT_RELU,
+                 h16, w16))
     return false;
-  if (!make_conv(P.dec[0], prefix + ".dec4.conv1", identity_perm(14 * n, 14 * n), 14 * n, 3, 1, 1, 1, ACT_RELU))
+  if (!make_conv(P.dec[0], prefix + ".dec4.conv1", identity_perm(14 * n, 14 * n), 14 * n, 3, 1, 1, 1, ACT_RELU, H / 8,
+                 W / 8))
     return false;
-  if (!make_conv(P.dec[1], prefix + ".dec3.conv1", identity_perm(10 * n, 10 * n), 10 * n, 3, 1, 1, 1, ACT_RELU))
+  if (!make_conv(P.dec[1], prefix + ".dec3.conv1", identity_perm(10 * n, 10 * n), 10 * n, 3, 1, 1, 1, ACT_RELU, H / 4,
+                 W / 4))
     return false;
   P.dec[2].rows_wide = true;   // dec2's upsample is fused into the row kernel whenever 4n is a multiple of 32
-  if (!make_conv(P.dec[2], prefix + ".dec2.conv1", identity_perm(6 * n, 6 * n), 6 * n, 3, 1, 1, 1, ACT_RELU))
+  if (!make_conv(P.dec[2], prefix + ".dec2.conv1", identity_perm(6 * n, 6 * n), 6 * n, 3, 1, 1, 1, ACT_RELU, H / 2,
+                 W / 2))
     return false;
   {
     // dec1 input in the reference: cat[ up(cat[h (2n), lstm (1)]) , e1 (n) ]  (lib/nets.py:38-39, layers.py:52-56)
@@ -268,7 +275,7 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
     for (int i = 0; i < n; ++i) perm[(size_t)(P.e1_off + i)] = 2 * n + 1 + i;
     // (the 64-wide tile was measured on dec1 as well - one N tile instead of two for n = 64 - and is no faster there:
     //  with its single accumulator set the epilogue no longer overlaps the next tile's products)
-    if (!make_conv(P.dec[3], prefix + ".dec1.conv1", perm, c1, 3, 1, 1, 1, ACT_RELU)) return false;
+    if (!make_conv(P.dec[3], prefix + ".dec1.conv1", perm, c1, 3, 1, 1, 1, ACT_RELU, H, W)) return false;
   }
 
   // ---- LSTM module (lib/layers.py:110-122) ----
@@ -395,9 +402,11 @@ bool Engine::finalize() {
     return false;
   if (!build_basenet(nets_[4], "stg3_full_band_net", a1 + a2 + 2, p3, C3, nout, max_bin, W, nin_lstm, cfg_.nout_lstm))
     return false;
-  if (!make_conv(bridge1_, "stg1_low_band_net.1", identity_perm(nout / 2, nout / 2), nout / 2, 1, 1, 1, 1, ACT_RELU))
+  if (!make_conv(bridge1_, "stg1_low_band_net.1", identity_perm(nout / 2, nout / 2), nout / 2, 1, 1, 1, 1, ACT_RELU,
+                 Hb, W))
     return false;
-  if (!make_conv(bridge2_, "stg2_low_band_net.1", identity_perm(nout, nout), nout, 1, 1, 1, 1, ACT_RELU)) return false;
+  if (!make_conv(bridge2_, "stg2_low_band_net.1", identity_perm(nout, nout), nout, 1, 1, 1, 1, ACT_RELU, Hb, W))
+    return false;
   const HostTensor *ow, *aw;
   if (!need("out.weight", {2, nout, 1, 1}, &ow)) return false;
   if (!need("aux_out.weight", {2, 3 * nout / 4, 1, 1}, &aw)) return false;   // dead in forward, but a strict key
@@ -481,7 +490,7 @@ bool Engine::profile_dump(std::string& text) {
 bool Engine::run_conv(ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, const ActView* up_src,
                       const ActView* extra) {
   ++launches;
-  const bool use_tc = L.tc && cfg_.conv_mode == 0 && tc_supported(L, in, out);
+  const bool use_tc = L.tc != nullptr;
   if (!use_tc && cfg_.conv_mode == 0 && L.Cout >= 4 && !warned_simt_) {
     // loud, once per context: this geometry does not tile for the wgmma kernels (e.g. a cropsize whose feature-map
     // widths are not powers of two / multiples of 128) and runs on the fp32 CUDA-core kernel, an order of magnitude slower
@@ -521,7 +530,7 @@ bool Engine::run_conv_inner(ConvLayer& L, const ActView& in, const ActView& out,
 bool Engine::run_decoder(ConvLayer& L, const ActView& low, const Buffer& cat, int N, const ActView& out,
                          cudaStream_t s) {
   const ActView cat_all = cat.all(N);
-  if (cfg_.conv_mode == 0 && L.tc && tc_supported(L, cat_all, out) && tc_can_fuse_upsample(L, cat_all, out, low))
+  if (L.tc && L.tc->fuses_upsample(low.C))
     return run_conv(L, cat_all, out, s, &low);   // channels [0, low.C) of cat are produced inside the kernel
   if (cat.C < low.C + 1) {
     err = "internal: " + L.name + " was laid out for the fused upsample but the fused kernel is not available";
@@ -570,8 +579,7 @@ bool Engine::run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, 
   // output: the row kernel's epilogue accumulates it from the fp32 activations it is about to store.
   LstmPlan& Q = P.lstm;
   const ActView d2v = P.d2.view(N, 0, H / 2, 0, 2 * n);
-  const bool dot_fused = cfg_.conv_mode == 0 && P.dec[2].tc && tc_supported(P.dec[2], P.cat2.all(N), d2v) &&
-                         tc_rows_supported(P.dec[2], *P.dec[2].tc, P.cat2.all(N), d2v);
+  const bool dot_fused = P.dec[2].tc && P.dec[2].tc->kind == TC_ROWS;
   if (dot_fused) {
     if (!ck(cudaMemsetAsync(Q.l0, 0, sizeof(float) * (size_t)N * Q.bins * Q.T, s), "lstm conv clear")) return false;
     P.dec[2].dot_w = Q.conv_w;
@@ -616,17 +624,13 @@ bool Engine::run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, 
         return false;
     }
     const ActView h = P.d2.all(N);
-    if (!tc_can_fuse_upsample(P.dec[3], P.cat1.all(N), out, h)) {
-      err = "internal: " + P.prefix + ".dec1 was laid out for the fused upsample but the fused kernel is not available";
-      return false;
-    }
     return run_conv(P.dec[3], P.cat1.all(N), out, s, &h, P.lstm_own ? &lstm_full : nullptr);
   }
   // staged layout: dec1 on cat[up(h, lstm), e1] (lib/nets.py:39)
   const int upc = P.e1_off;   // channels of d2 that are upsampled: 2n conv channels + the LSTM channel group
   if (overlap) {
     if (!ck(cudaEventRecord(ev_lstm_join_, side), "lstm join")) return false;
-    if (cfg_.conv_mode == 0 && tc_can_fuse_upsample(P.dec[3], P.cat1.all(N), out, P.d2.all(N))) {
+    if (P.dec[3].tc && P.dec[3].tc->fuses_upsample(P.d2.C)) {
       // fused: the convolution reads d2 (incl. the LSTM channel) itself, so it simply waits for the side stream
       if (!ck(cudaStreamWaitEvent(s, ev_lstm_join_, 0), "lstm join")) return false;
       return run_decoder(P.dec[3], P.d2.all(N), P.cat1, N, out, s);
@@ -1026,7 +1030,7 @@ bool Engine::debug_conv(const float* x_nchw, int N, int Cin, int H, int W, const
   Buffer bout = make_buffer(N, Ho, Wo, round_up(Cout, 8));
   ConvLayer L;
   L.name = "debug_conv";
-  L.rows_wide = g_tc_debug[2] == 1;   // vr_debug_set(2, 1): exercise the 64-wide row tile on a plain convolution
+  L.rows_wide = g_debug.rows_wide == 1;   // vr_debug_set(2, 1): exercise the 64-wide row tile on a plain convolution
   L.Cin = Cin; L.CinPad = cin_pad; L.Cout = Cout; L.CoutPad = round_up(Cout, 8);
   L.k = k; L.stride = stride; L.dil_h = dil_h; L.dil_w = dil_w; L.act = act;
   const int taps = k * k;
@@ -1050,17 +1054,15 @@ bool Engine::debug_conv(const float* x_nchw, int N, int Cin, int H, int W, const
     cudaMemcpy(L.bias, L.bias_host.data(), L.bias_host.size() * sizeof(float), cudaMemcpyHostToDevice);
     ok = ck(launch_nchw_to_act(x_nchw, Cin, bin.all(N), s), "nchw_to_act");
   }
-  const int saved_mode = cfg_.conv_mode;
   if (ok && use_tc) {
-    ok = tc_prepare(L, err, allocs_);
-    if (ok && !(L.tc && tc_supported(L, bin.all(N), bout.view(N, 0, Ho, 0, Cout)))) {
+    ok = tc_prepare(L, Ho, Wo, err, allocs_);
+    if (ok && !L.tc) {
       err = "debug_conv: geometry not supported by the wgmma kernel";
       ok = false;
     }
-    cfg_.conv_mode = 0;
-  } else {
-    cfg_.conv_mode = 1;
   }
+  const int saved_mode = cfg_.conv_mode;
+  cfg_.conv_mode = use_tc ? 0 : 1;   // a requested CUDA-core run is not warned about
   if (ok) ok = run_conv(L, bin.all(N), bout.view(N, 0, Ho, 0, Cout), s);
   cfg_.conv_mode = saved_mode;
   if (ok) ok = ck(launch_act_to_nchw(bout.view(N, 0, Ho, 0, Cout), Cout, y_nchw, s), "act_to_nchw");
@@ -1113,18 +1115,17 @@ bool Engine::debug_decoder(const float* low_nchw, int N, int Cl, int h, int w, c
     ok = ck(launch_nchw_to_act(low_nchw, Cl, blow.all(N), s), "nchw_to_act low") &&
          ck(launch_nchw_to_act(skip_nchw, Cs, bcat.view(N, 0, H, cl_pad, cin_pad - cl_pad), s), "nchw_to_act skip");
   }
-  if (ok) ok = tc_prepare(L, err, allocs_);
-  const int saved_mode = cfg_.conv_mode, saved_fuse = g_tc_debug[5];
-  cfg_.conv_mode = 0;
-  g_tc_debug[5] = fused ? 1 : 0;
-  if (ok && fused && !tc_can_fuse_upsample(L, bcat.all(N), bout.view(N, 0, H, 0, Cout), blow.all(N))) {
+  if (ok) ok = tc_prepare(L, H, W, err, allocs_);
+  if (ok && fused && !(L.tc && L.tc->fuses_upsample(blow.C))) {
     err = "debug_decoder: geometry not supported by the fused row kernel";
     ok = false;
   }
-  if (ok) ok = run_decoder(L, blow.all(N), bcat, N, bout.view(N, 0, H, 0, Cout), s);
-  cfg_.conv_mode = saved_mode;
-  g_tc_debug[5] = saved_fuse;
-  if (ok) ok = ck(launch_act_to_nchw(bout.view(N, 0, H, 0, Cout), Cout, y_nchw, s), "act_to_nchw");
+  const ActView out = bout.view(N, 0, H, 0, Cout);
+  if (ok && fused) ok = run_decoder(L, blow.all(N), bcat, N, out, s);
+  if (ok && !fused)
+    ok = ck(launch_upsample2x(blow.all(N), bcat.view(N, 0, H, 0, cl_pad), s), "debug_decoder upsample") &&
+         run_conv(L, bcat.all(N), out, s);
+  if (ok) ok = ck(launch_act_to_nchw(out, Cout, y_nchw, s), "act_to_nchw");
   if (ok) ok = ck(cudaStreamSynchronize(s), "debug_decoder sync");
   L.tc.reset();
   for (void* p : allocs_) cudaFree(p);

@@ -54,7 +54,7 @@ struct ConvLayer {
   // pre-zeroed plane dot_out[n][h][w] (the LSTM branch's 1x1 input convolution fused into dec2)
   const float* dot_w = nullptr;
   float* dot_out = nullptr;
-  std::shared_ptr<TcConv> tc;    // null -> CUDA-core kernel
+  std::shared_ptr<TcConv> tc;    // the tensor-core kernel and its packed weights; null -> CUDA-core kernel
 };
 
 struct LstmPlan {
@@ -82,8 +82,8 @@ struct BaseNetPlan {
   // up-sampled by a small kernel from lstm.y (half resolution, fp32 plane) into a 16-channel group at full
   // resolution: channels [n, n+16) of cat1 = [e1 n | up(lstm) 1 + 15 zeros] when e1 leaves room in its chunk (n = 16),
   // else an 8-channel group in the buffer lstm_up of its own (n = 32, 64: cat1 = [e1 n] stays dense for enc2.conv1, and
-  // the row kernel reads the group as its last chunk through a second tensor map whose box TMA zero-fills).  Otherwise (CUDA-core validation mode, nets whose
-  // 2n is not a multiple of 32): cat1 = [up(h) 2n | up(lstm) 1 + 15 zeros | e1 n | pad], d2 = [h 2n | lstm 1 | zeros].
+  // the row kernel reads the group as its last chunk through a second tensor map whose box TMA zero-fills).  Otherwise (dec1 not
+  // on the row kernel, nets whose 2n is not a multiple of 32): cat1 = [up(h) 2n | up(lstm) 1 + 15 zeros | e1 n | pad], d2 = [h 2n | lstm 1 | zeros].
   bool skip_only = false;
   int e1_coff = 0;          // channel offset of e1 inside cat1
   int lstm_coff = 0;        // skip_only: channel offset of the up-sampled LSTM channel inside cat1 (or 0 in lstm_up)
@@ -212,8 +212,9 @@ class Engine {
   void* dalloc(size_t bytes);
   Buffer make_buffer(int N, int H, int W, int C, int pad_w = 0);
   bool need(const std::string& key, std::initializer_list<int64_t> shape, const HostTensor** out);
+  // H x W: the layer's output maps, from which tc_prepare chooses its kernel
   bool make_conv(ConvLayer& L, const std::string& prefix, const std::vector<int>& perm, int cin_pad, int k, int stride,
-                 int dh, int dw, int act);
+                 int dh, int dw, int act, int H, int W);
   bool build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, const std::vector<int>& in_perm, int cin_pad,
                      int n, int H, int W, int nin_lstm, int nout_lstm);
   bool run_conv(ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, const ActView* up_src = nullptr,
@@ -230,11 +231,9 @@ class Engine {
   bool ck(cudaError_t e, const char* what);
 };
 
-// conv_tc.cu
-bool tc_supported(const ConvLayer& L, const ActView& in, const ActView& out);
-bool tc_prepare(ConvLayer& L, std::string& err, std::vector<void*>& allocs);
+// conv_tc.cu: plans L.tc for output maps of H x W (left null when the layer stays on the CUDA-core kernel)
+bool tc_prepare(ConvLayer& L, int H, int W, std::string& err, std::vector<void*>& allocs);
 cudaError_t tc_launch(ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, std::string& err,
                       const ActView* up_src = nullptr, const ActView* extra = nullptr);
-bool tc_can_fuse_upsample(const ConvLayer& L, const ActView& in, const ActView& out, const ActView& up_src);
 
 }  // namespace vr

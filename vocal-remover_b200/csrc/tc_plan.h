@@ -1,4 +1,7 @@
-// Host-side plan of one convolution layer for the wgmma kernels (conv_tc.cu, conv_tc_rows.cu).
+// Host-side plan of one convolution layer for the wgmma kernels (conv_tc.cu, conv_tc_rows.cu, conv_tc_halo.cu).
+// tc_prepare (conv_tc.cu) chooses the kernel of a layer once, from its fixed geometry (k, stride, dilation, channels and
+// the H x W of its output maps), and packs the weights once, in that kernel's layout.  The launches read the plan; only
+// the halo kernel's MB, which depends on the batch size, is chosen per launch.
 #pragma once
 #include <cuda.h>
 
@@ -9,56 +12,45 @@
 
 namespace vr {
 
-typedef std::tuple<const void*, const void*, int, int, int, int> ViewKey;
-
-struct TcRowsPlan {   // row-streaming variant: 3x3, stride 1, dilation 1, W % 128 == 0 (conv_tc_rows.cu)
-  bool ok = false;
-  int KB = 32, CinPadR = 0, chunks = 0, BN = 0, n_tiles = 0;
-  unsigned long long kmask = ~0ull;   // bit g: input channels [8g, 8g+8) carry a non-zero weight
-  bf16* w_planes = nullptr;   // [2][n_tiles*BN][9*CinPadR]
-  float* bias = nullptr;      // [n_tiles*BN]
-  CUtensorMap map_b;
-  std::map<ViewKey, CUtensorMap> map_a;
-  std::map<ViewKey, CUtensorMap> map_l;   // second activation map (the chunk read from its own buffer)
+enum TcKind {
+  TC_NONE,      // CUDA-core kernel (conv_simt.cu)
+  TC_GENERIC,   // one shifted pixel box per (tap, channel chunk) (conv_tc.cu)
+  TC_ROWS,      // row streaming: 3x3, stride 1, dilation 1, W % 128 == 0, H % 8 == 0 (conv_tc_rows.cu)
+  TC_HALO,      // halo tile: 3x3, stride 1, dilation 1, W in {16, 32, 64} (conv_tc_halo.cu)
 };
 
-struct TcHaloPlan {   // halo-tile variant: 3x3, stride 1, dilation 1, W in {16, 32, 64} (conv_tc_halo.cu)
-  bool ok = false;
-  int CinPadH = 0, chunks = 0;   // BN, n_tiles and the bias are the generic plan's
-  unsigned long long kmask = ~0ull;   // bit g: input channels [8g, 8g+8) carry a non-zero weight
-  bf16* w_planes = nullptr;   // [2][n_tiles*BN][9*CinPadH]
-  CUtensorMap map_b;
-  std::map<ViewKey, CUtensorMap> map_a[2];   // per MB (the halo box height depends on it)
-};
+// activation view (hi, lo, N, H, W, C) and TMA box (W, H, N extents)
+typedef std::tuple<const void*, const void*, int, int, int, int, int, int, int> ViewKey;
 
 struct TcConv {
-  int CinPadTC = 0, KB = 0, cchunks = 0, SUBS = 0, taps = 0, Ktot = 0, CoutPadN = 0, BN = 0, n_tiles = 0;
-  bf16* w_planes = nullptr;   // [2][CoutPadN][Ktot]
-  float* bias = nullptr;      // [n_tiles*BN]
+  TcKind kind = TC_NONE;
+  int H = 0, W = 0;   // output maps the kernel was chosen for
+  // KB: channels per chunk (generic: 64 / 32 / 16, rows and halo: 32); CinPad: input channels padded to whole chunks
+  int KB = 0, CinPad = 0, chunks = 0, BN = 0, n_tiles = 0;
+  unsigned long long kmask = ~0ull;   // bit g: input channels [8g, 8g+8) carry a non-zero weight (rows and halo)
+  // weights, hi plane then lo plane: generic / halo [2][n_tiles*BN][taps*CinPad] (tap-major K), rows
+  // [2][n_tiles*3*BN][3*CinPad] (the three kh taps of an N tile stacked along N, kw-major K)
+  bf16* w_planes = nullptr;
+  float* bias = nullptr;   // [n_tiles*BN]
   CUtensorMap map_b;
   std::map<ViewKey, CUtensorMap> map_a;
-  TcRowsPlan rows;
-  TcHaloPlan halo;
+  // the row kernel can produce the leading up_C channels of its input as the x2 upsample of a half-resolution tensor
+  bool fuses_upsample(int up_C) const { return kind == TC_ROWS && up_C % 32 == 0 && up_C <= CinPad; }
 };
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn tc_encode_fn();
-uint16_t tc_f2bf(float f);
-float tc_bf2f(uint16_t h);
+TcKind tc_choose(const ConvLayer& L, int H, int W);
+// tensor map of an activation view: both split-bf16 planes in one box of {tc.KB, bw, bh, bn, 2} elements, element
+// stride es along W and H; cached in the plan.  nullptr (err set) if TMA cannot read the view.
+const CUtensorMap* tc_activation_map(TcConv& tc, const ActView& v, int bw, int bh, int bn, int es, std::string& err,
+                                     const std::string& name);
 
 // conv_tc_rows.cu
-bool tc_rows_prepare(ConvLayer& L, TcConv& tc, std::string& err, std::vector<void*>& allocs);
-bool tc_rows_supported(const ConvLayer& L, const TcConv& tc, const ActView& in, const ActView& out);
 cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const ActView& out, cudaStream_t s,
-                           std::string& err, const ActView* up_src = nullptr, const ActView* extra = nullptr);
+                           std::string& err, const ActView* up_src, const ActView* extra);
 void tc_rows_set_attributes(int max_smem);
 int tc_rows_read_trace(unsigned long long* out, long long capacity);
 
 // conv_tc_halo.cu
-bool tc_halo_prepare(ConvLayer& L, TcConv& tc, std::string& err, std::vector<void*>& allocs);
-bool tc_halo_supported(const ConvLayer& L, const TcConv& tc, const ActView& in, const ActView& out);
 cudaError_t tc_halo_launch(ConvLayer& L, TcConv& tc, const ActView& in, const ActView& out, cudaStream_t s,
                            std::string& err);
 void tc_halo_set_attributes(int max_smem);
@@ -72,11 +64,14 @@ struct TcDevice {
 };
 const TcDevice& tc_device();
 
-// validation knobs (vr_debug_set): [0] = 1: CTA 0 of the row kernel records a timeline (vr_debug_trace), [2] = 1: vr_debug_conv uses the 64-wide row tile, [1] = 1 disables the row kernel, [4] = k: k of the row slots feed the interpolation
-// warps (default half), [5] = 1 (default): decoder upsample fused into the row kernel, [6] = 1 (default): the row
-// and halo kernels skip channel groups whose weights are all zero, [3] = 1: the layers of the halo kernel go to the
-// per-tap kernel instead, [3] = 2 / 3: the halo kernel uses MB = 1 / 2 (where the height tiles) for every layer;
-// the other entries are unused
-extern int g_tc_debug[8];
+// validation switches, set with vr_debug_set(key, value)
+struct TcDebug {
+  int trace = 0;       // key 0 = 1: CTA 0 of the row kernel records a timeline (-DVR_TRACE builds, vr_debug_trace)
+  int rows_wide = 0;   // key 2 = 1: vr_debug_conv uses the row kernel's 64-wide tile
+  int halo = 0;        // key 3 = 1: layers prepared from then on go to the generic kernel instead of the halo kernel;
+                       // 2 / 3: the halo kernel uses MB = 1 / 2 (where the height tiles) in every launch
+  int kskip = 1;       // key 6 = 1 (default): the row and halo kernels skip channel groups whose weights are all zero
+};
+extern TcDebug g_debug;
 
 }  // namespace vr

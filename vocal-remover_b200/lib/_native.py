@@ -80,14 +80,8 @@ def load_library():
         fn.restype = res
         fn.argtypes = args
     # validation knobs of the tensor-core kernels (see vr_debug_set in include/vr_b200.h)
-    if os.environ.get('VR_FUSE_UP'):
-        lib.vr_debug_set(5, int(os.environ['VR_FUSE_UP']))
     if os.environ.get('VR_KSKIP'):
         lib.vr_debug_set(6, int(os.environ['VR_KSKIP']))
-    if os.environ.get('VR_USLOTS'):
-        lib.vr_debug_set(4, int(os.environ['VR_USLOTS']))
-    if os.environ.get('VR_NO_ROWS'):
-        lib.vr_debug_set(1, int(os.environ['VR_NO_ROWS']))
     _lib = lib
     return lib
 
