@@ -176,9 +176,12 @@ VR_API int64_t vr_launch_count(const vr_ctx* ctx);
  * out[0..2] = tensor-core conv {ms, algorithmic FLOPs, launches}, out[3..5] = CUDA-core conv likewise.    */
 VR_API int vr_profile_enable(vr_ctx* ctx, int32_t on);
 VR_API int vr_profile_read(vr_ctx* ctx, double* out6);
-/* Per-launch detail of the same records as text, one line per convolution launch in launch order:
- * "<state_dict prefix of the layer>[+up] N Hout Wout tensor_core(0/1) ms gflop".  Writes at most cap bytes
- * (NUL-terminated) and stores the size needed in *needed (either may be NULL / 0 to query).                */
+/* Per-launch detail as text, one line per timed launch in launch order, convolutions and every other kernel of the
+ * path: "<name> N Hout Wout kind ms gflop".  A convolution is named by the state_dict prefix of its layer (+ "+up"
+ * when it produces its upsampled input itself) and has kind 1 (tensor cores) or 0 (CUDA cores); any other kernel has
+ * kind 2 and gflop 0, and one line may time a group of kernels launched together (e.g. the two of the lexmax
+ * normaliser).  Writes at most cap bytes (NUL-terminated) and stores the size needed in *needed (either may be
+ * NULL / 0 to query).                                                                                       */
 VR_API int vr_profile_dump(vr_ctx* ctx, char* text, int64_t cap, int64_t* needed);
 
 /* ---- validation hooks used by tests/ (not part of the reference surface) ---------------------------- */

@@ -139,18 +139,12 @@ int vr_apply_mask(vr_ctx* ctx, const void* spec, const float* mask, int64_t T, v
 
 int vr_mask_frame_min(vr_ctx* ctx, const float* mask, int64_t T, float* frame_min, void* stream) {
   CHECK_CTX(ctx);
-  cudaSetDevice(ctx->eng->cfg().device);
-  ++ctx->eng->launches;
-  cudaError_t e = vr::launch_mask_frame_min(mask, 2 * ctx->eng->bins(), T, frame_min, (cudaStream_t)stream);
-  return e == cudaSuccess ? 0 : fail(ctx, std::string("vr_mask_frame_min: ") + cudaGetErrorString(e));
+  return done(ctx, ctx->eng->mask_frame_min(mask, T, frame_min, (cudaStream_t)stream));
 }
 
 int vr_mask_apply_weight(vr_ctx* ctx, float* mask, int64_t T, const float* weight, void* stream) {
   CHECK_CTX(ctx);
-  cudaSetDevice(ctx->eng->cfg().device);
-  ++ctx->eng->launches;
-  cudaError_t e = vr::launch_mask_apply_weight(mask, 2 * ctx->eng->bins(), T, weight, (cudaStream_t)stream);
-  return e == cudaSuccess ? 0 : fail(ctx, std::string("vr_mask_apply_weight: ") + cudaGetErrorString(e));
+  return done(ctx, ctx->eng->mask_apply_weight(mask, T, weight, (cudaStream_t)stream));
 }
 
 int vr_apply_mask_istft(vr_ctx* ctx, const void* spec, const float* mask, int64_t T, float* wave_inst,

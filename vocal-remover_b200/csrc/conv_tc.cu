@@ -355,7 +355,7 @@ static bool encode_weight_map(TcConv& tc, int rows, int K, int box_rows, std::st
   cuuint64_t strides[2] = {(cuuint64_t)K * 2, (cuuint64_t)rows * K * 2};
   cuuint32_t box[3] = {(cuuint32_t)tc.KB, (cuuint32_t)box_rows, 2};
   cuuint32_t es[3] = {1, 1, 1};
-  CUresult r = tc_encode_fn()(&tc.map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, tc.w_planes, dims, strides, box, es,
+  CUresult r = tc_encode_fn()(&tc.map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, tc.w_planes.get(), dims, strides, box, es,
                               CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(tc.KB), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -391,7 +391,7 @@ const CUtensorMap* tc_activation_map(TcConv& tc, const ActView& v, int bw, int b
   return &tc.map_a.emplace(key, m).first->second;
 }
 
-bool tc_prepare(ConvLayer& L, int H, int W, std::string& err, std::vector<void*>& allocs) {
+bool tc_prepare(ConvLayer& L, int H, int W, std::string& err) {
   const TcKind kind = tc_choose(L, H, W);
   if (kind == TC_NONE) return true;   // stays on the CUDA-core kernel
   if (!tc_encode_fn()) {
@@ -427,19 +427,14 @@ bool tc_prepare(ConvLayer& L, int H, int W, std::string& err, std::vector<void*>
   }
   std::vector<float> bias((size_t)rows, 0.f);
   for (int co = 0; co < L.Cout; ++co) bias[(size_t)co] = L.bias_host[(size_t)co];
-  void* dw = nullptr;
-  void* db = nullptr;
-  if (cudaMalloc(&dw, planes.size() * 2) != cudaSuccess || cudaMalloc(&db, bias.size() * 4) != cudaSuccess) {
+  if (tc->w_planes.alloc(planes.size() * 2) != cudaSuccess || tc->bias.alloc(bias.size() * 4) != cudaSuccess) {
     err = "cudaMalloc failed while packing tensor-core weights for " + L.name;
     return false;
   }
-  allocs.push_back(dw);
-  allocs.push_back(db);
-  cudaMemcpy(dw, planes.data(), planes.size() * 2, cudaMemcpyHostToDevice);
-  cudaMemcpy(db, bias.data(), bias.size() * 4, cudaMemcpyHostToDevice);
-  tc->w_planes = (bf16*)dw;
-  tc->bias = (float*)db;
-  if (!encode_weight_map(*tc, brows, K, kind == TC_ROWS ? 3 * BN : BN, err, L.name)) return false;
+  if (!upload(tc->w_planes.get(), planes.data(), planes.size() * 2, err) ||
+      !upload(tc->bias.get(), bias.data(), bias.size() * 4, err) ||
+      !encode_weight_map(*tc, brows, K, kind == TC_ROWS ? 3 * BN : BN, err, L.name))
+    return false;
   L.tc = tc;
   return true;
 }
@@ -487,7 +482,7 @@ cudaError_t tc_launch(ConvLayer& L, const ActView& in, const ActView& out, cudaS
   }
   p.out_hi = out.hi; p.out_lo = out.lo;
   p.osn = out.sn; p.osh = out.sh; p.osw = out.sw;
-  p.bias = tc.bias;
+  p.bias = tc.bias.get();
   const int total_tiles = p.m_tiles * p.n_tiles;
   const int grid = total_tiles < dv.num_sms ? total_tiles : dv.num_sms;
 #define VR_TC_LAUNCH(KB_, BN_)                                                       \

@@ -291,7 +291,7 @@ cudaError_t tc_halo_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   p.kmask = g_debug.kskip == 1 ? tc.kmask : ~0ull;
   p.out_hi = out.hi; p.out_lo = out.lo;
   p.osn = out.sn; p.osh = out.sh; p.osw = out.sw;
-  p.bias = tc.bias;
+  p.bias = tc.bias.get();
   // the halo tile, both planes
   const CUtensorMap* map_a = tc_activation_map(tc, in, p.Wb, p.Ht + 2, 1, 1, err, L.name);
   if (!map_a) return cudaErrorInvalidValue;

@@ -567,7 +567,7 @@ cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   p.chunks = tc.chunks; p.CinPadR = tc.CinPad; p.Cout = L.Cout; p.act = L.act;
   p.out_hi = out.hi; p.out_lo = out.lo;
   p.osn = out.sn; p.osh = out.sh; p.osw = out.sw;
-  p.bias = tc.bias;
+  p.bias = tc.bias.get();
   p.up_chunks = 0; p.xH = p.xW = 0;
   p.x_hi = p.x_lo = nullptr; p.xsn = p.xsh = 0; p.xsw = 0;
   p.trace = g_debug.trace == 1 ? 1 : 0;

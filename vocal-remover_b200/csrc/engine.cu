@@ -19,26 +19,35 @@ bool Engine::ck(cudaError_t e, const char* what) {
   return false;
 }
 
-void* Engine::dalloc(size_t bytes) {
-  void* p = nullptr;
-  if (bytes == 0) bytes = 16;
-  cudaError_t e = cudaMalloc(&p, bytes);
-  if (e != cudaSuccess) {
-    err = std::string("cudaMalloc(") + std::to_string(bytes) + "): " + cudaGetErrorString(e);
-    return nullptr;
-  }
-  cudaMemset(p, 0, bytes);   // pad channels must be finite zeros forever (zero weights multiply them)
-  allocs_.push_back(p);
-  return p;
+bool upload(void* dst, const void* src, size_t bytes, std::string& err) {
+  const cudaError_t e = cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) return true;
+  err = std::string("cudaMemcpy(") + std::to_string(bytes) + ", host to device): " + cudaGetErrorString(e);
+  return false;
 }
 
-Buffer Engine::make_buffer(int N, int H, int W, int C, int pad_w) {
+void* Engine::dalloc(Arena& arena, size_t bytes, const void* host) {
+  const size_t n = bytes == 0 ? 16 : bytes;
+  DevPtr<void> m;
+  const cudaError_t e = m.alloc(n);
+  if (e != cudaSuccess) {
+    err = std::string("cudaMalloc(") + std::to_string(n) + "): " + cudaGetErrorString(e);
+    return nullptr;
+  }
+  // pad channels must be finite zeros forever (zero weights multiply them)
+  if (!ck(cudaMemset(m.get(), 0, n), "cudaMemset")) return nullptr;
+  if (host && !upload(m.get(), host, bytes, err)) return nullptr;
+  arena.push_back(std::move(m));
+  return arena.back().get();
+}
+
+Buffer Engine::make_buffer(Arena& arena, int N, int H, int W, int C, int pad_w) {
   Buffer b;
   b.N = N; b.H = H; b.W = W; b.C = C;
   b.Wp = W + pad_w;
   size_t plane = (size_t)N * H * b.Wp * C * sizeof(bf16);
   plane = (plane + 1023) / 1024 * 1024;
-  char* p = (char*)dalloc(2 * plane);
+  char* p = (char*)dalloc(arena, 2 * plane);
   if (p) {
     b.hi = (bf16*)p;
     b.lo = (bf16*)(p + plane);
@@ -59,13 +68,11 @@ Engine::Engine(const Config& cfg) : cfg_(cfg) {
     tw[q] = make_float2((float)cos(a), (float)sin(a));
   }
   for (int n = 0; n < NF; ++n) win[n] = (float)(0.5 - 0.5 * cos(2.0 * M_PI * (double)n / (double)NF));
-  twiddle_ = (float2*)dalloc(sizeof(float2) * tw.size());
-  window_ = (float*)dalloc(sizeof(float) * win.size());
-  ws_norm_ = (float*)dalloc(sizeof(float) * 4);
-  ws_lex_ = (unsigned long long*)dalloc(sizeof(unsigned long long));
+  twiddle_ = (float2*)dalloc(arena_, sizeof(float2) * tw.size(), tw.data());
+  window_ = (float*)dalloc(arena_, sizeof(float) * win.size(), win.data());
+  ws_norm_ = (float*)dalloc(arena_, sizeof(float) * 4);
+  ws_lex_ = (unsigned long long*)dalloc(arena_, sizeof(unsigned long long));
   if (!twiddle_ || !window_ || !ws_norm_ || !ws_lex_) return;
-  cudaMemcpy(twiddle_, tw.data(), sizeof(float2) * tw.size(), cudaMemcpyHostToDevice);
-  cudaMemcpy(window_, win.data(), sizeof(float) * win.size(), cudaMemcpyHostToDevice);
   cudaStreamCreateWithFlags(&s_hi_, cudaStreamNonBlocking);
   cudaStreamCreateWithFlags(&s_copy_, cudaStreamNonBlocking);
   cudaEventCreateWithFlags(&ev_span_, cudaEventDisableTiming);
@@ -75,15 +82,9 @@ Engine::Engine(const Config& cfg) : cfg_(cfg) {
   cudaEventCreateWithFlags(&ev_lstm_join_, cudaEventDisableTiming);
 }
 
+// the members that own device memory are destroyed after this body, with the context's device current
 Engine::~Engine() {
   cudaSetDevice(cfg_.device);
-  for (void* p : allocs_) cudaFree(p);
-  if (ws_spec_) cudaFree(ws_spec_);
-  if (ws_mask_) cudaFree(ws_mask_);
-  if (ws_frames_) cudaFree(ws_frames_);
-  if (ws_wave_) cudaFree(ws_wave_);
-  if (ws_img_) cudaFree(ws_img_);
-  if (ws_val_) cudaFree(ws_val_);
   profile_enable(false);
   if (s_hi_) cudaStreamDestroy(s_hi_);
   if (s_copy_) cudaStreamDestroy(s_copy_);
@@ -162,27 +163,35 @@ bool Engine::make_conv(ConvLayer& L, const std::string& prefix, const std::vecto
       !need(prefix + ".conv.1.running_mean", {Cout}, &m) || !need(prefix + ".conv.1.running_var", {Cout}, &v) ||
       !need(prefix + ".conv.1.num_batches_tracked", {}, &cnt))
     return false;
-  L.Cin = Cin; L.CinPad = cin_pad; L.Cout = Cout; L.CoutPad = round_up(Cout, 8);
-  const int taps = k * k;
+  std::vector<double> scale((size_t)Cout);
+  std::vector<float> bias((size_t)Cout);
+  for (int co = 0; co < Cout; ++co) {
+    scale[(size_t)co] = (double)g->data[co] / sqrt((double)v->data[co] + kBnEps);
+    bias[(size_t)co] = (float)((double)b->data[co] - (double)m->data[co] * scale[(size_t)co]);
+  }
+  if (!pack_conv(L, arena_, w.data.data(), Cout, Cin, scale.data(), bias.data(), perm)) return false;
+  return cfg_.conv_mode != 0 || tc_prepare(L, H, W, err);
+}
+
+bool Engine::pack_conv(ConvLayer& L, Arena& arena, const float* w, int Cout, int Cin, const double* scale,
+                       const float* bias, const std::vector<int>& perm) {
+  L.Cin = Cin; L.CinPad = (int)perm.size(); L.Cout = Cout; L.CoutPad = round_up(Cout, 8);
+  const int taps = L.k * L.k;
   L.w_host.assign((size_t)taps * L.CinPad * L.CoutPad, 0.f);
   L.bias_host.assign((size_t)L.CoutPad, 0.f);
   for (int co = 0; co < Cout; ++co) {
-    const double scale = (double)g->data[co] / sqrt((double)v->data[co] + kBnEps);
-    L.bias_host[co] = (float)((double)b->data[co] - (double)m->data[co] * scale);
-    for (int pc = 0; pc < cin_pad; ++pc) {
-      const int ci = perm[pc];
+    L.bias_host[(size_t)co] = bias[co];
+    for (int pc = 0; pc < L.CinPad; ++pc) {
+      const int ci = perm[(size_t)pc];
       if (ci < 0) continue;
       for (int t = 0; t < taps; ++t)
         L.w_host[((size_t)t * L.CinPad + pc) * L.CoutPad + co] =
-            (float)((double)w.data[((size_t)co * Cin + ci) * taps + t] * scale);
+            (float)((double)w[((size_t)co * Cin + ci) * taps + t] * scale[co]);
     }
   }
-  L.w = (float*)dalloc(L.w_host.size() * sizeof(float));
-  L.bias = (float*)dalloc(L.bias_host.size() * sizeof(float));
-  if (!L.w || !L.bias) return false;
-  cudaMemcpy(L.w, L.w_host.data(), L.w_host.size() * sizeof(float), cudaMemcpyHostToDevice);
-  cudaMemcpy(L.bias, L.bias_host.data(), L.bias_host.size() * sizeof(float), cudaMemcpyHostToDevice);
-  return cfg_.conv_mode != 0 || tc_prepare(L, H, W, err, allocs_);
+  L.w = (float*)dalloc(arena, L.w_host.size() * sizeof(float), L.w_host.data());
+  L.bias = (float*)dalloc(arena, L.bias_host.size() * sizeof(float), L.bias_host.data());
+  return L.w && L.bias;
 }
 
 static std::vector<int> identity_perm(int c, int pad) {
@@ -213,23 +222,24 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
   P.e1_off = P.skip_only ? 2 * n : 2 * n + lg;      // position of e1 in dec1's reduction (weight) order
   P.e1_coff = P.skip_only ? 0 : P.e1_off;           // position of e1 in the cat1 buffer
   P.lstm_coff = !P.skip_only ? 2 * n : P.lstm_own ? 0 : n;
-  P.cat1 = make_buffer(Nb, H, W, !P.skip_only ? c1 : P.lstm_own ? n : round_up(n + lg, 32));
-  if (P.lstm_own) P.lstm_up = make_buffer(Nb, H, W, 8);   // 8-channel group: the row kernel's TMA box zero-fills the rest
-  P.t2 = make_buffer(Nb, H / 2, W / 2, 2 * n);
-  P.cat2 = make_buffer(Nb, H / 2, W / 2, 6 * n);
-  P.t3 = make_buffer(Nb, H / 4, W / 4, 4 * n);
-  P.cat3 = make_buffer(Nb, H / 4, W / 4, 10 * n);
-  P.t4 = make_buffer(Nb, H / 8, W / 8, 6 * n);
-  P.cat4 = make_buffer(Nb, H / 8, W / 8, 14 * n);
-  P.t5 = make_buffer(Nb, H / 16, W / 16, 8 * n);
-  P.e5 = make_buffer(Nb, H / 16, W / 16, 8 * n);
-  P.pool = make_buffer(Nb, 1, W / 16, 8 * n);
-  P.f1 = make_buffer(Nb, 1, W / 16, 8 * n);
-  P.acat = make_buffer(Nb, H / 16, W / 16, 40 * n);
-  P.ao = make_buffer(Nb, H / 16, W / 16, 8 * n);
-  P.d4 = make_buffer(Nb, H / 8, W / 8, 6 * n);
-  P.d3 = make_buffer(Nb, H / 4, W / 4, 4 * n);
-  P.d2 = make_buffer(Nb, H / 2, W / 2, P.skip_only ? 2 * n : 2 * n + lg);
+  P.cat1 = make_buffer(arena_, Nb, H, W, !P.skip_only ? c1 : P.lstm_own ? n : round_up(n + lg, 32));
+  // 8-channel group: the row kernel's TMA box zero-fills the rest
+  if (P.lstm_own) P.lstm_up = make_buffer(arena_, Nb, H, W, 8);
+  P.t2 = make_buffer(arena_, Nb, H / 2, W / 2, 2 * n);
+  P.cat2 = make_buffer(arena_, Nb, H / 2, W / 2, 6 * n);
+  P.t3 = make_buffer(arena_, Nb, H / 4, W / 4, 4 * n);
+  P.cat3 = make_buffer(arena_, Nb, H / 4, W / 4, 10 * n);
+  P.t4 = make_buffer(arena_, Nb, H / 8, W / 8, 6 * n);
+  P.cat4 = make_buffer(arena_, Nb, H / 8, W / 8, 14 * n);
+  P.t5 = make_buffer(arena_, Nb, H / 16, W / 16, 8 * n);
+  P.e5 = make_buffer(arena_, Nb, H / 16, W / 16, 8 * n);
+  P.pool = make_buffer(arena_, Nb, 1, W / 16, 8 * n);
+  P.f1 = make_buffer(arena_, Nb, 1, W / 16, 8 * n);
+  P.acat = make_buffer(arena_, Nb, H / 16, W / 16, 40 * n);
+  P.ao = make_buffer(arena_, Nb, H / 16, W / 16, 8 * n);
+  P.d4 = make_buffer(arena_, Nb, H / 8, W / 8, 6 * n);
+  P.d3 = make_buffer(arena_, Nb, H / 4, W / 4, 4 * n);
+  P.d2 = make_buffer(arena_, Nb, H / 2, W / 2, P.skip_only ? 2 * n : 2 * n + lg);
   if (!P.d2.hi || !P.cat1.hi) return false;
 
   if (!make_conv(P.enc1, prefix + ".enc1", in_perm, cin_pad, 3, 1, 1, 1, ACT_RELU, H, W)) return false;
@@ -296,9 +306,8 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
     std::vector<float> w((size_t)Q.C);
     for (int c = 0; c < Q.C; ++c) w[(size_t)c] = (float)((double)cw->data[(size_t)c] * scale);
     Q.conv_bias = (float)((double)b->data[0] - (double)m->data[0] * scale);
-    Q.conv_w = (float*)dalloc(sizeof(float) * w.size());
+    Q.conv_w = (float*)dalloc(arena_, sizeof(float) * w.size(), w.data());
     if (!Q.conv_w) return false;
-    cudaMemcpy(Q.conv_w, w.data(), sizeof(float) * w.size(), cudaMemcpyHostToDevice);
   }
   {
     const int H4 = 4 * Q.hid;
@@ -314,13 +323,10 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
       memcpy(&whh[(size_t)d * H4 * Q.hid], h->data.data(), sizeof(float) * (size_t)H4 * Q.hid);
       for (int i = 0; i < H4; ++i) bih[(size_t)d * H4 + i] = b1->data[(size_t)i] + b2->data[(size_t)i];
     }
-    Q.wih = (float*)dalloc(sizeof(float) * wih.size());
-    Q.bih = (float*)dalloc(sizeof(float) * bih.size());
-    Q.whh = (float*)dalloc(sizeof(float) * whh.size());
+    Q.wih = (float*)dalloc(arena_, sizeof(float) * wih.size(), wih.data());
+    Q.bih = (float*)dalloc(arena_, sizeof(float) * bih.size(), bih.data());
+    Q.whh = (float*)dalloc(arena_, sizeof(float) * whh.size(), whh.data());
     if (!Q.wih || !Q.bih || !Q.whh) return false;
-    cudaMemcpy(Q.wih, wih.data(), sizeof(float) * wih.size(), cudaMemcpyHostToDevice);
-    cudaMemcpy(Q.bih, bih.data(), sizeof(float) * bih.size(), cudaMemcpyHostToDevice);
-    cudaMemcpy(Q.whh, whh.data(), sizeof(float) * whh.size(), cudaMemcpyHostToDevice);
   }
   {
     const int K = 2 * Q.hid;
@@ -337,18 +343,15 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
       sh[(size_t)bin] = (float)(s * ((double)db->data[(size_t)bin] - (double)m1->data[(size_t)bin]) +
                                 (double)b1->data[(size_t)bin]);
     }
-    Q.wd = (float*)dalloc(sizeof(float) * dw->data.size());
-    Q.dscale = (float*)dalloc(sizeof(float) * sc.size());
-    Q.dshift = (float*)dalloc(sizeof(float) * sh.size());
+    Q.wd = (float*)dalloc(arena_, sizeof(float) * dw->data.size(), dw->data.data());
+    Q.dscale = (float*)dalloc(arena_, sizeof(float) * sc.size(), sc.data());
+    Q.dshift = (float*)dalloc(arena_, sizeof(float) * sh.size(), sh.data());
     if (!Q.wd || !Q.dscale || !Q.dshift) return false;
-    cudaMemcpy(Q.wd, dw->data.data(), sizeof(float) * dw->data.size(), cudaMemcpyHostToDevice);
-    cudaMemcpy(Q.dscale, sc.data(), sizeof(float) * sc.size(), cudaMemcpyHostToDevice);
-    cudaMemcpy(Q.dshift, sh.data(), sizeof(float) * sh.size(), cudaMemcpyHostToDevice);
   }
-  Q.l0 = (float*)dalloc(sizeof(float) * (size_t)Nb * Q.T * Q.bins);
-  Q.xp = (float*)dalloc(sizeof(float) * (size_t)Nb * Q.T * 8 * Q.hid);
-  Q.hs = (float*)dalloc(sizeof(float) * (size_t)Nb * Q.T * 2 * Q.hid);
-  Q.y = (float*)dalloc(sizeof(float) * (size_t)Nb * Q.T * Q.bins);
+  Q.l0 = (float*)dalloc(arena_, sizeof(float) * (size_t)Nb * Q.T * Q.bins);
+  Q.xp = (float*)dalloc(arena_, sizeof(float) * (size_t)Nb * Q.T * 8 * Q.hid);
+  Q.hs = (float*)dalloc(arena_, sizeof(float) * (size_t)Nb * Q.T * 2 * Q.hid);
+  Q.y = (float*)dalloc(arena_, sizeof(float) * (size_t)Nb * Q.T * Q.bins);
   return Q.l0 && Q.xp && Q.hs && Q.y;
 }
 
@@ -368,10 +371,10 @@ bool Engine::finalize() {
   }
   pos_aux2_ = 0; pos_aux1_ = a2; pos_x_ = a2 + a1;
   const int C3 = round_up(a2 + a1 + 2, 16);
-  in3_ = make_buffer(Nb, max_bin, W, C3);
-  o1_ = make_buffer(Nb, max_bin / 2, W, nout / 2);
-  o2_ = make_buffer(Nb, max_bin / 2, W, nout);
-  f3_ = make_buffer(Nb, max_bin, W, nout);
+  in3_ = make_buffer(arena_, Nb, max_bin, W, C3);
+  o1_ = make_buffer(arena_, Nb, max_bin / 2, W, nout / 2);
+  o2_ = make_buffer(arena_, Nb, max_bin / 2, W, nout);
+  f3_ = make_buffer(arena_, Nb, max_bin, W, nout);
   if (!in3_.hi || !o1_.hi || !o2_.hi || !f3_.hi) return false;
 
   const int nin_lstm = max_bin / 2;
@@ -410,9 +413,8 @@ bool Engine::finalize() {
   const HostTensor *ow, *aw;
   if (!need("out.weight", {2, nout, 1, 1}, &ow)) return false;
   if (!need("aux_out.weight", {2, 3 * nout / 4, 1, 1}, &aw)) return false;   // dead in forward, but a strict key
-  out_w_ = (float*)dalloc(sizeof(float) * 2 * nout);
+  out_w_ = (float*)dalloc(arena_, sizeof(float) * 2 * nout, ow->data.data());
   if (!out_w_) return false;
-  cudaMemcpy(out_w_, ow->data.data(), sizeof(float) * 2 * nout, cudaMemcpyHostToDevice);
   // strict load: no unexpected keys (torch load_state_dict(strict=True), inference.py:131)
   {
     // every key outside the model's name space is unexpected
@@ -536,8 +538,7 @@ bool Engine::run_decoder(ConvLayer& L, const ActView& low, const Buffer& cat, in
     err = "internal: " + L.name + " was laid out for the fused upsample but the fused kernel is not available";
     return false;
   }
-  ++launches;
-  if (!timed("upsample2x", N, cat.H, cat.W, s, [&] { return ck(launch_upsample2x(low, cat.view(N, 0, cat.H, 0, low.C), s), "decoder upsample"); }))
+  if (!timed("upsample2x", 1, N, cat.H, cat.W, s, [&] { return ck(launch_upsample2x(low, cat.view(N, 0, cat.H, 0, low.C), s), "decoder upsample"); }))
     return false;
   return run_conv(L, cat_all, out, s);
 }
@@ -557,22 +558,20 @@ bool Engine::run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, 
   if (!run_conv(P.enc_a[3], e4, P.t5.all(N), s) || !run_conv(P.enc_b[3], P.t5.all(N), P.e5.all(N), s)) return false;
   // ASPP (lib/layers.py:92-105)
   const int c8 = 8 * n, h16 = H / 16;
-  launches += 2;
-  if (!timed("aspp.pool_freq_mean", N, h16, P.W / 16, s, [&] { return ck(launch_pool_freq_mean(P.e5.all(N), P.pool.all(N), s), "aspp pool"); }))
+  if (!timed("aspp.pool_freq_mean", 1, N, h16, P.W / 16, s, [&] { return ck(launch_pool_freq_mean(P.e5.all(N), P.pool.all(N), s), "aspp pool"); }))
     return false;
   if (!run_conv(P.aspp1, P.pool.all(N), P.f1.all(N), s)) return false;
-  if (!timed("aspp.broadcast_rows", N, h16, P.W / 16, s, [&] { return ck(launch_broadcast_rows(P.f1.all(N), P.acat.view(N, 0, h16, 0, c8), s), "aspp broadcast"); }))
+  if (!timed("aspp.broadcast_rows", 1, N, h16, P.W / 16, s, [&] { return ck(launch_broadcast_rows(P.f1.all(N), P.acat.view(N, 0, h16, 0, c8), s), "aspp broadcast"); }))
     return false;
   if (!run_conv(P.aspp2, P.e5.all(N), P.acat.view(N, 0, h16, c8, c8), s)) return false;
   for (int i = 0; i < 3; ++i)
     if (!run_conv(P.aspp_d[i], P.e5.all(N), P.acat.view(N, 0, h16, (2 + i) * c8, c8), s)) return false;
   if (!run_conv(P.bott, P.acat.all(N), P.ao.all(N), s)) return false;
   // decoders (lib/nets.py:35-37, lib/layers.py:51-64)
-  launches += 2;
-  if (!timed("upsample2x", N, H / 8, P.W / 8, s, [&] { return ck(launch_upsample2x(P.ao.all(N), P.cat4.view(N, 0, H / 8, 0, 8 * n), s), "up4"); }))
+  if (!timed("upsample2x", 1, N, H / 8, P.W / 8, s, [&] { return ck(launch_upsample2x(P.ao.all(N), P.cat4.view(N, 0, H / 8, 0, 8 * n), s), "up4"); }))
     return false;
   if (!run_conv(P.dec[0], P.cat4.all(N), P.d4.all(N), s)) return false;
-  if (!timed("upsample2x", N, H / 4, P.W / 4, s, [&] { return ck(launch_upsample2x(P.d4.all(N), P.cat3.view(N, 0, H / 4, 0, 6 * n), s), "up3"); }))
+  if (!timed("upsample2x", 1, N, H / 4, P.W / 4, s, [&] { return ck(launch_upsample2x(P.d4.all(N), P.cat3.view(N, 0, H / 4, 0, 6 * n), s), "up3"); }))
     return false;
   if (!run_conv(P.dec[1], P.cat3.all(N), P.d3.all(N), s)) return false;
   // The LSTM branch's 1x1 input convolution (2n -> 1, lib/layers.py:112,126) is one dot product per pixel of dec2's
@@ -598,26 +597,24 @@ bool Engine::run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, 
     if (!ck(cudaEventRecord(ev_lstm_fork_, s), "lstm fork") || !ck(cudaStreamWaitEvent(side, ev_lstm_fork_, 0), "lstm fork"))
       return false;
   }
-  launches += dot_fused ? 3 : 4;
   if (!dot_fused &&
-      !timed("lstm.inconv", N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_inconv(d2v, Q.conv_w, Q.l0, sl), "lstm conv"); }))
+      !timed("lstm.inconv", 1, N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_inconv(d2v, Q.conv_w, Q.l0, sl), "lstm conv"); }))
     return false;
-  if (!timed("lstm.input_projection", N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_input_projection(Q.l0, Q.conv_bias, Q.wih, Q.bih, Q.xp, N, Q.T, Q.bins, 8 * Q.hid, sl), "lstm input projection"); }))
+  if (!timed("lstm.input_projection", 1, N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_input_projection(Q.l0, Q.conv_bias, Q.wih, Q.bih, Q.xp, N, Q.T, Q.bins, 8 * Q.hid, sl), "lstm input projection"); }))
     return false;
-  if (!timed("lstm.recurrence", N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_recurrence(Q.xp, Q.whh, Q.hs, N, Q.T, Q.hid, sl), "lstm recurrence"); }))
+  if (!timed("lstm.recurrence", 1, N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_recurrence(Q.xp, Q.whh, Q.hs, N, Q.T, Q.hid, sl), "lstm recurrence"); }))
     return false;
   // the branch output at half resolution: fp32 plane y[bin][n][t]
-  if (!timed("lstm.dense", N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_dense(Q.hs, Q.wd, Q.dscale, Q.dshift, N * Q.T, 2 * Q.hid, Q.bins, Q.y, sl), "lstm dense"); }))
+  if (!timed("lstm.dense", 1, N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_dense(Q.hs, Q.wd, Q.dscale, Q.dshift, N * Q.T, 2 * Q.hid, Q.bins, Q.y, sl), "lstm dense"); }))
     return false;
-  ++launches;
   if (!P.skip_only &&   // staged layout: it becomes channel 2n of d2 and is up-sampled together with h
-      !timed("lstm.to_channel", N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_plane_to_channel(Q.y, N, Q.T, Q.bins, P.d2.all(N), 2 * n, sl), "lstm channel"); }))
+      !timed("lstm.to_channel", 1, N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_plane_to_channel(Q.y, N, Q.T, Q.bins, P.d2.all(N), 2 * n, sl), "lstm channel"); }))
     return false;
   if (P.skip_only) {
     // fused layout: up(lstm) -> its 16-channel group of cat1 / lstm_up (small kernel on the LSTM's stream), then the row
     // kernel reads [e1 | up(lstm)] by TMA and produces up(h) itself from d2
     const ActView lstm_full = P.lstm_own ? P.lstm_up.all(N) : P.cat1.view(N, 0, H, P.lstm_coff, 16);
-    if (!timed("lstm.upsample2x", N, H, P.W, sl, [&] { return ck(launch_upsample2x_c1(Q.y, Q.bins, Q.T, Q.T, (int64_t)N * Q.T, lstm_full, sl), "lstm upsample"); }))
+    if (!timed("lstm.upsample2x", 1, N, H, P.W, sl, [&] { return ck(launch_upsample2x_c1(Q.y, Q.bins, Q.T, Q.T, (int64_t)N * Q.T, lstm_full, sl), "lstm upsample"); }))
       return false;
     if (overlap) {
       if (!ck(cudaEventRecord(ev_lstm_join_, side), "lstm join") || !ck(cudaStreamWaitEvent(s, ev_lstm_join_, 0), "lstm join"))
@@ -629,17 +626,21 @@ bool Engine::run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, 
   // staged layout: dec1 on cat[up(h, lstm), e1] (lib/nets.py:39)
   const int upc = P.e1_off;   // channels of d2 that are upsampled: 2n conv channels + the LSTM channel group
   if (overlap) {
-    if (!ck(cudaEventRecord(ev_lstm_join_, side), "lstm join")) return false;
+    // Only stage 3 has a side stream, and its n is a multiple of 16: 2n fills whole 32-channel chunks, so a dec1 on the
+    // row kernel (the only one that fuses the upsample) always got the fused layout from build_basenet.
     if (P.dec[3].tc && P.dec[3].tc->fuses_upsample(P.d2.C)) {
-      // fused: the convolution reads d2 (incl. the LSTM channel) itself, so it simply waits for the side stream
-      if (!ck(cudaStreamWaitEvent(s, ev_lstm_join_, 0), "lstm join")) return false;
-      return run_decoder(P.dec[3], P.d2.all(N), P.cat1, N, out, s);
+      err = "internal: " + P.dec[3].name + " fuses its upsample but has the staged layout";
+      return false;
     }
-    ++launches;
-    if (!ck(launch_upsample2x(P.d2.view(N, 0, H / 2, 0, 2 * n), P.cat1.view(N, 0, H, 0, 2 * n), s), "up1")) return false;
+    if (!ck(cudaEventRecord(ev_lstm_join_, side), "lstm join")) return false;
+    if (!timed("upsample2x", 1, N, H, P.W, s, [&] {
+          return ck(launch_upsample2x(P.d2.view(N, 0, H / 2, 0, 2 * n), P.cat1.view(N, 0, H, 0, 2 * n), s), "up1");
+        }))
+      return false;
     if (!ck(cudaStreamWaitEvent(s, ev_lstm_join_, 0), "lstm join")) return false;
-    if (!ck(launch_upsample2x(P.d2.view(N, 0, H / 2, 2 * n, upc - 2 * n), P.cat1.view(N, 0, H, 2 * n, upc - 2 * n), s),
-            "up1 lstm"))
+    if (!timed("upsample2x", 1, N, H, P.W, s, [&] {
+          return ck(launch_upsample2x(P.d2.view(N, 0, H / 2, 2 * n, upc - 2 * n), P.cat1.view(N, 0, H, 2 * n, upc - 2 * n), s), "up1 lstm");
+        }))
       return false;
     return run_conv(P.dec[3], P.cat1.all(N), out, s);
   }
@@ -687,10 +688,9 @@ bool Engine::predict_mask(const float* mag, int N, float* mask_out, int offset, 
   const int max_bin = cfg_.n_fft / 2, nb = bins(), W = cfg_.cropsize, r = W - 2 * offset;
   for (int i = 0; i < N; i += cfg_.max_batch) {
     const int nb_now = N - i < cfg_.max_batch ? N - i : cfg_.max_batch;
-    ++launches;
-    if (!ck(launch_pack_mag_from_float(mag + (int64_t)i * 2 * nb * W, nb, max_bin,
-                                       in3_.view(nb_now, 0, max_bin, pos_x_, 2), s),
-            "pack"))
+    if (!timed("pack_mag_from_float", 1, nb_now, max_bin, W, s, [&] {
+          return ck(launch_pack_mag_from_float(mag + (int64_t)i * 2 * nb * W, nb, max_bin, in3_.view(nb_now, 0, max_bin, pos_x_, 2), s), "pack");
+        }))
       return false;
     if (!forward(nb_now, s)) return false;
     MaskOutParams p;
@@ -699,8 +699,7 @@ bool Engine::predict_mask(const float* mag, int N, float* mask_out, int offset, 
     p.out = mask_out + (int64_t)i * 2 * nb * r;
     p.stride_n = (int64_t)2 * nb * r; p.stride_c = (int64_t)nb * r; p.stride_bin = r;
     p.offset = offset; p.t_base0 = 0; p.t_limit = r; p.roi_t = 0; p.accumulate = 0;
-    ++launches;
-    if (!timed("mask_out", nb_now, max_bin, W, s, [&] { return ck(launch_mask_out(p, s), "mask_out"); })) return false;
+    if (!timed("mask_out", 1, nb_now, max_bin, W, s, [&] { return ck(launch_mask_out(p, s), "mask_out"); })) return false;
   }
   return true;
 }
@@ -717,8 +716,7 @@ bool Engine::separate_windows(const float2* spec, int64_t T, const float* norm, 
   for (int i = 0; i < count; i += cfg_.max_batch) {
     const int n_now = count - i < cfg_.max_batch ? count - i : cfg_.max_batch;
     const int g0 = first + i;
-    ++launches;
-    if (!timed("pack_mag_from_spec", n_now, max_bin, W, s, [&] {
+    if (!timed("pack_mag_from_spec", 1, n_now, max_bin, W, s, [&] {
           return ck(launch_pack_mag_from_spec(spec, nb, T, max_bin, W, r, pad_l, g0, norm, in3_.view(n_now, 0, max_bin, pos_x_, 2), s), "pack");
         }))
       return false;
@@ -731,8 +729,7 @@ bool Engine::separate_windows(const float2* spec, int64_t T, const float* norm, 
     p.offset = cfg_.offset;
     p.t_base0 = (int64_t)g0 * r - frame_shift;
     p.t_limit = mask_T; p.roi_t = r; p.accumulate = accumulate;
-    ++launches;
-    if (!timed("mask_out", n_now, max_bin, W, s, [&] { return ck(launch_mask_out(p, s), "mask_out"); })) return false;
+    if (!timed("mask_out", 1, n_now, max_bin, W, s, [&] { return ck(launch_mask_out(p, s), "mask_out"); })) return false;
     if (final_pass && on_frames_final_) {
       int64_t f = p.t_base0 + (int64_t)n_now * r;
       if (f > mask_T) f = mask_T;
@@ -744,10 +741,9 @@ bool Engine::separate_windows(const float2* spec, int64_t T, const float* norm, 
 
 bool Engine::normaliser(const float2* spec, int64_t T, int mode, float* out, cudaStream_t s) {
   cudaSetDevice(cfg_.device);
-  ++launches;
   const int64_t n = (int64_t)2 * bins() * T;
-  if (mode == 0) return timed("normaliser.absmax", 1, bins(), (int)T, s, [&] { return ck(launch_absmax(spec, n, out, s), "absmax"); });
-  return timed("normaliser.lexmax", 1, bins(), (int)T, s, [&] { return ck(launch_lexmax_abs(spec, n, ws_lex_, out, s), "lexmax"); });
+  if (mode == 0) return timed("normaliser.absmax", 1, 1, bins(), (int)T, s, [&] { return ck(launch_absmax(spec, n, out, s), "absmax"); });
+  return timed("normaliser.lexmax", 2, 1, bins(), (int)T, s, [&] { return ck(launch_lexmax_abs(spec, n, ws_lex_, out, s), "lexmax"); });
 }
 
 // mask [2][bins][T]; the full window range of one track on this device (inference.py:70-77 / 83-98)
@@ -770,8 +766,23 @@ bool Engine::separate(const float2* spec, int64_t T, int tta, float* mask, cudaS
 
 bool Engine::apply_mask(const float2* spec, const float* mask, int64_t T, float2* y, float2* v, cudaStream_t s) {
   cudaSetDevice(cfg_.device);
-  ++launches;
-  return ck(launch_apply_mask(spec, mask, (int64_t)2 * bins() * T, y, v, s), "apply_mask");
+  return timed("apply_mask", 1, 1, bins(), (int)T, s, [&] {
+    return ck(launch_apply_mask(spec, mask, (int64_t)2 * bins() * T, y, v, s), "apply_mask");
+  });
+}
+
+bool Engine::mask_frame_min(const float* mask, int64_t T, float* frame_min, cudaStream_t s) {
+  cudaSetDevice(cfg_.device);
+  return timed("mask_frame_min", 1, 1, bins(), (int)T, s, [&] {
+    return ck(launch_mask_frame_min(mask, 2 * bins(), T, frame_min, s), "vr_mask_frame_min");
+  });
+}
+
+bool Engine::mask_apply_weight(float* mask, int64_t T, const float* weight, cudaStream_t s) {
+  cudaSetDevice(cfg_.device);
+  return timed("mask_apply_weight", 1, 1, bins(), (int)T, s, [&] {
+    return ck(launch_mask_apply_weight(mask, 2 * bins(), T, weight, s), "vr_mask_apply_weight");
+  });
 }
 
 bool Engine::spec_image(const float2* spec, const float* mask, int64_t T, unsigned char* img_a, unsigned char* img_b,
@@ -782,9 +793,8 @@ bool Engine::spec_image(const float2* spec, const float* mask, int64_t T, unsign
     return false;
   }
   // allocated on first use, once per context
-  if (!ws_img_range_ && !(ws_img_range_ = (unsigned int*)dalloc(sizeof(unsigned int) * 4))) return false;
-  launches += 2;
-  return timed("spec_image", 1, bins(), (int)T, s, [&] {
+  if (!ws_img_range_ && !(ws_img_range_ = (unsigned int*)dalloc(arena_, sizeof(unsigned int) * 4))) return false;
+  return timed("spec_image", 2, 1, bins(), (int)T, s, [&] {
     return ck(launch_spec_image(spec, mask, (int64_t)bins() * T, ws_img_range_, img_a, img_b, s), "spec_image");
   });
 }
@@ -816,31 +826,19 @@ bool Engine::validation_loss(const float2* spec_x, const float2* spec_y, int64_t
   const int n = (int)n64;
   const int64_t mask_T = n64 * r;
   const int64_t nmask = (int64_t)2 * bins() * mask_T;
-  if (nmask > ws_mask_cap_) {
-    if (ws_mask_) cudaFree(ws_mask_);
-    ws_mask_ = nullptr;
-    if (!ck(cudaMalloc(&ws_mask_, sizeof(float) * nmask), "workspace mask")) return false;
-    ws_mask_cap_ = nmask;
-  }
-  const int64_t nval = validation_l1_scratch(n);
-  if (nval > ws_val_cap_) {
-    if (ws_val_) cudaFree(ws_val_);
-    ws_val_ = nullptr;
-    if (!ck(cudaMalloc(&ws_val_, sizeof(double) * nval), "workspace validation")) return false;
-    ws_val_cap_ = nval;
-  }
+  if (!ck(ws_mask_.ensure(nmask), "workspace mask") ||
+      !ck(ws_val_.ensure(validation_l1_scratch(n)), "workspace validation"))
+    return false;
   float* coef = coef_out ? coef_out : ws_norm_;
   const int64_t nspec = (int64_t)2 * bins() * T;
-  launches += 2;
-  if (!timed("normaliser.absmax", 1, bins(), (int)T, s, [&] {
+  if (!timed("normaliser.absmax", 2, 1, bins(), (int)T, s, [&] {
         return ck(launch_absmax(spec_x, nspec, coef, s), "absmax X") &&
                ck(launch_absmax(spec_y, nspec, coef, s, true), "absmax y");
       }))
     return false;
-  if (!separate_windows(spec_x, T, coef, cfg_.offset, 0, n, ws_mask_, mask_T, 0, 0, s)) return false;
-  launches += 2;
-  return timed("validation_l1", n, bins(), r, s, [&] {
-    return ck(launch_validation_l1(spec_x, spec_y, ws_mask_, bins(), T, r, n, coef, ws_val_, window_sums, s),
+  if (!separate_windows(spec_x, T, coef, cfg_.offset, 0, n, ws_mask_.get(), mask_T, 0, 0, s)) return false;
+  return timed("validation_l1", 2, n, bins(), r, s, [&] {
+    return ck(launch_validation_l1(spec_x, spec_y, ws_mask_.get(), bins(), T, r, n, coef, ws_val_.get(), window_sums, s),
               "validation_l1");
   });
 }
@@ -862,8 +860,7 @@ bool Engine::stft_range(const float* wave, int64_t L, float2* spec, int64_t T, i
     err = "stft: frame range outside [0, T]";
     return false;
   }
-  ++launches;
-  return timed("stft", 1, bins(), (int)(t1 - t0), s, [&] { return ck(launch_stft(wave, L, cfg_.n_fft, cfg_.hop, spec, T, t0, t1, twiddle_, window_, s), "stft"); });
+  return timed("stft", 1, 1, bins(), (int)(t1 - t0), s, [&] { return ck(launch_stft(wave, L, cfg_.n_fft, cfg_.hop, spec, T, t0, t1, twiddle_, window_, s), "stft"); });
 }
 
 bool Engine::normaliser_range(const float2* spec, int64_t T, int64_t t0, int64_t t1, float* out, cudaStream_t s) {
@@ -872,32 +869,15 @@ bool Engine::normaliser_range(const float2* spec, int64_t T, int64_t t0, int64_t
     err = "normaliser: frame range outside [0, T]";
     return false;
   }
-  ++launches;
-  return ck(launch_absmax_range(spec, 2 * bins(), T, t0, t1, out, s), "absmax range");
+  return timed("normaliser.absmax_range", 1, 1, bins(), (int)(t1 - t0), s, [&] {
+    return ck(launch_absmax_range(spec, 2 * bins(), T, t0, t1, out, s), "absmax range");
+  });
 }
 
 bool Engine::ensure_ws(int64_t T) {
   const int64_t nspec = (int64_t)2 * bins() * T;
-  if (nspec > ws_spec_cap_) {
-    if (ws_spec_) cudaFree(ws_spec_);
-    ws_spec_ = nullptr;
-    if (!ck(cudaMalloc(&ws_spec_, sizeof(float2) * nspec), "workspace spec")) return false;
-    ws_spec_cap_ = nspec;
-  }
-  if (nspec > ws_mask_cap_) {
-    if (ws_mask_) cudaFree(ws_mask_);
-    ws_mask_ = nullptr;
-    if (!ck(cudaMalloc(&ws_mask_, sizeof(float) * nspec), "workspace mask")) return false;
-    ws_mask_cap_ = nspec;
-  }
-  const int64_t nfr = (int64_t)4 * T * cfg_.n_fft;
-  if (nfr > ws_frames_cap_) {
-    if (ws_frames_) cudaFree(ws_frames_);
-    ws_frames_ = nullptr;
-    if (!ck(cudaMalloc(&ws_frames_, sizeof(float) * nfr), "workspace frames")) return false;
-    ws_frames_cap_ = nfr;
-  }
-  return true;
+  return ck(ws_spec_.ensure(nspec), "workspace spec") && ck(ws_mask_.ensure(nspec), "workspace mask") &&
+         ck(ws_frames_.ensure((int64_t)4 * T * cfg_.n_fft), "workspace frames");
 }
 
 bool Engine::istft(const float2* spec, const float* mask, int64_t T, float* wave_a, float* wave_b, cudaStream_t s) {
@@ -922,19 +902,12 @@ bool Engine::istft_range(const float2* spec, const float* mask, int64_t T, int64
   int64_t f1 = ((int64_t)hop * k1 - 1 + NF / 2) / hop;
   if (f1 > T - 1) f1 = T - 1;
   const int64_t nfr = f1 - f0 + 1;
-  const int64_t need = (int64_t)4 * nfr * NF;
-  if (need > ws_frames_cap_) {
-    if (ws_frames_) cudaFree(ws_frames_);
-    ws_frames_ = nullptr;
-    if (!ck(cudaMalloc(&ws_frames_, sizeof(float) * need), "workspace frames")) return false;
-    ws_frames_cap_ = need;
-  }
-  float* fa = ws_frames_;
-  float* fb = mask ? ws_frames_ + (int64_t)2 * nfr * NF : nullptr;
-  launches += 2;
-  if (!timed("istft.frames", 1, bins(), (int)nfr, s, [&] { return ck(launch_istft_frames(spec, mask, NF, T, f0, nfr, fa, fb, twiddle_, window_, s), "istft frames"); }))
+  if (!ck(ws_frames_.ensure((int64_t)4 * nfr * NF), "workspace frames")) return false;
+  float* fa = ws_frames_.get();
+  float* fb = mask ? fa + (int64_t)2 * nfr * NF : nullptr;
+  if (!timed("istft.frames", 1, 1, bins(), (int)nfr, s, [&] { return ck(launch_istft_frames(spec, mask, NF, T, f0, nfr, fa, fb, twiddle_, window_, s), "istft frames"); }))
     return false;
-  return timed("istft.overlap_add", 1, bins(), (int)nfr, s, [&] {
+  return timed("istft.overlap_add", 1, 1, bins(), (int)nfr, s, [&] {
     return ck(launch_istft_ola(fa, fb, NF, hop, T, f0, nfr, (int64_t)hop * k0, (int64_t)hop * k1, wave_a, mask ? wave_b : nullptr, window_, s), "istft ola");
   });
 }
@@ -944,9 +917,9 @@ bool Engine::separate_wave(const float* wave, int64_t L, int tta, float* inst, f
   cudaSetDevice(cfg_.device);
   const int64_t T = 1 + L / cfg_.hop;
   if (!ensure_ws(T)) return false;
-  if (!stft(wave, L, ws_spec_, T, nullptr, s)) return false;
-  if (!separate(ws_spec_, T, tta, ws_mask_, s)) return false;
-  return istft(ws_spec_, ws_mask_, T, inst, voc, s);
+  if (!stft(wave, L, ws_spec_.get(), T, nullptr, s)) return false;
+  if (!separate(ws_spec_.get(), T, tta, ws_mask_.get(), s)) return false;
+  return istft(ws_spec_.get(), ws_mask_.get(), T, inst, voc, s);
 }
 
 // Host-buffer entry (the end-to-end call): H2D of the wave, the whole path, D2H of both stems.
@@ -955,36 +928,27 @@ bool Engine::separate_wave_host(const float* wave, int64_t L, int tta, float* in
   cudaSetDevice(cfg_.device);
   const int64_t T = 1 + L / cfg_.hop;
   const int64_t Lo = (int64_t)cfg_.hop * (T - 1);
-  const int64_t need_f = 2 * L + 4 * Lo;
-  if (need_f > ws_wave_cap_) {
-    if (ws_wave_) cudaFree(ws_wave_);
-    ws_wave_ = nullptr;
-    if (!ck(cudaMalloc(&ws_wave_, sizeof(float) * need_f), "workspace wave")) return false;
-    ws_wave_cap_ = need_f;
-  }
+  if (!ck(ws_wave_.ensure(2 * L + 4 * Lo), "workspace wave")) return false;
   const int64_t img_bytes = (int64_t)3 * bins() * T;
-  if ((img_inst || img_voc) && 2 * img_bytes > ws_img_cap_) {
-    if (ws_img_) cudaFree(ws_img_);
-    ws_img_ = nullptr;
-    if (!ck(cudaMalloc(&ws_img_, 2 * img_bytes), "workspace images")) return false;
-    ws_img_cap_ = 2 * img_bytes;
-  }
-  float* d_in = ws_wave_;
-  float* d_inst = ws_wave_ + 2 * L;
+  if ((img_inst || img_voc) && !ck(ws_img_.ensure(2 * img_bytes), "workspace images")) return false;
+  float* d_in = ws_wave_.get();
+  float* d_inst = d_in + 2 * L;
   float* d_voc = d_inst + 2 * Lo;
   if (!ck(cudaMemcpyAsync(d_in, wave, sizeof(float) * 2 * L, cudaMemcpyHostToDevice, s), "H2D wave")) return false;
   // The stems leave the device span by span: as soon as a window batch of the last pass has written its mask frames,
   // the masked inverse STFT of the hops they complete runs on `s` and their device-to-host copy on the copy stream,
   // overlapped with the next batch of the net (the copies of a 4-minute track are 169 MB).
   if (!ensure_ws(T)) return false;
-  if (!stft(d_in, L, ws_spec_, T, nullptr, s)) return false;
+  float2* spec = ws_spec_.get();
+  float* mask = ws_mask_.get();
+  if (!stft(d_in, L, spec, T, nullptr, s)) return false;
   int64_t k_done = 0;
   bool ok = true;
   auto flush = [&](int64_t f) -> bool {
     // output hop k needs mask frames k and k+1
     int64_t k1 = f >= T ? T - 1 : f - 1;
     if (k1 <= k_done) return true;
-    if (!istft_range(ws_spec_, ws_mask_, T, k_done, k1, d_inst, d_voc, s)) return false;
+    if (!istft_range(spec, mask, T, k_done, k1, d_inst, d_voc, s)) return false;
     if (!ck(cudaEventRecord(ev_span_, s), "span event") || !ck(cudaStreamWaitEvent(s_copy_, ev_span_, 0), "span wait"))
       return false;
     const size_t off = (size_t)cfg_.hop * (size_t)k_done, cnt = (size_t)cfg_.hop * (size_t)(k1 - k_done);
@@ -999,15 +963,16 @@ bool Engine::separate_wave_host(const float* wave, int64_t L, int tta, float* in
     return true;
   };
   on_frames_final_ = flush;
-  ok = separate(ws_spec_, T, tta, ws_mask_, s);
+  ok = separate(spec, T, tta, mask, s);
   on_frames_final_ = nullptr;
   if (ok) ok = flush(T);
   if (ok && (img_inst || img_voc)) {
     // after the last span: the images of the final mask, copied back behind the stems on the copy stream
-    ok = spec_image(ws_spec_, ws_mask_, T, ws_img_, ws_img_ + img_bytes, s) &&
+    unsigned char* img = ws_img_.get();
+    ok = spec_image(spec, mask, T, img, img + img_bytes, s) &&
          ck(cudaEventRecord(ev_span_, s), "image event") && ck(cudaStreamWaitEvent(s_copy_, ev_span_, 0), "image wait") &&
-         (!img_inst || ck(cudaMemcpyAsync(img_inst, ws_img_, img_bytes, cudaMemcpyDeviceToHost, s_copy_), "D2H image")) &&
-         (!img_voc || ck(cudaMemcpyAsync(img_voc, ws_img_ + img_bytes, img_bytes, cudaMemcpyDeviceToHost, s_copy_),
+         (!img_inst || ck(cudaMemcpyAsync(img_inst, img, img_bytes, cudaMemcpyDeviceToHost, s_copy_), "D2H image")) &&
+         (!img_voc || ck(cudaMemcpyAsync(img_voc, img + img_bytes, img_bytes, cudaMemcpyDeviceToHost, s_copy_),
                          "D2H image"));
   }
   if (!ok) {
@@ -1019,59 +984,51 @@ bool Engine::separate_wave_host(const float* wave, int64_t L, int tta, float* in
 }
 
 // ---------------------------------------------------------------------------------------------
+bool Engine::debug_weights(ConvLayer& L, Arena& arena, const float* w, const float* bias, int Cout, int Cin,
+                           const std::vector<int>& perm, cudaStream_t s) {
+  std::vector<float> hw((size_t)Cout * Cin * L.k * L.k), hb((size_t)Cout);
+  if (!ck(cudaMemcpyAsync(hw.data(), w, hw.size() * sizeof(float), cudaMemcpyDeviceToHost, s), "weights to host") ||
+      !ck(cudaMemcpyAsync(hb.data(), bias, hb.size() * sizeof(float), cudaMemcpyDeviceToHost, s), "bias to host") ||
+      !ck(cudaStreamSynchronize(s), "weights to host"))
+    return false;
+  const std::vector<double> one((size_t)Cout, 1.0);
+  return pack_conv(L, arena, hw.data(), Cout, Cin, one.data(), hb.data(), perm);
+}
+
+bool Engine::to_nchw(const ActView& v, int C, float* y_nchw, cudaStream_t s) {
+  return timed("act_to_nchw", 1, v.N, v.H, v.W, s,
+               [&] { return ck(launch_act_to_nchw(v, C, y_nchw, s), "act_to_nchw"); });
+}
+
 bool Engine::debug_conv(const float* x_nchw, int N, int Cin, int H, int W, const float* w, const float* bias, int Cout,
                         int k, int stride, int dil_h, int dil_w, int act, int use_tc, float* y_nchw, cudaStream_t s) {
   cudaSetDevice(cfg_.device);
   const int cin_pad = round_up(Cin, 16);
   const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
-  std::vector<void*> tmp;
-  std::swap(tmp, allocs_);
-  Buffer bin = make_buffer(N, H, W, cin_pad);
-  Buffer bout = make_buffer(N, Ho, Wo, round_up(Cout, 8));
+  Arena arena;   // the hook's buffers and weights, freed on return
+  const Buffer bin = make_buffer(arena, N, H, W, cin_pad);
+  const Buffer bout = make_buffer(arena, N, Ho, Wo, round_up(Cout, 8));
   ConvLayer L;
   L.name = "debug_conv";
   L.rows_wide = g_debug.rows_wide == 1;   // vr_debug_set(2, 1): exercise the 64-wide row tile on a plain convolution
-  L.Cin = Cin; L.CinPad = cin_pad; L.Cout = Cout; L.CoutPad = round_up(Cout, 8);
   L.k = k; L.stride = stride; L.dil_h = dil_h; L.dil_w = dil_w; L.act = act;
-  const int taps = k * k;
-  std::vector<float> hw((size_t)Cout * Cin * taps), hb((size_t)Cout);
-  cudaMemcpyAsync(hw.data(), w, hw.size() * sizeof(float), cudaMemcpyDeviceToHost, s);
-  cudaMemcpyAsync(hb.data(), bias, hb.size() * sizeof(float), cudaMemcpyDeviceToHost, s);
-  cudaStreamSynchronize(s);
-  L.w_host.assign((size_t)taps * L.CinPad * L.CoutPad, 0.f);
-  L.bias_host.assign((size_t)L.CoutPad, 0.f);
-  for (int co = 0; co < Cout; ++co) {
-    L.bias_host[(size_t)co] = hb[(size_t)co];
-    for (int ci = 0; ci < Cin; ++ci)
-      for (int t = 0; t < taps; ++t)
-        L.w_host[((size_t)t * L.CinPad + ci) * L.CoutPad + co] = hw[((size_t)co * Cin + ci) * taps + t];
-  }
-  L.w = (float*)dalloc(L.w_host.size() * sizeof(float));
-  L.bias = (float*)dalloc(L.bias_host.size() * sizeof(float));
-  bool ok = bin.hi && bout.hi && L.w && L.bias;
-  if (ok) {
-    cudaMemcpy(L.w, L.w_host.data(), L.w_host.size() * sizeof(float), cudaMemcpyHostToDevice);
-    cudaMemcpy(L.bias, L.bias_host.data(), L.bias_host.size() * sizeof(float), cudaMemcpyHostToDevice);
-    ok = ck(launch_nchw_to_act(x_nchw, Cin, bin.all(N), s), "nchw_to_act");
-  }
-  if (ok && use_tc) {
-    ok = tc_prepare(L, Ho, Wo, err, allocs_);
-    if (ok && !L.tc) {
+  if (!bin.hi || !bout.hi || !debug_weights(L, arena, w, bias, Cout, Cin, identity_perm(Cin, cin_pad), s)) return false;
+  if (!timed("nchw_to_act", 1, N, H, W, s,
+             [&] { return ck(launch_nchw_to_act(x_nchw, Cin, bin.all(N), s), "nchw_to_act"); }))
+    return false;
+  if (use_tc) {
+    if (!tc_prepare(L, Ho, Wo, err)) return false;
+    if (!L.tc) {
       err = "debug_conv: geometry not supported by the wgmma kernel";
-      ok = false;
+      return false;
     }
   }
+  const ActView out = bout.view(N, 0, Ho, 0, Cout);
   const int saved_mode = cfg_.conv_mode;
   cfg_.conv_mode = use_tc ? 0 : 1;   // a requested CUDA-core run is not warned about
-  if (ok) ok = run_conv(L, bin.all(N), bout.view(N, 0, Ho, 0, Cout), s);
+  const bool ok = run_conv(L, bin.all(N), out, s);
   cfg_.conv_mode = saved_mode;
-  if (ok) ok = ck(launch_act_to_nchw(bout.view(N, 0, Ho, 0, Cout), Cout, y_nchw, s), "act_to_nchw");
-  if (ok) ok = ck(cudaStreamSynchronize(s), "debug_conv sync");
-  L.tc.reset();
-  for (void* p : allocs_) cudaFree(p);
-  allocs_.clear();
-  std::swap(tmp, allocs_);
-  return ok;
+  return ok && to_nchw(out, Cout, y_nchw, s) && ck(cudaStreamSynchronize(s), "debug_conv sync");
 }
 
 // Test hook for the decoder path: y = act(conv3x3(cat[up2x(low), skip]) + bias), fused (upsample inside the row
@@ -1080,58 +1037,41 @@ bool Engine::debug_decoder(const float* low_nchw, int N, int Cl, int h, int w, c
                            const float* wgt, const float* bias, int Cout, int act, int fused, float* y_nchw,
                            cudaStream_t s) {
   cudaSetDevice(cfg_.device);
-  const int H = 2 * h, W = 2 * w, Cin = Cl + Cs;
+  const int H = 2 * h, W = 2 * w;
   const int cl_pad = round_up(Cl, 32), cin_pad = round_up(cl_pad + Cs, 16);
-  std::vector<void*> tmp;
-  std::swap(tmp, allocs_);
-  Buffer blow = make_buffer(N, h, w, cl_pad);
-  Buffer bcat = make_buffer(N, H, W, cin_pad);
-  Buffer bout = make_buffer(N, H, W, round_up(Cout, 16));
+  Arena arena;   // the hook's buffers and weights, freed on return
+  const Buffer blow = make_buffer(arena, N, h, w, cl_pad);
+  const Buffer bcat = make_buffer(arena, N, H, W, cin_pad);
+  const Buffer bout = make_buffer(arena, N, H, W, round_up(Cout, 16));
   ConvLayer L;
   L.name = "debug_decoder";
   L.rows_wide = true;
-  L.Cin = Cin; L.CinPad = cin_pad; L.Cout = Cout; L.CoutPad = round_up(Cout, 8);
-  L.k = 3; L.stride = 1; L.dil_h = 1; L.dil_w = 1; L.act = act;
-  std::vector<float> hw((size_t)Cout * Cin * 9), hb((size_t)Cout);
-  cudaMemcpyAsync(hw.data(), wgt, hw.size() * sizeof(float), cudaMemcpyDeviceToHost, s);
-  cudaMemcpyAsync(hb.data(), bias, hb.size() * sizeof(float), cudaMemcpyDeviceToHost, s);
-  cudaStreamSynchronize(s);
-  L.w_host.assign((size_t)9 * L.CinPad * L.CoutPad, 0.f);
-  L.bias_host.assign((size_t)L.CoutPad, 0.f);
-  for (int co = 0; co < Cout; ++co) {
-    L.bias_host[(size_t)co] = hb[(size_t)co];
-    for (int ci = 0; ci < Cin; ++ci) {
-      const int pc = ci < Cl ? ci : cl_pad + (ci - Cl);   // packed position: [up Cl | pad | skip Cs]
-      for (int t = 0; t < 9; ++t)
-        L.w_host[((size_t)t * L.CinPad + pc) * L.CoutPad + co] = hw[((size_t)co * Cin + ci) * 9 + t];
-    }
-  }
-  L.w = (float*)dalloc(L.w_host.size() * sizeof(float));
-  L.bias = (float*)dalloc(L.bias_host.size() * sizeof(float));
-  bool ok = blow.hi && bcat.hi && bout.hi && L.w && L.bias;
-  if (ok) {
-    cudaMemcpy(L.w, L.w_host.data(), L.w_host.size() * sizeof(float), cudaMemcpyHostToDevice);
-    cudaMemcpy(L.bias, L.bias_host.data(), L.bias_host.size() * sizeof(float), cudaMemcpyHostToDevice);
-    ok = ck(launch_nchw_to_act(low_nchw, Cl, blow.all(N), s), "nchw_to_act low") &&
-         ck(launch_nchw_to_act(skip_nchw, Cs, bcat.view(N, 0, H, cl_pad, cin_pad - cl_pad), s), "nchw_to_act skip");
-  }
-  if (ok) ok = tc_prepare(L, H, W, err, allocs_);
-  if (ok && fused && !(L.tc && L.tc->fuses_upsample(blow.C))) {
-    err = "debug_decoder: geometry not supported by the fused row kernel";
-    ok = false;
-  }
+  L.k = 3; L.act = act;
+  std::vector<int> perm((size_t)cin_pad, -1);   // packed input channels: [up Cl | pad | skip Cs]
+  for (int i = 0; i < Cl; ++i) perm[(size_t)i] = i;
+  for (int i = 0; i < Cs; ++i) perm[(size_t)(cl_pad + i)] = Cl + i;
+  if (!blow.hi || !bcat.hi || !bout.hi || !debug_weights(L, arena, wgt, bias, Cout, Cl + Cs, perm, s)) return false;
+  const ActView skip = bcat.view(N, 0, H, cl_pad, cin_pad - cl_pad);
+  if (!timed("nchw_to_act", 1, N, h, w, s,
+             [&] { return ck(launch_nchw_to_act(low_nchw, Cl, blow.all(N), s), "nchw_to_act low"); }) ||
+      !timed("nchw_to_act", 1, N, H, W, s,
+             [&] { return ck(launch_nchw_to_act(skip_nchw, Cs, skip, s), "nchw_to_act skip"); }) ||
+      !tc_prepare(L, H, W, err))
+    return false;
   const ActView out = bout.view(N, 0, H, 0, Cout);
-  if (ok && fused) ok = run_decoder(L, blow.all(N), bcat, N, out, s);
-  if (ok && !fused)
-    ok = ck(launch_upsample2x(blow.all(N), bcat.view(N, 0, H, 0, cl_pad), s), "debug_decoder upsample") &&
-         run_conv(L, bcat.all(N), out, s);
-  if (ok) ok = ck(launch_act_to_nchw(out, Cout, y_nchw, s), "act_to_nchw");
-  if (ok) ok = ck(cudaStreamSynchronize(s), "debug_decoder sync");
-  L.tc.reset();
-  for (void* p : allocs_) cudaFree(p);
-  allocs_.clear();
-  std::swap(tmp, allocs_);
-  return ok;
+  bool ok;
+  if (fused) {
+    if (!(L.tc && L.tc->fuses_upsample(blow.C))) {
+      err = "debug_decoder: geometry not supported by the fused row kernel";
+      return false;
+    }
+    ok = run_decoder(L, blow.all(N), bcat, N, out, s);
+  } else {
+    ok = timed("upsample2x", 1, N, H, W, s, [&] {
+           return ck(launch_upsample2x(blow.all(N), bcat.view(N, 0, H, 0, cl_pad), s), "debug_decoder upsample");
+         }) && run_conv(L, bcat.all(N), out, s);
+  }
+  return ok && to_nchw(out, Cout, y_nchw, s) && ck(cudaStreamSynchronize(s), "debug_decoder sync");
 }
 
 bool Engine::debug_read(const char* what, float* out, int64_t cap, int64_t* dims, cudaStream_t s) {
@@ -1162,7 +1102,7 @@ bool Engine::debug_read(const char* what, float* out, int64_t cap, int64_t* dims
   const int64_t total = (int64_t)N * C * v.H * v.W;
   dims[0] = N; dims[1] = C; dims[2] = v.H; dims[3] = v.W;
   if (total > cap) { err = "debug_read: output buffer too small"; return false; }
-  return ck(launch_act_to_nchw(v, C, out, s), "debug_read");
+  return to_nchw(v, C, out, s);
 }
 
 }  // namespace vr

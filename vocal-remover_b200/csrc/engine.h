@@ -15,6 +15,59 @@
 
 namespace vr {
 
+// Owner of one cudaMalloc allocation.  It is freed on destruction, so the device it was made on must be current then.
+template <class T>
+class DevPtr {
+ public:
+  DevPtr() = default;
+  DevPtr(DevPtr&& o) noexcept : p_(o.p_) { o.p_ = nullptr; }
+  DevPtr(const DevPtr&) = delete;
+  DevPtr& operator=(const DevPtr&) = delete;
+  ~DevPtr() { reset(); }
+  // frees what it holds, then allocates `bytes` (not initialised)
+  cudaError_t alloc(size_t bytes) {
+    reset();
+    void* p = nullptr;
+    const cudaError_t e = cudaMalloc(&p, bytes);
+    if (e == cudaSuccess) p_ = static_cast<T*>(p);
+    return e;
+  }
+  void reset() {
+    if (p_) cudaFree(p_);
+    p_ = nullptr;
+  }
+  T* get() const { return p_; }
+
+ private:
+  T* p_ = nullptr;
+};
+
+// Allocations that live as long as their owner: the engine's weights and activation buffers, or a test hook's
+// temporaries.
+typedef std::vector<DevPtr<void>> Arena;
+
+// Grow-only workspace of T: ensure(n) keeps an allocation of at least n elements, else frees it and allocates exactly n.
+// The contents are neither kept nor zeroed.
+template <class T>
+class GrowArray {
+ public:
+  cudaError_t ensure(int64_t n) {
+    if (n <= cap_) return cudaSuccess;
+    cap_ = 0;
+    const cudaError_t e = mem_.alloc(sizeof(T) * (size_t)n);
+    if (e == cudaSuccess) cap_ = n;
+    return e;
+  }
+  T* get() const { return mem_.get(); }
+
+ private:
+  DevPtr<T> mem_;
+  int64_t cap_ = 0;
+};
+
+// Synchronous host-to-device copy of weights or tables; on failure sets err and returns false.
+bool upload(void* dst, const void* src, size_t bytes, std::string& err);
+
 struct HostTensor {
   std::vector<int64_t> shape;
   std::vector<float> data;
@@ -124,6 +177,9 @@ class Engine {
                         bool final_pass = false);
   bool separate(const float2* spec, int64_t T, int tta, float* mask, cudaStream_t s);
   bool apply_mask(const float2* spec, const float* mask, int64_t T, float2* y, float2* v, cudaStream_t s);
+  // --postprocess: per-frame minimum of mask [2][bins][T], then the mask pulled towards 1 by per-frame weights
+  bool mask_frame_min(const float* mask, int64_t T, float* frame_min, cudaStream_t s);
+  bool mask_apply_weight(float* mask, int64_t T, const float* weight, cudaStream_t s);
   bool separate_wave(const float* wave, int64_t L, int tta, float* inst, float* voc, cudaStream_t s);
   // img_inst / img_voc: HOST [bins][T][3] uint8 spectrogram images of the two stems, or nullptr for none
   bool separate_wave_host(const float* wave, int64_t L, int tta, float* inst, float* voc, cudaStream_t s,
@@ -147,9 +203,9 @@ class Engine {
   const Config& cfg() const { return cfg_; }
   int bins() const { return cfg_.n_fft / 2 + 1; }
   int roi() const { int r = cfg_.cropsize - 2 * cfg_.offset; return r == 0 ? cfg_.cropsize : r; }
-  int64_t launches = 0;   // kernels launched by this engine (bench 'gpu_launches')
+  int64_t launches = 0;   // kernels launched by this engine (bench 'gpu_launches'); counted by timed and run_conv
 
-  // optional CUDA-event timing of every convolution launch (bench.py roofline object)
+  // optional CUDA-event timing of every launch (bench.py roofline object and --layers table)
   void profile_enable(bool on);
   // sums over the events recorded since enable: [0] tensor-core conv ms, [1] tensor-core conv algorithmic FLOPs,
   // [2] tensor-core launches, [3] CUDA-core conv ms, [4] CUDA-core conv FLOPs, [5] CUDA-core launches
@@ -161,7 +217,7 @@ class Engine {
   bool finalized_ = false;
   bool warned_simt_ = false;   // the CUDA-core fallback warning was printed
   std::map<std::string, HostTensor> sd_;
-  std::vector<void*> allocs_;
+  Arena arena_;   // weights, tables and activation buffers
   int last_n_ = 0;
   // tc: 1 = tensor-core convolution, 0 = CUDA-core convolution, 2 = any other kernel of the path
   struct ProfRec { cudaEvent_t a, b; double flops; int tc; std::string name; int N, H, W; };
@@ -169,25 +225,27 @@ class Engine {
   std::vector<ProfRec> prof_;
   int prof_begin(const std::string& name, int kind, double flops, int N, int H, int W, cudaStream_t s);
   void prof_end(int idx, cudaStream_t s);
-  // a non-convolution launch, bracketed by a CUDA-event pair while profiling is on
+  // Every launch that is not a convolution (those go through run_conv): `launch` enqueues `kernels` kernels on s,
+  // which are counted and, while profiling is on, bracketed by one CUDA-event pair.
   template <class F>
-  bool timed(const char* name, int N, int H, int W, cudaStream_t s, F&& launch) {
+  bool timed(const char* name, int kernels, int N, int H, int W, cudaStream_t s, F&& launch) {
+    launches += kernels;
     const int i = prof_begin(name, 2, 0.0, N, H, W, s);
     const bool ok = launch();
     prof_end(i, s);
     return ok;
   }
 
-  // whole-track workspace (grow-only)
-  float2* ws_spec_ = nullptr; int64_t ws_spec_cap_ = 0;
-  float* ws_mask_ = nullptr; int64_t ws_mask_cap_ = 0;
-  float* ws_frames_ = nullptr; int64_t ws_frames_cap_ = 0;
-  float* ws_wave_ = nullptr; int64_t ws_wave_cap_ = 0;   // [2][L] in + 2 x [2][Lo] out (host-buffer entry)
+  // whole-track workspaces
+  GrowArray<float2> ws_spec_;
+  GrowArray<float> ws_mask_;
+  GrowArray<float> ws_frames_;
+  GrowArray<float> ws_wave_;   // [2][L] in + 2 x [2][Lo] out (host-buffer entry)
   float* ws_norm_ = nullptr;            // [4] floats: absmax, lexmax-abs
   unsigned long long* ws_lex_ = nullptr;
   unsigned int* ws_img_range_ = nullptr;   // [4] min / max keys of the spectrogram image pass (first use)
-  unsigned char* ws_img_ = nullptr; int64_t ws_img_cap_ = 0;   // two [bins][T][3] images (host-buffer entry)
-  double* ws_val_ = nullptr; int64_t ws_val_cap_ = 0;   // per-slice partial sums of the validation loss
+  GrowArray<unsigned char> ws_img_;   // two [bins][T][3] images (host-buffer entry)
+  GrowArray<double> ws_val_;   // per-slice partial sums of the validation loss
 
   // the high-band BaseNets of stages 1-2 run on their own stream next to the low-band chain (independent until
   // stage 3, lib/nets.py:88-99); disabled while per-kernel profiling is on so event timings stay per-kernel
@@ -209,12 +267,22 @@ class Engine {
   ConvLayer bridge1_, bridge2_;
   float* out_w_ = nullptr;     // [2][nout]
 
-  void* dalloc(size_t bytes);
-  Buffer make_buffer(int N, int H, int W, int C, int pad_w = 0);
+  // zero-filled allocation in `arena`, holding a copy of host[0, bytes) when host is given; nullptr (err set) on failure
+  void* dalloc(Arena& arena, size_t bytes, const void* host = nullptr);
+  Buffer make_buffer(Arena& arena, int N, int H, int W, int C, int pad_w = 0);
   bool need(const std::string& key, std::initializer_list<int64_t> shape, const HostTensor** out);
   // H x W: the layer's output maps, from which tc_prepare chooses its kernel
   bool make_conv(ConvLayer& L, const std::string& prefix, const std::vector<int>& perm, int cin_pad, int k, int stride,
                  int dh, int dw, int act, int H, int W);
+  // Packs OIHW weights w [Cout][Cin][L.k][L.k], output channel co times scale[co] (in double, rounded to float once),
+  // to L.w_host [tap][CinPad][CoutPad] with CinPad = perm.size(): packed input channel pc holds channel perm[pc], or
+  // zeros where that is -1.  Sets L's channel counts and uploads the weights and the bias [Cout] to L.w / L.bias.
+  bool pack_conv(ConvLayer& L, Arena& arena, const float* w, int Cout, int Cin, const double* scale, const float* bias,
+                 const std::vector<int>& perm);
+  // test hooks: pack_conv of the caller's device weights / bias, unscaled
+  bool debug_weights(ConvLayer& L, Arena& arena, const float* w, const float* bias, int Cout, int Cin,
+                     const std::vector<int>& perm, cudaStream_t s);
+  bool to_nchw(const ActView& v, int C, float* y_nchw, cudaStream_t s);
   bool build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, const std::vector<int>& in_perm, int cin_pad,
                      int n, int H, int W, int nin_lstm, int nout_lstm);
   bool run_conv(ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, const ActView* up_src = nullptr,
@@ -232,7 +300,7 @@ class Engine {
 };
 
 // conv_tc.cu: plans L.tc for output maps of H x W (left null when the layer stays on the CUDA-core kernel)
-bool tc_prepare(ConvLayer& L, int H, int W, std::string& err, std::vector<void*>& allocs);
+bool tc_prepare(ConvLayer& L, int H, int W, std::string& err);
 cudaError_t tc_launch(ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, std::string& err,
                       const ActView* up_src = nullptr, const ActView* extra = nullptr);
 

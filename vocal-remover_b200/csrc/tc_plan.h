@@ -30,8 +30,8 @@ struct TcConv {
   unsigned long long kmask = ~0ull;   // bit g: input channels [8g, 8g+8) carry a non-zero weight (rows and halo)
   // weights, hi plane then lo plane: generic / halo [2][n_tiles*BN][taps*CinPad] (tap-major K), rows
   // [2][n_tiles*3*BN][3*CinPad] (the three kh taps of an N tile stacked along N, kw-major K)
-  bf16* w_planes = nullptr;
-  float* bias = nullptr;   // [n_tiles*BN]
+  DevPtr<bf16> w_planes;
+  DevPtr<float> bias;   // [n_tiles*BN]
   CUtensorMap map_b;
   std::map<ViewKey, CUtensorMap> map_a;
   // the row kernel can produce the leading up_C channels of its input as the x2 upsample of a half-resolution tensor
