@@ -138,6 +138,16 @@ VR_API int vr_separate_wave_host_images(vr_ctx* ctx, const float* wave_host, int
 VR_API int vr_spec_image(vr_ctx* ctx, const void* spec, const float* mask, int64_t T, uint8_t* img_a, uint8_t* img_b,
                          void* stream);
 
+/* The vocal JPG of the dataset inspection tool (lib/dataset.py:280-287): spectrogram_to_image(v_mag) with
+ * v_mag = |X| - |y|, kept where v_mag > |y| (zero elsewhere), for the mixture spec_x and instruments spec_y, both
+ * device complex64 [2][bins][T].  img: device uint8 [bins][T][3], levels, min / max and constant-array rule as in
+ * vr_spec_image.                                                                                              */
+VR_API int vr_vocal_image(vr_ctx* ctx, const void* spec_x, const void* spec_y, int64_t T, uint8_t* img, void* stream);
+
+/* v_spec = X_spec - y_spec of the pair check (lib/spec_utils.py:186): out = a - b elementwise over the device
+ * complex64 [2][bins][T] arrays a, b, out (IEEE fp32 subtraction, numpy's bits).                               */
+VR_API int vr_spec_sub(vr_ctx* ctx, const void* a, const void* b, int64_t T, void* out, void* stream);
+
 /* train.py:108-134 validate_epoch over lib/dataset.py:220-248 make_validation_set, one track pair:
  * window_sums[j], j < ceil(T/roi), = sum over (2, bins, roi) of |mask*|X|/coef - |y|/coef| for patch j,
  * coef = max(max|X|, max|y|) written to *coef_out (device float, may be NULL).

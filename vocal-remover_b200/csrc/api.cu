@@ -198,6 +198,16 @@ int vr_spec_image(vr_ctx* ctx, const void* spec, const float* mask, int64_t T, u
   return done(ctx, ctx->eng->spec_image((const float2*)spec, mask, T, img_a, img_b, (cudaStream_t)stream));
 }
 
+int vr_vocal_image(vr_ctx* ctx, const void* spec_x, const void* spec_y, int64_t T, uint8_t* img, void* stream) {
+  CHECK_CTX(ctx);
+  return done(ctx, ctx->eng->vocal_image((const float2*)spec_x, (const float2*)spec_y, T, img, (cudaStream_t)stream));
+}
+
+int vr_spec_sub(vr_ctx* ctx, const void* a, const void* b, int64_t T, void* out, void* stream) {
+  CHECK_CTX(ctx);
+  return done(ctx, ctx->eng->spec_sub((const float2*)a, (const float2*)b, T, (float2*)out, (cudaStream_t)stream));
+}
+
 int vr_validation_loss(vr_ctx* ctx, const void* spec_x, const void* spec_y, int64_t T, float* coef_out,
                        double* window_sums, void* stream) {
   CHECK_CTX(ctx);

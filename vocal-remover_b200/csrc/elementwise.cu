@@ -477,7 +477,8 @@ cudaError_t launch_apply_mask(const float2* spec, const float* mask, int64_t n, 
 
 // ------------------------------------------------------------------------------------------------
 // --output_image (reference spectrogram_to_image, magnitude mode): log10(a^2 + 1e-8) per (channel, bin, frame) with
-// a = m|X| (instruments), (1-m)|X| (vocals) or |X| (no mask), scaled to [0, 255] by the min / max over the whole stem.
+// a = m|X| (instruments), (1-m)|X| (vocals), |X| (no mask) or the dataset tool's vocal residual of a track pair
+// (VocalLevels), scaled to [0, 255] by the min / max over the whole stem.
 // Every step is a separately rounded fp32 operation (no fma contraction), as numpy's float32 arithmetic is; |X| and
 // log10 are evaluated in fp64 and rounded once, which gives the correctly rounded fp32 results of the host's hypotf /
 // log10f where CUDA's fp32 versions may be 1-2 ulp off and move a pixel across a truncation boundary.
@@ -485,26 +486,51 @@ __device__ __forceinline__ float log_level(float a) {
   return (float)log10((double)__fadd_rn(__fmul_rn(a, a), 1e-8f));
 }
 
-__device__ __forceinline__ void image_levels(float2 x, const float* mask, int64_t i, float& la, float& lb) {
-  const float mag = (float)sqrt(fma((double)x.x, (double)x.x, (double)x.y * (double)x.y));
-  float a = mag, b = 0.f;
-  if (mask) {
-    const float m = mask[i];
-    a = __fmul_rn(m, mag);
-    b = __fmul_rn(__fsub_rn(1.f, m), mag);
-  }
-  la = log_level(a);
-  lb = log_level(b);
+__device__ __forceinline__ float image_mag(float2 x) {
+  return (float)sqrt(fma((double)x.x, (double)x.x, (double)x.y * (double)x.y));
 }
+
+// The source of the image kernels, a compile-time parameter: the levels la (image a) and lb (image b) of element i of
+// the [2][plane] inputs `spec` and `aux`, and whether image b is made.
+// spectrogram_to_image of mask * spec and (1 - mask) * spec, or of spec itself when mask == nullptr
+struct MaskedLevels {
+  using Aux = float;
+  __device__ static bool two(const float* mask) { return mask != nullptr; }
+  __device__ static void levels(const float2* spec, const float* mask, int64_t i, float& la, float& lb) {
+    const float mag = image_mag(spec[i]);
+    float a = mag, b = 0.f;
+    if (mask) {
+      const float m = mask[i];
+      a = __fmul_rn(m, mag);
+      b = __fmul_rn(__fsub_rn(1.f, m), mag);
+    }
+    la = log_level(a);
+    lb = log_level(b);
+  }
+};
+
+// the dataset tool's vocal residual (reference lib/dataset.py:280-287) of mixture x = spec and instruments y = aux:
+// v = |x| - |y|, then v *= (v > |y|), one image
+struct VocalLevels {
+  using Aux = float2;
+  __device__ static bool two(const float2*) { return false; }
+  __device__ static void levels(const float2* x, const float2* y, int64_t i, float& la, float& lb) {
+    const float my = image_mag(y[i]);
+    const float v = __fsub_rn(image_mag(x[i]), my);
+    la = log_level(__fmul_rn(v, v > my ? 1.f : 0.f));
+    lb = 0.f;
+  }
+};
 
 // range[0..3] = {~key(min a), key(max a), ~key(min b), key(max b)} (order_key above, zero-initialised): atomicMax only,
 // which is order-independent, so the result does not depend on scheduling.  NaN levels do not take part.
-__global__ void image_range_kernel(const float2* __restrict__ spec, const float* __restrict__ mask, int64_t n,
-                                   unsigned int* range) {
+template <class Src>
+__global__ void image_range_kernel(const float2* __restrict__ spec, const typename Src::Aux* __restrict__ aux,
+                                   int64_t n, unsigned int* range) {
   unsigned int k[4] = {0u, 0u, 0u, 0u};
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     float la, lb;
-    image_levels(spec[i], mask, i, la, lb);
+    Src::levels(spec, aux, i, la, lb);
     if (la == la) {
       k[0] = max(k[0], ~order_key(la));
       k[1] = max(k[1], order_key(la));
@@ -521,7 +547,7 @@ __global__ void image_range_kernel(const float2* __restrict__ spec, const float*
   if ((threadIdx.x & 31) == 0) {
     atomicMax(range + 0, k[0]);
     atomicMax(range + 1, k[1]);
-    if (mask) {
+    if (Src::two(aux)) {
       atomicMax(range + 2, k[2]);
       atomicMax(range + 3, k[3]);
     }
@@ -548,23 +574,24 @@ __device__ __forceinline__ void image_scale(const unsigned int* range, float& lo
 }
 
 // one thread per (bin, frame): img[bin][t][3] = {max(qL, qR), qL, qR}
-__global__ void image_pixels_kernel(const float2* __restrict__ spec, const float* __restrict__ mask, int64_t plane,
-                                    const unsigned int* __restrict__ range, unsigned char* __restrict__ img_a,
-                                    unsigned char* __restrict__ img_b) {
+template <class Src>
+__global__ void image_pixels_kernel(const float2* __restrict__ spec, const typename Src::Aux* __restrict__ aux,
+                                    int64_t plane, const unsigned int* __restrict__ range,
+                                    unsigned char* __restrict__ img_a, unsigned char* __restrict__ img_b) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= plane) return;
   float lo_a, s_a, lo_b = 0.f, s_b = 0.f;
   image_scale(range, lo_a, s_a);
-  if (mask) image_scale(range + 2, lo_b, s_b);
+  if (Src::two(aux)) image_scale(range + 2, lo_b, s_b);
   float la0, lb0, la1, lb1;
-  image_levels(spec[i], mask, i, la0, lb0);
-  image_levels(spec[plane + i], mask, plane + i, la1, lb1);
+  Src::levels(spec, aux, i, la0, lb0);
+  Src::levels(spec, aux, plane + i, la1, lb1);
   unsigned char l = image_pixel(la0, lo_a, s_a), r = image_pixel(la1, lo_a, s_a);
   unsigned char* p = img_a + 3 * i;
   p[0] = l > r ? l : r;
   p[1] = l;
   p[2] = r;
-  if (mask) {
+  if (Src::two(aux)) {
     l = image_pixel(lb0, lo_b, s_b);
     r = image_pixel(lb1, lo_b, s_b);
     p = img_b + 3 * i;
@@ -574,16 +601,42 @@ __global__ void image_pixels_kernel(const float2* __restrict__ spec, const float
   }
 }
 
-cudaError_t launch_spec_image(const float2* spec, const float* mask, int64_t plane, unsigned int* range,
-                              unsigned char* img_a, unsigned char* img_b, cudaStream_t stream) {
+// the range pass over both channels, then the pixel pass
+template <class Src>
+static cudaError_t launch_image(const float2* spec, const typename Src::Aux* aux, int64_t plane, unsigned int* range,
+                                unsigned char* img_a, unsigned char* img_b, cudaStream_t stream) {
   cudaError_t e = cudaMemsetAsync(range, 0, 4 * sizeof(unsigned int), stream);
   if (e != cudaSuccess || plane == 0) return e;
   const int64_t n = 2 * plane;
   const int grid = (int)(((n + 255) / 256) < 132 * 8 ? ((n + 255) / 256) : 132 * 8);
-  image_range_kernel<<<grid, 256, 0, stream>>>(spec, mask, n, range);
+  image_range_kernel<Src><<<grid, 256, 0, stream>>>(spec, aux, n, range);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  image_pixels_kernel<<<(unsigned)((plane + 255) / 256), 256, 0, stream>>>(spec, mask, plane, range, img_a, img_b);
+  image_pixels_kernel<Src><<<(unsigned)((plane + 255) / 256), 256, 0, stream>>>(spec, aux, plane, range, img_a, img_b);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_spec_image(const float2* spec, const float* mask, int64_t plane, unsigned int* range,
+                              unsigned char* img_a, unsigned char* img_b, cudaStream_t stream) {
+  return launch_image<MaskedLevels>(spec, mask, plane, range, img_a, img_b, stream);
+}
+
+cudaError_t launch_vocal_image(const float2* spec_x, const float2* spec_y, int64_t plane, unsigned int* range,
+                               unsigned char* img, cudaStream_t stream) {
+  return launch_image<VocalLevels>(spec_x, spec_y, plane, range, img, nullptr, stream);
+}
+
+__global__ void spec_sub_kernel(const float2* __restrict__ a, const float2* __restrict__ b, int64_t n,
+                                float2* __restrict__ out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float2 x = a[i], y = b[i];
+  out[i] = make_float2(__fsub_rn(x.x, y.x), __fsub_rn(x.y, y.y));
+}
+
+cudaError_t launch_spec_sub(const float2* a, const float2* b, int64_t n, float2* out, cudaStream_t stream) {
+  if (n == 0) return cudaSuccess;
+  spec_sub_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(a, b, n, out);
   return cudaGetLastError();
 }
 

@@ -799,6 +799,29 @@ bool Engine::spec_image(const float2* spec, const float* mask, int64_t T, unsign
   });
 }
 
+bool Engine::vocal_image(const float2* spec_x, const float2* spec_y, int64_t T, unsigned char* img, cudaStream_t s) {
+  cudaSetDevice(cfg_.device);
+  if (T < 0 || !spec_x || !spec_y || !img) {
+    err = "vocal_image: needs spec_x, spec_y, img and T >= 0";
+    return false;
+  }
+  if (!ws_img_range_ && !(ws_img_range_ = (unsigned int*)dalloc(arena_, sizeof(unsigned int) * 4))) return false;
+  return timed("vocal_image", 2, 1, bins(), (int)T, s, [&] {
+    return ck(launch_vocal_image(spec_x, spec_y, (int64_t)bins() * T, ws_img_range_, img, s), "vocal_image");
+  });
+}
+
+bool Engine::spec_sub(const float2* a, const float2* b, int64_t T, float2* out, cudaStream_t s) {
+  cudaSetDevice(cfg_.device);
+  if (T < 0 || !a || !b || !out) {
+    err = "spec_sub: needs a, b, out and T >= 0";
+    return false;
+  }
+  return timed("spec_sub", 1, 1, bins(), (int)T, s, [&] {
+    return ck(launch_spec_sub(a, b, (int64_t)2 * bins() * T, out, s), "spec_sub");
+  });
+}
+
 // train.py:108-134 validate_epoch over lib/dataset.py:220-248 make_validation_set, one pair: coef = max(max|X|, max|y|),
 // ceil(T / roi) windows of X / coef padded by make_padding (left = offset) through the net, then the L1 sums of the
 // kept mask frames.  Only the mask workspace is needed (no inverse STFT, so not ensure_ws's frame workspace).

@@ -187,6 +187,9 @@ class Engine {
   // spectrogram images of mask * spec and (1 - mask) * spec (mask == nullptr: of spec itself, img_b unused)
   bool spec_image(const float2* spec, const float* mask, int64_t T, unsigned char* img_a, unsigned char* img_b,
                   cudaStream_t s);
+  // dataset tools: image of the vocal residual of a track pair, and out = a - b; see include/vr_b200.h
+  bool vocal_image(const float2* spec_x, const float2* spec_y, int64_t T, unsigned char* img, cudaStream_t s);
+  bool spec_sub(const float2* a, const float2* b, int64_t T, float2* out, cudaStream_t s);
   bool normaliser(const float2* spec, int64_t T, int mode, float* out, cudaStream_t s);
   // validation loss of one (mixture, instruments) pair; see vr_validation_loss in include/vr_b200.h
   bool validation_loss(const float2* spec_x, const float2* spec_y, int64_t T, float* coef_out, double* window_sums,

@@ -56,6 +56,12 @@ cudaError_t launch_apply_mask(const float2* spec, const float* mask, int64_t n, 
 // range: 4 unsigned ints of scratch
 cudaError_t launch_spec_image(const float2* spec, const float* mask, int64_t plane, unsigned int* range,
                               unsigned char* img_a, unsigned char* img_b, cudaStream_t stream);
+// the same image of the vocal residual v = |X| - |y|, kept where v > |y| (reference lib/dataset.py:280-287), of
+// spec_x / spec_y [2][plane] -> img [plane][3]; range: 4 unsigned ints of scratch
+cudaError_t launch_vocal_image(const float2* spec_x, const float2* spec_y, int64_t plane, unsigned int* range,
+                               unsigned char* img, cudaStream_t stream);
+// out[i] = a[i] - b[i] over n complex elements
+cudaError_t launch_spec_sub(const float2* a, const float2* b, int64_t n, float2* out, cudaStream_t stream);
 // validation loss (reference train.py:108-134): window_sums[j] = sum over (channel, bin, frames [j*roi, (j+1)*roi) of
 // the track) of |mask * |X| / coef - |y| / coef|, spec_x / spec_y [2][bins][T], mask [2][bins][n_windows * roi],
 // *coef on the device; partial: validation_l1_scratch(n_windows) doubles of scratch

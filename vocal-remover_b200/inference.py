@@ -179,7 +179,7 @@ class Separator(object):
 
 MODEL_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'models')
 DEFAULT_MODEL_PATH = os.path.join(MODEL_DIR, 'baseline.pth')
-JPEG_MAX_WIDTH = 65500   # widest image the JPEG encoder accepts; one pixel per STFT frame
+JPEG_MAX_WIDTH = utils.JPEG_MAX_WIDTH
 
 
 def main():

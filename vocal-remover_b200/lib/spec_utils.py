@@ -4,7 +4,24 @@ wave_to_spectrogram / spectrogram_to_wave keep the reference signatures and nump
 contract (lib/spec_utils.py:26-31, 157-165) but run the framed FFT / inverse FFT + overlap-add on the
 GPU through libvr_b200.so (csrc/fft.cu) instead of librosa on the host.  spectrogram_to_image (--output_image) builds
 its uint8 image on the GPU as well (csrc/elementwise.cu).
+
+Run as a script, it is the reference's pair check (lib/spec_utils.py:168-198): one (mixture, instruments) pair is
+loaded at 44.1 kHz and aligned, and test_X / test_y / test_v .jpg and .wav, of the mixture, the instruments and
+their difference v = X - y, are written to the working directory::
+
+    python lib/spec_utils.py <mix> <inst>        (or python -m lib.spec_utils ...)
 """
+import os
+import sys
+
+if __name__ == '__main__' and not __package__:
+    # run as a file: import the package this file belongs to instead of its modules as top-level ones
+    _LIB_DIR = os.path.dirname(os.path.abspath(__file__))
+    if sys.path and os.path.abspath(sys.path[0] or os.curdir) == _LIB_DIR:
+        del sys.path[0]
+    sys.path.insert(0, os.path.dirname(_LIB_DIR))
+    __package__ = 'lib'
+
 import numpy as np
 import torch
 
@@ -99,16 +116,42 @@ def spectrogram_to_image(spec, mode='magnitude'):
     ctx = _spectral_ctx(2 * (bins - 1), bins - 1)
     dev = torch.device('cuda', ctx.device_index)
     with torch.cuda.device(dev):
-        if on_device:
-            if spec.device != dev:
-                raise ValueError('spectrogram_to_image: spec is on %s, the spectral functions use %s' % (spec.device, dev))
-            d_spec = spec.to(torch.complex64).contiguous()
-        else:
-            d_spec = torch.from_numpy(np.ascontiguousarray(np.asarray(spec, dtype=np.complex64))).to(dev)
+        d_spec = _to_device(spec, dev, 'spectrogram_to_image')
         img = torch.empty((bins, T, 3), dtype=torch.uint8, device=dev)
         ctx.check(ctx.lib.vr_spec_image(ctx.handle, _native.ptr(d_spec), None, T, _native.ptr(img), None,
                                         _native.stream_ptr()), 'vr_spec_image')
         return img if on_device else img.cpu().numpy()
+
+
+def _to_device(spec, dev, what):
+    """A contiguous complex64 copy (or the tensor itself) of ``spec`` on ``dev``."""
+    if torch.is_tensor(spec):
+        if spec.device != dev:
+            raise ValueError('%s: spec is on %s, the spectral functions use %s' % (what, spec.device, dev))
+        return spec.to(torch.complex64).contiguous()
+    return torch.from_numpy(np.ascontiguousarray(np.asarray(spec, dtype=np.complex64))).to(dev)
+
+
+def spectrogram_difference(a, b):
+    """complex (2, bins, T) a - b, the pair check's v_spec = X_spec - y_spec (lib/spec_utils.py:186), on the GPU
+    (vr_spec_sub): complex64 with numpy's bits.  Numpy arrays give a numpy array, CUDA tensors a CUDA tensor."""
+    on_device = torch.is_tensor(a)
+    if torch.is_tensor(b) != on_device:
+        raise TypeError('spectrogram_difference: a and b must both be numpy arrays or both CUDA tensors')
+    if not on_device:
+        a, b = np.asarray(a), np.asarray(b)
+    if a.ndim != 3 or a.shape[0] != 2 or tuple(a.shape) != tuple(b.shape):
+        raise ValueError('spectrogram_difference: a and b must both have shape (2, bins, T), got %s and %s'
+                         % (tuple(a.shape), tuple(b.shape)))
+    bins, T = a.shape[1], a.shape[2]
+    ctx = _spectral_ctx(2 * (bins - 1), bins - 1)
+    dev = torch.device('cuda', ctx.device_index)
+    with torch.cuda.device(dev):
+        d_a, d_b = (_to_device(s, dev, 'spectrogram_difference') for s in (a, b))
+        out = torch.empty((2, bins, T), dtype=torch.complex64, device=dev)
+        ctx.check(ctx.lib.vr_spec_sub(ctx.handle, _native.ptr(d_a), _native.ptr(d_b), T, _native.ptr(out),
+                                      _native.stream_ptr()), 'vr_spec_sub')
+        return out if on_device else out.cpu().numpy()
 
 
 def artifact_weights(frame_min, thres=0.05, min_range=64, fade_size=32):
@@ -234,3 +277,47 @@ def cache_or_load(mix_path, inst_path, sr, hop_length, n_fft):
         np.save(inst_cache_path, y.transpose(2, 0, 1))
     assert X.shape == y.shape
     return X, y, mix_cache_path, inst_cache_path
+
+
+def main(argv=None):
+    """The reference's pair check: test_X / test_y / test_v .jpg and .wav of one aligned pair, in the working
+    directory."""
+    import argparse
+    from . import audio_io, utils
+    p = argparse.ArgumentParser(prog='lib/spec_utils.py',
+                                description='aligns one (mixture, instruments) pair and writes test_X, test_y and '
+                                            'test_v (= X - y) .jpg and .wav to the working directory')
+    p.add_argument('mix')
+    p.add_argument('inst')
+    args = p.parse_args(argv)
+
+    # missing requirements fail before any file is written
+    try:
+        import cv2  # noqa: F401  (the JPEG encoder of lib/utils.imwrite)
+    except ImportError as e:
+        raise ImportError('the pair check needs OpenCV (the cv2 module) to encode the JPGs: %s' % e) from e
+    if not torch.cuda.is_available():
+        raise RuntimeError('no CUDA device: the H100 build of vocal-remover has no CPU path')
+
+    sr, hop_length, n_fft = 44100, 1024, 2048
+    X, _ = audio_io.load(args.mix, sr=sr, mono=False, dtype=np.float32, device=_DEVICE_INDEX)
+    y, _ = audio_io.load(args.inst, sr=sr, mono=False, dtype=np.float32, device=_DEVICE_INDEX)
+    X, y = align_wave_head_and_tail(X, y, sr)
+    X_spec = wave_to_spectrogram(X, hop_length, n_fft)
+    y_spec = wave_to_spectrogram(y, hop_length, n_fft)
+    v_spec = spectrogram_difference(X_spec, y_spec)
+
+    specs = (('X', X_spec), ('y', y_spec), ('v', v_spec))
+    if X_spec.shape[2] > utils.JPEG_MAX_WIDTH:
+        # the encoder refuses the images: no JPG, the WAVs are still written
+        print('skipping test_X.jpg, test_y.jpg and test_v.jpg: {} frames exceed the {}-pixel width limit of '
+              'JPEG'.format(X_spec.shape[2], utils.JPEG_MAX_WIDTH))
+    else:
+        for name, spec in specs:
+            utils.imwrite('test_{}.jpg'.format(name), spectrogram_to_image(spec))
+    for name, spec in specs:
+        audio_io.write('test_{}.wav'.format(name), spectrogram_to_wave(spec, hop_length).T, sr)
+
+
+if __name__ == '__main__':
+    main()

@@ -7,6 +7,8 @@ import os
 
 import numpy as np
 
+JPEG_MAX_WIDTH = 65500   # widest image the JPEG encoder accepts; one pixel per STFT frame
+
 
 def imread(filename, flags=None, dtype=np.uint8):
     """Decodes an image file (cv2.IMREAD_COLOR by default); None if it cannot be read or decoded."""
