@@ -212,11 +212,9 @@ VR_API int vr_debug_decoder(vr_ctx* ctx, const float* low, int32_t N, int32_t Cl
  * one, key 3 = 2 / 3 makes the halo-tile kernel use MB = 1 / 2, key 6 = 1 (default) skips channel groups whose weights
  * are all zero.  Returns -1 for any other key.                                                                      */
 VR_API int vr_debug_set(int32_t key, int32_t value);
-/* Internal activation of the last forward as NCHW float32; dims receives [N,C,H,W].                       */
 /* timeline of CTA 0 of the last row-kernel launch made with vr_debug_set(0, 1): 3 roles x 2048 events x 3 clock64 stamps
  * (unused / TMA producer / interpolation warp 0), copied to HOST memory; returns the number of values or -1 */
 VR_API int64_t vr_debug_trace(uint64_t* host_out, int64_t capacity);
-VR_API int vr_debug_read(vr_ctx* ctx, const char* what, float* out, int64_t capacity, int64_t* dims, void* stream);
 
 #ifdef __cplusplus
 }

@@ -329,9 +329,4 @@ int64_t vr_debug_trace(uint64_t* host_out, int64_t capacity) {
   return vr::tc_rows_read_trace((unsigned long long*)host_out, (long long)capacity);
 }
 
-int vr_debug_read(vr_ctx* ctx, const char* what, float* out, int64_t capacity, int64_t* dims, void* stream) {
-  CHECK_CTX(ctx);
-  return done(ctx, ctx->eng->debug_read(what, out, capacity, dims, (cudaStream_t)stream));
-}
-
 }  // extern "C"

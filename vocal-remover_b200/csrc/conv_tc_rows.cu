@@ -542,13 +542,17 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
 }
 
 // ------------------------------------------------------------------------------------------------
-// up_src != nullptr: the first up_src->C channels of `in` are NOT read; they are produced inside the kernel as the
-// bilinear x2 upsample of *up_src (half resolution, tc.fuses_upsample(up_src->C)).
+// up_src != nullptr: the first up_src->C reduction channels are produced inside the kernel as the bilinear x2 upsample
+// of *up_src (half resolution, tc.fuses_upsample(up_src->C)); `in` holds only the channels after them.
 // extra != nullptr: the LAST channel chunk is read from *extra (channels [0, extra->C), zero-filled up to the chunk).
 cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const ActView& out, cudaStream_t s,
                            std::string& err, const ActView* up_src, const ActView* extra) {
   if (up_src && (!tc.fuses_upsample(up_src->C) || up_src->H * 2 != in.H || up_src->W * 2 != in.W || up_src->sw % 8)) {
     err = "tc_rows_launch: fused upsample needs a half-resolution source of 32k channels";
+    return cudaErrorInvalidValue;
+  }
+  if (up_src && up_src->C + in.C > tc.CinPad) {
+    err = "tc_rows_launch: with a fused upsample the input must hold only the channels after the up-sampled ones";
     return cudaErrorInvalidValue;
   }
   if (extra && (extra->H != in.H || extra->W != in.W || extra->N != in.N || extra->C > tc.KB)) {
@@ -577,9 +581,7 @@ cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   p.l_chunk = extra ? tc.chunks - 1 : -1;
   p.kmask = g_debug.kskip == 1 ? tc.kmask : ~0ull;   // VR_KSKIP=0 issues the all-zero-weight channel groups too
   if (up_src) {
-    // `in` is either the whole concat buffer (its first up_src->C channels are then never read) or only the skip
-    // tensor, which starts at reduction index up_src->C
-    if (in.C + up_src->C + (extra ? tc.KB : 0) <= tc.CinPad) p.a_c_off = -up_src->C;
+    p.a_c_off = -up_src->C;   // `in` starts at reduction channel up_src->C
     p.up_chunks = up_src->C / 32;
     p.xH = up_src->H; p.xW = up_src->W;
     p.x_hi = up_src->hi; p.x_lo = up_src->lo;

@@ -209,39 +209,6 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
     err = "unsupported geometry: band height and cropsize must be multiples of 16 and nout a multiple of 16";
     return false;
   }
-  // Layouts of the dec1 input (see BaseNetPlan::skip_only in engine.h).  The fused layout needs the row kernel with
-  // dec1's up-sampled half (h, 2n channels) in whole 32-channel chunks.  dec1 is a 3x3 convolution to n channels at
-  // H x W; its weights are packed below, once the layout is known.
-  ConvLayer dec1;
-  dec1.k = 3;
-  dec1.Cout = n;
-  P.skip_only = cfg_.conv_mode == 0 && (2 * n) % 32 == 0 && tc_choose(dec1, H, W) == TC_ROWS;
-  const int lg = 16;   // the lstm channel + 15 zeros keep every slice 32-byte aligned (full-sector 256-bit stores)
-  P.lstm_own = P.skip_only && n % 32 == 0;
-  const int c1 = P.skip_only ? 2 * n + round_up(n, 32) + (P.lstm_own ? lg : 0) : round_up(3 * n + lg, 16);
-  P.e1_off = P.skip_only ? 2 * n : 2 * n + lg;      // position of e1 in dec1's reduction (weight) order
-  P.e1_coff = P.skip_only ? 0 : P.e1_off;           // position of e1 in the cat1 buffer
-  P.lstm_coff = !P.skip_only ? 2 * n : P.lstm_own ? 0 : n;
-  P.cat1 = make_buffer(arena_, Nb, H, W, !P.skip_only ? c1 : P.lstm_own ? n : round_up(n + lg, 32));
-  // 8-channel group: the row kernel's TMA box zero-fills the rest
-  if (P.lstm_own) P.lstm_up = make_buffer(arena_, Nb, H, W, 8);
-  P.t2 = make_buffer(arena_, Nb, H / 2, W / 2, 2 * n);
-  P.cat2 = make_buffer(arena_, Nb, H / 2, W / 2, 6 * n);
-  P.t3 = make_buffer(arena_, Nb, H / 4, W / 4, 4 * n);
-  P.cat3 = make_buffer(arena_, Nb, H / 4, W / 4, 10 * n);
-  P.t4 = make_buffer(arena_, Nb, H / 8, W / 8, 6 * n);
-  P.cat4 = make_buffer(arena_, Nb, H / 8, W / 8, 14 * n);
-  P.t5 = make_buffer(arena_, Nb, H / 16, W / 16, 8 * n);
-  P.e5 = make_buffer(arena_, Nb, H / 16, W / 16, 8 * n);
-  P.pool = make_buffer(arena_, Nb, 1, W / 16, 8 * n);
-  P.f1 = make_buffer(arena_, Nb, 1, W / 16, 8 * n);
-  P.acat = make_buffer(arena_, Nb, H / 16, W / 16, 40 * n);
-  P.ao = make_buffer(arena_, Nb, H / 16, W / 16, 8 * n);
-  P.d4 = make_buffer(arena_, Nb, H / 8, W / 8, 6 * n);
-  P.d3 = make_buffer(arena_, Nb, H / 4, W / 4, 4 * n);
-  P.d2 = make_buffer(arena_, Nb, H / 2, W / 2, P.skip_only ? 2 * n : 2 * n + lg);
-  if (!P.d2.hi || !P.cat1.hi) return false;
-
   if (!make_conv(P.enc1, prefix + ".enc1", in_perm, cin_pad, 3, 1, 1, 1, ACT_RELU, H, W)) return false;
   const int mult[5] = {1, 2, 4, 6, 8};
   for (int i = 0; i < 4; ++i) {
@@ -276,17 +243,44 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
   if (!make_conv(P.dec[2], prefix + ".dec2.conv1", identity_perm(6 * n, 6 * n), 6 * n, 3, 1, 1, 1, ACT_RELU, H / 2,
                  W / 2))
     return false;
+  // dec1 input in the reference: cat[ up(cat[h (2n), lstm (1)]) , e1 (n) ]  (lib/nets.py:38-39, layers.py:52-56),
+  // reduced as [ up(h) 2n | zeros up to Up | e1 n | zeros up to Lp | up(lstm) 1 | 15 zeros ] (BaseNetPlan, engine.h)
+  const int lg = 16;   // the lstm channel + 15 zeros keep every slice 32-byte aligned (full-sector 256-bit stores)
+  const int Up = round_up(2 * n, 32), Lp = round_up(Up + n, 16), c1 = Lp + lg;
   {
-    // dec1 input in the reference: cat[ up(cat[h (2n), lstm (1)]) , e1 (n) ]  (lib/nets.py:38-39, layers.py:52-56)
-    // packed as [ up(h) 2n | up(lstm) 1 | 15 zeros | e1 n | zeros ], or (skip_only) [ up(h) 2n | e1 n | up(lstm) 1 | zeros ]
     std::vector<int> perm((size_t)c1, -1);
     for (int i = 0; i < 2 * n; ++i) perm[(size_t)i] = i;
-    perm[(size_t)(!P.skip_only ? 2 * n : P.lstm_own ? 2 * n + round_up(n, 32) : 2 * n + n)] = 2 * n;
-    for (int i = 0; i < n; ++i) perm[(size_t)(P.e1_off + i)] = 2 * n + 1 + i;
+    for (int i = 0; i < n; ++i) perm[(size_t)(Up + i)] = 2 * n + 1 + i;
+    perm[(size_t)Lp] = 2 * n;
     // (the 64-wide tile was measured on dec1 as well - one N tile instead of two for n = 64 - and is no faster there:
     //  with its single accumulator set the epilogue no longer overlaps the next tile's products)
     if (!make_conv(P.dec[3], prefix + ".dec1.conv1", perm, c1, 3, 1, 1, 1, ACT_RELU, H, W)) return false;
   }
+
+  // activation buffers: the decoders' plans decide what their concat buffers hold
+  P.fused2 = P.dec[2].tc && P.dec[2].tc->fuses_upsample(4 * n);
+  P.fused1 = P.dec[3].tc && P.dec[3].tc->fuses_upsample(Up);
+  P.lstm_own = P.fused1 && n % 32 == 0;
+  const int c1_first = P.fused1 ? Up : 0;   // the first of dec1's reduction channels that cat1 holds
+  P.lstm_coff = Lp - c1_first;
+  P.cat1 = make_buffer(arena_, Nb, H, W, (P.lstm_own ? Lp : c1) - c1_first);
+  if (P.lstm_own) P.lstm_up = make_buffer(arena_, Nb, H, W, 8);
+  P.t2 = make_buffer(arena_, Nb, H / 2, W / 2, 2 * n);
+  P.cat2 = make_buffer(arena_, Nb, H / 2, W / 2, P.fused2 ? 2 * n : 6 * n);
+  P.t3 = make_buffer(arena_, Nb, H / 4, W / 4, 4 * n);
+  P.cat3 = make_buffer(arena_, Nb, H / 4, W / 4, 10 * n);
+  P.t4 = make_buffer(arena_, Nb, H / 8, W / 8, 6 * n);
+  P.cat4 = make_buffer(arena_, Nb, H / 8, W / 8, 14 * n);
+  P.t5 = make_buffer(arena_, Nb, H / 16, W / 16, 8 * n);
+  P.e5 = make_buffer(arena_, Nb, H / 16, W / 16, 8 * n);
+  P.pool = make_buffer(arena_, Nb, 1, W / 16, 8 * n);
+  P.f1 = make_buffer(arena_, Nb, 1, W / 16, 8 * n);
+  P.acat = make_buffer(arena_, Nb, H / 16, W / 16, 40 * n);
+  P.ao = make_buffer(arena_, Nb, H / 16, W / 16, 8 * n);
+  P.d4 = make_buffer(arena_, Nb, H / 8, W / 8, 6 * n);
+  P.d3 = make_buffer(arena_, Nb, H / 4, W / 4, 4 * n);
+  P.d2 = make_buffer(arena_, Nb, H / 2, W / 2, Up);
+  if (!P.d2.hi || !P.cat1.hi) return false;
 
   // ---- LSTM module (lib/layers.py:110-122) ----
   LstmPlan& Q = P.lstm;
@@ -529,27 +523,21 @@ bool Engine::run_conv_inner(ConvLayer& L, const ActView& in, const ActView& out,
   return ck(launch_conv_simt(p, s), L.name.c_str());
 }
 
-bool Engine::run_decoder(ConvLayer& L, const ActView& low, const Buffer& cat, int N, const ActView& out,
+bool Engine::run_decoder(ConvLayer& L, const ActView& low, const Buffer& cat, int N, const ActView& out, bool fused,
                          cudaStream_t s) {
-  const ActView cat_all = cat.all(N);
-  if (L.tc && L.tc->fuses_upsample(low.C))
-    return run_conv(L, cat_all, out, s, &low);   // channels [0, low.C) of cat are produced inside the kernel
-  if (cat.C < low.C + 1) {
-    err = "internal: " + L.name + " was laid out for the fused upsample but the fused kernel is not available";
-    return false;
-  }
+  if (fused) return run_conv(L, cat.all(N), out, s, &low);
   if (!timed("upsample2x", 1, N, cat.H, cat.W, s, [&] { return ck(launch_upsample2x(low, cat.view(N, 0, cat.H, 0, low.C), s), "decoder upsample"); }))
     return false;
-  return run_conv(L, cat_all, out, s);
+  return run_conv(L, cat.all(N), out, s);
 }
 
 bool Engine::run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, int N, cudaStream_t s,
                          cudaStream_t side) {
   const int n = P.n, H = P.H;
   // encoders (lib/nets.py:27-31); each skip tensor is written straight into its decoder's concat buffer
-  ActView e1 = P.cat1.view(N, 0, H, P.e1_coff, n);
+  ActView e1 = P.cat1.view(N, 0, H, P.fused1 ? 0 : P.d2.C, n);   // staged: after up(h), which is as wide as d2
   if (!run_conv(P.enc1, in, e1, s)) return false;
-  ActView e2 = P.cat2.view(N, 0, H / 2, 4 * n, 2 * n);
+  ActView e2 = P.cat2.view(N, 0, H / 2, P.fused2 ? 0 : 4 * n, 2 * n);
   if (!run_conv(P.enc_a[0], e1, P.t2.all(N), s) || !run_conv(P.enc_b[0], P.t2.all(N), e2, s)) return false;
   ActView e3 = P.cat3.view(N, 0, H / 4, 6 * n, 4 * n);
   if (!run_conv(P.enc_a[1], e2, P.t3.all(N), s) || !run_conv(P.enc_b[1], P.t3.all(N), e3, s)) return false;
@@ -577,20 +565,20 @@ bool Engine::run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, 
   // The LSTM branch's 1x1 input convolution (2n -> 1, lib/layers.py:112,126) is one dot product per pixel of dec2's
   // output: the row kernel's epilogue accumulates it from the fp32 activations it is about to store.
   LstmPlan& Q = P.lstm;
-  const ActView d2v = P.d2.view(N, 0, H / 2, 0, 2 * n);
+  const ActView d2 = P.d2.all(N), h = P.d2.view(N, 0, H / 2, 0, 2 * n);
   const bool dot_fused = P.dec[2].tc && P.dec[2].tc->kind == TC_ROWS;
   if (dot_fused) {
     if (!ck(cudaMemsetAsync(Q.l0, 0, sizeof(float) * (size_t)N * Q.bins * Q.T, s), "lstm conv clear")) return false;
     P.dec[2].dot_w = Q.conv_w;
     P.dec[2].dot_out = Q.l0;
   }
-  const bool dec2_ok = run_decoder(P.dec[2], P.d3.all(N), P.cat2, N, d2v, s);
+  const bool dec2_ok = run_decoder(P.dec[2], P.d3.all(N), P.cat2, N, h, P.fused2, s);
   P.dec[2].dot_w = nullptr;
   P.dec[2].dot_out = nullptr;
   if (!dec2_ok) return false;
-  // LSTM branch -> channel 2n of d2 (lib/nets.py:38, lib/layers.py:124-133).  Its 128-step recurrence keeps only
-  // 2N CTAs busy, so when a side stream is free (stage 3) it runs there while the main stream upsamples the 2n
-  // convolution channels of d2; only the LSTM channel's 16-channel group is upsampled after the join.
+  // LSTM branch -> up(lstm), dec1's last reduction group (lib/nets.py:38, lib/layers.py:124-133).  Its 128-step
+  // recurrence keeps only 2N CTAs busy, so when a side stream is free (stage 3) it runs there while the main stream
+  // upsamples h for a staged dec1.
   const bool overlap = side != nullptr && !profiling_;
   cudaStream_t sl = overlap ? side : s;
   if (overlap) {
@@ -598,7 +586,7 @@ bool Engine::run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, 
       return false;
   }
   if (!dot_fused &&
-      !timed("lstm.inconv", 1, N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_inconv(d2v, Q.conv_w, Q.l0, sl), "lstm conv"); }))
+      !timed("lstm.inconv", 1, N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_inconv(h, Q.conv_w, Q.l0, sl), "lstm conv"); }))
     return false;
   if (!timed("lstm.input_projection", 1, N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_input_projection(Q.l0, Q.conv_bias, Q.wih, Q.bih, Q.xp, N, Q.T, Q.bins, 8 * Q.hid, sl), "lstm input projection"); }))
     return false;
@@ -607,51 +595,24 @@ bool Engine::run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, 
   // the branch output at half resolution: fp32 plane y[bin][n][t]
   if (!timed("lstm.dense", 1, N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_dense(Q.hs, Q.wd, Q.dscale, Q.dshift, N * Q.T, 2 * Q.hid, Q.bins, Q.y, sl), "lstm dense"); }))
     return false;
-  if (!P.skip_only &&   // staged layout: it becomes channel 2n of d2 and is up-sampled together with h
-      !timed("lstm.to_channel", 1, N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_plane_to_channel(Q.y, N, Q.T, Q.bins, P.d2.all(N), 2 * n, sl), "lstm channel"); }))
+  const ActView up_lstm = P.lstm_own ? P.lstm_up.all(N) : P.cat1.view(N, 0, H, P.lstm_coff, 16);
+  if (!timed("lstm.upsample2x", 1, N, H, P.W, sl, [&] { return ck(launch_upsample2x_c1(Q.y, Q.bins, Q.T, Q.T, (int64_t)N * Q.T, up_lstm, sl), "lstm upsample"); }))
     return false;
-  if (P.skip_only) {
-    // fused layout: up(lstm) -> its 16-channel group of cat1 / lstm_up (small kernel on the LSTM's stream), then the row
-    // kernel reads [e1 | up(lstm)] by TMA and produces up(h) itself from d2
-    const ActView lstm_full = P.lstm_own ? P.lstm_up.all(N) : P.cat1.view(N, 0, H, P.lstm_coff, 16);
-    if (!timed("lstm.upsample2x", 1, N, H, P.W, sl, [&] { return ck(launch_upsample2x_c1(Q.y, Q.bins, Q.T, Q.T, (int64_t)N * Q.T, lstm_full, sl), "lstm upsample"); }))
-      return false;
-    if (overlap) {
-      if (!ck(cudaEventRecord(ev_lstm_join_, side), "lstm join") || !ck(cudaStreamWaitEvent(s, ev_lstm_join_, 0), "lstm join"))
-        return false;
-    }
-    const ActView h = P.d2.all(N);
-    return run_conv(P.dec[3], P.cat1.all(N), out, s, &h, P.lstm_own ? &lstm_full : nullptr);
-  }
-  // staged layout: dec1 on cat[up(h, lstm), e1] (lib/nets.py:39)
-  const int upc = P.e1_off;   // channels of d2 that are upsampled: 2n conv channels + the LSTM channel group
+  // dec1 on cat[up(cat[h, lstm]), e1] (lib/nets.py:39): a fused dec1 produces up(d2) itself
+  if (!P.fused1 &&
+      !timed("upsample2x", 1, N, H, P.W, s, [&] { return ck(launch_upsample2x(h, P.cat1.view(N, 0, H, 0, 2 * n), s), "up1"); }))
+    return false;
   if (overlap) {
-    // Only stage 3 has a side stream, and its n is a multiple of 16: 2n fills whole 32-channel chunks, so a dec1 on the
-    // row kernel (the only one that fuses the upsample) always got the fused layout from build_basenet.
-    if (P.dec[3].tc && P.dec[3].tc->fuses_upsample(P.d2.C)) {
-      err = "internal: " + P.dec[3].name + " fuses its upsample but has the staged layout";
+    if (!ck(cudaEventRecord(ev_lstm_join_, side), "lstm join") || !ck(cudaStreamWaitEvent(s, ev_lstm_join_, 0), "lstm join"))
       return false;
-    }
-    if (!ck(cudaEventRecord(ev_lstm_join_, side), "lstm join")) return false;
-    if (!timed("upsample2x", 1, N, H, P.W, s, [&] {
-          return ck(launch_upsample2x(P.d2.view(N, 0, H / 2, 0, 2 * n), P.cat1.view(N, 0, H, 0, 2 * n), s), "up1");
-        }))
-      return false;
-    if (!ck(cudaStreamWaitEvent(s, ev_lstm_join_, 0), "lstm join")) return false;
-    if (!timed("upsample2x", 1, N, H, P.W, s, [&] {
-          return ck(launch_upsample2x(P.d2.view(N, 0, H / 2, 2 * n, upc - 2 * n), P.cat1.view(N, 0, H, 2 * n, upc - 2 * n), s), "up1 lstm");
-        }))
-      return false;
-    return run_conv(P.dec[3], P.cat1.all(N), out, s);
   }
-  return run_decoder(P.dec[3], P.d2.all(N), P.cat1, N, out, s);
+  return run_conv(P.dec[3], P.cat1.all(N), out, s, P.fused1 ? &d2 : nullptr, P.lstm_own ? &up_lstm : nullptr);
 }
 
 bool Engine::forward(int N, cudaStream_t s) {
   const int max_bin = cfg_.n_fft / 2, Hb = max_bin / 2;
   const int nout = cfg_.nout, a1 = nout / 4, a2 = nout / 2;
   const int c0_1 = pos_x_ / 16 * 16, c0_2 = pos_aux1_ / 16 * 16;
-  last_n_ = N;
   // Stages 1 and 2 (lib/nets.py:91-99): the low-band chain (stg1_low -> bridge -> stg2_low -> bridge) and the
   // high-band chain (stg1_high -> stg2_high) only meet at stage 3, so they run on two streams.
   const bool two = s_hi_ != nullptr && !profiling_;
@@ -1055,77 +1016,40 @@ bool Engine::debug_conv(const float* x_nchw, int N, int Cin, int H, int W, const
 }
 
 // Test hook for the decoder path: y = act(conv3x3(cat[up2x(low), skip]) + bias), fused (upsample inside the row
-// kernel) or staged (upsample kernel, then convolution).
+// kernel) or staged (upsample kernel, then convolution), with the concat buffer laid out as the engine's decoders'.
 bool Engine::debug_decoder(const float* low_nchw, int N, int Cl, int h, int w, const float* skip_nchw, int Cs,
                            const float* wgt, const float* bias, int Cout, int act, int fused, float* y_nchw,
                            cudaStream_t s) {
   cudaSetDevice(cfg_.device);
   const int H = 2 * h, W = 2 * w;
   const int cl_pad = round_up(Cl, 32), cin_pad = round_up(cl_pad + Cs, 16);
+  const int skip_off = fused ? 0 : cl_pad;   // the fused kernel's concat buffer holds only the skip channels
   Arena arena;   // the hook's buffers and weights, freed on return
   const Buffer blow = make_buffer(arena, N, h, w, cl_pad);
-  const Buffer bcat = make_buffer(arena, N, H, W, cin_pad);
+  const Buffer bcat = make_buffer(arena, N, H, W, cin_pad - cl_pad + skip_off);
   const Buffer bout = make_buffer(arena, N, H, W, round_up(Cout, 16));
   ConvLayer L;
   L.name = "debug_decoder";
   L.rows_wide = true;
   L.k = 3; L.act = act;
-  std::vector<int> perm((size_t)cin_pad, -1);   // packed input channels: [up Cl | pad | skip Cs]
+  std::vector<int> perm((size_t)cin_pad, -1);   // reduction order: [up Cl | pad | skip Cs]
   for (int i = 0; i < Cl; ++i) perm[(size_t)i] = i;
   for (int i = 0; i < Cs; ++i) perm[(size_t)(cl_pad + i)] = Cl + i;
   if (!blow.hi || !bcat.hi || !bout.hi || !debug_weights(L, arena, wgt, bias, Cout, Cl + Cs, perm, s)) return false;
-  const ActView skip = bcat.view(N, 0, H, cl_pad, cin_pad - cl_pad);
+  const ActView skip = bcat.view(N, 0, H, skip_off, cin_pad - cl_pad);
   if (!timed("nchw_to_act", 1, N, h, w, s,
              [&] { return ck(launch_nchw_to_act(low_nchw, Cl, blow.all(N), s), "nchw_to_act low"); }) ||
       !timed("nchw_to_act", 1, N, H, W, s,
              [&] { return ck(launch_nchw_to_act(skip_nchw, Cs, skip, s), "nchw_to_act skip"); }) ||
       !tc_prepare(L, H, W, err))
     return false;
+  if (fused && !(L.tc && L.tc->fuses_upsample(blow.C))) {
+    err = "debug_decoder: geometry not supported by the fused row kernel";
+    return false;
+  }
   const ActView out = bout.view(N, 0, H, 0, Cout);
-  bool ok;
-  if (fused) {
-    if (!(L.tc && L.tc->fuses_upsample(blow.C))) {
-      err = "debug_decoder: geometry not supported by the fused row kernel";
-      return false;
-    }
-    ok = run_decoder(L, blow.all(N), bcat, N, out, s);
-  } else {
-    ok = timed("upsample2x", 1, N, H, W, s, [&] {
-           return ck(launch_upsample2x(blow.all(N), bcat.view(N, 0, H, 0, cl_pad), s), "debug_decoder upsample");
-         }) && run_conv(L, bcat.all(N), out, s);
-  }
-  return ok && to_nchw(out, Cout, y_nchw, s) && ck(cudaStreamSynchronize(s), "debug_decoder sync");
-}
-
-bool Engine::debug_read(const char* what, float* out, int64_t cap, int64_t* dims, cudaStream_t s) {
-  cudaSetDevice(cfg_.device);
-  const std::string w(what);
-  const int N = last_n_;
-  const int nout = cfg_.nout, max_bin = cfg_.n_fft / 2;
-  ActView v;
-  int C = 0;
-  if (w == "f3") { v = f3_.all(N); C = nout; }
-  else if (w == "aux1") { v = in3_.view(N, 0, max_bin, pos_aux1_, nout / 4); C = nout / 4; }
-  else if (w == "aux2") { v = in3_.view(N, 0, max_bin, pos_aux2_, nout / 2); C = nout / 2; }
-  else if (w == "x") { v = in3_.view(N, 0, max_bin, pos_x_, 2); C = 2; }
-  else {
-    // "<net index>.<buffer>" e.g. "4.e5", "0.d2"
-    int ni = w.size() > 2 && w[1] == '.' ? w[0] - '0' : -1;
-    if (ni < 0 || ni > 4) { err = "debug_read: unknown tensor " + w; return false; }
-    BaseNetPlan& P = nets_[ni];
-    const std::string b = w.substr(2);
-    const Buffer* buf = nullptr;
-    if (b == "cat1") buf = &P.cat1; else if (b == "cat2") buf = &P.cat2; else if (b == "cat3") buf = &P.cat3;
-    else if (b == "cat4") buf = &P.cat4; else if (b == "e5") buf = &P.e5; else if (b == "acat") buf = &P.acat;
-    else if (b == "ao") buf = &P.ao; else if (b == "d4") buf = &P.d4; else if (b == "d3") buf = &P.d3;
-    else if (b == "d2") buf = &P.d2; else if (b == "t2") buf = &P.t2; else if (b == "f1") buf = &P.f1;
-    else { err = "debug_read: unknown buffer " + b; return false; }
-    v = buf->all(N); C = buf->C;
-  }
-  const int64_t total = (int64_t)N * C * v.H * v.W;
-  dims[0] = N; dims[1] = C; dims[2] = v.H; dims[3] = v.W;
-  if (total > cap) { err = "debug_read: output buffer too small"; return false; }
-  return to_nchw(v, C, out, s);
+  return run_decoder(L, blow.all(N), bcat, N, out, fused != 0, s) && to_nchw(out, Cout, y_nchw, s) &&
+         ck(cudaStreamSynchronize(s), "debug_decoder sync");
 }
 
 }  // namespace vr

@@ -131,18 +131,19 @@ struct BaseNetPlan {
   int n = 0, H = 0, W = 0;
   ConvLayer enc1, enc_a[4], enc_b[4], aspp1, aspp2, aspp_d[3], bott, dec[4];   // dec[0]=dec4 .. dec[3]=dec1
   LstmPlan lstm;
-  // skip_only: dec1's upsample of h is fused into the row kernel and d2 = [h 2n] only; the single LSTM channel is
-  // up-sampled by a small kernel from lstm.y (half resolution, fp32 plane) into a 16-channel group at full
-  // resolution: channels [n, n+16) of cat1 = [e1 n | up(lstm) 1 + 15 zeros] when e1 leaves room in its chunk (n = 16),
-  // else an 8-channel group in the buffer lstm_up of its own (n = 32, 64: cat1 = [e1 n] stays dense for enc2.conv1, and
-  // the row kernel reads the group as its last chunk through a second tensor map whose box TMA zero-fills).  Otherwise (dec1 not
-  // on the row kernel, nets whose 2n is not a multiple of 32): cat1 = [up(h) 2n | up(lstm) 1 + 15 zeros | e1 n | pad], d2 = [h 2n | lstm 1 | zeros].
-  bool skip_only = false;
-  int e1_coff = 0;          // channel offset of e1 inside cat1
-  int lstm_coff = 0;        // skip_only: channel offset of the up-sampled LSTM channel inside cat1 (or 0 in lstm_up)
-  bool lstm_own = false;    // skip_only: the up-sampled LSTM group lives in lstm_up, not in cat1
+  // A decoder is fused when its plan produces its up-sampled input channels inside the row kernel
+  // (TcConv::fuses_upsample); its concat buffer then holds only the reduction channels no kernel produces on the fly.
+  //   dec2 reduces over [up(d3) 4n | e2 2n]: cat2 = [up(d3) 4n | e2 2n], or [e2 2n] when fused.
+  //   dec1 reduces over [up(d2) Up | e1 n | zeros up to Lp = round_up(Up + n, 16) | up(lstm) 1 + 15 zeros], where
+  //   d2 = [h 2n | zeros up to Up = round_up(2n, 32)] (whole chunks, which the row kernel can up-sample): cat1 holds
+  //   channels [fused1 ? Up : 0, Lp + 16) of it.  up(lstm) is up-sampled from lstm.y (half resolution, fp32 plane) into
+  //   its group by a small kernel.  When dec1 is fused and n % 32 == 0 the group is instead an 8-channel buffer lstm_up
+  //   of its own, so that cat1 = [e1 n] stays dense for enc2.conv1; the row kernel reads it as its last chunk through a
+  //   second tensor map whose box TMA zero-fills.
+  bool fused2 = false, fused1 = false;   // dec2 / dec1 fuse their upsample
+  bool lstm_own = false;                 // the up(lstm) group is lstm_up, not in cat1
+  int lstm_coff = 0;                     // channel offset of the up(lstm) group in cat1 (when not lstm_own)
   Buffer cat1, t2, cat2, t3, cat3, t4, cat4, t5, e5, pool, f1, acat, ao, d4, d3, d2, lstm_up;
-  int e1_off = 0;   // position of e1 in dec1's reduction (weight) order
 };
 
 struct Config {
@@ -200,8 +201,6 @@ class Engine {
                   int k, int stride, int dil_h, int dil_w, int act, int use_tc, float* y_nchw, cudaStream_t s);
   bool debug_decoder(const float* low_nchw, int N, int Cl, int h, int w, const float* skip_nchw, int Cs, const float* wgt,
                      const float* bias, int Cout, int act, int fused, float* y_nchw, cudaStream_t s);
-  // debug: copy an internal activation (by name) of the last forward to NCHW fp32
-  bool debug_read(const char* what, float* out, int64_t cap, int64_t* dims, cudaStream_t s);
 
   const Config& cfg() const { return cfg_; }
   int bins() const { return cfg_.n_fft / 2 + 1; }
@@ -221,7 +220,6 @@ class Engine {
   bool warned_simt_ = false;   // the CUDA-core fallback warning was printed
   std::map<std::string, HostTensor> sd_;
   Arena arena_;   // weights, tables and activation buffers
-  int last_n_ = 0;
   // tc: 1 = tensor-core convolution, 0 = CUDA-core convolution, 2 = any other kernel of the path
   struct ProfRec { cudaEvent_t a, b; double flops; int tc; std::string name; int N, H, W; };
   bool profiling_ = false;
@@ -292,9 +290,10 @@ class Engine {
                 const ActView* extra = nullptr);
   bool run_conv_inner(ConvLayer& L, const ActView& in, const ActView& out, bool use_tc, cudaStream_t s,
                       const ActView* up_src, const ActView* extra);
-  // Decoder (lib/layers.py:51-64): upsample `low` into channels [0, low.C) of `cat`, then conv(cat) -> out; the
-  // upsample is fused into the convolution's operand producer when the row kernel can do it
-  bool run_decoder(ConvLayer& L, const ActView& low, const Buffer& cat, int N, const ActView& out, cudaStream_t s);
+  // Decoder (lib/layers.py:51-64): conv(cat[up(low), skip]) -> out.  fused: the row kernel produces up(low) itself and
+  // `cat` holds only the skip channels; else up(low) is first written into channels [0, low.C) of `cat`.
+  bool run_decoder(ConvLayer& L, const ActView& low, const Buffer& cat, int N, const ActView& out, bool fused,
+                   cudaStream_t s);
   bool run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, int N, cudaStream_t s,
                    cudaStream_t side = nullptr);
   bool forward(int N, cudaStream_t s);   // in3_ x-channels already packed for N windows -> f3_

@@ -84,9 +84,6 @@ cudaError_t launch_lstm_recurrence(const float* xp, const float* whh, float* hs,
 // y[bin][(n,t)] = relu(scale[bin] * (wd[bin][:] . hs[(n,t)][:]) + shift[bin]),  wd: [bins][K], NT = N * T
 cudaError_t launch_lstm_dense(const float* hs, const float* wd, const float* scale, const float* shift, int NT, int K,
                               int bins, float* y, cudaStream_t stream);
-// y[bin][n][t] -> channel `ch` of dst[n][bin][t][.] (split bf16)
-cudaError_t launch_lstm_plane_to_channel(const float* y, int N, int T, int bins, ActView dst, int ch,
-                                         cudaStream_t stream);
 
 // ---- STFT / iSTFT (fft.cu), reference lib/spec_utils.py:26-31,157-165 (librosa semantics, SURVEY App. A)
 // frames [t0, t1) only (the full-track call is t0 = 0, t1 = T)

@@ -197,25 +197,6 @@ cudaError_t launch_lstm_dense(const float* hs, const float* wd, const float* sca
   return cudaGetLastError();
 }
 
-// the branch output y[bin][n][t] -> channel `ch` of dst (staged dec1 layout: the LSTM channel of d2)
-__global__ void lstm_plane_to_channel_kernel(const float* __restrict__ y, int N, int T, int bins, ActView dst, int ch) {
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= (int64_t)bins * N * T) return;
-  const int t = (int)(idx % T);
-  const int64_t r = idx / T;
-  const int n = (int)(r % N), bin = (int)(r / N);
-  const int64_t o = (int64_t)n * dst.sn + (int64_t)bin * dst.sh + (int64_t)t * dst.sw + ch;
-  split_bf16(y[idx], dst.hi[o], dst.lo[o]);
-}
-
-cudaError_t launch_lstm_plane_to_channel(const float* y, int N, int T, int bins, ActView dst, int ch,
-                                         cudaStream_t stream) {
-  const int64_t total = (int64_t)bins * N * T;
-  if (total == 0) return cudaSuccess;
-  lstm_plane_to_channel_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(y, N, T, bins, dst, ch);
-  return cudaGetLastError();
-}
-
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float sigmoid_acc(float x) { return 1.f / (1.f + expf(-x)); }
 

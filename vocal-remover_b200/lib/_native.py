@@ -61,7 +61,6 @@ SIGNATURES = {
                                  c_fp, c_vp]),
     'vr_debug_set': (c_i32, [c_i32, c_i32]),
     'vr_debug_trace': (c_i64, [c_vp, c_i64]),
-    'vr_debug_read': (c_i32, [c_vp, ctypes.c_char_p, c_fp, c_i64, ctypes.POINTER(c_i64), c_vp]),
 }
 
 _lib = None
