@@ -210,7 +210,8 @@ VR_API int vr_debug_decoder(vr_ctx* ctx, const float* low, int32_t N, int32_t Cl
  * timeline (builds with -DVR_TRACE), key 2 = 1 makes vr_debug_conv use its 64-channel output tile, key 3 = 1 sends the
  * layers prepared afterwards (every vr_debug_conv call prepares its layer) from the halo-tile kernel to the generic
  * one, key 3 = 2 / 3 makes the halo-tile kernel use MB = 1 / 2, key 6 = 1 (default) skips channel groups whose weights
- * are all zero.  Returns -1 for any other key.                                                                      */
+ * are all zero, key 7 = 1 (default) lets stage 3's last convolution compute only the frames the mask keeps and write
+ * the mask itself (0: every frame, then a separate output-layer kernel).  Returns -1 for any other key.              */
 VR_API int vr_debug_set(int32_t key, int32_t value);
 /* timeline of CTA 0 of the last row-kernel launch made with vr_debug_set(0, 1): 3 roles x 2048 events x 3 clock64 stamps
  * (unused / TMA producer / interpolation warp 0), copied to HOST memory; returns the number of values or -1 */

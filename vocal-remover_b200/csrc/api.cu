@@ -319,7 +319,7 @@ int vr_debug_decoder(vr_ctx* ctx, const float* low, int32_t N, int32_t Cl, int32
 
 int vr_debug_set(int32_t key, int32_t value) {
   int* knob = key == 0 ? &vr::g_debug.trace : key == 2 ? &vr::g_debug.rows_wide : key == 3 ? &vr::g_debug.halo
-            : key == 6 ? &vr::g_debug.kskip : nullptr;
+            : key == 6 ? &vr::g_debug.kskip : key == 7 ? &vr::g_debug.crop_mask : nullptr;
   if (!knob) return -1;
   *knob = value;
   return 0;

@@ -447,8 +447,8 @@ cudaError_t tc_launch(ConvLayer& L, const ActView& in, const ActView& out, cudaS
     return cudaErrorInvalidValue;
   }
   if (tc.kind == TC_ROWS) return tc_rows_launch(L, tc, in, out, s, err, up_src, extra);
-  if (up_src || extra) {
-    err = "tc_launch: fused upsample is only implemented in the row-streaming kernel";
+  if (up_src || extra || L.mask) {
+    err = "tc_launch: fused upsample and output layer are only implemented in the row-streaming kernel";
     return cudaErrorInvalidValue;
   }
   if (tc.kind == TC_HALO) return tc_halo_launch(L, tc, in, out, s, err);

@@ -24,6 +24,11 @@
 // interpolate each 130-pixel row from half-resolution rows into the swizzled operand slot
 // (plain stores + mbarrier arrive; the consumers read the slot with ldmatrix), bit-identical to upsample2x_kernel up to the
 // order of the two blends.
+//
+// Fused output layer (optional, stage 3's dec1 only): the tiles cover only the columns [col0, W - col0) whose mask
+// frames the network keeps (lib/nets.py:127-129), and the epilogue applies the 1x1 output convolution and the sigmoid
+// (mask_out_kernel) instead of storing the layer.  A runtime branch of the BN <= 32 instantiations with the fused
+// upsample, like the fused single-channel dot product, so that no other instantiation changes.
 #include <stdio.h>
 
 #include "engine.h"
@@ -78,6 +83,7 @@ struct RowsGeom {
 
 struct RowsParams {
   int N, H, W, tiles_w, tiles_h, n_tiles, total_tiles;
+  int col0;   // first output column computed: tiles cover columns [col0, col0 + 128 tiles_w) of the W-wide image
   int chunks, CinPadR, Cout, act;
   int n_aslots;
   bf16* out_hi;
@@ -104,7 +110,28 @@ struct RowsParams {
   // adds sum_c dot_w[c] * y[c] over this tile's output channels to dot_out[(n * H + h) * W + w] (pre-zeroed fp32 plane)
   const float* dot_w;
   float* dot_out;
+  // fused output layer of the network (mask_out_kernel, elementwise.cu) when mask.out is set: the consumers apply the
+  // 1x1 convolution to two channels and the sigmoid to each computed pixel, column w being kept frame w - col0, and
+  // store no activation.  mask.f3 is not used.
+  MaskOutParams mask;
 };
+
+// The tile decomposition, shared by the consumers, the TMA producer and the interpolation warps: N tile fastest,
+// then the 128-pixel column tile, the R-row tile and the image.
+struct RowsTile {
+  int nt, w0, h0, n;
+};
+template <int R>
+__device__ __forceinline__ RowsTile rows_tile(const RowsParams& p, int tile) {
+  RowsTile t;
+  t.nt = tile % p.n_tiles;
+  int mt = tile / p.n_tiles;
+  t.w0 = p.col0 + (mt % p.tiles_w) * 128;
+  mt /= p.tiles_w;
+  t.h0 = (mt % p.tiles_h) * R;
+  t.n = mt / p.tiles_h;
+  return t;
+}
 
 // Consumer state across the rows of a tile: the A ring position of each producer's ring, the B buffer, and the weight
 // buffer whose last wgmma group may still be in flight (released once the NEXT group has been committed and the older
@@ -185,6 +212,42 @@ __device__ __forceinline__ float dot_pair(float v0, float v1, const float* bias_
   return fmaf(fmaxf(t0, 0.f) + slope * fminf(t0, 0.f), dot_s[c], (fmaxf(t1, 0.f) + slope * fminf(t1, 0.f)) * dot_s[c + 1]);
 }
 
+// The fused output layer on pixel (n, bin, w) of a one-N-tile layer (BN = Cout = nout), with mask_out_kernel's exact
+// arithmetic.  v holds this lane's accumulators of the pixel, channels 8 j + 2 (lane % 4) + {0, 1}: the quad of lanes
+// that shares the pixel holds all of its channels.  Each channel becomes act(acc + bias) split to hi / lo bf16 as
+// epilogue_pair stores it, then hi + lo: the value mask_out_kernel reads back.  The quad gathers the values in channel
+// order by shuffle; lanes 0 / 1 (mod 4) take the dot product with row 0 / 1 of out.weight (mask_s) and write that mask
+// channel, lanes 2 / 3 write the same value into the replicated Nyquist row (lib/nets.py:111-115).
+template <int BN>
+__device__ __forceinline__ void mask_pixel(const RowsParams& p, const float* v, const float* bias_s,
+                                           const float* mask_s, float slope, int lane, int n, int bin, int w) {
+  float x[BN / 4];
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int c = 8 * j + 2 * (lane & 3);
+    const float t0 = v[4 * j] + bias_s[c], t1 = v[4 * j + 1] + bias_s[c + 1];
+    const float y0 = fmaxf(t0, 0.f) + slope * fminf(t0, 0.f);
+    const float y1 = fmaxf(t1, 0.f) + slope * fminf(t1, 0.f);
+    const float2 hf = bf2_to_f2(f2_to_bf2(y0, y1));
+    const float2 lf = bf2_to_f2(f2_to_bf2(y0 - hf.x, y1 - hf.y));
+    x[2 * j] = hf.x + lf.x;
+    x[2 * j + 1] = hf.y + lf.y;
+  }
+  const float* wm = mask_s + (lane & 1) * BN;
+  float a = 0.f;
+#pragma unroll
+  for (int c = 0; c < BN; ++c)
+    a = fmaf(__shfl_sync(0xffffffffu, x[2 * (c >> 3) + (c & 1)], (lane & ~3) | ((c >> 1) & 3)), wm[c], a);
+  const float m = 1.f / (1.f + expf(-a));
+  const int tr = w - p.col0;
+  const int64_t t = p.mask.t_base0 + (int64_t)n * p.mask.roi_t + tr;
+  const bool nyquist = (lane & 2) != 0;
+  if (t < 0 || t >= p.mask.t_limit || (nyquist && bin != p.H - 1)) return;
+  float* d = p.mask.out + (int64_t)n * p.mask.stride_n + (int64_t)(nyquist ? bin + 1 : bin) * p.mask.stride_bin +
+             p.mask.t_base0 + tr + ((lane & 1) ? p.mask.stride_c : 0);
+  *d = p.mask.accumulate ? (*d + m) * 0.5f : m;
+}
+
 template <int BN, bool UP>
 __global__ void __launch_bounds__(rows_threads(UP), 1)
     conv_tc_rows_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -222,6 +285,12 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
   for (int i = threadIdx.x; i < p.n_tiles * BN; i += blockDim.x) {
     bias_s[i] = __ldg(p.bias + i);
     dot_s[i] = p.dot_out && i < p.Cout ? __ldg(p.dot_w + i) : 0.f;
+  }
+  // the fused output layer only exists where stage 3's dec1 can run (kMaskable); dot_s then holds out.weight [2][BN]
+  constexpr bool kMaskable = UP && BN <= 32;
+  if constexpr (kMaskable) {
+    if (p.mask.out)
+      for (int i = threadIdx.x; i < 2 * BN; i += blockDim.x) dot_s[i] = __ldg(p.mask.w + i);
   }
   __syncthreads();
   // Consumers and producers split first: each producer warpgroup (with UP: the TMA warp with interpolation warps 0-2,
@@ -277,19 +346,21 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
       if (lane == 0 && st.pend_b >= 0) mbar_arrive(bempty0 + (uint32_t)st.pend_b * 8u);
       st.pend_b = -1;
 
-      const int nt = tile % p.n_tiles;
-      int mt = tile / p.n_tiles;
-      const int w0 = (mt % p.tiles_w) * 128;
-      mt /= p.tiles_w;
-      const int h0 = (mt % p.tiles_h) * R;
-      const int n = mt / p.tiles_h;
-      const int c_lane = nt * BN + 2 * (lane & 3);
+      const RowsTile tl = rows_tile<R>(p, tile);
+      const int w0 = tl.w0, h0 = tl.h0, n = tl.n;
+      const int c_lane = tl.nt * BN + 2 * (lane & 3);
 #pragma unroll
       for (int orow = 0; orow < R; ++orow) {
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
           const int px = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
           const float* v = acc + orow * (BN / 2) + 2 * hr;
+          if constexpr (kMaskable) {
+            if (p.mask.out) {
+              mask_pixel<BN>(p, v, bias_s, dot_s, slope, lane, n, h0 + orow, w0 + px);
+              continue;
+            }
+          }
           if (p.dot_out) {
             float d = 0.f;
 #pragma unroll
@@ -321,12 +392,8 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
 #endif
         int tn = 0;
         for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-          const int nt = tile % p.n_tiles;
-          int mt = tile / p.n_tiles;
-          const int w0 = (mt % p.tiles_w) * 128;
-          mt /= p.tiles_w;
-          const int h0 = (mt % p.tiles_h) * R;
-          const int n = mt / p.tiles_h;
+          const RowsTile tl = rows_tile<R>(p, tile);
+          const int nt = tl.nt, w0 = tl.w0, h0 = tl.h0, n = tl.n;
           for (int cc = 0; cc < p.chunks; ++cc) {
             mbar_wait(smem_u32(&bar_bempty[bs]), bph ^ 1u);
             const uint32_t bfull = smem_u32(&bar_bfull[bs]);
@@ -397,13 +464,11 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
         int64_t f_base = 0;
         bool f_px = false;
         auto fetch_tile = [&]() {
-          int mt = f_tile / p.n_tiles;
-          const int w0 = (mt % p.tiles_w) * 128;
-          mt /= p.tiles_w;
-          f_h0 = (mt % p.tiles_h) * R - 1;
-          f_X = (int)(p.up_sw * (w0 > 0 ? w0 - 1 : 0)) + sx;
+          const RowsTile tl = rows_tile<R>(p, f_tile);
+          f_h0 = tl.h0 - 1;
+          f_X = (int)(p.up_sw * (tl.w0 > 0 ? tl.w0 - 1 : 0)) + sx;
           f_px = sx < kSrcPx && f_X < p.xW;
-          f_base = (int64_t)(mt / p.tiles_h) * p.xsn + (int64_t)f_X * p.xsw + j * 8;
+          f_base = (int64_t)tl.n * p.xsn + (int64_t)f_X * p.xsw + j * 8;
         };
         fetch_tile();
         // Two rows are in flight: the loads of row k+2 are issued right after row k has been stored and announced, so
@@ -445,8 +510,7 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
           fetch();   // row 1 (row 0 moves to q*)
         }
         for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-          int mt = tile / p.n_tiles;
-          const int w0 = (mt % p.tiles_w) * 128;
+          const int w0 = rows_tile<R>(p, tile).w0;
           const int X = (int)(p.up_sw * (w0 > 0 ? w0 - 1 : 0)) + sx;   // absolute source pixel
           // the output pixels w with (int)(up_sw * w) == X lie in [wc - 1, wc + 3] and there are at most 3 of them
           int e_off[3];
@@ -563,10 +627,18 @@ cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   const CUtensorMap* map_a = tc_activation_map(tc, in, kBoxPx, 1, 1, 1, err, L.name);
   const CUtensorMap* map_l = extra ? tc_activation_map(tc, *extra, kBoxPx, 1, 1, 1, err, L.name) : map_a;
   if (!map_a || !map_l) return cudaErrorInvalidValue;
+  // with the fused output layer only the kept columns [offset, W - offset) are computed
+  const int col0 = L.mask ? L.mask->offset : 0, kept = out.W - 2 * col0;
+  if (L.mask && (!up_src || !tc.fuses_mask(L.Cout) || col0 < 0 || kept <= 0 || kept % 128)) {
+    err = "tc_rows_launch: the fused output layer needs a fused upsample, one N tile of Cout <= 32 channels and a "
+          "kept width that is a multiple of 128";
+    return cudaErrorInvalidValue;
+  }
   RowsParams p;
   p.N = out.N; p.H = out.H; p.W = out.W;
   const bool up = up_src != nullptr;
-  p.tiles_w = out.W / 128; p.tiles_h = out.H / rows_per_tile(tc.BN); p.n_tiles = tc.n_tiles;
+  p.col0 = col0;
+  p.tiles_w = kept / 128; p.tiles_h = out.H / rows_per_tile(tc.BN); p.n_tiles = tc.n_tiles;
   p.total_tiles = p.tiles_w * p.tiles_h * out.N * tc.n_tiles;
   p.chunks = tc.chunks; p.CinPadR = tc.CinPad; p.Cout = L.Cout; p.act = L.act;
   p.out_hi = out.hi; p.out_lo = out.lo;
@@ -577,6 +649,7 @@ cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   p.trace = g_debug.trace == 1 ? 1 : 0;
   p.up_sh = p.up_sw = 0.f;
   p.dot_w = L.dot_w; p.dot_out = L.dot_w ? L.dot_out : nullptr;
+  p.mask = L.mask ? *L.mask : MaskOutParams{};
   p.a_c_off = 0;
   p.l_chunk = extra ? tc.chunks - 1 : -1;
   p.kmask = g_debug.kskip == 1 ? tc.kmask : ~0ull;   // VR_KSKIP=0 issues the all-zero-weight channel groups too

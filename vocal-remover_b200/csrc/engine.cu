@@ -496,9 +496,12 @@ bool Engine::run_conv(ConvLayer& L, const ActView& in, const ActView& out, cudaS
             "CUDA-core convolution; use a cropsize whose maps tile (e.g. 256) for full speed\n",
             L.name.c_str(), in.N, in.H, in.W, out.H, out.W);
   }
-  // algorithmic FLOPs with the real (un-padded) channel counts: 2 * pixels * Cout * Cin * taps
-  const int pi = prof_begin(up_src ? L.name + "+up" : L.name, use_tc ? 1 : 0,
-                            2.0 * (double)out.N * out.H * out.W * L.Cout * L.Cin * L.k * L.k, out.N, out.H, out.W, s);
+  // algorithmic FLOPs with the real (un-padded) channel counts: 2 * pixels * Cout * Cin * taps, over the computed
+  // columns only (a fused output layer computes the kept ones)
+  const int cols = L.mask ? out.W - 2 * L.mask->offset : out.W;
+  const std::string name = L.name + (up_src ? "+up" : "") + (L.mask ? "+mask" : "");
+  const int pi = prof_begin(name, use_tc ? 1 : 0, 2.0 * (double)out.N * out.H * cols * L.Cout * L.Cin * L.k * L.k,
+                            out.N, out.H, out.W, s);
   bool ok = run_conv_inner(L, in, out, use_tc, s, up_src, extra);
   prof_end(pi, s);
   return ok;
@@ -507,8 +510,8 @@ bool Engine::run_conv(ConvLayer& L, const ActView& in, const ActView& out, cudaS
 bool Engine::run_conv_inner(ConvLayer& L, const ActView& in, const ActView& out, bool use_tc, cudaStream_t s,
                             const ActView* up_src, const ActView* extra) {
   if (use_tc) return ck(tc_launch(L, in, out, s, err, up_src, extra), L.name.c_str());
-  if (up_src || extra) {
-    err = "internal: fused upsample requested for a CUDA-core convolution";
+  if (up_src || extra || L.mask) {
+    err = "internal: fused upsample or output layer requested for a CUDA-core convolution";
     return false;
   }
   ConvParams p;
@@ -609,7 +612,7 @@ bool Engine::run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, 
   return run_conv(P.dec[3], P.cat1.all(N), out, s, P.fused1 ? &d2 : nullptr, P.lstm_own ? &up_lstm : nullptr);
 }
 
-bool Engine::forward(int N, cudaStream_t s) {
+bool Engine::forward(int N, const MaskOutParams& mask, cudaStream_t s) {
   const int max_bin = cfg_.n_fft / 2, Hb = max_bin / 2;
   const int nout = cfg_.nout, a1 = nout / 4, a2 = nout / 2;
   const int c0_1 = pos_x_ / 16 * 16, c0_2 = pos_aux1_ / 16 * 16;
@@ -635,8 +638,19 @@ bool Engine::forward(int N, cudaStream_t s) {
     if (!ck(cudaEventRecord(ev_join_, s_hi_), "join") || !ck(cudaStreamWaitEvent(s, ev_join_, 0), "join wait"))
       return false;
   }
-  // stage 3 (lib/nets.py:101-102)
-  return run_basenet(nets_[4], in3_.all(N), f3_.all(N), N, s, two ? s_hi_ : nullptr);
+  // Stage 3 (lib/nets.py:101-102) and the output layer (lib/nets.py:109-115, 127-129).  dec1 is a 3x3 convolution and
+  // `out` a 1x1 one, so a kept frame needs dec1 at that frame only: where the row kernel can apply the output layer,
+  // dec1 computes just the kept frames and writes the mask, and f3_ is not written.
+  ConvLayer& dec1 = nets_[4].dec[3];
+  const int kept = cfg_.cropsize - 2 * mask.offset;
+  const bool crop = g_debug.crop_mask == 1 && nets_[4].fused1 && dec1.tc && dec1.tc->fuses_mask(dec1.Cout) &&
+                    mask.offset >= 0 && kept > 0 && kept % 128 == 0;
+  if (crop) dec1.mask = &mask;
+  const bool ok = run_basenet(nets_[4], in3_.all(N), f3_.all(N), N, s, two ? s_hi_ : nullptr);
+  dec1.mask = nullptr;
+  if (!ok) return false;
+  if (crop) return true;
+  return timed("mask_out", 1, N, mask.f3.H, mask.f3.W, s, [&] { return ck(launch_mask_out(mask, s), "mask_out"); });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -653,14 +667,13 @@ bool Engine::predict_mask(const float* mag, int N, float* mask_out, int offset, 
           return ck(launch_pack_mag_from_float(mag + (int64_t)i * 2 * nb * W, nb, max_bin, in3_.view(nb_now, 0, max_bin, pos_x_, 2), s), "pack");
         }))
       return false;
-    if (!forward(nb_now, s)) return false;
     MaskOutParams p;
     p.f3 = f3_.all(nb_now);
     p.w = out_w_;
     p.out = mask_out + (int64_t)i * 2 * nb * r;
     p.stride_n = (int64_t)2 * nb * r; p.stride_c = (int64_t)nb * r; p.stride_bin = r;
     p.offset = offset; p.t_base0 = 0; p.t_limit = r; p.roi_t = 0; p.accumulate = 0;
-    if (!timed("mask_out", 1, nb_now, max_bin, W, s, [&] { return ck(launch_mask_out(p, s), "mask_out"); })) return false;
+    if (!forward(nb_now, p, s)) return false;
   }
   return true;
 }
@@ -681,7 +694,6 @@ bool Engine::separate_windows(const float2* spec, int64_t T, const float* norm, 
           return ck(launch_pack_mag_from_spec(spec, nb, T, max_bin, W, r, pad_l, g0, norm, in3_.view(n_now, 0, max_bin, pos_x_, 2), s), "pack");
         }))
       return false;
-    if (!forward(n_now, s)) return false;
     MaskOutParams p;
     p.f3 = f3_.all(n_now);
     p.w = out_w_;
@@ -690,7 +702,7 @@ bool Engine::separate_windows(const float2* spec, int64_t T, const float* norm, 
     p.offset = cfg_.offset;
     p.t_base0 = (int64_t)g0 * r - frame_shift;
     p.t_limit = mask_T; p.roi_t = r; p.accumulate = accumulate;
-    if (!timed("mask_out", 1, n_now, max_bin, W, s, [&] { return ck(launch_mask_out(p, s), "mask_out"); })) return false;
+    if (!forward(n_now, p, s)) return false;
     if (final_pass && on_frames_final_) {
       int64_t f = p.t_base0 + (int64_t)n_now * r;
       if (f > mask_T) f = mask_T;

@@ -107,6 +107,9 @@ struct ConvLayer {
   // pre-zeroed plane dot_out[n][h][w] (the LSTM branch's 1x1 input convolution fused into dec2)
   const float* dot_w = nullptr;
   float* dot_out = nullptr;
+  // set around ONE launch by the caller (stage 3's dec1): the row kernel computes only the output columns
+  // [mask->offset, W - mask->offset) and writes the network's mask there (mask_out_kernel's work) instead of the layer
+  const MaskOutParams* mask = nullptr;
   std::shared_ptr<TcConv> tc;    // the tensor-core kernel and its packed weights; null -> CUDA-core kernel
 };
 
@@ -296,7 +299,9 @@ class Engine {
                    cudaStream_t s);
   bool run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, int N, cudaStream_t s,
                    cudaStream_t side = nullptr);
-  bool forward(int N, cudaStream_t s);   // in3_ x-channels already packed for N windows -> f3_
+  // in3_ x-channels already packed for N windows -> the mask of frames [mask.offset, W - mask.offset) of every window,
+  // written as mask describes (mask.f3 = f3_.all(N))
+  bool forward(int N, const MaskOutParams& mask, cudaStream_t s);
   bool ensure_ws(int64_t T);
   bool ck(cudaError_t e, const char* what);
 };

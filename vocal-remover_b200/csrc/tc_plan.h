@@ -36,6 +36,9 @@ struct TcConv {
   std::map<ViewKey, CUtensorMap> map_a;
   // the row kernel can produce the leading up_C channels of its input as the x2 upsample of a half-resolution tensor
   bool fuses_upsample(int up_C) const { return kind == TC_ROWS && up_C % 32 == 0 && up_C <= CinPad; }
+  // the row kernel can apply the network's output layer (mask_out_kernel) in its epilogue: one quad of lanes must hold
+  // all Cout channels of a pixel, and only the BN <= 32 instantiations with a fused upsample carry that epilogue
+  bool fuses_mask(int Cout) const { return kind == TC_ROWS && n_tiles == 1 && BN <= 32 && BN == Cout; }
 };
 
 TcKind tc_choose(const ConvLayer& L, int H, int W);
@@ -71,6 +74,8 @@ struct TcDebug {
   int halo = 0;        // key 3 = 1: layers prepared from then on go to the generic kernel instead of the halo kernel;
                        // 2 / 3: the halo kernel uses MB = 1 / 2 (where the height tiles) in every launch
   int kskip = 1;       // key 6 = 1 (default): the row and halo kernels skip channel groups whose weights are all zero
+  int crop_mask = 1;   // key 7 = 1 (default): stage 3's dec1 computes only the kept frames and applies the output layer
+                       // in its epilogue where it can; 0: it computes every frame into f3_, then mask_out_kernel runs
 };
 extern TcDebug g_debug;
 
