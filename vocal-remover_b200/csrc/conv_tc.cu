@@ -31,6 +31,7 @@ namespace vr {
 static constexpr int kMaxStages = 8;
 static constexpr int kConsumerWarps = 8;                 // two warpgroups
 static constexpr int kThreads = 32 * kConsumerWarps + 32;   // + the TMA producer warp
+static constexpr int kStaticSmem = 2048;   // shared memory not given to the dynamic part: barriers and staged bias
 
 struct TcParams {
   int N, Ho, Wo, Wt, Ht, Nt, tiles_w, tiles_h, m_tiles, n_tiles;
@@ -216,7 +217,7 @@ const TcDevice& tc_device() {
         cudaDeviceGetAttribute(&d.num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
       return none;
 #define VR_TC_SET_SMEM(KB, BN) \
-  cudaFuncSetAttribute(conv_tc_kernel<KB, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem - 2048);
+  cudaFuncSetAttribute(conv_tc_kernel<KB, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem - kStaticSmem);
     VR_TC_FOR_ALL(VR_TC_SET_SMEM)
 #undef VR_TC_SET_SMEM
     tc_rows_set_attributes(d.max_smem);
@@ -285,35 +286,32 @@ static TileGeom tile_geom(int Ho, int Wo) {
 struct NTiling {
   int BN, n_tiles;
 };
-static NTiling n_tiling(const ConvLayer& L, bool rows) {
+static NTiling n_tiling(const ConvLayer& L, bool rows, bool rows_wide) {
   const int cout16 = round_up(L.Cout, 16);
   if (rows) {
     // 64 output channels per tile for the decoder layers with a fused upsample: one N = 64 MMA per product and output
     // row instead of two N = 32 ones (half the A-operand reads from shared memory) and every input row is interpolated
     // once instead of once per N tile.  Plain TMA layers stay at 32: the 64-wide tile has a single accumulator set (no
     // epilogue overlap) and only four operand slots next to its 147 KB of weights, and measured slower there.
-    const int BN = cout16 == 16 ? 16 : (L.rows_wide && cout16 % 64 == 0 ? 64 : 32);
+    const int BN = cout16 == 16 ? 16 : (rows_wide && cout16 % 64 == 0 ? 64 : 32);
     return {BN, ceil_div(cout16, BN)};
   }
   const int n_tiles = ceil_div(cout16, 128);
   return {round_up(ceil_div(cout16, n_tiles), 16), n_tiles};
 }
 
-// the BN values conv_tc_halo.cu instantiates
-static bool halo_has_bn(int BN) { return BN == 16 || BN == 32 || BN == 48 || BN == 64 || BN == 96 || BN == 128; }
-
 // The kernel of a layer whose output maps are H x W: the row kernel where it applies, else the halo kernel, else the
 // generic one.  The row and halo kernels stage the bias of every N tile in 256 floats of shared memory.
-TcKind tc_choose(const ConvLayer& L, int H, int W) {
+TcKind tc_choose(const ConvLayer& L, int H, int W, bool rows_wide) {
   if (!(L.k == 1 || L.k == 3) || !(L.stride == 1 || L.stride == 2) || L.Cout < 4) return TC_NONE;
   const TileGeom g = tile_geom(H, W);
   if (!g.ok || g.Wt * L.stride > 256 || g.Ht * L.stride > 256) return TC_NONE;
   const bool k3s1 = L.k == 3 && L.stride == 1 && L.dil_h == 1 && L.dil_w == 1;
-  const NTiling r = n_tiling(L, true), t = n_tiling(L, false);
+  const NTiling r = n_tiling(L, true, rows_wide), t = n_tiling(L, false, false);
   // whole 128-pixel row tiles of 2, 4 or 8 rows (rows_per_tile, conv_tc_rows.cu)
-  if (k3s1 && W % 128 == 0 && H % 8 == 0 && r.n_tiles * r.BN <= 256) return TC_ROWS;
+  if (k3s1 && W % 128 == 0 && H % 8 == 0 && tc_rows_has(r.BN) && r.n_tiles * r.BN <= 256) return TC_ROWS;
   // whole tiles of 128 / W rows (MB = 1)
-  if (k3s1 && (W == 16 || W == 32 || W == 64) && H % (128 / W) == 0 && halo_has_bn(t.BN) &&
+  if (k3s1 && (W == 16 || W == 32 || W == 64) && H % (128 / W) == 0 && tc_halo_has(t.BN) &&
       t.n_tiles * t.BN <= 256 && g_debug.halo != 1)
     return TC_HALO;
   return TC_GENERIC;
@@ -391,8 +389,8 @@ const CUtensorMap* tc_activation_map(TcConv& tc, const ActView& v, int bw, int b
   return &tc.map_a.emplace(key, m).first->second;
 }
 
-bool tc_prepare(ConvLayer& L, int H, int W, std::string& err) {
-  const TcKind kind = tc_choose(L, H, W);
+bool tc_prepare(ConvLayer& L, int H, int W, bool rows_wide, std::string& err) {
+  const TcKind kind = tc_choose(L, H, W, rows_wide);
   if (kind == TC_NONE) return true;   // stays on the CUDA-core kernel
   if (!tc_encode_fn()) {
     err = "cuTensorMapEncodeTiled is not available from the driver";
@@ -401,7 +399,7 @@ bool tc_prepare(ConvLayer& L, int H, int W, std::string& err) {
   auto tc = std::make_shared<TcConv>();
   tc->kind = kind;
   tc->H = H; tc->W = W;
-  const NTiling nt = n_tiling(L, kind == TC_ROWS);
+  const NTiling nt = n_tiling(L, kind == TC_ROWS, rows_wide);
   const int BN = nt.BN, cin16 = round_up(L.CinPad, 16);
   tc->BN = BN; tc->n_tiles = nt.n_tiles;
   tc->KB = kind != TC_GENERIC ? 32 : cin16 % 64 == 0 ? 64 : cin16 % 32 == 0 ? 32 : 16;
@@ -439,16 +437,16 @@ bool tc_prepare(ConvLayer& L, int H, int W, std::string& err) {
   return true;
 }
 
-cudaError_t tc_launch(ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, std::string& err,
-                      const ActView* up_src, const ActView* extra) {
+cudaError_t tc_launch(const ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, std::string& err,
+                      const ConvFusion& f) {
   TcConv& tc = *L.tc;
   if (out.H != tc.H || out.W != tc.W || (in.H - 1) / L.stride + 1 != out.H || (in.W - 1) / L.stride + 1 != out.W) {
     err = "internal: " + L.name + " is launched on maps of another size than it was prepared for";
     return cudaErrorInvalidValue;
   }
-  if (tc.kind == TC_ROWS) return tc_rows_launch(L, tc, in, out, s, err, up_src, extra);
-  if (up_src || extra || L.mask) {
-    err = "tc_launch: fused upsample and output layer are only implemented in the row-streaming kernel";
+  if (tc.kind == TC_ROWS) return tc_rows_launch(L, tc, in, out, s, err, f);
+  if (!f.empty()) {
+    err = "tc_launch: fused work is only implemented in the row-streaming kernel";
     return cudaErrorInvalidValue;
   }
   if (tc.kind == TC_HALO) return tc_halo_launch(L, tc, in, out, s, err);
@@ -473,7 +471,7 @@ cudaError_t tc_launch(ConvLayer& L, const ActView& in, const ActView& out, cudaS
     err = "tc_launch: cannot query the current device";
     return cudaErrorInvalidValue;
   }
-  const int dyn = dv.max_smem - 2048;   // static barriers + staged bias live in the remaining 2 KiB
+  const int dyn = dv.max_smem - kStaticSmem;
   p.stages = (dyn - 1024) / stage_bytes;
   if (p.stages > kMaxStages) p.stages = kMaxStages;
   if (p.stages < 2) {

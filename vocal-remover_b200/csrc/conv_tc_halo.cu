@@ -36,6 +36,7 @@ static constexpr int kProducerRegs = 40;
 static_assert(kConsumerWarps * kConsumerRegs + kProducerWarps * kProducerRegs <=
                   (kConsumerWarps + kProducerWarps) * kLaunchRegs,
               "setmaxnreg.inc would wait forever for registers the block does not own");
+static constexpr int kStaticSmem = 2048;   // shared memory not given to the dynamic part: barriers and staged bias
 static constexpr int kMaxHSlots = 4;
 static constexpr int kMaxWStages = 18;      // two chunks of nine taps
 static constexpr uint32_t kKB = 32;         // channels per chunk (SWIZZLE_64B rows of 64 bytes)
@@ -253,14 +254,21 @@ __global__ void __launch_bounds__(kThreads, 1)
   }
 }
 
-// every (BN, MB) instantiation the host can launch: the BN values tc_choose accepts for these layers (halo_has_bn)
+// every (BN, MB) instantiation the host can launch, and so the BN values tc_choose accepts for these layers
 #define VR_HALO_FOR_MB(X, BN) X(BN, 1) X(BN, 2)
 #define VR_HALO_FOR_ALL(X) \
   VR_HALO_FOR_MB(X, 16) VR_HALO_FOR_MB(X, 32) VR_HALO_FOR_MB(X, 48) VR_HALO_FOR_MB(X, 64) VR_HALO_FOR_MB(X, 96) \
   VR_HALO_FOR_MB(X, 128)
 
+bool tc_halo_has(int BN) {
+#define VR_HALO_HAS(BN_, MB_) if (BN == BN_) return true;
+  VR_HALO_FOR_ALL(VR_HALO_HAS)
+#undef VR_HALO_HAS
+  return false;
+}
+
 // ------------------------------------------------------------------------------------------------
-cudaError_t tc_halo_launch(ConvLayer& L, TcConv& tc, const ActView& in, const ActView& out, cudaStream_t s,
+cudaError_t tc_halo_launch(const ConvLayer& L, TcConv& tc, const ActView& in, const ActView& out, cudaStream_t s,
                            std::string& err) {
   const TcDevice& dv = tc_device();
   if (!dv.ok) {
@@ -297,7 +305,7 @@ cudaError_t tc_halo_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   if (!map_a) return cudaErrorInvalidValue;
   // shared memory: up to kMaxHSlots halo slots next to one chunk's nine weight stages, the rest to weight stages
   const int w_stage = tc.BN * 2 * (int)kRowB;
-  const int dyn = dv.max_smem - 2048;   // static barriers + staged bias live in the remaining 2 KiB
+  const int dyn = dv.max_smem - kStaticSmem;
   const int avail = dyn - 1024;
   p.n_hslots = (avail - 9 * w_stage) / (int)p.hslot;
   if (p.n_hslots > kMaxHSlots) p.n_hslots = kMaxHSlots;
@@ -324,7 +332,7 @@ cudaError_t tc_halo_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
 // cudaFuncSetAttribute is per device: called by tc_device() the first time a device is used (conv_tc.cu)
 void tc_halo_set_attributes(int max_smem) {
 #define VR_HALO_SET(BN_, MB_) \
-  cudaFuncSetAttribute(conv_tc_halo_kernel<BN_, MB_>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem - 2048);
+  cudaFuncSetAttribute(conv_tc_halo_kernel<BN_, MB_>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem - kStaticSmem);
   VR_HALO_FOR_ALL(VR_HALO_SET)
 #undef VR_HALO_SET
 }

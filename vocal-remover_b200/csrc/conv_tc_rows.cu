@@ -61,6 +61,7 @@ static constexpr int kRowPx = 130;                 // 128 + 2 halo pixels
 static constexpr int kBoxPx = 136;                 // pixels per TMA row box: makes one plane 17 x 512 B, so that the lo plane
                                                    // of the two-plane box starts on the SWIZZLE_64B repeat (8 rows x 64 B)
 static constexpr int kMaxASlots = 8;
+static constexpr int kStaticSmem = 3072;           // shared memory not given to the dynamic part: barriers, bias, dot_s
 static constexpr int kSrcPx = 68;                  // half-resolution pixels a 130-pixel row interpolates from (fused upsample)
 static constexpr uint32_t kKB = 32;                 // channels per chunk (SWIZZLE_64B rows of 64 bytes)
 static constexpr uint32_t kRowB = kKB * 2;          // bytes of one pixel of a chunk
@@ -605,12 +606,24 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
   }
 }
 
+// every (BN, UP) instantiation the host can launch, and so the BN values tc_choose accepts for this kernel
+#define VR_ROWS_FOR_ALL(X) X(16, true) X(16, false) X(32, true) X(32, false) X(64, true) X(64, false)
+
+// bytes of the two weight buffers of the BN instantiations; 0 if there are none
+static int rows_b_bytes(int BN) {
+#define VR_ROWS_B(BN_, UP_) if (BN == BN_) return (int)(2 * RowsGeom<BN_>::kBBuf);
+  VR_ROWS_FOR_ALL(VR_ROWS_B)
+#undef VR_ROWS_B
+  return 0;
+}
+
+bool tc_rows_has(int BN) { return rows_b_bytes(BN) > 0; }
+
 // ------------------------------------------------------------------------------------------------
-// up_src != nullptr: the first up_src->C reduction channels are produced inside the kernel as the bilinear x2 upsample
-// of *up_src (half resolution, tc.fuses_upsample(up_src->C)); `in` holds only the channels after them.
-// extra != nullptr: the LAST channel chunk is read from *extra (channels [0, extra->C), zero-filled up to the chunk).
-cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const ActView& out, cudaStream_t s,
-                           std::string& err, const ActView* up_src, const ActView* extra) {
+// f: the fused work (ConvFusion), checked against what the plan can do (TcConv::fuses_*)
+cudaError_t tc_rows_launch(const ConvLayer& L, TcConv& tc, const ActView& in, const ActView& out, cudaStream_t s,
+                           std::string& err, const ConvFusion& f) {
+  const ActView* up_src = f.up;
   if (up_src && (!tc.fuses_upsample(up_src->C) || up_src->H * 2 != in.H || up_src->W * 2 != in.W || up_src->sw % 8)) {
     err = "tc_rows_launch: fused upsample needs a half-resolution source of 32k channels";
     return cudaErrorInvalidValue;
@@ -619,26 +632,27 @@ cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
     err = "tc_rows_launch: with a fused upsample the input must hold only the channels after the up-sampled ones";
     return cudaErrorInvalidValue;
   }
-  if (extra && (extra->H != in.H || extra->W != in.W || extra->N != in.N || extra->C > tc.KB)) {
-    err = "tc_rows_launch: the extra last-chunk tensor must match the input geometry and fit one chunk";
+  const ActView* last = f.last_chunk;
+  if (last && (last->H != in.H || last->W != in.W || last->N != in.N || last->C > tc.KB)) {
+    err = "tc_rows_launch: the last-chunk tensor must match the input geometry and fit one chunk";
     return cudaErrorInvalidValue;
   }
   // both planes of one row in one box
   const CUtensorMap* map_a = tc_activation_map(tc, in, kBoxPx, 1, 1, 1, err, L.name);
-  const CUtensorMap* map_l = extra ? tc_activation_map(tc, *extra, kBoxPx, 1, 1, 1, err, L.name) : map_a;
+  const CUtensorMap* map_l = last ? tc_activation_map(tc, *last, kBoxPx, 1, 1, 1, err, L.name) : map_a;
   if (!map_a || !map_l) return cudaErrorInvalidValue;
   // with the fused output layer only the kept columns [offset, W - offset) are computed
-  const int col0 = L.mask ? L.mask->offset : 0, kept = out.W - 2 * col0;
-  if (L.mask && (!up_src || !tc.fuses_mask(L.Cout) || col0 < 0 || kept <= 0 || kept % 128)) {
+  if (f.mask && !tc.fuses_mask(L.Cout, f.mask->offset, up_src != nullptr)) {
     err = "tc_rows_launch: the fused output layer needs a fused upsample, one N tile of Cout <= 32 channels and a "
           "kept width that is a multiple of 128";
     return cudaErrorInvalidValue;
   }
+  const int col0 = f.mask ? f.mask->offset : 0;
   RowsParams p;
   p.N = out.N; p.H = out.H; p.W = out.W;
   const bool up = up_src != nullptr;
   p.col0 = col0;
-  p.tiles_w = kept / 128; p.tiles_h = out.H / rows_per_tile(tc.BN); p.n_tiles = tc.n_tiles;
+  p.tiles_w = (out.W - 2 * col0) / 128; p.tiles_h = out.H / rows_per_tile(tc.BN); p.n_tiles = tc.n_tiles;
   p.total_tiles = p.tiles_w * p.tiles_h * out.N * tc.n_tiles;
   p.chunks = tc.chunks; p.CinPadR = tc.CinPad; p.Cout = L.Cout; p.act = L.act;
   p.out_hi = out.hi; p.out_lo = out.lo;
@@ -648,10 +662,10 @@ cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   p.x_hi = p.x_lo = nullptr; p.xsn = p.xsh = 0; p.xsw = 0;
   p.trace = g_debug.trace == 1 ? 1 : 0;
   p.up_sh = p.up_sw = 0.f;
-  p.dot_w = L.dot_w; p.dot_out = L.dot_w ? L.dot_out : nullptr;
-  p.mask = L.mask ? *L.mask : MaskOutParams{};
+  p.dot_w = f.dot_w; p.dot_out = f.dot_w ? f.dot_out : nullptr;
+  p.mask = f.mask ? *f.mask : MaskOutParams{};
   p.a_c_off = 0;
-  p.l_chunk = extra ? tc.chunks - 1 : -1;
+  p.l_chunk = last ? tc.chunks - 1 : -1;
   p.kmask = g_debug.kskip == 1 ? tc.kmask : ~0ull;   // VR_KSKIP=0 issues the all-zero-weight channel groups too
   if (up_src) {
     p.a_c_off = -up_src->C;   // `in` starts at reduction channel up_src->C
@@ -671,8 +685,8 @@ cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
     err = "tc_rows_launch: cannot query the current device";
     return cudaErrorInvalidValue;
   }
-  const int b_bytes = tc.BN == 16 ? (int)(2 * RowsGeom<16>::kBBuf) : tc.BN == 32 ? (int)(2 * RowsGeom<32>::kBBuf) : (int)(2 * RowsGeom<64>::kBBuf);
-  p.n_aslots = (dv.max_smem - 3072 - 1024 - b_bytes) / (int)kASlot;
+  const int b_bytes = rows_b_bytes(tc.BN);
+  p.n_aslots = (dv.max_smem - kStaticSmem - 1024 - b_bytes) / (int)kASlot;
   if (p.n_aslots > kMaxASlots) p.n_aslots = kMaxASlots;
   if (p.n_aslots < (p.up_chunks > 0 ? 4 : 2)) {
     err = "tc_rows_launch: shared memory too small";
@@ -684,17 +698,12 @@ cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const Ac
   const int dyn = p.n_aslots * (int)kASlot + b_bytes + 1024;
   const int grid = p.total_tiles < dv.num_sms ? p.total_tiles : dv.num_sms;   // persistent: one CTA per SM
   const int threads = rows_threads(up);
-#define VR_ROWS_LAUNCH(BN_)                                                                      \
-  if (tc.BN == BN_) {                                                                            \
-    if (up)                                                                                      \
-      conv_tc_rows_kernel<BN_, true><<<grid, threads, dyn, s>>>(*map_a, tc.map_b, *map_l, p);    \
-    else                                                                                         \
-      conv_tc_rows_kernel<BN_, false><<<grid, threads, dyn, s>>>(*map_a, tc.map_b, *map_l, p);   \
-    return cudaGetLastError();                                                                   \
+#define VR_ROWS_LAUNCH(BN_, UP_)                                                              \
+  if (tc.BN == BN_ && up == UP_) {                                                            \
+    conv_tc_rows_kernel<BN_, UP_><<<grid, threads, dyn, s>>>(*map_a, tc.map_b, *map_l, p);    \
+    return cudaGetLastError();                                                                \
   }
-  VR_ROWS_LAUNCH(16)
-  VR_ROWS_LAUNCH(32)
-  VR_ROWS_LAUNCH(64)
+  VR_ROWS_FOR_ALL(VR_ROWS_LAUNCH)
 #undef VR_ROWS_LAUNCH
   err = "tc_rows_launch: no kernel instantiation for this channel tile";
   return cudaErrorInvalidValue;
@@ -711,12 +720,11 @@ int tc_rows_read_trace(unsigned long long* out, long long capacity) {
 
 // cudaFuncSetAttribute is per device: called by tc_device() the first time a device is used (conv_tc.cu)
 void tc_rows_set_attributes(int max_smem) {
-#define VR_ROWS_SET(BN_, UP_)                                                                                     \
-  cudaFuncSetAttribute(conv_tc_rows_kernel<BN_, UP_>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem - 3072); \
+#define VR_ROWS_SET(BN_, UP_)                                                                        \
+  cudaFuncSetAttribute(conv_tc_rows_kernel<BN_, UP_>, cudaFuncAttributeMaxDynamicSharedMemorySize,   \
+                       max_smem - kStaticSmem);                                                      \
   cudaFuncSetAttribute(conv_tc_rows_kernel<BN_, UP_>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-  VR_ROWS_SET(16, false) VR_ROWS_SET(16, true)
-  VR_ROWS_SET(32, false) VR_ROWS_SET(32, true)
-  VR_ROWS_SET(64, false) VR_ROWS_SET(64, true)
+  VR_ROWS_FOR_ALL(VR_ROWS_SET)
 #undef VR_ROWS_SET
 }
 

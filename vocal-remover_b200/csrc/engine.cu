@@ -138,7 +138,7 @@ bool Engine::need(const std::string& key, std::initializer_list<int64_t> shape, 
 // Fold BatchNorm2d(eval) into the bias-free conv and pack to [tap][CinPad][CoutPad] (lib/layers.py:12-23).
 // perm[packed_ci] = original input channel, or -1 for a zero (padding) channel.
 bool Engine::make_conv(ConvLayer& L, const std::string& prefix, const std::vector<int>& perm, int cin_pad, int k,
-                       int stride, int dh, int dw, int act, int H, int W) {
+                       int stride, int dh, int dw, int act, int H, int W, bool rows_wide) {
   L.name = prefix;
   L.k = k; L.stride = stride; L.dil_h = dh; L.dil_w = dw; L.act = act;
   auto itw = sd_.find(prefix + ".conv.0.weight");
@@ -170,7 +170,7 @@ bool Engine::make_conv(ConvLayer& L, const std::string& prefix, const std::vecto
     bias[(size_t)co] = (float)((double)b->data[co] - (double)m->data[co] * scale[(size_t)co]);
   }
   if (!pack_conv(L, arena_, w.data.data(), Cout, Cin, scale.data(), bias.data(), perm)) return false;
-  return cfg_.conv_mode != 0 || tc_prepare(L, H, W, err);
+  return cfg_.conv_mode != 0 || tc_prepare(L, H, W, rows_wide, err);
 }
 
 bool Engine::pack_conv(ConvLayer& L, Arena& arena, const float* w, int Cout, int Cin, const double* scale,
@@ -239,9 +239,9 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
   if (!make_conv(P.dec[1], prefix + ".dec3.conv1", identity_perm(10 * n, 10 * n), 10 * n, 3, 1, 1, 1, ACT_RELU, H / 4,
                  W / 4))
     return false;
-  P.dec[2].rows_wide = true;   // dec2's upsample is fused into the row kernel whenever 4n is a multiple of 32
+  // rows_wide: dec2's upsample is fused into the row kernel whenever 4n is a multiple of 32
   if (!make_conv(P.dec[2], prefix + ".dec2.conv1", identity_perm(6 * n, 6 * n), 6 * n, 3, 1, 1, 1, ACT_RELU, H / 2,
-                 W / 2))
+                 W / 2, true))
     return false;
   // dec1 input in the reference: cat[ up(cat[h (2n), lstm (1)]) , e1 (n) ]  (lib/nets.py:38-39, layers.py:52-56),
   // reduced as [ up(h) 2n | zeros up to Up | e1 n | zeros up to Lp | up(lstm) 1 | 15 zeros ] (BaseNetPlan, engine.h)
@@ -260,6 +260,7 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
   // activation buffers: the decoders' plans decide what their concat buffers hold
   P.fused2 = P.dec[2].tc && P.dec[2].tc->fuses_upsample(4 * n);
   P.fused1 = P.dec[3].tc && P.dec[3].tc->fuses_upsample(Up);
+  P.dot2 = P.dec[2].tc && P.dec[2].tc->fuses_dot();
   P.lstm_own = P.fused1 && n % 32 == 0;
   const int c1_first = P.fused1 ? Up : 0;   // the first of dec1's reduction channels that cat1 holds
   P.lstm_coff = Lp - c1_first;
@@ -483,10 +484,13 @@ bool Engine::profile_dump(std::string& text) {
   return true;
 }
 
-bool Engine::run_conv(ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, const ActView* up_src,
-                      const ActView* extra) {
-  ++launches;
+bool Engine::run_conv(const ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, const ConvFusion& f) {
   const bool use_tc = L.tc != nullptr;
+  if (!use_tc && !f.empty()) {
+    err = "internal: fused work requested for a CUDA-core convolution";
+    return false;
+  }
+  ++launches;
   if (!use_tc && cfg_.conv_mode == 0 && L.Cout >= 4 && !warned_simt_) {
     // loud, once per context: this geometry does not tile for the wgmma kernels (e.g. a cropsize whose feature-map
     // widths are not powers of two / multiples of 128) and runs on the fp32 CUDA-core kernel, an order of magnitude slower
@@ -498,44 +502,42 @@ bool Engine::run_conv(ConvLayer& L, const ActView& in, const ActView& out, cudaS
   }
   // algorithmic FLOPs with the real (un-padded) channel counts: 2 * pixels * Cout * Cin * taps, over the computed
   // columns only (a fused output layer computes the kept ones)
-  const int cols = L.mask ? out.W - 2 * L.mask->offset : out.W;
-  const std::string name = L.name + (up_src ? "+up" : "") + (L.mask ? "+mask" : "");
+  const int cols = f.mask ? out.W - 2 * f.mask->offset : out.W;
+  const std::string name = L.name + (f.up ? "+up" : "") + (f.mask ? "+mask" : "");
   const int pi = prof_begin(name, use_tc ? 1 : 0, 2.0 * (double)out.N * out.H * cols * L.Cout * L.Cin * L.k * L.k,
                             out.N, out.H, out.W, s);
-  bool ok = run_conv_inner(L, in, out, use_tc, s, up_src, extra);
+  bool ok;
+  if (use_tc) {
+    ok = ck(tc_launch(L, in, out, s, err, f), L.name.c_str());
+  } else {
+    ConvParams p;
+    p.in = in; p.out = out;
+    p.w = L.w; p.bias = L.bias;
+    p.CinPad = L.CinPad; p.Cout = L.Cout; p.CoutPad = L.CoutPad;
+    p.KH = L.k; p.KW = L.k; p.stride = L.stride;
+    p.dil_h = L.dil_h; p.dil_w = L.dil_w;
+    p.pad_h = L.dil_h * (L.k / 2); p.pad_w = L.dil_w * (L.k / 2);
+    p.act = L.act;
+    p.in.C = L.CinPad;
+    ok = ck(launch_conv_simt(p, s), L.name.c_str());
+  }
   prof_end(pi, s);
   return ok;
 }
 
-bool Engine::run_conv_inner(ConvLayer& L, const ActView& in, const ActView& out, bool use_tc, cudaStream_t s,
-                            const ActView* up_src, const ActView* extra) {
-  if (use_tc) return ck(tc_launch(L, in, out, s, err, up_src, extra), L.name.c_str());
-  if (up_src || extra || L.mask) {
-    err = "internal: fused upsample or output layer requested for a CUDA-core convolution";
-    return false;
+bool Engine::run_decoder(const ConvLayer& L, const ActView& low, const Buffer& cat, int N, const ActView& out,
+                         bool fused, cudaStream_t s, ConvFusion f) {
+  if (fused) {
+    f.up = &low;
+    return run_conv(L, cat.all(N), out, s, f);
   }
-  ConvParams p;
-  p.in = in; p.out = out;
-  p.w = L.w; p.bias = L.bias;
-  p.CinPad = L.CinPad; p.Cout = L.Cout; p.CoutPad = L.CoutPad;
-  p.KH = L.k; p.KW = L.k; p.stride = L.stride;
-  p.dil_h = L.dil_h; p.dil_w = L.dil_w;
-  p.pad_h = L.dil_h * (L.k / 2); p.pad_w = L.dil_w * (L.k / 2);
-  p.act = L.act;
-  p.in.C = L.CinPad;
-  return ck(launch_conv_simt(p, s), L.name.c_str());
-}
-
-bool Engine::run_decoder(ConvLayer& L, const ActView& low, const Buffer& cat, int N, const ActView& out, bool fused,
-                         cudaStream_t s) {
-  if (fused) return run_conv(L, cat.all(N), out, s, &low);
   if (!timed("upsample2x", 1, N, cat.H, cat.W, s, [&] { return ck(launch_upsample2x(low, cat.view(N, 0, cat.H, 0, low.C), s), "decoder upsample"); }))
     return false;
-  return run_conv(L, cat.all(N), out, s);
+  return run_conv(L, cat.all(N), out, s, f);
 }
 
 bool Engine::run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, int N, cudaStream_t s,
-                         cudaStream_t side) {
+                         cudaStream_t side, const MaskOutParams* mask) {
   const int n = P.n, H = P.H;
   // encoders (lib/nets.py:27-31); each skip tensor is written straight into its decoder's concat buffer
   ActView e1 = P.cat1.view(N, 0, H, P.fused1 ? 0 : P.d2.C, n);   // staged: after up(h), which is as wide as d2
@@ -569,16 +571,13 @@ bool Engine::run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, 
   // output: the row kernel's epilogue accumulates it from the fp32 activations it is about to store.
   LstmPlan& Q = P.lstm;
   const ActView d2 = P.d2.all(N), h = P.d2.view(N, 0, H / 2, 0, 2 * n);
-  const bool dot_fused = P.dec[2].tc && P.dec[2].tc->kind == TC_ROWS;
-  if (dot_fused) {
+  ConvFusion dot;
+  if (P.dot2) {
     if (!ck(cudaMemsetAsync(Q.l0, 0, sizeof(float) * (size_t)N * Q.bins * Q.T, s), "lstm conv clear")) return false;
-    P.dec[2].dot_w = Q.conv_w;
-    P.dec[2].dot_out = Q.l0;
+    dot.dot_w = Q.conv_w;
+    dot.dot_out = Q.l0;
   }
-  const bool dec2_ok = run_decoder(P.dec[2], P.d3.all(N), P.cat2, N, h, P.fused2, s);
-  P.dec[2].dot_w = nullptr;
-  P.dec[2].dot_out = nullptr;
-  if (!dec2_ok) return false;
+  if (!run_decoder(P.dec[2], P.d3.all(N), P.cat2, N, h, P.fused2, s, dot)) return false;
   // LSTM branch -> up(lstm), dec1's last reduction group (lib/nets.py:38, lib/layers.py:124-133).  Its 128-step
   // recurrence keeps only 2N CTAs busy, so when a side stream is free (stage 3) it runs there while the main stream
   // upsamples h for a staged dec1.
@@ -588,7 +587,7 @@ bool Engine::run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, 
     if (!ck(cudaEventRecord(ev_lstm_fork_, s), "lstm fork") || !ck(cudaStreamWaitEvent(side, ev_lstm_fork_, 0), "lstm fork"))
       return false;
   }
-  if (!dot_fused &&
+  if (!P.dot2 &&
       !timed("lstm.inconv", 1, N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_inconv(h, Q.conv_w, Q.l0, sl), "lstm conv"); }))
     return false;
   if (!timed("lstm.input_projection", 1, N, H / 2, P.W / 2, sl, [&] { return ck(launch_lstm_input_projection(Q.l0, Q.conv_bias, Q.wih, Q.bih, Q.xp, N, Q.T, Q.bins, 8 * Q.hid, sl), "lstm input projection"); }))
@@ -609,7 +608,11 @@ bool Engine::run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, 
     if (!ck(cudaEventRecord(ev_lstm_join_, side), "lstm join") || !ck(cudaStreamWaitEvent(s, ev_lstm_join_, 0), "lstm join"))
       return false;
   }
-  return run_conv(P.dec[3], P.cat1.all(N), out, s, P.fused1 ? &d2 : nullptr, P.lstm_own ? &up_lstm : nullptr);
+  ConvFusion f1;
+  f1.up = P.fused1 ? &d2 : nullptr;
+  f1.last_chunk = P.lstm_own ? &up_lstm : nullptr;
+  f1.mask = mask;
+  return run_conv(P.dec[3], P.cat1.all(N), out, s, f1);
 }
 
 bool Engine::forward(int N, const MaskOutParams& mask, cudaStream_t s) {
@@ -641,14 +644,10 @@ bool Engine::forward(int N, const MaskOutParams& mask, cudaStream_t s) {
   // Stage 3 (lib/nets.py:101-102) and the output layer (lib/nets.py:109-115, 127-129).  dec1 is a 3x3 convolution and
   // `out` a 1x1 one, so a kept frame needs dec1 at that frame only: where the row kernel can apply the output layer,
   // dec1 computes just the kept frames and writes the mask, and f3_ is not written.
-  ConvLayer& dec1 = nets_[4].dec[3];
-  const int kept = cfg_.cropsize - 2 * mask.offset;
-  const bool crop = g_debug.crop_mask == 1 && nets_[4].fused1 && dec1.tc && dec1.tc->fuses_mask(dec1.Cout) &&
-                    mask.offset >= 0 && kept > 0 && kept % 128 == 0;
-  if (crop) dec1.mask = &mask;
-  const bool ok = run_basenet(nets_[4], in3_.all(N), f3_.all(N), N, s, two ? s_hi_ : nullptr);
-  dec1.mask = nullptr;
-  if (!ok) return false;
+  const ConvLayer& dec1 = nets_[4].dec[3];
+  const bool crop = g_debug.crop_mask == 1 && dec1.tc && dec1.tc->fuses_mask(dec1.Cout, mask.offset, nets_[4].fused1);
+  if (!run_basenet(nets_[4], in3_.all(N), f3_.all(N), N, s, two ? s_hi_ : nullptr, crop ? &mask : nullptr))
+    return false;
   if (crop) return true;
   return timed("mask_out", 1, N, mask.f3.H, mask.f3.W, s, [&] { return ck(launch_mask_out(mask, s), "mask_out"); });
 }
@@ -1006,14 +1005,14 @@ bool Engine::debug_conv(const float* x_nchw, int N, int Cin, int H, int W, const
   const Buffer bout = make_buffer(arena, N, Ho, Wo, round_up(Cout, 8));
   ConvLayer L;
   L.name = "debug_conv";
-  L.rows_wide = g_debug.rows_wide == 1;   // vr_debug_set(2, 1): exercise the 64-wide row tile on a plain convolution
   L.k = k; L.stride = stride; L.dil_h = dil_h; L.dil_w = dil_w; L.act = act;
   if (!bin.hi || !bout.hi || !debug_weights(L, arena, w, bias, Cout, Cin, identity_perm(Cin, cin_pad), s)) return false;
   if (!timed("nchw_to_act", 1, N, H, W, s,
              [&] { return ck(launch_nchw_to_act(x_nchw, Cin, bin.all(N), s), "nchw_to_act"); }))
     return false;
   if (use_tc) {
-    if (!tc_prepare(L, Ho, Wo, err)) return false;
+    // vr_debug_set(2, 1): exercise the 64-wide row tile on a plain convolution
+    if (!tc_prepare(L, Ho, Wo, g_debug.rows_wide == 1, err)) return false;
     if (!L.tc) {
       err = "debug_conv: geometry not supported by the wgmma kernel";
       return false;
@@ -1042,7 +1041,6 @@ bool Engine::debug_decoder(const float* low_nchw, int N, int Cl, int h, int w, c
   const Buffer bout = make_buffer(arena, N, H, W, round_up(Cout, 16));
   ConvLayer L;
   L.name = "debug_decoder";
-  L.rows_wide = true;
   L.k = 3; L.act = act;
   std::vector<int> perm((size_t)cin_pad, -1);   // reduction order: [up Cl | pad | skip Cs]
   for (int i = 0; i < Cl; ++i) perm[(size_t)i] = i;
@@ -1053,7 +1051,7 @@ bool Engine::debug_decoder(const float* low_nchw, int N, int Cl, int h, int w, c
              [&] { return ck(launch_nchw_to_act(low_nchw, Cl, blow.all(N), s), "nchw_to_act low"); }) ||
       !timed("nchw_to_act", 1, N, H, W, s,
              [&] { return ck(launch_nchw_to_act(skip_nchw, Cs, skip, s), "nchw_to_act skip"); }) ||
-      !tc_prepare(L, H, W, err))
+      !tc_prepare(L, H, W, true, err))
     return false;
   if (fused && !(L.tc && L.tc->fuses_upsample(blow.C))) {
     err = "debug_decoder: geometry not supported by the fused row kernel";

@@ -102,15 +102,22 @@ struct ConvLayer {
   float* bias = nullptr;   // device fp32 [CoutPad]
   std::vector<float> w_host;     // packed copy kept for the tensor-core packer
   std::vector<float> bias_host;
-  bool rows_wide = false;        // row kernel: 64 output channels per tile (decoder layers whose upsample is fused)
-  // set around ONE launch by the caller: the row kernel also accumulates sum_c dot_w[c] * y[c] per output pixel into the
-  // pre-zeroed plane dot_out[n][h][w] (the LSTM branch's 1x1 input convolution fused into dec2)
+  std::shared_ptr<TcConv> tc;    // the tensor-core kernel and its packed weights; null -> CUDA-core kernel
+};
+
+// Work one convolution launch does besides the layer; the default is none.  Only the row kernel implements it (what a
+// plan can fuse: TcConv::fuses_*); every other path rejects a launch that asks for any.
+struct ConvFusion {
+  const ActView* up = nullptr;           // the leading up->C input channels are the x2 upsample of *up; `in` the rest
+  const ActView* last_chunk = nullptr;   // the last channel chunk is read from here, zero-filled up to the chunk
+  // sum_c dot_w[c] * y[c] of every output pixel is added to the pre-zeroed plane dot_out[n][h][w] (the LSTM branch's
+  // 1x1 input convolution fused into dec2)
   const float* dot_w = nullptr;
   float* dot_out = nullptr;
-  // set around ONE launch by the caller (stage 3's dec1): the row kernel computes only the output columns
-  // [mask->offset, W - mask->offset) and writes the network's mask there (mask_out_kernel's work) instead of the layer
+  // stage 3's dec1: only the output columns [mask->offset, W - mask->offset) are computed, and the network's mask is
+  // written there (mask_out_kernel's work) instead of the layer
   const MaskOutParams* mask = nullptr;
-  std::shared_ptr<TcConv> tc;    // the tensor-core kernel and its packed weights; null -> CUDA-core kernel
+  bool empty() const { return !up && !last_chunk && !dot_w && !dot_out && !mask; }
 };
 
 struct LstmPlan {
@@ -144,6 +151,7 @@ struct BaseNetPlan {
   //   of its own, so that cat1 = [e1 n] stays dense for enc2.conv1; the row kernel reads it as its last chunk through a
   //   second tensor map whose box TMA zero-fills.
   bool fused2 = false, fused1 = false;   // dec2 / dec1 fuse their upsample
+  bool dot2 = false;                     // dec2's epilogue computes the LSTM branch's 1x1 input convolution (fuses_dot)
   bool lstm_own = false;                 // the up(lstm) group is lstm_up, not in cat1
   int lstm_coff = 0;                     // channel offset of the up(lstm) group in cat1 (when not lstm_own)
   Buffer cat1, t2, cat2, t3, cat3, t4, cat4, t5, e5, pool, f1, acat, ao, d4, d3, d2, lstm_up;
@@ -275,9 +283,9 @@ class Engine {
   void* dalloc(Arena& arena, size_t bytes, const void* host = nullptr);
   Buffer make_buffer(Arena& arena, int N, int H, int W, int C, int pad_w = 0);
   bool need(const std::string& key, std::initializer_list<int64_t> shape, const HostTensor** out);
-  // H x W: the layer's output maps, from which tc_prepare chooses its kernel
+  // H x W: the layer's output maps, from which tc_prepare chooses its kernel (rows_wide: see tc_prepare)
   bool make_conv(ConvLayer& L, const std::string& prefix, const std::vector<int>& perm, int cin_pad, int k, int stride,
-                 int dh, int dw, int act, int H, int W);
+                 int dh, int dw, int act, int H, int W, bool rows_wide = false);
   // Packs OIHW weights w [Cout][Cin][L.k][L.k], output channel co times scale[co] (in double, rounded to float once),
   // to L.w_host [tap][CinPad][CoutPad] with CinPad = perm.size(): packed input channel pc holds channel perm[pc], or
   // zeros where that is -1.  Sets L's channel counts and uploads the weights and the bias [Cout] to L.w / L.bias.
@@ -289,16 +297,14 @@ class Engine {
   bool to_nchw(const ActView& v, int C, float* y_nchw, cudaStream_t s);
   bool build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, const std::vector<int>& in_perm, int cin_pad,
                      int n, int H, int W, int nin_lstm, int nout_lstm);
-  bool run_conv(ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, const ActView* up_src = nullptr,
-                const ActView* extra = nullptr);
-  bool run_conv_inner(ConvLayer& L, const ActView& in, const ActView& out, bool use_tc, cudaStream_t s,
-                      const ActView* up_src, const ActView* extra);
+  bool run_conv(const ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, const ConvFusion& f = {});
   // Decoder (lib/layers.py:51-64): conv(cat[up(low), skip]) -> out.  fused: the row kernel produces up(low) itself and
   // `cat` holds only the skip channels; else up(low) is first written into channels [0, low.C) of `cat`.
-  bool run_decoder(ConvLayer& L, const ActView& low, const Buffer& cat, int N, const ActView& out, bool fused,
-                   cudaStream_t s);
+  bool run_decoder(const ConvLayer& L, const ActView& low, const Buffer& cat, int N, const ActView& out, bool fused,
+                   cudaStream_t s, ConvFusion f = {});
+  // mask != nullptr: dec1 writes the network's mask in its epilogue instead of `out` (dec1.tc->fuses_mask)
   bool run_basenet(BaseNetPlan& P, const ActView& in, const ActView& out, int N, cudaStream_t s,
-                   cudaStream_t side = nullptr);
+                   cudaStream_t side = nullptr, const MaskOutParams* mask = nullptr);
   // in3_ x-channels already packed for N windows -> the mask of frames [mask.offset, W - mask.offset) of every window,
   // written as mask describes (mask.f3 = f3_.all(N))
   bool forward(int N, const MaskOutParams& mask, cudaStream_t s);
@@ -306,9 +312,10 @@ class Engine {
   bool ck(cudaError_t e, const char* what);
 };
 
-// conv_tc.cu: plans L.tc for output maps of H x W (left null when the layer stays on the CUDA-core kernel)
-bool tc_prepare(ConvLayer& L, int H, int W, std::string& err);
-cudaError_t tc_launch(ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, std::string& err,
-                      const ActView* up_src = nullptr, const ActView* extra = nullptr);
+// conv_tc.cu: plans L.tc for output maps of H x W (left null when the layer stays on the CUDA-core kernel).
+// rows_wide: the row kernel may use its 64-output-channel tile (decoder layers whose upsample it fuses).
+bool tc_prepare(ConvLayer& L, int H, int W, bool rows_wide, std::string& err);
+cudaError_t tc_launch(const ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, std::string& err,
+                      const ConvFusion& f);
 
 }  // namespace vr

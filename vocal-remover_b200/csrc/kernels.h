@@ -71,8 +71,8 @@ cudaError_t launch_validation_l1(const float2* spec_x, const float2* spec_y, con
                                  cudaStream_t stream);
 
 // ---- LSTM branch (lstm.cu), reference lib/layers.py:108-133 ------------------------------------
-// 1x1 conv (C -> 1), pre-activation sums as an fp32 plane l0[n][bin][t] (the row kernel's epilogue accumulates the same
-// sums when the layer that produces `in` runs there: RowsDot in tc_plan.h)
+// 1x1 conv (C -> 1), pre-activation sums as an fp32 plane l0[n][bin][t] (dec2's epilogue accumulates the same sums
+// instead where its plan can: ConvFusion::dot_w in engine.h, TcConv::fuses_dot)
 cudaError_t launch_lstm_inconv(ActView in, const float* w, float* l0, cudaStream_t stream);
 // xp[(n,t)][gates] = relu(l0[n][:][t] + conv_bias) . wih[gates][:]^T + bih   (gates = 8 * hid)
 cudaError_t launch_lstm_input_projection(const float* l0, float conv_bias, const float* wih, const float* bih, float* xp,

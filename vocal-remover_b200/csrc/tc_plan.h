@@ -34,29 +34,39 @@ struct TcConv {
   DevPtr<float> bias;   // [n_tiles*BN]
   CUtensorMap map_b;
   std::map<ViewKey, CUtensorMap> map_a;
+  // What a launch of this plan can fuse (ConvFusion); the launchers reject anything else.
   // the row kernel can produce the leading up_C channels of its input as the x2 upsample of a half-resolution tensor
   bool fuses_upsample(int up_C) const { return kind == TC_ROWS && up_C % 32 == 0 && up_C <= CinPad; }
-  // the row kernel can apply the network's output layer (mask_out_kernel) in its epilogue: one quad of lanes must hold
-  // all Cout channels of a pixel, and only the BN <= 32 instantiations with a fused upsample carry that epilogue
-  bool fuses_mask(int Cout) const { return kind == TC_ROWS && n_tiles == 1 && BN <= 32 && BN == Cout; }
+  // the row kernel can accumulate a 1x1 convolution to one channel in its epilogue
+  bool fuses_dot() const { return kind == TC_ROWS; }
+  // the row kernel can compute only the columns [offset, W - offset), in whole 128-pixel tiles, and apply the network's
+  // output layer (mask_out_kernel) there in its epilogue: one quad of lanes must hold all Cout channels of a pixel, and
+  // only the BN <= 32 instantiations with a fused upsample (up) carry that epilogue
+  bool fuses_mask(int Cout, int offset, bool up) const {
+    const int kept = W - 2 * offset;
+    return kind == TC_ROWS && up && n_tiles == 1 && BN <= 32 && BN == Cout && offset >= 0 && kept > 0 &&
+           kept % 128 == 0;
+  }
 };
 
-TcKind tc_choose(const ConvLayer& L, int H, int W);
+TcKind tc_choose(const ConvLayer& L, int H, int W, bool rows_wide);
 // tensor map of an activation view: both split-bf16 planes in one box of {tc.KB, bw, bh, bn, 2} elements, element
 // stride es along W and H; cached in the plan.  nullptr (err set) if TMA cannot read the view.
 const CUtensorMap* tc_activation_map(TcConv& tc, const ActView& v, int bw, int bh, int bn, int es, std::string& err,
                                      const std::string& name);
 
 // conv_tc_rows.cu
-cudaError_t tc_rows_launch(ConvLayer& L, TcConv& tc, const ActView& in, const ActView& out, cudaStream_t s,
-                           std::string& err, const ActView* up_src, const ActView* extra);
+cudaError_t tc_rows_launch(const ConvLayer& L, TcConv& tc, const ActView& in, const ActView& out, cudaStream_t s,
+                           std::string& err, const ConvFusion& f);
 void tc_rows_set_attributes(int max_smem);
+bool tc_rows_has(int BN);   // the row kernel is instantiated for this BN
 int tc_rows_read_trace(unsigned long long* out, long long capacity);
 
 // conv_tc_halo.cu
-cudaError_t tc_halo_launch(ConvLayer& L, TcConv& tc, const ActView& in, const ActView& out, cudaStream_t s,
+cudaError_t tc_halo_launch(const ConvLayer& L, TcConv& tc, const ActView& in, const ActView& out, cudaStream_t s,
                            std::string& err);
 void tc_halo_set_attributes(int max_smem);
+bool tc_halo_has(int BN);   // the halo kernel is instantiated for this BN
 
 // Properties of the CURRENT device, cached per device ordinal.  The first use on a device also opts the tensor-core
 // kernels in to their dynamic shared memory there (cudaFuncSetAttribute is per device, so a process that drives
