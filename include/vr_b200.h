@@ -170,6 +170,25 @@ VR_API int vr_resample(vr_ctx* ctx, const float* x, int32_t channels, int64_t n_
                        double sample_ratio, const double* win, const double* delta, int32_t nwin,
                        int32_t table_per_crossing, void* stream);
 
+/* FLAC decoding on the device (RFC 9639; lib/flac.py is the caller, oracle/flac_oracle.py restates the format).  All
+ * buffers are DEVICE memory owned by the caller; neither call allocates.  ctx may be NULL, as for vr_resample: the
+ * call then runs on the calling thread's current device and its error message is read with vr_last_error(NULL).
+ *
+ * vr_flac_scan: every frame-header candidate (sync 0xFFF8 / 0xFFF9, a parsable header, matching CRC-8) at a byte
+ * offset in [begin, n_bytes) of data.  Writes min(count, max_cands) rows of 4 int64, in no particular order:
+ * (offset, coded frame or sample number, block size | header length << 17 | variable-strategy bit << 22,
+ * header byte 2 | byte 3 << 8 | coded sample-rate value << 16); *count (one int32) is set to the number found.
+ *
+ * vr_flac_decode: one warp per frame.  frames: n_frames rows of 4 int64 (start byte, the next frame's start byte or,
+ * for the last frame, the end of the audio data, first sample, block size | header length << 17 | channel code << 24 |
+ * bits per sample << 28).  out: [channels][n_samples] float32, float32(x) / 2^(bps-1).  status: one
+ * int64 per frame, 0 when the frame decoded, ends 2 bytes before the next frame's start and its CRC-16 matches, else
+ * code << 40 | bit offset in the frame (codes: lib/flac.py).  Malformed bytes never fault: they give a status. */
+VR_API int vr_flac_scan(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, int64_t begin, int64_t* cands,
+                        int32_t max_cands, int32_t* count, void* stream);
+VR_API int vr_flac_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int64_t* frames, int32_t n_frames,
+                          int32_t channels, int64_t n_samples, float* out, int64_t* status, void* stream);
+
 /* Multi-GPU mask exchange over NVLink peer memory (one process per GPU).  The owner (rank 0) allocates the
  * whole-track mask with vr_shared_alloc and publishes the 64-byte CUDA IPC handle; every other rank maps it
  * with vr_shared_open and passes the mapped pointer as `mask` to vr_separate_windows, so the mask epilogue

@@ -234,6 +234,30 @@ int vr_resample(vr_ctx* ctx, const float* x, int32_t channels, int64_t n_in, flo
   return 0;
 }
 
+// ctx may be NULL for both FLAC calls, as for vr_resample
+static int flac_result(vr_ctx* ctx, const char* what, cudaError_t e) {
+  if (e == cudaSuccess) return 0;
+  const std::string m = std::string(what) + ": " + cudaGetErrorString(e);
+  if (ctx) return fail(ctx, m);
+  g_create_err = m;
+  return -1;
+}
+
+int vr_flac_scan(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, int64_t begin, int64_t* cands, int32_t max_cands,
+                 int32_t* count, void* stream) {
+  if (ctx && ctx->eng) cudaSetDevice(ctx->eng->cfg().device);
+  return flac_result(ctx, "vr_flac_scan",
+                     vr::launch_flac_scan(data, n_bytes, begin, cands, max_cands, count, (cudaStream_t)stream));
+}
+
+int vr_flac_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int64_t* frames, int32_t n_frames,
+                   int32_t channels, int64_t n_samples, float* out, int64_t* status, void* stream) {
+  if (ctx && ctx->eng) cudaSetDevice(ctx->eng->cfg().device);
+  return flac_result(ctx, "vr_flac_decode",
+                     vr::launch_flac_decode(data, n_bytes, frames, n_frames, channels, n_samples, out, status,
+                                            (cudaStream_t)stream));
+}
+
 int vr_shared_alloc(vr_ctx* ctx, int64_t bytes, void** dev_ptr, unsigned char* handle64) {
   CHECK_CTX(ctx);
   if (!dev_ptr || !handle64 || bytes <= 0) return fail(ctx, "vr_shared_alloc: bad arguments");

@@ -106,4 +106,14 @@ cudaError_t launch_istft_ola(const float* frames_a, const float* frames_b, int n
 cudaError_t launch_resample_sinc(const float* x, int C, int64_t n_in, float* y, int64_t n_out, double sample_ratio,
                                  const double* win, const double* delta, int nwin, int num_table, cudaStream_t stream);
 
+// ---- FLAC frame decoding (flac.cu), the decode in front of the path for .flac input (lib/flac.py) --------------------
+// scan: every frame-header candidate at byte offsets [begin, n_bytes) -> cands[*count][4] (at most max_cands written;
+// *count is zeroed first and counts them all); decode: one warp per chained frame, frames[n_frames][4] = (start byte,
+// next frame's start byte or n_bytes, first sample, block size | header length << 17 | channel code << 24 |
+// bps << 28) -> out [channels][n_samples] float32, status[n_frames]
+cudaError_t launch_flac_scan(const uint8_t* data, int64_t n_bytes, int64_t begin, int64_t* cands, int max_cands,
+                             int* count, cudaStream_t stream);
+cudaError_t launch_flac_decode(const uint8_t* data, int64_t n_bytes, const int64_t* frames, int n_frames, int channels,
+                               int64_t n_samples, float* out, int64_t* status, cudaStream_t stream);
+
 }  // namespace vr

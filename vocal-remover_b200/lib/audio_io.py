@@ -1,8 +1,9 @@
 """Audio file I/O either side of the hot path (SURVEY 8(f) rank 2).
 
 The reference uses ``librosa.load(path, sr=sr, mono=False, dtype=np.float32, res_type='kaiser_fast')`` and
-``soundfile.write`` (inference.py:136-138,173,178).  Decoding and encoding stay on the host (librosa / soundfile when
-installed, else a stdlib ``wave`` reader / writer for PCM WAV); the sample-rate conversion of non-``sr`` input - the
+``soundfile.write`` (inference.py:136-138,173,178).  FLAC input is decoded on the GPU when there is one (lib/flac.py,
+csrc/flac.cu); other decoding and all encoding stay on the host (soundfile when installed, else a stdlib ``wave``
+reader for 8/16/24/32-bit PCM WAV and writer for 16-bit); the sample-rate conversion of non-``sr`` input - the
 expensive part of ``librosa.load`` - runs on the GPU (``vr_resample``, csrc/resample.cu): resampy 0.4's algorithm with the
 ``kaiser_fast`` table taken from an installed resampy, or regenerated from its documented parameters otherwise
 (oracle/resample_oracle.py states what is and is not pinned).
@@ -72,19 +73,33 @@ def resample(y, orig_sr, target_sr, device=None, filt=None):
     return out if is_tensor else out.cpu().numpy().astype(np.asarray(y).dtype if np.asarray(y).dtype.kind == 'f' else np.float32)
 
 
-def _decode(path):
-    """(channels, n) float32 at the file's own rate."""
+def _decode(path, device=None):
+    """(channels, n) float32 at the file's own rate.  FLAC (recognised by content) is decoded on the GPU whenever a
+    CUDA device is visible (lib/flac.py); otherwise soundfile reads it if it is installed."""
+    from . import flac
+    is_flac = flac.sniff(path)
+    if is_flac:
+        import torch
+        if torch.cuda.is_available():
+            x, rate, _ = flac.decode(path, device)
+            return x.cpu().numpy(), rate
     try:
         import soundfile as sf
         data, rate = sf.read(path, dtype='float32', always_2d=True)
         return np.ascontiguousarray(data.T), rate
     except ImportError:
         pass
+    if is_flac:
+        raise RuntimeError('%s is a FLAC file: decoding it needs a CUDA device (lib/flac.py) or the soundfile module, '
+                           'and neither is available' % path)
     with _wave.open(path, 'rb') as f:
         nch, width, rate, nframes = f.getnchannels(), f.getsampwidth(), f.getframerate(), f.getnframes()
         raw = f.readframes(nframes)
     if width == 2:
         x = np.frombuffer(raw, dtype='<i2').astype(np.float32) / 32768.0
+    elif width == 3:
+        b = np.frombuffer(raw, dtype=np.uint8).reshape(-1, 3).astype(np.int32)
+        x = ((b[:, 0] | (b[:, 1] << 8) | (b[:, 2] << 16)) << 8 >> 8).astype(np.float32) / 8388608.0
     elif width == 4:
         x = np.frombuffer(raw, dtype='<i4').astype(np.float32) / 2147483648.0
     elif width == 1:
@@ -97,7 +112,7 @@ def _decode(path):
 def load(path, sr, mono=False, dtype=np.float32, device=None):
     """librosa.load(path, sr=sr, mono=mono, dtype=dtype, res_type='kaiser_fast'): (channels, n) or (n,) array, sr.
     As in librosa, the channels are averaged first (mono=True) and the result is then resampled."""
-    x, rate = _decode(path)
+    x, rate = _decode(path, device)
     if mono or x.shape[0] == 1:
         x = x.mean(axis=0)
     if sr is not None and rate != sr:
