@@ -71,12 +71,9 @@ __global__ void __launch_bounds__(kThreads, 1)
   const int num_iters = (p.total_sub + SUBS - 1) / SUBS;
 
   if (warp == kConsumerWarps && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-    for (int s = 0; s < p.stages; ++s) {
-      mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), kConsumerWarps);
-    }
+    tma_prefetch(&tmA);
+    tma_prefetch(&tmB);
+    MbarRing(smem_u32(&bar_full[0]), smem_u32(&bar_empty[0]), 0, p.stages).init(1, kConsumerWarps);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   for (int i = threadIdx.x; i < p.n_tiles * BN; i += blockDim.x) bias_s[i] = __ldg(p.bias + i);
@@ -85,9 +82,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   if (warp == kConsumerWarps) {
     // ===================== TMA producer (one elected lane runs the whole loop nest) =====================
     if (elect_one_sync()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      const uint32_t full0 = smem_u32(&bar_full[0]), empty0 = smem_u32(&bar_empty[0]);
+      MbarRing ring(smem_u32(&bar_full[0]), smem_u32(&bar_empty[0]), 0, p.stages);
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int nt = tile % p.n_tiles;
         const int mt = tile / p.n_tiles;
@@ -98,10 +93,10 @@ __global__ void __launch_bounds__(kThreads, 1)
         const int nrow = nt * BN;
         int cc = 0, kw = 0, kh = 0, sub = 0;   // (tap, channel chunk) of the next sub-tile, advanced without divisions
         for (int it = 0; it < num_iters; ++it) {
-          mbar_wait(empty0 + (uint32_t)stage * 8u, phase ^ 1u);
+          ring.wait_empty();
           const int nsub = min(SUBS, p.total_sub - sub);
-          const uint32_t full = full0 + (uint32_t)stage * 8u;
-          const uint32_t sbase = smem_base + (uint32_t)stage * kStageBytes;
+          const uint32_t full = ring.full();
+          const uint32_t sbase = smem_base + (uint32_t)ring.slot * kStageBytes;
           mbar_expect_tx(full, (uint32_t)nsub * (kASub + kBSub));
 #pragma unroll
           for (int j = 0; j < SUBS; ++j) {
@@ -119,10 +114,7 @@ __global__ void __launch_bounds__(kThreads, 1)
               }
             }
           }
-          if (++stage == p.stages) {
-            stage = 0;
-            phase ^= 1u;
-          }
+          ring.advance();
         }
       }
     }
@@ -130,20 +122,18 @@ __global__ void __launch_bounds__(kThreads, 1)
   } else {
     // ===================== consumer warpgroups: wgmma into registers, then the epilogue =====================
     const int wg = warp >> 2;   // pixels [64 wg, 64 wg + 64) of the tile
-    const float slope = p.act == ACT_RELU ? 0.f : p.act == ACT_LEAKY ? 0.01f : 1.f;
+    const float slope = act_slope(p.act);
     const uint32_t dhi = desc_hi(8 * KB * 2, kLayout);
-    const uint32_t full0 = smem_u32(&bar_full[0]), empty0 = smem_u32(&bar_empty[0]);
-    int stage = 0;
-    uint32_t phase = 0;
+    MbarRing ring(smem_u32(&bar_full[0]), smem_u32(&bar_empty[0]), 0, p.stages);
     float acc[BN / 2];
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-      int prev = -1;
+      HeldSlot held;
       for (int it = 0; it < num_iters; ++it) {
         const int nsub = min(SUBS, p.total_sub - it * SUBS);
-        mbar_wait(full0 + (uint32_t)stage * 8u, phase);
-        const uint32_t sdesc = desc_lo(smem_base + (uint32_t)stage * kStageBytes);
+        ring.wait_full();
+        const uint32_t sdesc = desc_lo(smem_base + (uint32_t)ring.slot * kStageBytes);
         wg_fence();
 #pragma unroll
         for (int j = 0; j < SUBS; ++j) {
@@ -159,19 +149,12 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
         wg_commit();
         wg_wait<1>();   // the group of the previous stage has read its operands: hand that slot back
-        if (prev >= 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(empty0 + (uint32_t)prev * 8u);
-        }
-        prev = stage;
-        if (++stage == p.stages) {
-          stage = 0;
-          phase ^= 1u;
-        }
+        held.release(ring, lane);
+        held.hold(ring);
+        ring.advance();
       }
       wg_wait<0>();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(empty0 + (uint32_t)prev * 8u);
+      held.release_last(ring, lane);
 
       const int nt = tile % p.n_tiles;
       const int mt = tile / p.n_tiles;

@@ -61,11 +61,10 @@ struct HaloParams {
   const float* bias;
 };
 
-// Consumer ring positions: halo slot, weight stage, and the weight stage whose last wgmma group may still be in flight
-// (released once the next group has been committed and the older one waited for).
+// The consumers' positions in the halo ring and the weight ring, and the weight stage still held
 struct HaloConsumer {
-  int hs, ws, pend_w;
-  uint32_t hph, wph;
+  MbarRing h, w;
+  HeldSlot held_w;
 };
 
 // One channel chunk.  Each (tap, k-step) is one commit group: the warp loads the 16 x 16 hi and lo fragments of its MB
@@ -79,11 +78,10 @@ struct HaloConsumer {
 template <int BN, int MB>
 __device__ __forceinline__ void consume_halo(HaloConsumer& st, const HaloParams& p, float* acc,
                                              uint32_t (&fr)[2][MB * 8], const uint32_t* q0, uint32_t h_base,
-                                             uint32_t w_base, uint32_t dhi, uint32_t hfull0,
-                                             uint32_t hempty0, uint32_t wfull0, uint32_t wempty0, int lane) {
+                                             uint32_t w_base, uint32_t dhi, int lane) {
   typedef HaloGeom<BN> G;
-  mbar_wait(hfull0 + (uint32_t)st.hs * 8u, st.hph);
-  const uint32_t slot = h_base + (uint32_t)st.hs * p.hslot;
+  st.h.wait_full();
+  const uint32_t slot = h_base + (uint32_t)st.h.slot * p.hslot;
 #pragma unroll
   for (int t = 0; t < 9; ++t) {
     const int kh = t / 3, kw = t % 3;
@@ -98,34 +96,21 @@ __device__ __forceinline__ void consume_halo(HaloConsumer& st, const HaloParams&
         ldsm_x4(f + 8 * b, a);
         ldsm_x4(f + 8 * b + 4, a + p.hplane);
       }
-      if (ks == 0) mbar_wait(wfull0 + (uint32_t)st.ws * 8u, st.wph);
-      const uint32_t b_hi = desc_lo(w_base + (uint32_t)st.ws * G::kWStage) + (uint32_t)(ks * 32 >> 4);
+      if (ks == 0) st.w.wait_full();
+      const uint32_t b_hi = desc_lo(w_base + (uint32_t)st.w.slot * G::kWStage) + (uint32_t)(ks * 32 >> 4);
       wg_fence();
 #pragma unroll
       for (int b = 0; b < MB; ++b)
         wgmma_split3_rs<BN>(acc + b * (BN / 2), f + 8 * b, f + 8 * b + 4, b_hi, b_hi + (G::kBPlane >> 4), dhi);
       wg_commit();
-      if (t == 8 && ks == 1) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(hempty0 + (uint32_t)st.hs * 8u);
-      }
+      if (t == 8 && ks == 1) warp_arrive(st.h.empty(), lane);
       wg_wait<1>();   // every group but this one is complete: its fragments and the weights it read can be reused
-      if (st.pend_w >= 0) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(wempty0 + (uint32_t)st.pend_w * 8u);
-        st.pend_w = -1;
-      }
+      st.held_w.release(st.w, lane);
     }
-    st.pend_w = st.ws;   // released after the next group, once this tap's k-step 1 group has completed
-    if (++st.ws == p.n_wstages) {
-      st.ws = 0;
-      st.wph ^= 1u;
-    }
+    st.held_w.hold(st.w);   // released after the next group, once this tap's k-step 1 group has completed
+    st.w.advance();
   }
-  if (++st.hs == p.n_hslots) {
-    st.hs = 0;
-    st.hph ^= 1u;
-  }
+  st.h.advance();
 }
 
 template <int BN, int MB>
@@ -145,24 +130,18 @@ __global__ void __launch_bounds__(kThreads, 1)
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t h_base = smem_base;
   const uint32_t w_base = smem_base + (uint32_t)p.n_hslots * p.hslot;
+  MbarRing hring(smem_u32(&bar_hfull[0]), smem_u32(&bar_hempty[0]), 0, p.n_hslots);
+  MbarRing wring(smem_u32(&bar_wfull[0]), smem_u32(&bar_wempty[0]), 0, p.n_wstages);
 
   if (warp == kConsumerWarps && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-    for (int s = 0; s < p.n_hslots; ++s) {
-      mbar_init(smem_u32(&bar_hfull[s]), 1);
-      mbar_init(smem_u32(&bar_hempty[s]), kConsumerWarps);
-    }
-    for (int s = 0; s < p.n_wstages; ++s) {
-      mbar_init(smem_u32(&bar_wfull[s]), 1);
-      mbar_init(smem_u32(&bar_wempty[s]), kConsumerWarps);
-    }
+    tma_prefetch(&tmA);
+    tma_prefetch(&tmB);
+    hring.init(1, kConsumerWarps);
+    wring.init(1, kConsumerWarps);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   for (int i = threadIdx.x; i < p.n_tiles * BN; i += blockDim.x) bias_s[i] = __ldg(p.bias + i);
   __syncthreads();
-  const uint32_t hfull0 = smem_u32(&bar_hfull[0]), hempty0 = smem_u32(&bar_hempty[0]);
-  const uint32_t wfull0 = smem_u32(&bar_wfull[0]), wempty0 = smem_u32(&bar_wempty[0]);
 
   // Consumers and producers split first: all four producer warps execute the one setmaxnreg.dec, as setmaxnreg requires
   // of every thread of a warpgroup, and ptxas allocates the consumer code for kConsumerRegs.
@@ -170,8 +149,6 @@ __global__ void __launch_bounds__(kThreads, 1)
     setmaxnreg_dec<kProducerRegs>();
     // ===================== TMA producer: one elected lane of warp 8 runs the whole loop nest =====================
     if (warp == kConsumerWarps && elect_one_sync()) {
-      int hs = 0, ws = 0;
-      uint32_t hph = 0, wph = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
         const int nt = tile % p.n_tiles;
         const int mt = tile / p.n_tiles;
@@ -179,23 +156,16 @@ __global__ void __launch_bounds__(kThreads, 1)
         const int n = mt / p.tiles_h;
         for (int cc = 0; cc < p.chunks; ++cc) {
           if (!chunk_groups(p.kmask, cc)) continue;   // no weights on this chunk: the consumers skip it too
-          mbar_wait(hempty0 + (uint32_t)hs * 8u, hph ^ 1u);
-          const uint32_t hfull = hfull0 + (uint32_t)hs * 8u;
-          mbar_expect_tx(hfull, p.hslot);
-          tma_load_5d(h_base + (uint32_t)hs * p.hslot, &tmA, cc * (int)kKB, -1, h0 - 1, n, 0, hfull);
-          if (++hs == p.n_hslots) {
-            hs = 0;
-            hph ^= 1u;
-          }
+          hring.wait_empty();
+          mbar_expect_tx(hring.full(), p.hslot);
+          tma_load_5d(h_base + (uint32_t)hring.slot * p.hslot, &tmA, cc * (int)kKB, -1, h0 - 1, n, 0, hring.full());
+          hring.advance();
           for (int t = 0; t < 9; ++t) {
-            mbar_wait(wempty0 + (uint32_t)ws * 8u, wph ^ 1u);
-            const uint32_t wfull = wfull0 + (uint32_t)ws * 8u;
-            mbar_expect_tx(wfull, G::kWStage);
-            tma_load_3d(w_base + (uint32_t)ws * G::kWStage, &tmB, t * p.CinPadH + cc * (int)kKB, nt * BN, 0, wfull);
-            if (++ws == p.n_wstages) {
-              ws = 0;
-              wph ^= 1u;
-            }
+            wring.wait_empty();
+            mbar_expect_tx(wring.full(), G::kWStage);
+            tma_load_3d(w_base + (uint32_t)wring.slot * G::kWStage, &tmB, t * p.CinPadH + cc * (int)kKB, nt * BN, 0,
+                        wring.full());
+            wring.advance();
           }
         }
       }
@@ -205,7 +175,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     // ===================== consumer warpgroups: wgmma into registers, then the epilogue =====================
     setmaxnreg_inc<kConsumerRegs>();
     const int wg = warp >> 2;   // m64 blocks [MB wg, MB wg + MB) of the tile
-    const float slope = p.act == ACT_RELU ? 0.f : p.act == ACT_LEAKY ? 0.01f : 1.f;
+    const float slope = act_slope(p.act);
     const uint32_t dhi = desc_hi(8 * kRowB, 2u);   // SWIZZLE_64B, 8-row groups of 64-byte rows
     uint32_t q0[MB];
 #pragma unroll
@@ -213,9 +183,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       const int px = 64 * (MB * wg + b) + 16 * (warp & 3) + (lane & 15);
       q0[b] = (uint32_t)((px >> p.lw) * p.Wb + (px & (p.W - 1)));
     }
-    HaloConsumer st;
-    st.hs = 0; st.ws = 0; st.pend_w = -1;
-    st.hph = 0; st.wph = 0;
+    HaloConsumer st{hring, wring};
     float acc[MB * BN / 2];
     uint32_t fr[2][MB * 8];
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
@@ -224,12 +192,10 @@ __global__ void __launch_bounds__(kThreads, 1)
       for (int cc = 0; cc < p.chunks; ++cc) {
         // a chunk whose weights are all zero is not issued: exact, since the products would be 0
         if (!chunk_groups(p.kmask, cc)) continue;
-        consume_halo<BN, MB>(st, p, acc, fr, q0, h_base, w_base, dhi, hfull0, hempty0, wfull0, wempty0, lane);
+        consume_halo<BN, MB>(st, p, acc, fr, q0, h_base, w_base, dhi, lane);
       }
       wg_wait<0>();
-      __syncwarp();
-      if (lane == 0 && st.pend_w >= 0) mbar_arrive(wempty0 + (uint32_t)st.pend_w * 8u);
-      st.pend_w = -1;
+      st.held_w.release_last(st.w, lane);
 
       const int nt = tile % p.n_tiles;
       const int mt = tile / p.n_tiles;

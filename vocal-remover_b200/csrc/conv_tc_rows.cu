@@ -134,13 +134,11 @@ __device__ __forceinline__ RowsTile rows_tile(const RowsParams& p, int tile) {
   return t;
 }
 
-// Consumer state across the rows of a tile: the A ring position of each producer's ring, the B buffer, and the weight
-// buffer whose last wgmma group may still be in flight (released once the NEXT group has been committed and the older
-// one waited for).
+// The consumers' positions in the two A rings (one per producer, see RowsParams::n_uslots) and in the weight ring,
+// and the weight buffer still held
 struct RowsConsumer {
-  int as_t, as_u, bs, as, pend_b;
-  uint32_t aph_t, aph_u, bph, aph;
-  int ring_lo, ring_hi;
+  MbarRing a_up, a_tma, b;
+  HeldSlot held_b;
 };
 
 // Input row r of one chunk.  For each kw tap the warp loads its 16 x 16 A fragments (hi and lo plane, both k-steps) of
@@ -152,16 +150,16 @@ struct RowsConsumer {
 // `wait_group 1` has retired it.  The wgmma read only weights from shared memory: the A slot is free once the last
 // ldmatrix of the row has returned.  Every accumulator receives its products in the order chunk, row, kw, k-step,
 // hi*hi, lo*hi, hi*lo.
-// ksm: k-steps (16 channels) of the chunk that carry weights (bit 0 / 1).  lrow: shared-memory address of this lane's
-// ldmatrix row (pixel 64 wg + 16 (warp % 4) + lane % 16) in slot 0; bsrc: descriptor low word of the weight buffer.
+// a: the A ring this chunk's rows come from; returned advanced past them.  ksm: k-steps (16 channels) of the chunk that
+// carry weights (bit 0 / 1).  lrow: shared-memory address of this lane's ldmatrix row (pixel 64 wg + 16 (warp % 4) +
+// lane % 16) in slot 0; bsrc: descriptor low word of the weight buffer.
 template <int BN, int R, int r>
-__device__ __forceinline__ void consume_rows(RowsConsumer& st, float* acc, uint32_t (&fr)[2][16], uint32_t lrow,
-                                             uint32_t bsrc, uint32_t dhi, uint32_t ksm, uint32_t afull0,
-                                             uint32_t aempty0, uint32_t bempty0, int lane) {
+__device__ __forceinline__ MbarRing consume_rows(MbarRing a, RowsConsumer& st, float* acc, uint32_t (&fr)[2][16],
+                                                 uint32_t lrow, uint32_t bsrc, uint32_t dhi, uint32_t ksm, int lane) {
   constexpr int o_lo = r - 2 < 0 ? 0 : r - 2;
   constexpr int o_hi = r > R - 1 ? R - 1 : r;
-  mbar_wait(afull0 + (uint32_t)st.as * 8u, st.aph);
-  const uint32_t row = lrow + (uint32_t)st.as * kASlot;
+  a.wait_full();
+  const uint32_t row = lrow + (uint32_t)a.slot * kASlot;
 #pragma unroll
   for (int kw = 0; kw < 3; ++kw) {
     uint32_t* f = fr[(3 * r + kw) & 1];
@@ -187,23 +185,15 @@ __device__ __forceinline__ void consume_rows(RowsConsumer& st, float* acc, uint3
       }
     }
     wg_commit();
-    if (kw == 2) {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(aempty0 + (uint32_t)st.as * 8u);
-    }
+    if (kw == 2) warp_arrive(a.empty(), lane);
     wg_wait<1>();   // every group but this one is complete: its fragments and the weights it read can be reused
-    if (st.pend_b >= 0) {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bempty0 + (uint32_t)st.pend_b * 8u);
-      st.pend_b = -1;
-    }
+    st.held_b.release(st.b, lane);
   }
-  if (++st.as == st.ring_hi) {
-    st.as = st.ring_lo;
-    st.aph ^= 1u;
-  }
+  a.advance();
   if constexpr (r + 1 < R + 2)
-    consume_rows<BN, R, r + 1>(st, acc, fr, lrow, bsrc, dhi, ksm, afull0, aempty0, bempty0, lane);
+    return consume_rows<BN, R, r + 1>(a, st, acc, fr, lrow, bsrc, dhi, ksm, lane);
+  else
+    return a;
 }
 
 // w[c] * act(v0 + bias[c]) + w[c + 1] * act(v1 + bias[c + 1]): this thread's share of the fused single-channel 1x1
@@ -268,19 +258,18 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_base = smem_base;
   const uint32_t b_base = smem_base + (uint32_t)p.n_aslots * kASlot;
+  // the A slots hold one ring per producer: [0, n_uslots) for the interpolation warps, [n_uslots, n_aslots) for TMA
+  MbarRing a_up(smem_u32(&bar_afull[0]), smem_u32(&bar_aempty[0]), 0, p.n_uslots);
+  MbarRing a_tma(smem_u32(&bar_afull[0]), smem_u32(&bar_aempty[0]), p.n_uslots, p.n_aslots);
+  MbarRing b_ring(smem_u32(&bar_bfull[0]), smem_u32(&bar_bempty[0]), 0, 2);
 
   if (warp == kTmaWarp && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-    for (int s = 0; s < p.n_aslots; ++s) {
-      // slots of the interpolation ring are filled by kInterpWarps producers (one arrive each), the others by one TMA box
-      mbar_init(smem_u32(&bar_afull[s]), s < p.n_uslots ? (uint32_t)kInterpWarps : 1u);
-      mbar_init(smem_u32(&bar_aempty[s]), kConsumerWarps);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&bar_bfull[s]), 1);
-      mbar_init(smem_u32(&bar_bempty[s]), kConsumerWarps);
-    }
+    tma_prefetch(&tmA);
+    tma_prefetch(&tmB);
+    // an interpolation slot is filled by kInterpWarps producers (one arrive each), a TMA slot by one box
+    a_up.init(kInterpWarps, kConsumerWarps);
+    a_tma.init(1, kConsumerWarps);
+    b_ring.init(1, kConsumerWarps);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   for (int i = threadIdx.x; i < p.n_tiles * BN; i += blockDim.x) {
@@ -302,50 +291,36 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
     // ===================== consumer warpgroups: wgmma into registers, then the epilogue =====================
     if constexpr (UP) setmaxnreg_inc<kUpConsumerRegs>();
     const int wg = warp >> 2;   // pixels [64 wg, 64 wg + 64) of the tile
-    const float slope = p.act == ACT_RELU ? 0.f : p.act == ACT_LEAKY ? 0.01f : 1.f;
+    const float slope = act_slope(p.act);
     const uint32_t dhi = desc_hi(8 * kRowB, 2u);   // SWIZZLE_64B, 8-row groups of 64-byte rows
-    const uint32_t afull0 = smem_u32(&bar_afull[0]), aempty0 = smem_u32(&bar_aempty[0]);
-    const uint32_t bempty0 = smem_u32(&bar_bempty[0]);
     const uint32_t lrow = a_base + (uint32_t)(64 * wg + 16 * (warp & 3) + (lane & 15)) * kRowB;
-    RowsConsumer st;
-    st.as_t = p.n_uslots; st.as_u = 0; st.bs = 0; st.pend_b = -1;
-    st.aph_t = 0; st.aph_u = 0; st.bph = 0;
+    RowsConsumer st{a_up, a_tma, b_ring};
     float acc[R * BN / 2];
     uint32_t fr[2][16];
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
 #pragma unroll
       for (int i = 0; i < R * BN / 2; ++i) acc[i] = 0.f;
       for (int cc = 0; cc < p.chunks; ++cc) {
-        mbar_wait(smem_u32(&bar_bfull[st.bs]), st.bph);
-        const uint32_t bsrc = desc_lo(b_base + (uint32_t)st.bs * G::kBBuf);
+        st.b.wait_full();
+        const uint32_t bsrc = desc_lo(b_base + (uint32_t)st.b.slot * G::kBBuf);
         const bool up = cc < p.up_chunks;
         // k-steps (16 channels = two groups) whose weights are all zero are not issued: exact, since the products
         // would be 0 (lstm / pad channel groups of the concat layouts)
         const uint32_t gm = chunk_groups(p.kmask, cc);
         const uint32_t ksm = ((gm & 0x3u) ? 1u : 0u) | ((gm & 0xCu) ? 2u : 0u);
-        // this chunk's ring of A slots: the interpolation ring [0, n_uslots) or the TMA ring [n_uslots, n_aslots)
-        st.as = up ? st.as_u : st.as_t;
-        st.aph = up ? st.aph_u : st.aph_t;
-        st.ring_lo = up ? 0 : p.n_uslots;
-        st.ring_hi = up ? p.n_uslots : p.n_aslots;
-        consume_rows<BN, R, 0>(st, acc, fr, lrow, bsrc, dhi, ksm, afull0, aempty0, bempty0, lane);
-        if (up) {
-          st.as_u = st.as;
-          st.aph_u = st.aph;
-        } else {
-          st.as_t = st.as;
-          st.aph_t = st.aph;
-        }
-        st.pend_b = st.bs;   // released with the last row's slot, once the next group has been committed
-        if (++st.bs == 2) {
-          st.bs = 0;
-          st.bph ^= 1u;
-        }
+        // The chosen ring goes by value and its position comes back by select: a ring chosen through a reference can be
+        // placed in local memory, and writing back whole rings (the barrier addresses and ranges never change) costs
+        // ptxas 8 to 13 more consumer registers.
+        const MbarRing a = consume_rows<BN, R, 0>(up ? st.a_up : st.a_tma, st, acc, fr, lrow, bsrc, dhi, ksm, lane);
+        st.a_up.slot = up ? a.slot : st.a_up.slot;
+        st.a_up.phase = up ? a.phase : st.a_up.phase;
+        st.a_tma.slot = up ? st.a_tma.slot : a.slot;
+        st.a_tma.phase = up ? st.a_tma.phase : a.phase;
+        st.held_b.hold(st.b);   // released with the last row's slot, once the next group has been committed
+        st.b.advance();
       }
       wg_wait<0>();
-      __syncwarp();
-      if (lane == 0 && st.pend_b >= 0) mbar_arrive(bempty0 + (uint32_t)st.pend_b * 8u);
-      st.pend_b = -1;
+      st.held_b.release_last(st.b, lane);
 
       const RowsTile tl = rows_tile<R>(p, tile);
       const int w0 = tl.w0, h0 = tl.h0, n = tl.n;
@@ -383,9 +358,6 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
     if (warp == kTmaWarp) {
       // ===================== TMA producer: one elected lane runs the whole loop nest =====================
       if (elect_one_sync()) {
-        int as = p.n_uslots, bs = 0;
-        uint32_t aph = 0, bph = 0;
-        const uint32_t afull0 = smem_u32(&bar_afull[0]), aempty0 = smem_u32(&bar_aempty[0]);
 #ifdef VR_TRACE
         const bool tr = p.trace && blockIdx.x == 0;
 #else
@@ -396,36 +368,30 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
           const RowsTile tl = rows_tile<R>(p, tile);
           const int nt = tl.nt, w0 = tl.w0, h0 = tl.h0, n = tl.n;
           for (int cc = 0; cc < p.chunks; ++cc) {
-            mbar_wait(smem_u32(&bar_bempty[bs]), bph ^ 1u);
-            const uint32_t bfull = smem_u32(&bar_bfull[bs]);
-            const uint32_t bdst = b_base + (uint32_t)bs * G::kBBuf;
-            mbar_expect_tx(bfull, G::kBBuf);
+            b_ring.wait_empty();
+            const uint32_t bdst = b_base + (uint32_t)b_ring.slot * G::kBBuf;
+            mbar_expect_tx(b_ring.full(), G::kBBuf);
 #pragma unroll
             for (int kw = 0; kw < 3; ++kw)
-              tma_load_3d(bdst + (uint32_t)kw * G::kBKw, &tmB, kw * p.CinPadR + cc * (int)kKB, nt * 3 * BN, 0, bfull);
-            if (++bs == 2) {
-              bs = 0;
-              bph ^= 1u;
-            }
+              tma_load_3d(bdst + (uint32_t)kw * G::kBKw, &tmB, kw * p.CinPadR + cc * (int)kKB, nt * 3 * BN, 0,
+                          b_ring.full());
+            b_ring.advance();
             if (cc < p.up_chunks) continue;   // rows of this chunk are produced by the interpolation warps
             const bool from_l = cc == p.l_chunk;
             const int c0 = from_l ? 0 : cc * (int)kKB + p.a_c_off;
             for (int r = 0; r < R + 2; ++r) {
               const unsigned long long t0 = tr ? clock64() : 0ull;
-              mbar_wait(aempty0 + (uint32_t)as * 8u, aph ^ 1u);
-              const uint32_t afull = afull0 + (uint32_t)as * 8u;
-              mbar_expect_tx(afull, kASlot);
-              tma_load_5d(a_base + (uint32_t)as * kASlot, from_l ? &tmL : &tmA, c0, w0 - 1, h0 - 1 + r, n, 0, afull);
+              a_tma.wait_empty();
+              mbar_expect_tx(a_tma.full(), kASlot);
+              tma_load_5d(a_base + (uint32_t)a_tma.slot * kASlot, from_l ? &tmL : &tmA, c0, w0 - 1, h0 - 1 + r, n, 0,
+                          a_tma.full());
               if (tr && tn < kTraceEvents) {
                 g_rows_trace[(1 * kTraceEvents + tn) * 3 + 0] = t0;
                 g_rows_trace[(1 * kTraceEvents + tn) * 3 + 1] = clock64();
                 g_rows_trace[(1 * kTraceEvents + tn) * 3 + 2] = 0ull;
                 ++tn;
               }
-              if (++as == p.n_aslots) {
-                as = p.n_uslots;
-                aph ^= 1u;
-              }
+              a_tma.advance();
             }
           }
         }
@@ -447,9 +413,6 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
         const int xi = lane >> 2, j = lane & 3;
         const int sx = 7 * wk + xi;              // source pixel of this lane, relative to xs
         const bool emit = xi < 7 && sx < kSrcPx; // xi == 7 only provides the neighbour of xi == 6
-        int as = 0;
-        uint32_t aph = 0;
-        const uint32_t afull0 = smem_u32(&bar_afull[0]), aempty0 = smem_u32(&bar_aempty[0]);
         const float inv_sw = p.up_sw > 0.f ? 1.f / p.up_sw : 0.f;
 #ifdef VR_TRACE
         const bool tr = p.trace && blockIdx.x == 0 && wk == 0;
@@ -564,9 +527,9 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
                 nv[i] = last_px ? v[i] : t;
               }
               const unsigned long long t1 = tr ? clock64() : 0ull;
-              mbar_wait(aempty0 + (uint32_t)as * 8u, aph ^ 1u);
+              a_up.wait_empty();
               const unsigned long long t2 = tr ? clock64() : 0ull;
-              uint8_t* slot = smem_raw + (a_base - smem_u32(smem_raw)) + (size_t)as * kASlot;
+              uint8_t* slot = smem_raw + (a_base - smem_u32(smem_raw)) + (size_t)a_up.slot * kASlot;
 #pragma unroll
               for (int k = 0; k < 3; ++k) {
                 if (e_off[k] < 0) continue;
@@ -585,8 +548,7 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
               }
               // no fence.proxy.async: the slot is read by the consumers' ldmatrix (generic proxy), never by wgmma or TMA;
               // the arrive's release and the consumers' acquiring wait order the stores before those reads
-              __syncwarp();
-              if (lane == 0) mbar_arrive(afull0 + (uint32_t)as * 8u);
+              warp_arrive(a_up.full(), lane);
               fetch();   // row k+2 (after the arrive, see above); past the last row it only shifts the pipeline
               if (tr && lane == 0 && tn < kTraceEvents) {
                 g_rows_trace[(2 * kTraceEvents + tn) * 3 + 0] = t0;
@@ -594,10 +556,7 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
                 g_rows_trace[(2 * kTraceEvents + tn) * 3 + 2] = clock64();
               }
               ++tn;
-              if (++as == p.n_uslots) {
-                as = 0;
-                aph ^= 1u;
-              }
+              a_up.advance();
             }
           }
         }

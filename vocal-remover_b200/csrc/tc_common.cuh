@@ -1,4 +1,5 @@
-// Raw-PTX device helpers shared by the wgmma convolution kernels (mbarrier, TMA, GMMA descriptors, wgmma).
+// Raw-PTX device helpers shared by the wgmma convolution kernels (mbarrier rings, TMA, GMMA descriptors, wgmma) and
+// their epilogue.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -67,7 +68,70 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       : "memory");
 #endif
 }
+// __syncwarp, then one arrive for the warp (an empty barrier counts one arrive per consumer warp)
+__device__ __forceinline__ void warp_arrive(uint32_t bar, int lane) {
+  __syncwarp();
+  if (lane == 0) mbar_arrive(bar);
+}
 
+// A ring of shared-memory slots [lo, hi) guarded by two mbarrier arrays: full[s] completes once slot s has been filled
+// (the TMA transaction bytes, or one arrive per producer warp), empty[s] once every consumer warp has released it (one
+// arrive each).  Every role keeps
+// its own copy and walks the slots in the same order: the producer waits for a slot's empty phase, fills it and moves
+// on; a consumer waits for its full phase, reads it, releases it and moves on.  `phase` is the parity of the slot's
+// current use.  It flips each time the ring wraps, and the producer's first pass waits on the parity before the
+// initial one, which a fresh barrier reports complete.
+struct MbarRing {
+  uint32_t full0, empty0;   // shared addresses of full[0] and empty[0]
+  int lo, hi, slot;
+  uint32_t phase;
+
+  __device__ __forceinline__ MbarRing(uint32_t full0_, uint32_t empty0_, int lo_, int hi_)
+      : full0(full0_), empty0(empty0_), lo(lo_), hi(hi_), slot(lo_), phase(0) {}
+  __device__ __forceinline__ uint32_t full(int s) const { return full0 + (uint32_t)s * 8u; }
+  __device__ __forceinline__ uint32_t empty(int s) const { return empty0 + (uint32_t)s * 8u; }
+  __device__ __forceinline__ uint32_t full() const { return full(slot); }
+  __device__ __forceinline__ uint32_t empty() const { return empty(slot); }
+  __device__ __forceinline__ void wait_full() const { mbar_wait(full(), phase); }
+  __device__ __forceinline__ void wait_empty() const { mbar_wait(empty(), phase ^ 1u); }
+  __device__ __forceinline__ void advance() {
+    if (++slot == hi) {
+      slot = lo;
+      phase ^= 1u;
+    }
+  }
+  // one thread, before the block's first barrier: the barriers of every slot of the ring
+  __device__ __forceinline__ void init(uint32_t full_count, uint32_t empty_count) const {
+    for (int s = lo; s < hi; ++s) {
+      mbar_init(full(s), full_count);
+      mbar_init(empty(s), empty_count);
+    }
+  }
+};
+
+// The slot of a ring whose last wgmma group may still be in flight.  A consumer holds it once it has committed that
+// group.  release() after the wg_wait<1> that follows the next commit hands it back; release_last() after the
+// wg_wait<0> at the end of a tile hands back the last one.  Every tile commits at least one group, so a slot is always
+// held there.  A slot that no wgmma reads (an A slot read with ldmatrix) is released right after its last ldmatrix
+// instead, with warp_arrive.
+struct HeldSlot {
+  int slot = -1;
+  __device__ __forceinline__ void hold(const MbarRing& r) { slot = r.slot; }
+  __device__ __forceinline__ void release(const MbarRing& r, int lane) {
+    if (slot >= 0) {
+      warp_arrive(r.empty(slot), lane);
+      slot = -1;
+    }
+  }
+  __device__ __forceinline__ void release_last(const MbarRing& r, int lane) {
+    warp_arrive(r.empty(slot), lane);
+    slot = -1;
+  }
+};
+
+__device__ __forceinline__ void tma_prefetch(const CUtensorMap* map) {
+  asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
+}
 __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3,
                                             int c4, uint32_t bar) {
   asm volatile(
@@ -287,8 +351,11 @@ __device__ __forceinline__ void setmaxnreg_dec() {
   asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
 }
 
-// bias + activation + split-bf16 store of the two adjacent channels (c, c + 1) a thread holds of one pixel.
-// slope: 0 = ReLU, 0.01 = LeakyReLU, 1 = identity  (y = max(v,0) + slope*min(v,0), branch-free)
+// The epilogue applies the activation as y = max(v,0) + slope*min(v,0), branch-free: slope 0 = ReLU, 0.01 = LeakyReLU,
+// 1 = identity.
+__device__ __forceinline__ float act_slope(int act) { return act == ACT_RELU ? 0.f : act == ACT_LEAKY ? 0.01f : 1.f; }
+
+// bias + activation + split-bf16 store of the two adjacent channels (c, c + 1) a thread holds of one pixel
 __device__ __forceinline__ void epilogue_pair(float v0, float v1, const float* bias_s, int c, int Cout, float slope,
                                               bf16* out_hi, bf16* out_lo) {
   if (c >= Cout) return;
