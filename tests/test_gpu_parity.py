@@ -300,6 +300,31 @@ def test_load_state_dict_is_strict():
         ctx.load_state_dict(bad)
 
 
+def test_context_without_weights():
+    """A context whose weights were never finalized still runs the spectral calls (lib/spec_utils.py uses such
+    contexts), and every call that runs the net fails with "weights not finalized"."""
+    from lib import _native
+    dev = _dev()
+    ctx = _native.Context(0, 2048, 1024, 32, 128, 256, 1)
+    st = _native.stream_ptr()
+    L = 1024 * 20
+    T = 1 + L // 1024
+    wave = torch.randn((2, L), generator=torch.Generator().manual_seed(7)).to(dev)
+    spec = torch.empty((2, 1025, T), dtype=torch.complex64, device=dev)
+    back = torch.empty((2, 1024 * (T - 1)), device=dev)
+    ctx.check(ctx.lib.vr_stft(ctx.handle, _native.ptr(wave), L, _native.ptr(spec), T, None, st), 'vr_stft')
+    ctx.check(ctx.lib.vr_istft(ctx.handle, _native.ptr(spec), T, _native.ptr(back), st), 'vr_istft')
+    torch.cuda.synchronize()
+    assert (back - wave[:, :back.shape[1]]).abs().max().item() < 1e-4
+    mag = torch.zeros((1, 2, 1025, 256), device=dev)
+    mask = torch.empty((1, 2, 1025, 256), device=dev)
+    assert ctx.lib.vr_forward(ctx.handle, _native.ptr(mag), 1, _native.ptr(mask), st) == -1
+    assert ctx.lib.vr_last_error(ctx.handle) == b'weights not finalized'
+    inst, voc = torch.empty_like(back), torch.empty_like(back)
+    assert ctx.lib.vr_separate_wave(ctx.handle, _native.ptr(wave), L, 0, _native.ptr(inst), _native.ptr(voc), st) == -1
+    assert ctx.lib.vr_last_error(ctx.handle) == b'weights not finalized'
+
+
 @pytest.mark.parametrize('n_frames', [3, 128, 129, 256])
 def test_edge_lengths_vs_oracle(default_model, n_frames):
     """Ragged / tiny / exactly-aligned tracks: make_padding corner cases (lib/dataset.py:198-205)."""

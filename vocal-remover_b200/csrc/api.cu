@@ -26,8 +26,14 @@ static int done(vr_ctx* c, bool ok) {
   c->err = c->eng->err;
   return -1;
 }
-#define CHECK_CTX(c) \
-  if (!(c) || !(c)->eng) return -2;
+// Every entry point that takes a context runs on the context's device ...
+#define CHECK_CTX(c)                  \
+  if (!(c) || !(c)->eng) return -2;   \
+  cudaSetDevice((c)->eng->cfg().device);
+// ... and one that runs the net needs its weights finalized.
+#define CHECK_NET(c) \
+  CHECK_CTX(c)       \
+  if (!(c)->eng->ready()) return fail(c, "weights not finalized");
 
 extern "C" {
 
@@ -103,12 +109,12 @@ int vr_istft(vr_ctx* ctx, const void* spec, int64_t T, float* wave, void* stream
 }
 
 int vr_predict_mask(vr_ctx* ctx, const float* mag, int32_t N, float* mask, void* stream) {
-  CHECK_CTX(ctx);
+  CHECK_NET(ctx);
   return done(ctx, ctx->eng->predict_mask(mag, N, mask, ctx->eng->cfg().offset, (cudaStream_t)stream));
 }
 
 int vr_forward(vr_ctx* ctx, const float* mag, int32_t N, float* mask, void* stream) {
-  CHECK_CTX(ctx);
+  CHECK_NET(ctx);
   return done(ctx, ctx->eng->predict_mask(mag, N, mask, 0, (cudaStream_t)stream));
 }
 
@@ -120,13 +126,13 @@ int vr_normaliser(vr_ctx* ctx, const void* spec, int64_t T, int32_t norm_mode, f
 int vr_separate_windows(vr_ctx* ctx, const void* spec, int64_t T, const float* norm, int32_t pad_l,
                         int32_t first_window, int32_t n_windows, float* mask, int64_t mask_T, int64_t frame_shift,
                         int32_t accumulate, void* stream) {
-  CHECK_CTX(ctx);
+  CHECK_NET(ctx);
   return done(ctx, ctx->eng->separate_windows((const float2*)spec, T, norm, pad_l, first_window, n_windows, mask,
                                               mask_T, frame_shift, accumulate, (cudaStream_t)stream));
 }
 
 int vr_separate(vr_ctx* ctx, const void* spec, int64_t T, int32_t tta, float* mask, void* stream) {
-  CHECK_CTX(ctx);
+  CHECK_NET(ctx);
   return done(ctx, ctx->eng->separate((const float2*)spec, T, tta, mask, (cudaStream_t)stream));
 }
 
@@ -175,19 +181,19 @@ int vr_apply_mask_istft_range(vr_ctx* ctx, const void* spec, const float* mask, 
 
 int vr_separate_wave(vr_ctx* ctx, const float* wave, int64_t L, int32_t tta, float* wave_inst, float* wave_voc,
                      void* stream) {
-  CHECK_CTX(ctx);
+  CHECK_NET(ctx);
   return done(ctx, ctx->eng->separate_wave(wave, L, tta, wave_inst, wave_voc, (cudaStream_t)stream));
 }
 
 int vr_separate_wave_host(vr_ctx* ctx, const float* wave_host, int64_t L, int32_t tta, float* inst_host,
                           float* voc_host, void* stream) {
-  CHECK_CTX(ctx);
+  CHECK_NET(ctx);
   return done(ctx, ctx->eng->separate_wave_host(wave_host, L, tta, inst_host, voc_host, (cudaStream_t)stream));
 }
 
 int vr_separate_wave_host_images(vr_ctx* ctx, const float* wave_host, int64_t L, int32_t tta, float* inst_host,
                                  float* voc_host, uint8_t* img_inst_host, uint8_t* img_voc_host, void* stream) {
-  CHECK_CTX(ctx);
+  CHECK_NET(ctx);
   return done(ctx, ctx->eng->separate_wave_host(wave_host, L, tta, inst_host, voc_host, (cudaStream_t)stream,
                                                 img_inst_host, img_voc_host));
 }
@@ -210,7 +216,7 @@ int vr_spec_sub(vr_ctx* ctx, const void* a, const void* b, int64_t T, void* out,
 
 int vr_validation_loss(vr_ctx* ctx, const void* spec_x, const void* spec_y, int64_t T, float* coef_out,
                        double* window_sums, void* stream) {
-  CHECK_CTX(ctx);
+  CHECK_NET(ctx);
   return done(ctx, ctx->eng->validation_loss((const float2*)spec_x, (const float2*)spec_y, T, coef_out, window_sums,
                                              (cudaStream_t)stream));
 }
@@ -262,7 +268,6 @@ int vr_shared_alloc(vr_ctx* ctx, int64_t bytes, void** dev_ptr, unsigned char* h
   CHECK_CTX(ctx);
   if (!dev_ptr || !handle64 || bytes <= 0) return fail(ctx, "vr_shared_alloc: bad arguments");
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "CUDA IPC handle is 64 bytes");
-  cudaSetDevice(ctx->eng->cfg().device);
   void* p = nullptr;
   cudaError_t e = cudaMalloc(&p, (size_t)bytes);
   if (e != cudaSuccess) return fail(ctx, std::string("vr_shared_alloc: cudaMalloc: ") + cudaGetErrorString(e));
@@ -280,7 +285,6 @@ int vr_shared_alloc(vr_ctx* ctx, int64_t bytes, void** dev_ptr, unsigned char* h
 int vr_shared_open(vr_ctx* ctx, const unsigned char* handle64, void** dev_ptr) {
   CHECK_CTX(ctx);
   if (!dev_ptr || !handle64) return fail(ctx, "vr_shared_open: bad arguments");
-  cudaSetDevice(ctx->eng->cfg().device);
   cudaIpcMemHandle_t h;
   memcpy(&h, handle64, 64);
   void* p = nullptr;
@@ -293,7 +297,6 @@ int vr_shared_open(vr_ctx* ctx, const unsigned char* handle64, void** dev_ptr) {
 int vr_shared_close(vr_ctx* ctx, void* dev_ptr, int32_t owner) {
   CHECK_CTX(ctx);
   if (!dev_ptr) return 0;
-  cudaSetDevice(ctx->eng->cfg().device);
   cudaError_t e = owner ? cudaFree(dev_ptr) : cudaIpcCloseMemHandle(dev_ptr);
   if (e != cudaSuccess) return fail(ctx, std::string("vr_shared_close: ") + cudaGetErrorString(e));
   return 0;

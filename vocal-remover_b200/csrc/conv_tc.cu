@@ -300,15 +300,16 @@ TcKind tc_choose(const ConvLayer& L, int H, int W, bool rows_wide) {
   return TC_GENERIC;
 }
 
-// The folded fp32 weights split into bf16 hi / lo planes of rows x K; at(co, tap, ci) = row * K + k of one weight.
+// The folded fp32 weights w [tap][L.CinPad][L.CoutPad] split into bf16 hi / lo planes of rows x K; at(co, tap, ci) =
+// row * K + k of one weight.
 template <class At>
-static std::vector<uint16_t> split_bf16(const ConvLayer& L, int rows, int K, At at) {
+static std::vector<uint16_t> split_bf16(const ConvLayer& L, const float* wp, int rows, int K, At at) {
   std::vector<uint16_t> planes((size_t)2 * rows * K, 0);
   const size_t lo = (size_t)rows * K;
   for (int co = 0; co < L.Cout; ++co)
     for (int t = 0; t < L.k * L.k; ++t)
       for (int ci = 0; ci < L.CinPad; ++ci) {
-        const float w = L.w_host[((size_t)t * L.CinPad + ci) * L.CoutPad + co];
+        const float w = wp[((size_t)t * L.CinPad + ci) * L.CoutPad + co];
         const uint16_t hi = tc_f2bf(w);
         const size_t i = at(co, t, ci);
         planes[i] = hi;
@@ -318,13 +319,13 @@ static std::vector<uint16_t> split_bf16(const ConvLayer& L, int rows, int K, At 
 }
 
 // which 8-channel input groups carry any weight at all (the lstm / pad groups of the concat layouts do not)
-static unsigned long long weight_group_mask(const ConvLayer& L, int CinPad) {
+static unsigned long long weight_group_mask(const ConvLayer& L, const float* wp, int CinPad) {
   if (CinPad / 8 > 64) return ~0ull;
   unsigned long long m = 0x3ull;   // k-step 0 of chunk 0 initialises the accumulators: never skipped
   for (int ci = 0; ci < L.CinPad; ++ci) {
     bool any = false;
     for (int t = 0; t < L.k * L.k && !any; ++t)
-      for (int co = 0; co < L.Cout && !any; ++co) any = L.w_host[((size_t)t * L.CinPad + ci) * L.CoutPad + co] != 0.f;
+      for (int co = 0; co < L.Cout && !any; ++co) any = wp[((size_t)t * L.CinPad + ci) * L.CoutPad + co] != 0.f;
     if (any) m |= 1ull << (ci / 8);
   }
   return m;
@@ -372,7 +373,7 @@ const CUtensorMap* tc_activation_map(TcConv& tc, const ActView& v, int bw, int b
   return &tc.map_a.emplace(key, m).first->second;
 }
 
-bool tc_prepare(ConvLayer& L, int H, int W, bool rows_wide, std::string& err) {
+bool tc_prepare(ConvLayer& L, const float* w, const float* b, int H, int W, bool rows_wide, std::string& err) {
   const TcKind kind = tc_choose(L, H, W, rows_wide);
   if (kind == TC_NONE) return true;   // stays on the CUDA-core kernel
   if (!tc_encode_fn()) {
@@ -389,7 +390,7 @@ bool tc_prepare(ConvLayer& L, int H, int W, bool rows_wide, std::string& err) {
   const int CinPad = round_up(L.CinPad, tc->KB);
   tc->CinPad = CinPad;
   tc->chunks = CinPad / tc->KB;
-  tc->kmask = weight_group_mask(L, CinPad);
+  tc->kmask = weight_group_mask(L, w, CinPad);
   const int rows = nt.n_tiles * BN;
   std::vector<uint16_t> planes;
   int brows, K;
@@ -397,17 +398,17 @@ bool tc_prepare(ConvLayer& L, int H, int W, bool rows_wide, std::string& err) {
     // B[plane][nt*3*BN + (2-kh)*BN + co][kw*CinPad + ci]: the three kh taps stacked along the MMA N dimension
     brows = 3 * rows;
     K = 3 * CinPad;
-    planes = split_bf16(L, brows, K, [&](int co, int t, int ci) {
+    planes = split_bf16(L, w, brows, K, [&](int co, int t, int ci) {
       return (size_t)(co / BN * 3 * BN + (2 - t / 3) * BN + co % BN) * K + (size_t)(t % 3) * CinPad + ci;
     });
   } else {
     // B[plane][co][tap*CinPad + ci]: every tap padded to whole chunks, so no chunk reads another tap's weights
     brows = rows;
     K = L.k * L.k * CinPad;
-    planes = split_bf16(L, brows, K, [&](int co, int t, int ci) { return (size_t)co * K + (size_t)t * CinPad + ci; });
+    planes = split_bf16(L, w, brows, K, [&](int co, int t, int ci) { return (size_t)co * K + (size_t)t * CinPad + ci; });
   }
   std::vector<float> bias((size_t)rows, 0.f);
-  for (int co = 0; co < L.Cout; ++co) bias[(size_t)co] = L.bias_host[(size_t)co];
+  for (int co = 0; co < L.Cout; ++co) bias[(size_t)co] = b[co];
   if (tc->w_planes.alloc(planes.size() * 2) != cudaSuccess || tc->bias.alloc(bias.size() * 4) != cudaSuccess) {
     err = "cudaMalloc failed while packing tensor-core weights for " + L.name;
     return false;

@@ -135,10 +135,56 @@ bool Engine::need(const std::string& key, std::initializer_list<int64_t> shape, 
   return true;
 }
 
-// Fold BatchNorm2d(eval) into the bias-free conv and pack to [tap][CinPad][CoutPad] (lib/layers.py:12-23).
+bool Engine::fold_bn(const std::string& bn, int C, const float* pre_bias, std::vector<double>& scale,
+                     std::vector<double>& shift) {
+  const HostTensor *g, *b, *m, *v, *cnt;
+  if (!need(bn + ".weight", {C}, &g) || !need(bn + ".bias", {C}, &b) || !need(bn + ".running_mean", {C}, &m) ||
+      !need(bn + ".running_var", {C}, &v) || !need(bn + ".num_batches_tracked", {}, &cnt))
+    return false;
+  scale.resize((size_t)C);
+  shift.resize((size_t)C);
+  for (int c = 0; c < C; ++c) {
+    scale[(size_t)c] = (double)g->data[(size_t)c] / sqrt((double)v->data[(size_t)c] + kBnEps);
+    shift[(size_t)c] = scale[(size_t)c] * ((pre_bias ? (double)pre_bias[c] : 0.0) - (double)m->data[(size_t)c]) +
+                       (double)b->data[(size_t)c];
+  }
+  return true;
+}
+
+// Packs OIHW weights w [Cout][Cin][L.k][L.k], output channel co times scale[co] (in double, rounded to float once), to
+// wp [tap][CinPad][CoutPad] with CinPad = perm.size(): packed input channel pc holds channel perm[pc], or zeros where
+// that is -1.  bp [CoutPad] is shift rounded to float.  Sets L's channel counts.
+static void pack_conv(ConvLayer& L, const float* w, int Cout, int Cin, const double* scale, const double* shift,
+                      const std::vector<int>& perm, std::vector<float>& wp, std::vector<float>& bp) {
+  L.Cin = Cin; L.CinPad = (int)perm.size(); L.Cout = Cout; L.CoutPad = round_up(Cout, 8);
+  const int taps = L.k * L.k;
+  wp.assign((size_t)taps * L.CinPad * L.CoutPad, 0.f);
+  bp.assign((size_t)L.CoutPad, 0.f);
+  for (int co = 0; co < Cout; ++co) {
+    bp[(size_t)co] = (float)shift[co];
+    for (int pc = 0; pc < L.CinPad; ++pc) {
+      const int ci = perm[(size_t)pc];
+      if (ci < 0) continue;
+      for (int t = 0; t < taps; ++t)
+        wp[((size_t)t * L.CinPad + pc) * L.CoutPad + co] =
+            (float)((double)w[((size_t)co * Cin + ci) * taps + t] * scale[co]);
+    }
+  }
+}
+
+bool Engine::prepare_conv(ConvLayer& L, Arena& arena, const std::vector<float>& wp, const std::vector<float>& bp,
+                          bool use_tc, int H, int W, bool rows_wide) {
+  if (use_tc && !tc_prepare(L, wp.data(), bp.data(), H, W, rows_wide, err)) return false;
+  if (L.tc) return true;
+  L.w = (float*)dalloc(arena, wp.size() * sizeof(float), wp.data());
+  L.bias = (float*)dalloc(arena, bp.size() * sizeof(float), bp.data());
+  return L.w && L.bias;
+}
+
+// Fold BatchNorm2d(eval) into the bias-free conv (lib/layers.py:12-23) and prepare it for its kernel.
 // perm[packed_ci] = original input channel, or -1 for a zero (padding) channel.
-bool Engine::make_conv(ConvLayer& L, const std::string& prefix, const std::vector<int>& perm, int cin_pad, int k,
-                       int stride, int dh, int dw, int act, int H, int W, bool rows_wide) {
+bool Engine::make_conv(ConvLayer& L, const std::string& prefix, const std::vector<int>& perm, int k, int stride,
+                       int dh, int dw, int act, int H, int W, bool rows_wide) {
   L.name = prefix;
   L.k = k; L.stride = stride; L.dil_h = dh; L.dil_w = dw; L.act = act;
   auto itw = sd_.find(prefix + ".conv.0.weight");
@@ -154,44 +200,15 @@ bool Engine::make_conv(ConvLayer& L, const std::string& prefix, const std::vecto
   const int Cout = (int)w.shape[0], Cin = (int)w.shape[1];
   int used = 0;
   for (int v : perm) used += v >= 0;
-  if (used != Cin || (int)perm.size() != cin_pad) {
+  if (used != Cin) {
     err = "internal: channel permutation does not cover the input channels of " + prefix;
     return false;
   }
-  const HostTensor *g, *b, *m, *v, *cnt;
-  if (!need(prefix + ".conv.1.weight", {Cout}, &g) || !need(prefix + ".conv.1.bias", {Cout}, &b) ||
-      !need(prefix + ".conv.1.running_mean", {Cout}, &m) || !need(prefix + ".conv.1.running_var", {Cout}, &v) ||
-      !need(prefix + ".conv.1.num_batches_tracked", {}, &cnt))
-    return false;
-  std::vector<double> scale((size_t)Cout);
-  std::vector<float> bias((size_t)Cout);
-  for (int co = 0; co < Cout; ++co) {
-    scale[(size_t)co] = (double)g->data[co] / sqrt((double)v->data[co] + kBnEps);
-    bias[(size_t)co] = (float)((double)b->data[co] - (double)m->data[co] * scale[(size_t)co]);
-  }
-  if (!pack_conv(L, arena_, w.data.data(), Cout, Cin, scale.data(), bias.data(), perm)) return false;
-  return cfg_.conv_mode != 0 || tc_prepare(L, H, W, rows_wide, err);
-}
-
-bool Engine::pack_conv(ConvLayer& L, Arena& arena, const float* w, int Cout, int Cin, const double* scale,
-                       const float* bias, const std::vector<int>& perm) {
-  L.Cin = Cin; L.CinPad = (int)perm.size(); L.Cout = Cout; L.CoutPad = round_up(Cout, 8);
-  const int taps = L.k * L.k;
-  L.w_host.assign((size_t)taps * L.CinPad * L.CoutPad, 0.f);
-  L.bias_host.assign((size_t)L.CoutPad, 0.f);
-  for (int co = 0; co < Cout; ++co) {
-    L.bias_host[(size_t)co] = bias[co];
-    for (int pc = 0; pc < L.CinPad; ++pc) {
-      const int ci = perm[(size_t)pc];
-      if (ci < 0) continue;
-      for (int t = 0; t < taps; ++t)
-        L.w_host[((size_t)t * L.CinPad + pc) * L.CoutPad + co] =
-            (float)((double)w[((size_t)co * Cin + ci) * taps + t] * scale[co]);
-    }
-  }
-  L.w = (float*)dalloc(arena, L.w_host.size() * sizeof(float), L.w_host.data());
-  L.bias = (float*)dalloc(arena, L.bias_host.size() * sizeof(float), L.bias_host.data());
-  return L.w && L.bias;
+  std::vector<double> scale, shift;
+  if (!fold_bn(prefix + ".conv.1", Cout, nullptr, scale, shift)) return false;
+  std::vector<float> wp, bp;
+  pack_conv(L, w.data.data(), Cout, Cin, scale.data(), shift.data(), perm, wp, bp);
+  return prepare_conv(L, arena_, wp, bp, cfg_.conv_mode == 0, H, W, rows_wide);
 }
 
 static std::vector<int> identity_perm(int c, int pad) {
@@ -200,48 +217,42 @@ static std::vector<int> identity_perm(int c, int pad) {
   return p;
 }
 
-bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, const std::vector<int>& in_perm,
-                           int cin_pad, int n, int H, int W, int nin_lstm, int nout_lstm) {
-  (void)nin;
+bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, const std::vector<int>& in_perm, int n, int H,
+                           int W, int nin_lstm, int nout_lstm) {
   P.prefix = prefix; P.n = n; P.H = H; P.W = W;
   const int Nb = cfg_.max_batch;
   if (H % 16 || W % 16 || n % 4) {
     err = "unsupported geometry: band height and cropsize must be multiples of 16 and nout a multiple of 16";
     return false;
   }
-  if (!make_conv(P.enc1, prefix + ".enc1", in_perm, cin_pad, 3, 1, 1, 1, ACT_RELU, H, W)) return false;
+  if (!make_conv(P.enc1, prefix + ".enc1", in_perm, 3, 1, 1, 1, ACT_RELU, H, W)) return false;
   const int mult[5] = {1, 2, 4, 6, 8};
   for (int i = 0; i < 4; ++i) {
     const int cin = n * mult[i], cout = n * mult[i + 1], Ho = H >> (i + 1), Wo = W >> (i + 1);
     const std::string e = prefix + ".enc" + std::to_string(i + 2);
-    if (!make_conv(P.enc_a[i], e + ".conv1", identity_perm(cin, round_up(cin, 8)), round_up(cin, 8), 3, 2, 1, 1,
-                   ACT_LEAKY, Ho, Wo))
+    if (!make_conv(P.enc_a[i], e + ".conv1", identity_perm(cin, round_up(cin, 8)), 3, 2, 1, 1, ACT_LEAKY, Ho, Wo))
       return false;
-    if (!make_conv(P.enc_b[i], e + ".conv2", identity_perm(cout, cout), cout, 3, 1, 1, 1, ACT_LEAKY, Ho, Wo))
-      return false;
+    if (!make_conv(P.enc_b[i], e + ".conv2", identity_perm(cout, cout), 3, 1, 1, 1, ACT_LEAKY, Ho, Wo)) return false;
   }
   const int c8 = 8 * n, h16 = H / 16, w16 = W / 16;
-  if (!make_conv(P.aspp1, prefix + ".aspp.conv1.1", identity_perm(c8, c8), c8, 1, 1, 1, 1, ACT_RELU, 1, w16))
+  if (!make_conv(P.aspp1, prefix + ".aspp.conv1.1", identity_perm(c8, c8), 1, 1, 1, 1, ACT_RELU, 1, w16))
     return false;
-  if (!make_conv(P.aspp2, prefix + ".aspp.conv2", identity_perm(c8, c8), c8, 1, 1, 1, 1, ACT_RELU, h16, w16))
+  if (!make_conv(P.aspp2, prefix + ".aspp.conv2", identity_perm(c8, c8), 1, 1, 1, 1, ACT_RELU, h16, w16))
     return false;
   const int dil[3][2] = {{4, 2}, {8, 4}, {12, 6}};   // lib/nets.py:10
   for (int i = 0; i < 3; ++i)
-    if (!make_conv(P.aspp_d[i], prefix + ".aspp.conv" + std::to_string(i + 3), identity_perm(c8, c8), c8, 3, 1,
+    if (!make_conv(P.aspp_d[i], prefix + ".aspp.conv" + std::to_string(i + 3), identity_perm(c8, c8), 3, 1,
                    dil[i][0], dil[i][1], ACT_RELU, h16, w16))
       return false;
-  if (!make_conv(P.bott, prefix + ".aspp.bottleneck", identity_perm(5 * c8, 5 * c8), 5 * c8, 1, 1, 1, 1, ACT_RELU,
-                 h16, w16))
+  if (!make_conv(P.bott, prefix + ".aspp.bottleneck", identity_perm(5 * c8, 5 * c8), 1, 1, 1, 1, ACT_RELU, h16, w16))
     return false;
-  if (!make_conv(P.dec[0], prefix + ".dec4.conv1", identity_perm(14 * n, 14 * n), 14 * n, 3, 1, 1, 1, ACT_RELU, H / 8,
-                 W / 8))
+  if (!make_conv(P.dec[0], prefix + ".dec4.conv1", identity_perm(14 * n, 14 * n), 3, 1, 1, 1, ACT_RELU, H / 8, W / 8))
     return false;
-  if (!make_conv(P.dec[1], prefix + ".dec3.conv1", identity_perm(10 * n, 10 * n), 10 * n, 3, 1, 1, 1, ACT_RELU, H / 4,
-                 W / 4))
+  if (!make_conv(P.dec[1], prefix + ".dec3.conv1", identity_perm(10 * n, 10 * n), 3, 1, 1, 1, ACT_RELU, H / 4, W / 4))
     return false;
   // rows_wide: dec2's upsample is fused into the row kernel whenever 4n is a multiple of 32
-  if (!make_conv(P.dec[2], prefix + ".dec2.conv1", identity_perm(6 * n, 6 * n), 6 * n, 3, 1, 1, 1, ACT_RELU, H / 2,
-                 W / 2, true))
+  if (!make_conv(P.dec[2], prefix + ".dec2.conv1", identity_perm(6 * n, 6 * n), 3, 1, 1, 1, ACT_RELU, H / 2, W / 2,
+                 true))
     return false;
   // dec1 input in the reference: cat[ up(cat[h (2n), lstm (1)]) , e1 (n) ]  (lib/nets.py:38-39, layers.py:52-56),
   // reduced as [ up(h) 2n | zeros up to Up | e1 n | zeros up to Lp | up(lstm) 1 | 15 zeros ] (BaseNetPlan, engine.h)
@@ -254,7 +265,7 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
     perm[(size_t)Lp] = 2 * n;
     // (the 64-wide tile was measured on dec1 as well - one N tile instead of two for n = 64 - and is no faster there:
     //  with its single accumulator set the epilogue no longer overlaps the next tile's products)
-    if (!make_conv(P.dec[3], prefix + ".dec1.conv1", perm, c1, 3, 1, 1, 1, ACT_RELU, H, W)) return false;
+    if (!make_conv(P.dec[3], prefix + ".dec1.conv1", perm, 3, 1, 1, 1, ACT_RELU, H, W)) return false;
   }
 
   // activation buffers: the decoders' plans decide what their concat buffers hold
@@ -291,16 +302,15 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
     err = "LSTM input size does not match band height / 2 for " + lp;
     return false;
   }
-  const HostTensor *cw, *g, *b, *m, *v, *cnt;
-  if (!need(lp + ".conv.conv.0.weight", {1, Q.C, 1, 1}, &cw) || !need(lp + ".conv.conv.1.weight", {1}, &g) ||
-      !need(lp + ".conv.conv.1.bias", {1}, &b) || !need(lp + ".conv.conv.1.running_mean", {1}, &m) ||
-      !need(lp + ".conv.conv.1.running_var", {1}, &v) || !need(lp + ".conv.conv.1.num_batches_tracked", {}, &cnt))
+  const HostTensor* cw;
+  std::vector<double> scale, shift;
+  if (!need(lp + ".conv.conv.0.weight", {1, Q.C, 1, 1}, &cw) ||
+      !fold_bn(lp + ".conv.conv.1", 1, nullptr, scale, shift))
     return false;
   {
-    const double scale = (double)g->data[0] / sqrt((double)v->data[0] + kBnEps);
     std::vector<float> w((size_t)Q.C);
-    for (int c = 0; c < Q.C; ++c) w[(size_t)c] = (float)((double)cw->data[(size_t)c] * scale);
-    Q.conv_bias = (float)((double)b->data[0] - (double)m->data[0] * scale);
+    for (int c = 0; c < Q.C; ++c) w[(size_t)c] = (float)((double)cw->data[(size_t)c] * scale[0]);
+    Q.conv_bias = (float)shift[0];
     Q.conv_w = (float*)dalloc(arena_, sizeof(float) * w.size(), w.data());
     if (!Q.conv_w) return false;
   }
@@ -325,19 +335,11 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
   }
   {
     const int K = 2 * Q.hid;
-    const HostTensor *dw, *db, *g1, *b1, *m1, *v1, *c1t;
+    const HostTensor *dw, *db;
     if (!need(lp + ".dense.0.weight", {Q.bins, K}, &dw) || !need(lp + ".dense.0.bias", {Q.bins}, &db) ||
-        !need(lp + ".dense.1.weight", {Q.bins}, &g1) || !need(lp + ".dense.1.bias", {Q.bins}, &b1) ||
-        !need(lp + ".dense.1.running_mean", {Q.bins}, &m1) || !need(lp + ".dense.1.running_var", {Q.bins}, &v1) ||
-        !need(lp + ".dense.1.num_batches_tracked", {}, &c1t))
+        !fold_bn(lp + ".dense.1", Q.bins, db->data.data(), scale, shift))
       return false;
-    std::vector<float> sc((size_t)Q.bins), sh((size_t)Q.bins);
-    for (int bin = 0; bin < Q.bins; ++bin) {
-      const double s = (double)g1->data[(size_t)bin] / sqrt((double)v1->data[(size_t)bin] + kBnEps);
-      sc[(size_t)bin] = (float)s;
-      sh[(size_t)bin] = (float)(s * ((double)db->data[(size_t)bin] - (double)m1->data[(size_t)bin]) +
-                                (double)b1->data[(size_t)bin]);
-    }
+    const std::vector<float> sc(scale.begin(), scale.end()), sh(shift.begin(), shift.end());
     Q.wd = (float*)dalloc(arena_, sizeof(float) * dw->data.size(), dw->data.data());
     Q.dscale = (float*)dalloc(arena_, sizeof(float) * sc.size(), sc.data());
     Q.dshift = (float*)dalloc(arena_, sizeof(float) * sh.size(), sh.data());
@@ -353,7 +355,6 @@ bool Engine::build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, c
 bool Engine::finalize() {
   if (finalized_) return true;
   if (!err.empty() && !twiddle_) return false;
-  cudaSetDevice(cfg_.device);
   const int max_bin = cfg_.n_fft / 2, W = cfg_.cropsize, Nb = cfg_.max_batch;
   const int nout = cfg_.nout, a1 = nout / 4, a2 = nout / 2;
   if (nout % 16) {
@@ -389,21 +390,14 @@ bool Engine::finalize() {
   for (int j = 0; j < a2; ++j) p3[(size_t)(pos_aux2_ + j)] = 2 + a1 + j;
 
   const int Hb = max_bin / 2;
-  if (!build_basenet(nets_[0], "stg1_low_band_net.0", 2, p1, cp1, nout / 2, Hb, W, nin_lstm / 2, cfg_.nout_lstm))
+  if (!build_basenet(nets_[0], "stg1_low_band_net.0", p1, nout / 2, Hb, W, nin_lstm / 2, cfg_.nout_lstm) ||
+      !build_basenet(nets_[1], "stg1_high_band_net", p1, nout / 4, Hb, W, nin_lstm / 2, cfg_.nout_lstm / 2) ||
+      !build_basenet(nets_[2], "stg2_low_band_net.0", p2, nout, Hb, W, nin_lstm / 2, cfg_.nout_lstm) ||
+      !build_basenet(nets_[3], "stg2_high_band_net", p2, nout / 2, Hb, W, nin_lstm / 2, cfg_.nout_lstm / 2) ||
+      !build_basenet(nets_[4], "stg3_full_band_net", p3, nout, max_bin, W, nin_lstm, cfg_.nout_lstm))
     return false;
-  if (!build_basenet(nets_[1], "stg1_high_band_net", 2, p1, cp1, nout / 4, Hb, W, nin_lstm / 2, cfg_.nout_lstm / 2))
-    return false;
-  if (!build_basenet(nets_[2], "stg2_low_band_net.0", a1 + 2, p2, cp2, nout, Hb, W, nin_lstm / 2, cfg_.nout_lstm))
-    return false;
-  if (!build_basenet(nets_[3], "stg2_high_band_net", a1 + 2, p2, cp2, nout / 2, Hb, W, nin_lstm / 2,
-                     cfg_.nout_lstm / 2))
-    return false;
-  if (!build_basenet(nets_[4], "stg3_full_band_net", a1 + a2 + 2, p3, C3, nout, max_bin, W, nin_lstm, cfg_.nout_lstm))
-    return false;
-  if (!make_conv(bridge1_, "stg1_low_band_net.1", identity_perm(nout / 2, nout / 2), nout / 2, 1, 1, 1, 1, ACT_RELU,
-                 Hb, W))
-    return false;
-  if (!make_conv(bridge2_, "stg2_low_band_net.1", identity_perm(nout, nout), nout, 1, 1, 1, 1, ACT_RELU, Hb, W))
+  if (!make_conv(bridge1_, "stg1_low_band_net.1", identity_perm(nout / 2, nout / 2), 1, 1, 1, 1, ACT_RELU, Hb, W) ||
+      !make_conv(bridge2_, "stg2_low_band_net.1", identity_perm(nout, nout), 1, 1, 1, 1, ACT_RELU, Hb, W))
     return false;
   const HostTensor *ow, *aw;
   if (!need("out.weight", {2, nout, 1, 1}, &ow)) return false;
@@ -654,11 +648,6 @@ bool Engine::forward(int N, const MaskOutParams& mask, cudaStream_t s) {
 
 // ---------------------------------------------------------------------------------------------
 bool Engine::predict_mask(const float* mag, int N, float* mask_out, int offset, cudaStream_t s) {
-  if (!finalized_) {
-    err = "weights not finalized";
-    return false;
-  }
-  cudaSetDevice(cfg_.device);
   const int max_bin = cfg_.n_fft / 2, nb = bins(), W = cfg_.cropsize, r = W - 2 * offset;
   for (int i = 0; i < N; i += cfg_.max_batch) {
     const int nb_now = N - i < cfg_.max_batch ? N - i : cfg_.max_batch;
@@ -680,11 +669,6 @@ bool Engine::predict_mask(const float* mag, int N, float* mask_out, int offset, 
 bool Engine::separate_windows(const float2* spec, int64_t T, const float* norm, int pad_l, int first, int count,
                               float* mask, int64_t mask_T, int64_t frame_shift, int accumulate, cudaStream_t s,
                               bool final_pass) {
-  if (!finalized_) {
-    err = "weights not finalized";
-    return false;
-  }
-  cudaSetDevice(cfg_.device);
   const int max_bin = cfg_.n_fft / 2, nb = bins(), W = cfg_.cropsize, r = roi();
   for (int i = 0; i < count; i += cfg_.max_batch) {
     const int n_now = count - i < cfg_.max_batch ? count - i : cfg_.max_batch;
@@ -712,7 +696,6 @@ bool Engine::separate_windows(const float2* spec, int64_t T, const float* norm, 
 }
 
 bool Engine::normaliser(const float2* spec, int64_t T, int mode, float* out, cudaStream_t s) {
-  cudaSetDevice(cfg_.device);
   const int64_t n = (int64_t)2 * bins() * T;
   if (mode == 0) return timed("normaliser.absmax", 1, 1, bins(), (int)T, s, [&] { return ck(launch_absmax(spec, n, out, s), "absmax"); });
   return timed("normaliser.lexmax", 2, 1, bins(), (int)T, s, [&] { return ck(launch_lexmax_abs(spec, n, ws_lex_, out, s), "lexmax"); });
@@ -737,21 +720,18 @@ bool Engine::separate(const float2* spec, int64_t T, int tta, float* mask, cudaS
 }
 
 bool Engine::apply_mask(const float2* spec, const float* mask, int64_t T, float2* y, float2* v, cudaStream_t s) {
-  cudaSetDevice(cfg_.device);
   return timed("apply_mask", 1, 1, bins(), (int)T, s, [&] {
     return ck(launch_apply_mask(spec, mask, (int64_t)2 * bins() * T, y, v, s), "apply_mask");
   });
 }
 
 bool Engine::mask_frame_min(const float* mask, int64_t T, float* frame_min, cudaStream_t s) {
-  cudaSetDevice(cfg_.device);
   return timed("mask_frame_min", 1, 1, bins(), (int)T, s, [&] {
     return ck(launch_mask_frame_min(mask, 2 * bins(), T, frame_min, s), "vr_mask_frame_min");
   });
 }
 
 bool Engine::mask_apply_weight(float* mask, int64_t T, const float* weight, cudaStream_t s) {
-  cudaSetDevice(cfg_.device);
   return timed("mask_apply_weight", 1, 1, bins(), (int)T, s, [&] {
     return ck(launch_mask_apply_weight(mask, 2 * bins(), T, weight, s), "vr_mask_apply_weight");
   });
@@ -759,7 +739,6 @@ bool Engine::mask_apply_weight(float* mask, int64_t T, const float* weight, cuda
 
 bool Engine::spec_image(const float2* spec, const float* mask, int64_t T, unsigned char* img_a, unsigned char* img_b,
                         cudaStream_t s) {
-  cudaSetDevice(cfg_.device);
   if (T < 0 || !spec || !img_a || (mask && !img_b)) {
     err = "spec_image: needs spec, img_a, T >= 0 and, with a mask, img_b";
     return false;
@@ -772,7 +751,6 @@ bool Engine::spec_image(const float2* spec, const float* mask, int64_t T, unsign
 }
 
 bool Engine::vocal_image(const float2* spec_x, const float2* spec_y, int64_t T, unsigned char* img, cudaStream_t s) {
-  cudaSetDevice(cfg_.device);
   if (T < 0 || !spec_x || !spec_y || !img) {
     err = "vocal_image: needs spec_x, spec_y, img and T >= 0";
     return false;
@@ -784,7 +762,6 @@ bool Engine::vocal_image(const float2* spec_x, const float2* spec_y, int64_t T, 
 }
 
 bool Engine::spec_sub(const float2* a, const float2* b, int64_t T, float2* out, cudaStream_t s) {
-  cudaSetDevice(cfg_.device);
   if (T < 0 || !a || !b || !out) {
     err = "spec_sub: needs a, b, out and T >= 0";
     return false;
@@ -799,11 +776,6 @@ bool Engine::spec_sub(const float2* a, const float2* b, int64_t T, float2* out, 
 // kept mask frames.  Only the mask workspace is needed (no inverse STFT, so not ensure_ws's frame workspace).
 bool Engine::validation_loss(const float2* spec_x, const float2* spec_y, int64_t T, float* coef_out,
                              double* window_sums, cudaStream_t s) {
-  if (!finalized_) {
-    err = "weights not finalized";
-    return false;
-  }
-  cudaSetDevice(cfg_.device);
   if (T < 1 || !spec_x || !spec_y || !window_sums) {
     err = "validation_loss: needs spec_x, spec_y, window_sums and T >= 1";
     return false;
@@ -846,7 +818,6 @@ bool Engine::stft(const float* wave, int64_t L, float2* spec, int64_t T, float* 
 
 // frames [t0, t1) of the track only: what a rank of the window-sharded path needs (lib/distributed.py)
 bool Engine::stft_range(const float* wave, int64_t L, float2* spec, int64_t T, int64_t t0, int64_t t1, cudaStream_t s) {
-  cudaSetDevice(cfg_.device);
   if (T != 1 + L / cfg_.hop) {
     err = "stft: T must equal 1 + L // hop_length";
     return false;
@@ -859,7 +830,6 @@ bool Engine::stft_range(const float* wave, int64_t L, float2* spec, int64_t T, i
 }
 
 bool Engine::normaliser_range(const float2* spec, int64_t T, int64_t t0, int64_t t1, float* out, cudaStream_t s) {
-  cudaSetDevice(cfg_.device);
   if (t0 < 0 || t1 > T || t0 > t1) {
     err = "normaliser: frame range outside [0, T]";
     return false;
@@ -884,7 +854,6 @@ bool Engine::istft(const float2* spec, const float* mask, int64_t T, float* wave
 // wave_a / wave_b may point into another GPU's memory (peer-mapped).
 bool Engine::istft_range(const float2* spec, const float* mask, int64_t T, int64_t k0, int64_t k1, float* wave_a,
                          float* wave_b, cudaStream_t s) {
-  cudaSetDevice(cfg_.device);
   if (k0 < 0 || k1 > T - 1 || k0 > k1) {
     err = "istft: hop range outside [0, T-1]";
     return false;
@@ -909,7 +878,6 @@ bool Engine::istft_range(const float2* spec, const float* mask, int64_t T, int64
 
 // wave (2, L) in HBM -> instruments / vocals waves (2, hop*(T-1)) in HBM: the whole inference.py:147-176 path.
 bool Engine::separate_wave(const float* wave, int64_t L, int tta, float* inst, float* voc, cudaStream_t s) {
-  cudaSetDevice(cfg_.device);
   const int64_t T = 1 + L / cfg_.hop;
   if (!ensure_ws(T)) return false;
   if (!stft(wave, L, ws_spec_.get(), T, nullptr, s)) return false;
@@ -920,7 +888,6 @@ bool Engine::separate_wave(const float* wave, int64_t L, int tta, float* inst, f
 // Host-buffer entry (the end-to-end call): H2D of the wave, the whole path, D2H of both stems.
 bool Engine::separate_wave_host(const float* wave, int64_t L, int tta, float* inst, float* voc, cudaStream_t s,
                                 unsigned char* img_inst, unsigned char* img_voc) {
-  cudaSetDevice(cfg_.device);
   const int64_t T = 1 + L / cfg_.hop;
   const int64_t Lo = (int64_t)cfg_.hop * (T - 1);
   if (!ck(ws_wave_.ensure(2 * L + 4 * Lo), "workspace wave")) return false;
@@ -980,14 +947,16 @@ bool Engine::separate_wave_host(const float* wave, int64_t L, int tta, float* in
 
 // ---------------------------------------------------------------------------------------------
 bool Engine::debug_weights(ConvLayer& L, Arena& arena, const float* w, const float* bias, int Cout, int Cin,
-                           const std::vector<int>& perm, cudaStream_t s) {
+                           const std::vector<int>& perm, bool use_tc, int H, int W, bool rows_wide, cudaStream_t s) {
   std::vector<float> hw((size_t)Cout * Cin * L.k * L.k), hb((size_t)Cout);
   if (!ck(cudaMemcpyAsync(hw.data(), w, hw.size() * sizeof(float), cudaMemcpyDeviceToHost, s), "weights to host") ||
       !ck(cudaMemcpyAsync(hb.data(), bias, hb.size() * sizeof(float), cudaMemcpyDeviceToHost, s), "bias to host") ||
       !ck(cudaStreamSynchronize(s), "weights to host"))
     return false;
-  const std::vector<double> one((size_t)Cout, 1.0);
-  return pack_conv(L, arena, hw.data(), Cout, Cin, one.data(), hb.data(), perm);
+  const std::vector<double> one((size_t)Cout, 1.0), shift(hb.begin(), hb.end());
+  std::vector<float> wp, bp;
+  pack_conv(L, hw.data(), Cout, Cin, one.data(), shift.data(), perm, wp, bp);
+  return prepare_conv(L, arena, wp, bp, use_tc, H, W, rows_wide);
 }
 
 bool Engine::to_nchw(const ActView& v, int C, float* y_nchw, cudaStream_t s) {
@@ -997,7 +966,6 @@ bool Engine::to_nchw(const ActView& v, int C, float* y_nchw, cudaStream_t s) {
 
 bool Engine::debug_conv(const float* x_nchw, int N, int Cin, int H, int W, const float* w, const float* bias, int Cout,
                         int k, int stride, int dil_h, int dil_w, int act, int use_tc, float* y_nchw, cudaStream_t s) {
-  cudaSetDevice(cfg_.device);
   const int cin_pad = round_up(Cin, 16);
   const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
   Arena arena;   // the hook's buffers and weights, freed on return
@@ -1006,18 +974,18 @@ bool Engine::debug_conv(const float* x_nchw, int N, int Cin, int H, int W, const
   ConvLayer L;
   L.name = "debug_conv";
   L.k = k; L.stride = stride; L.dil_h = dil_h; L.dil_w = dil_w; L.act = act;
-  if (!bin.hi || !bout.hi || !debug_weights(L, arena, w, bias, Cout, Cin, identity_perm(Cin, cin_pad), s)) return false;
+  // vr_debug_set(2, 1): exercise the 64-wide row tile on a plain convolution
+  if (!bin.hi || !bout.hi ||
+      !debug_weights(L, arena, w, bias, Cout, Cin, identity_perm(Cin, cin_pad), use_tc != 0, Ho, Wo,
+                     g_debug.rows_wide == 1, s))
+    return false;
+  if (use_tc && !L.tc) {
+    err = "debug_conv: geometry not supported by the wgmma kernel";
+    return false;
+  }
   if (!timed("nchw_to_act", 1, N, H, W, s,
              [&] { return ck(launch_nchw_to_act(x_nchw, Cin, bin.all(N), s), "nchw_to_act"); }))
     return false;
-  if (use_tc) {
-    // vr_debug_set(2, 1): exercise the 64-wide row tile on a plain convolution
-    if (!tc_prepare(L, Ho, Wo, g_debug.rows_wide == 1, err)) return false;
-    if (!L.tc) {
-      err = "debug_conv: geometry not supported by the wgmma kernel";
-      return false;
-    }
-  }
   const ActView out = bout.view(N, 0, Ho, 0, Cout);
   const int saved_mode = cfg_.conv_mode;
   cfg_.conv_mode = use_tc ? 0 : 1;   // a requested CUDA-core run is not warned about
@@ -1031,7 +999,6 @@ bool Engine::debug_conv(const float* x_nchw, int N, int Cin, int H, int W, const
 bool Engine::debug_decoder(const float* low_nchw, int N, int Cl, int h, int w, const float* skip_nchw, int Cs,
                            const float* wgt, const float* bias, int Cout, int act, int fused, float* y_nchw,
                            cudaStream_t s) {
-  cudaSetDevice(cfg_.device);
   const int H = 2 * h, W = 2 * w;
   const int cl_pad = round_up(Cl, 32), cin_pad = round_up(cl_pad + Cs, 16);
   const int skip_off = fused ? 0 : cl_pad;   // the fused kernel's concat buffer holds only the skip channels
@@ -1045,18 +1012,19 @@ bool Engine::debug_decoder(const float* low_nchw, int N, int Cl, int h, int w, c
   std::vector<int> perm((size_t)cin_pad, -1);   // reduction order: [up Cl | pad | skip Cs]
   for (int i = 0; i < Cl; ++i) perm[(size_t)i] = i;
   for (int i = 0; i < Cs; ++i) perm[(size_t)(cl_pad + i)] = Cl + i;
-  if (!blow.hi || !bcat.hi || !bout.hi || !debug_weights(L, arena, wgt, bias, Cout, Cl + Cs, perm, s)) return false;
-  const ActView skip = bcat.view(N, 0, H, skip_off, cin_pad - cl_pad);
-  if (!timed("nchw_to_act", 1, N, h, w, s,
-             [&] { return ck(launch_nchw_to_act(low_nchw, Cl, blow.all(N), s), "nchw_to_act low"); }) ||
-      !timed("nchw_to_act", 1, N, H, W, s,
-             [&] { return ck(launch_nchw_to_act(skip_nchw, Cs, skip, s), "nchw_to_act skip"); }) ||
-      !tc_prepare(L, H, W, true, err))
+  if (!blow.hi || !bcat.hi || !bout.hi ||
+      !debug_weights(L, arena, wgt, bias, Cout, Cl + Cs, perm, true, H, W, true, s))
     return false;
   if (fused && !(L.tc && L.tc->fuses_upsample(blow.C))) {
     err = "debug_decoder: geometry not supported by the fused row kernel";
     return false;
   }
+  const ActView skip = bcat.view(N, 0, H, skip_off, cin_pad - cl_pad);
+  if (!timed("nchw_to_act", 1, N, h, w, s,
+             [&] { return ck(launch_nchw_to_act(low_nchw, Cl, blow.all(N), s), "nchw_to_act low"); }) ||
+      !timed("nchw_to_act", 1, N, H, W, s,
+             [&] { return ck(launch_nchw_to_act(skip_nchw, Cs, skip, s), "nchw_to_act skip"); }))
+    return false;
   const ActView out = bout.view(N, 0, H, 0, Cout);
   return run_decoder(L, blow.all(N), bcat, N, out, fused != 0, s) && to_nchw(out, Cout, y_nchw, s) &&
          ck(cudaStreamSynchronize(s), "debug_decoder sync");

@@ -94,14 +94,14 @@ struct Buffer {   // a whole NHWC split-bf16 allocation
 
 struct TcConv;   // tensor-core plan (conv_tc.cu)
 
+// A prepared layer holds the device weights of the one kernel that runs it: w / bias are non-null exactly when tc is
+// null.  No host copy of its weights is kept.
 struct ConvLayer {
   std::string name;
   int Cin = 0, CinPad = 0, Cout = 0, CoutPad = 0;
   int k = 1, stride = 1, dil_h = 1, dil_w = 1, act = ACT_RELU;
-  float* w = nullptr;      // device fp32 [taps][CinPad][CoutPad]
-  float* bias = nullptr;   // device fp32 [CoutPad]
-  std::vector<float> w_host;     // packed copy kept for the tensor-core packer
-  std::vector<float> bias_host;
+  float* w = nullptr;      // CUDA-core kernel: device fp32 [taps][CinPad][CoutPad]
+  float* bias = nullptr;   // CUDA-core kernel: device fp32 [CoutPad]
   std::shared_ptr<TcConv> tc;    // the tensor-core kernel and its packed weights; null -> CUDA-core kernel
 };
 
@@ -164,6 +164,9 @@ struct Config {
   int conv_mode = 0;   // 0: wgmma where eligible, 1: CUDA-core kernel everywhere (validation)
 };
 
+// Every method but the constructor and the destructor runs on the current device, which the caller makes cfg().device;
+// the methods that run the net (predict_mask, separate_windows, separate, separate_wave[_host], validation_loss) need
+// ready().  api.cu does both for every entry point.
 class Engine {
  public:
   explicit Engine(const Config& cfg);
@@ -283,20 +286,26 @@ class Engine {
   void* dalloc(Arena& arena, size_t bytes, const void* host = nullptr);
   Buffer make_buffer(Arena& arena, int N, int H, int W, int C, int pad_w = 0);
   bool need(const std::string& key, std::initializer_list<int64_t> shape, const HostTensor** out);
-  // H x W: the layer's output maps, from which tc_prepare chooses its kernel (rows_wide: see tc_prepare)
-  bool make_conv(ConvLayer& L, const std::string& prefix, const std::vector<int>& perm, int cin_pad, int k, int stride,
-                 int dh, int dw, int act, int H, int W, bool rows_wide = false);
-  // Packs OIHW weights w [Cout][Cin][L.k][L.k], output channel co times scale[co] (in double, rounded to float once),
-  // to L.w_host [tap][CinPad][CoutPad] with CinPad = perm.size(): packed input channel pc holds channel perm[pc], or
-  // zeros where that is -1.  Sets L's channel counts and uploads the weights and the bias [Cout] to L.w / L.bias.
-  bool pack_conv(ConvLayer& L, Arena& arena, const float* w, int Cout, int Cin, const double* scale, const float* bias,
-                 const std::vector<int>& perm);
-  // test hooks: pack_conv of the caller's device weights / bias, unscaled
+  // The eval-mode BatchNorm at `bn` (its weight, bias, running_mean, running_var and num_batches_tracked, C channels)
+  // after a layer with bias pre_bias (nullptr: none) as y = scale * x + shift per channel, in double:
+  // scale = gamma / sqrt(var + eps), shift = scale * (pre_bias - mean) + beta.
+  bool fold_bn(const std::string& bn, int C, const float* pre_bias, std::vector<double>& scale,
+               std::vector<double>& shift);
+  // H x W: the layer's output maps, from which tc_prepare chooses its kernel (rows_wide: see tc_prepare).
+  // The layer's padded input width is perm.size().
+  bool make_conv(ConvLayer& L, const std::string& prefix, const std::vector<int>& perm, int k, int stride, int dh,
+                 int dw, int act, int H, int W, bool rows_wide = false);
+  // Makes the device weights of L's kernel from its host-packed weights wp [tap][CinPad][CoutPad] and bias bp
+  // [CoutPad]: use_tc lets tc_prepare plan a tensor-core kernel for output maps of H x W; a layer left on the CUDA-core
+  // kernel gets wp / bp uploaded to L.w / L.bias in `arena`.
+  bool prepare_conv(ConvLayer& L, Arena& arena, const std::vector<float>& wp, const std::vector<float>& bp,
+                    bool use_tc, int H, int W, bool rows_wide);
+  // test hooks: pack_conv and prepare_conv of the caller's device weights / bias, unscaled
   bool debug_weights(ConvLayer& L, Arena& arena, const float* w, const float* bias, int Cout, int Cin,
-                     const std::vector<int>& perm, cudaStream_t s);
+                     const std::vector<int>& perm, bool use_tc, int H, int W, bool rows_wide, cudaStream_t s);
   bool to_nchw(const ActView& v, int C, float* y_nchw, cudaStream_t s);
-  bool build_basenet(BaseNetPlan& P, const std::string& prefix, int nin, const std::vector<int>& in_perm, int cin_pad,
-                     int n, int H, int W, int nin_lstm, int nout_lstm);
+  bool build_basenet(BaseNetPlan& P, const std::string& prefix, const std::vector<int>& in_perm, int n, int H, int W,
+                     int nin_lstm, int nout_lstm);
   bool run_conv(const ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, const ConvFusion& f = {});
   // Decoder (lib/layers.py:51-64): conv(cat[up(low), skip]) -> out.  fused: the row kernel produces up(low) itself and
   // `cat` holds only the skip channels; else up(low) is first written into channels [0, low.C) of `cat`.
@@ -312,9 +321,10 @@ class Engine {
   bool ck(cudaError_t e, const char* what);
 };
 
-// conv_tc.cu: plans L.tc for output maps of H x W (left null when the layer stays on the CUDA-core kernel).
+// conv_tc.cu: plans L.tc for output maps of H x W (left null when the layer stays on the CUDA-core kernel) and uploads
+// its weights from the host-packed w [tap][L.CinPad][L.CoutPad] and bias [L.Cout].
 // rows_wide: the row kernel may use its 64-output-channel tile (decoder layers whose upsample it fuses).
-bool tc_prepare(ConvLayer& L, int H, int W, bool rows_wide, std::string& err);
+bool tc_prepare(ConvLayer& L, const float* w, const float* bias, int H, int W, bool rows_wide, std::string& err);
 cudaError_t tc_launch(const ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, std::string& err,
                       const ConvFusion& f);
 
