@@ -225,6 +225,19 @@ VR_API int vr_debug_conv(vr_ctx* ctx, const float* x, int32_t N, int32_t Cin, in
 VR_API int vr_debug_decoder(vr_ctx* ctx, const float* low, int32_t N, int32_t Cl, int32_t h, int32_t w, const float* skip,
                      int32_t Cs, const float* wgt, const float* bias, int32_t Cout, int32_t act, int32_t fused, float* y,
                      void* stream);
+/* Images [n0, n0 + n) of one tensor the last forward (vr_predict_mask, vr_forward, vr_separate*) left on the device,
+ * copied to out (device float32) asynchronously on stream; synchronise the forward first.  Names:
+ *   "in3", "o1", "o2", "f3"         the stage-input buffer, the stage-1 / stage-2 low-band outputs, stage 3's output
+ *   "<prefix>.<buf>"                a BaseNet buffer, <prefix> its state_dict prefix (e.g. "stg3_full_band_net") and
+ *                                   <buf> one of cat1 lstm_up t2 cat2 t3 cat3 t4 cat4 t5 e5 pool f1 acat ao d4 d3 d2
+ *   "<prefix>.lstm.{l0,xp,hs,y}"    the LSTM branch's planes
+ * An activation buffer comes back as NCHW [n][C][H][W] with every channel of the buffer, pads included; its channel
+ * layout is DESIGN.md section 4's.  The LSTM planes come back as l0 / y [n][bins][T] (l0: the 1x1 input convolution
+ * before its bias), xp [n][T][8*hid] (gate pre-activations, forward then reverse) and hs [n][T][2*hid], with
+ * shape4[3] = 1.  out == NULL only fills shape4 = {n, C, H, W}.  Fails for an unknown name, n0 < 0, n0 + n > max_batch,
+ * "lstm_up" in a BaseNet whose up(lstm) group lives in cat1, and y images the last forward did not compute.      */
+VR_API int vr_debug_tensor(vr_ctx* ctx, const char* name, int32_t n0, int32_t n, float* out, int64_t* shape4,
+                           void* stream);
 /* Process-wide debug knobs of the tensor-core kernels: key 0 = 1 makes CTA 0 of the row-streaming kernel record a
  * timeline (builds with -DVR_TRACE), key 2 = 1 makes vr_debug_conv use its 64-channel output tile, key 3 = 1 sends the
  * layers prepared afterwards (every vr_debug_conv call prepares its layer) from the halo-tile kernel to the generic

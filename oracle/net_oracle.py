@@ -85,6 +85,14 @@ def aspp(sd, p, x, dilations=((4, 2), (8, 4), (12, 6))):
     return conv_bn_act(sd, p + '.bottleneck', torch.cat(feats, dim=1), pad=0)
 
 
+def lstm_dense(sd, p, h):
+    """lib/layers.py:119-122,131: Linear + BatchNorm1d + ReLU of the BiLSTM output h (M, 2*hid) -> (M, nbins)."""
+    h = F.linear(h, _t(sd, p + '.dense.0.weight'), _t(sd, p + '.dense.0.bias'))
+    h = F.batch_norm(h, _t(sd, p + '.dense.1.running_mean'), _t(sd, p + '.dense.1.running_var'),
+                     _t(sd, p + '.dense.1.weight'), _t(sd, p + '.dense.1.bias'), False, 0.0, BN_EPS)
+    return F.relu(h)
+
+
 def lstm_module(sd, p, x):
     """lib/layers.py:124-133: returns (N, 1, nbins, nframes)."""
     N, _, nbins, nframes = x.shape
@@ -97,11 +105,8 @@ def lstm_module(sd, p, x):
                 for n in ('weight_ih', 'weight_hh', 'bias_ih', 'bias_hh')]
         zeros = torch.zeros(2, N, hid, device=x.device, dtype=x.dtype)
         out, _, _ = torch._VF.lstm(h, (zeros, zeros), flat, True, 1, 0.0, False, True, False)
-        h2 = out.reshape(nframes * N, 2 * hid)
-        h2 = F.linear(h2, _t(sd, p + '.dense.0.weight'), _t(sd, p + '.dense.0.bias'))
-        h2 = F.batch_norm(h2, _t(sd, p + '.dense.1.running_mean'), _t(sd, p + '.dense.1.running_var'),
-                          _t(sd, p + '.dense.1.weight'), _t(sd, p + '.dense.1.bias'), False, 0.0, BN_EPS)
-        return F.relu(h2).reshape(nframes, N, 1, nbins).permute(1, 2, 3, 0)
+        h2 = lstm_dense(sd, p, out.reshape(nframes * N, 2 * hid))
+        return h2.reshape(nframes, N, 1, nbins).permute(1, 2, 3, 0)
     outs = []
     for sfx, rev in (('', False), ('_reverse', True)):
         w_ih = _t(sd, f'{p}.lstm.weight_ih_l0{sfx}')
@@ -119,11 +124,7 @@ def lstm_module(sd, p, x):
             hs = torch.sigmoid(o) * torch.tanh(cs)
             out[t] = hs
         outs.append(out)
-    h = torch.cat(outs, dim=2).reshape(nframes * N, 2 * hid)
-    h = F.linear(h, _t(sd, p + '.dense.0.weight'), _t(sd, p + '.dense.0.bias'))
-    h = F.batch_norm(h, _t(sd, p + '.dense.1.running_mean'), _t(sd, p + '.dense.1.running_var'),
-                     _t(sd, p + '.dense.1.weight'), _t(sd, p + '.dense.1.bias'), False, 0.0, BN_EPS)
-    h = F.relu(h)
+    h = lstm_dense(sd, p, torch.cat(outs, dim=2).reshape(nframes * N, 2 * hid))
     return h.reshape(nframes, N, 1, nbins).permute(1, 2, 3, 0)
 
 

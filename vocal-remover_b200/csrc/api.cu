@@ -344,6 +344,12 @@ int vr_debug_decoder(vr_ctx* ctx, const float* low, int32_t N, int32_t Cl, int32
                                            (cudaStream_t)stream));
 }
 
+int vr_debug_tensor(vr_ctx* ctx, const char* name, int32_t n0, int32_t n, float* out, int64_t* shape4, void* stream) {
+  CHECK_NET(ctx);
+  if (!name || !shape4) return fail(ctx, "vr_debug_tensor: name and shape4 are required");
+  return done(ctx, ctx->eng->debug_tensor(name, n0, n, out, shape4, (cudaStream_t)stream));
+}
+
 int vr_debug_set(int32_t key, int32_t value) {
   int* knob = key == 0 ? &vr::g_debug.trace : key == 2 ? &vr::g_debug.rows_wide : key == 3 ? &vr::g_debug.halo
             : key == 6 ? &vr::g_debug.kskip : key == 7 ? &vr::g_debug.crop_mask : nullptr;

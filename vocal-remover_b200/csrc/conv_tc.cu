@@ -284,7 +284,8 @@ static NTiling n_tiling(const ConvLayer& L, bool rows, bool rows_wide) {
 }
 
 // The kernel of a layer whose output maps are H x W: the row kernel where it applies, else the halo kernel, else the
-// generic one.  The row and halo kernels stage the bias of every N tile in 256 floats of shared memory.
+// generic one.  All three kernels stage the bias of every N tile in 256 floats of shared memory, so a layer with more
+// output channels than that stays on the CUDA-core kernel.
 TcKind tc_choose(const ConvLayer& L, int H, int W, bool rows_wide) {
   if (!(L.k == 1 || L.k == 3) || !(L.stride == 1 || L.stride == 2) || L.Cout < 4) return TC_NONE;
   const TileGeom g = tile_geom(H, W);
@@ -297,6 +298,7 @@ TcKind tc_choose(const ConvLayer& L, int H, int W, bool rows_wide) {
   if (k3s1 && (W == 16 || W == 32 || W == 64) && H % (128 / W) == 0 && tc_halo_has(t.BN) &&
       t.n_tiles * t.BN <= 256 && g_debug.halo != 1)
     return TC_HALO;
+  if (t.n_tiles * t.BN > 256) return TC_NONE;
   return TC_GENERIC;
 }
 

@@ -613,6 +613,7 @@ bool Engine::forward(int N, const MaskOutParams& mask, cudaStream_t s) {
   const int max_bin = cfg_.n_fft / 2, Hb = max_bin / 2;
   const int nout = cfg_.nout, a1 = nout / 4, a2 = nout / 2;
   const int c0_1 = pos_x_ / 16 * 16, c0_2 = pos_aux1_ / 16 * 16;
+  last_n_ = N;
   // Stages 1 and 2 (lib/nets.py:91-99): the low-band chain (stg1_low -> bridge -> stg2_low -> bridge) and the
   // high-band chain (stg1_high -> stg2_high) only meet at stage 3, so they run on two streams.
   const bool two = s_hi_ != nullptr && !profiling_;
@@ -1028,6 +1029,76 @@ bool Engine::debug_decoder(const float* low_nchw, int N, int Cl, int h, int w, c
   const ActView out = bout.view(N, 0, H, 0, Cout);
   return run_decoder(L, blow.all(N), bcat, N, out, fused != 0, s) && to_nchw(out, Cout, y_nchw, s) &&
          ck(cudaStreamSynchronize(s), "debug_decoder sync");
+}
+
+// Every activation buffer and LSTM plane is an allocation of its own (build_basenet, finalize), so after a forward each
+// one still holds what that forward wrote into it.
+bool Engine::debug_tensor(const std::string& name, int n0, int n, float* out, int64_t* shape4, cudaStream_t s) {
+  if (n0 < 0 || n < 0 || n0 + n > cfg_.max_batch) {
+    err = "debug_tensor: images [" + std::to_string(n0) + ", " + std::to_string(n0 + n) + ") outside [0, max_batch = " +
+          std::to_string(cfg_.max_batch) + ")";
+    return false;
+  }
+  const Buffer* buf = name == "in3" ? &in3_ : name == "o1" ? &o1_ : name == "o2" ? &o2_ : name == "f3" ? &f3_ : nullptr;
+  const BaseNetPlan* P = nullptr;
+  std::string member;
+  for (const BaseNetPlan& q : nets_)
+    if (name.size() > q.prefix.size() + 1 && name.compare(0, q.prefix.size() + 1, q.prefix + ".") == 0) {
+      P = &q;
+      member = name.substr(q.prefix.size() + 1);
+    }
+  if (P) {
+    const std::pair<const char*, const Buffer*> members[] = {
+        {"cat1", &P->cat1}, {"lstm_up", &P->lstm_up}, {"t2", &P->t2}, {"cat2", &P->cat2}, {"t3", &P->t3},
+        {"cat3", &P->cat3}, {"t4", &P->t4}, {"cat4", &P->cat4}, {"t5", &P->t5}, {"e5", &P->e5}, {"pool", &P->pool},
+        {"f1", &P->f1}, {"acat", &P->acat}, {"ao", &P->ao}, {"d4", &P->d4}, {"d3", &P->d3}, {"d2", &P->d2}};
+    for (const auto& m : members)
+      if (member == m.first) buf = m.second;
+    if (member == "lstm_up" && !P->lstm_own) {
+      err = "debug_tensor: " + P->prefix + " has no lstm_up buffer (its up(lstm) group is a channel slice of cat1)";
+      return false;
+    }
+  }
+  if (buf) {
+    const int64_t shape[4] = {n, buf->C, buf->H, buf->W};
+    for (int i = 0; i < 4; ++i) shape4[i] = shape[i];
+    if (!out) return true;
+    ActView v = buf->all(n);
+    v.hi += (int64_t)n0 * v.sn;
+    v.lo += (int64_t)n0 * v.sn;
+    return to_nchw(v, buf->C, out, s);
+  }
+  // LSTM planes in logical layouts: l0 / y (n, bins, T), xp (n, T, 8 hid), hs (n, T, 2 hid); shape4[3] = 1
+  const LstmPlan* Q = P ? &P->lstm : nullptr;
+  const float* src = nullptr;
+  int64_t d1 = 0, d2 = 0;
+  if (Q && member == "lstm.l0") { src = Q->l0; d1 = Q->bins; d2 = Q->T; }
+  if (Q && member == "lstm.xp") { src = Q->xp; d1 = Q->T; d2 = 8 * Q->hid; }
+  if (Q && member == "lstm.hs") { src = Q->hs; d1 = Q->T; d2 = 2 * Q->hid; }
+  if (Q && member == "lstm.y") { src = Q->y; d1 = Q->bins; d2 = Q->T; }
+  if (!src) {
+    err = "debug_tensor: unknown tensor name " + name;
+    return false;
+  }
+  const int64_t shape[4] = {n, d1, d2, 1};
+  for (int i = 0; i < 4; ++i) shape4[i] = shape[i];
+  if (!out) return true;
+  if (member != "lstm.y")
+    return ck(cudaMemcpyAsync(out, src + (int64_t)n0 * d1 * d2, sizeof(float) * (size_t)(n * d1 * d2),
+                              cudaMemcpyDeviceToDevice, s), "debug_tensor copy");
+  // y is stored [bin][image][t] with the last forward's batch as the image count
+  if (n0 + n > last_n_) {
+    err = "debug_tensor: the last forward ran " + std::to_string(last_n_) + " images; " + name + " has no image " +
+          std::to_string(n0 + n - 1);
+    return false;
+  }
+  for (int i = 0; i < n; ++i)
+    if (!ck(cudaMemcpy2DAsync(out + (int64_t)i * d1 * d2, sizeof(float) * (size_t)d2,
+                              src + (int64_t)(n0 + i) * d2, sizeof(float) * (size_t)last_n_ * d2,
+                              sizeof(float) * (size_t)d2, (size_t)d1, cudaMemcpyDeviceToDevice, s),
+            "debug_tensor copy"))
+      return false;
+  return true;
 }
 
 }  // namespace vr

@@ -215,6 +215,9 @@ class Engine {
                   int k, int stride, int dil_h, int dil_w, int act, int use_tc, float* y_nchw, cudaStream_t s);
   bool debug_decoder(const float* low_nchw, int N, int Cl, int h, int w, const float* skip_nchw, int Cs, const float* wgt,
                      const float* bias, int Cout, int act, int fused, float* y_nchw, cudaStream_t s);
+  // debug / tests: images [n0, n0 + n) of an activation buffer or LSTM plane as the last forward left it; see
+  // vr_debug_tensor in include/vr_b200.h.  out == nullptr: only shape4 is filled.
+  bool debug_tensor(const std::string& name, int n0, int n, float* out, int64_t* shape4, cudaStream_t s);
 
   const Config& cfg() const { return cfg_; }
   int bins() const { return cfg_.n_fft / 2 + 1; }
@@ -279,6 +282,7 @@ class Engine {
   Buffer o1_, o2_;             // low-band BaseNet outputs before the 1x1 bridge (stage 1 / stage 2)
   Buffer f3_;                  // stage-3 output (Nb, max_bin, W, nout)
   BaseNetPlan nets_[5];        // stg1_low, stg1_high, stg2_low, stg2_high, stg3_full
+  int last_n_ = 0;             // window batch of the last forward: the row stride of every LSTM plane y
   ConvLayer bridge1_, bridge2_;
   float* out_w_ = nullptr;     // [2][nout]
 
