@@ -20,6 +20,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle import net_oracle
+from oracle.precision_oracle import activation, bf16, fold_bn, folded_conv
 
 CONV_GATE = 2.0 ** -12
 NONVACUOUS = 8.0
@@ -48,40 +49,11 @@ def state_dict64(sd, device):
     return out
 
 
-def bf16(x):
-    return x.to(torch.bfloat16).to(x.dtype)
-
-
-def split_bf16(x):
-    """(hi, lo) of the product's activation storage: hi = bf16(x), lo = bf16(x - hi)"""
-    hi = bf16(x)
-    return hi, bf16(x - hi)
-
-
-def fold_bn(sd, bn, pre_bias=None):
-    """eval BatchNorm at ``bn`` as y = scale * x + shift per channel, in float64 (engine.cu fold_bn)."""
-    g, b = net_oracle._t(sd, bn + '.weight').double(), net_oracle._t(sd, bn + '.bias').double()
-    m, v = net_oracle._t(sd, bn + '.running_mean').double(), net_oracle._t(sd, bn + '.running_var').double()
-    scale = g / torch.sqrt(v + net_oracle.BN_EPS)
-    shift = scale * ((0.0 if pre_bias is None else pre_bias.double()) - m) + b
-    return scale, shift
-
-
-def folded_conv(sd, p):
-    """(w', b') of Conv2DBNActiv ``p``: its weights and bias with the BatchNorm folded in, float64."""
-    scale, shift = fold_bn(sd, p + '.conv.1')
-    return net_oracle._t(sd, p + '.conv.0.weight').double() * scale[:, None, None, None], shift
-
-
 def max_ratio(err, den):
     """max of |err| / den, where 0 / 0 counts as 0"""
     num = err.abs()
     r = torch.where(num == 0, torch.zeros_like(num), num / den)
     return float(r.max()) if r.numel() else 0.0
-
-
-def _act(y, act):
-    return F.relu(y) if act == 'relu' else F.leaky_relu(y, 0.01)
 
 
 def conv_ratios(sd, p, x, y, stride=1, pad=1, dil=1, act='relu'):
@@ -91,8 +63,8 @@ def conv_ratios(sd, p, x, y, stride=1, pad=1, dil=1, act='relu'):
     w, b = folded_conv(sd, p)
     kw = dict(stride=stride, padding=pad, dilation=dil)
     den = F.conv2d(x * x, w * w, None, **kw).sqrt() + 2.0 ** -4 * ref.abs()
-    no_wlo = _act(F.conv2d(x, bf16(w), b, **kw), act)
-    no_xlo = _act(F.conv2d(bf16(x), w, b, **kw), act)
+    no_wlo = activation(F.conv2d(x, bf16(w), b, **kw), act)
+    no_xlo = activation(F.conv2d(bf16(x), w, b, **kw), act)
     r = None if y is None else max_ratio(y - ref, den)
     return r, max_ratio(no_wlo - ref, den), max_ratio(no_xlo - ref, den), ref, den
 

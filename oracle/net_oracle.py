@@ -48,10 +48,10 @@ def conv_bn_act(sd, p, x, stride=1, pad=1, dil=1, act='relu'):
     raise ValueError(act)
 
 
-def encoder(sd, p, x):
+def encoder(sd, p, x, conv=conv_bn_act):
     """lib/layers.py:29-40 (ksize 3, stride 2, pad 1, LeakyReLU)."""
-    h = conv_bn_act(sd, p + '.conv1', x, stride=2, pad=1, act='leaky')
-    return conv_bn_act(sd, p + '.conv2', h, stride=1, pad=1, act='leaky')
+    h = conv(sd, p + '.conv1', x, stride=2, pad=1, act='leaky')
+    return conv(sd, p + '.conv2', h, stride=1, pad=1, act='leaky')
 
 
 def crop_center(h1, h2):
@@ -64,25 +64,25 @@ def crop_center(h1, h2):
     return h1[:, :, :, s:s + h2.shape[3]]
 
 
-def decoder(sd, p, x, skip):
+def decoder(sd, p, x, skip, conv=conv_bn_act):
     """lib/layers.py:51-64."""
     x = F.interpolate(x, scale_factor=2, mode='bilinear', align_corners=True)
     skip = crop_center(skip, x)
     x = torch.cat([x, skip], dim=1)
-    return conv_bn_act(sd, p + '.conv1', x, stride=1, pad=1, act='relu')
+    return conv(sd, p + '.conv1', x, stride=1, pad=1, act='relu')
 
 
-def aspp(sd, p, x, dilations=((4, 2), (8, 4), (12, 6))):
+def aspp(sd, p, x, dilations=((4, 2), (8, 4), (12, 6)), conv=conv_bn_act):
     """lib/layers.py:92-105 (dropout is identity in eval)."""
     _, _, h, w = x.shape
     pooled = x.mean(dim=2, keepdim=True)  # AdaptiveAvgPool2d((1, None))
-    f1 = conv_bn_act(sd, p + '.conv1.1', pooled, pad=0)
+    f1 = conv(sd, p + '.conv1.1', pooled, pad=0)
     f1 = F.interpolate(f1, size=(h, w), mode='bilinear', align_corners=True)
-    f2 = conv_bn_act(sd, p + '.conv2', x, pad=0)
+    f2 = conv(sd, p + '.conv2', x, pad=0)
     feats = [f1, f2]
     for i, d in zip((3, 4, 5), dilations):
-        feats.append(conv_bn_act(sd, f'{p}.conv{i}', x, pad=d, dil=d))
-    return conv_bn_act(sd, p + '.bottleneck', torch.cat(feats, dim=1), pad=0)
+        feats.append(conv(sd, f'{p}.conv{i}', x, pad=d, dil=d))
+    return conv(sd, p + '.bottleneck', torch.cat(feats, dim=1), pad=0)
 
 
 def lstm_dense(sd, p, h):
@@ -93,10 +93,10 @@ def lstm_dense(sd, p, h):
     return F.relu(h)
 
 
-def lstm_module(sd, p, x):
+def lstm_module(sd, p, x, conv=conv_bn_act):
     """lib/layers.py:124-133: returns (N, 1, nbins, nframes)."""
     N, _, nbins, nframes = x.shape
-    h = conv_bn_act(sd, p + '.conv', x, pad=0)[:, 0]          # N, nbins, nframes
+    h = conv(sd, p + '.conv', x, pad=0)[:, 0]                 # N, nbins, nframes
     h = h.permute(2, 0, 1).contiguous()                       # nframes, N, nbins
     hid = _t(sd, p + '.lstm.weight_hh_l0').shape[1]
     if x.is_cuda:
@@ -128,23 +128,24 @@ def lstm_module(sd, p, x):
     return h.reshape(nframes, N, 1, nbins).permute(1, 2, 3, 0)
 
 
-def basenet(sd, p, x):
+def basenet(sd, p, x, conv=conv_bn_act):
     """lib/nets.py:26-41."""
-    e1 = conv_bn_act(sd, p + '.enc1', x)
-    e2 = encoder(sd, p + '.enc2', e1)
-    e3 = encoder(sd, p + '.enc3', e2)
-    e4 = encoder(sd, p + '.enc4', e3)
-    e5 = encoder(sd, p + '.enc5', e4)
-    h = aspp(sd, p + '.aspp', e5)
-    h = decoder(sd, p + '.dec4', h, e4)
-    h = decoder(sd, p + '.dec3', h, e3)
-    h = decoder(sd, p + '.dec2', h, e2)
-    h = torch.cat([h, lstm_module(sd, p + '.lstm_dec2', h)], dim=1)
-    return decoder(sd, p + '.dec1', h, e1)
+    e1 = conv(sd, p + '.enc1', x)
+    e2 = encoder(sd, p + '.enc2', e1, conv)
+    e3 = encoder(sd, p + '.enc3', e2, conv)
+    e4 = encoder(sd, p + '.enc4', e3, conv)
+    e5 = encoder(sd, p + '.enc5', e4, conv)
+    h = aspp(sd, p + '.aspp', e5, conv=conv)
+    h = decoder(sd, p + '.dec4', h, e4, conv)
+    h = decoder(sd, p + '.dec3', h, e3, conv)
+    h = decoder(sd, p + '.dec2', h, e2, conv)
+    h = torch.cat([h, lstm_module(sd, p + '.lstm_dec2', h, conv)], dim=1)
+    return decoder(sd, p + '.dec1', h, e1, conv)
 
 
-def forward(sd, x, n_fft=2048, return_stages=False):
-    """lib/nets.py:82-117 (real mask).  x: float32 (N, 2, n_fft//2+1, W) -> mask same shape."""
+def forward(sd, x, n_fft=2048, return_stages=False, conv=conv_bn_act):
+    """lib/nets.py:82-117 (real mask).  x: float32 (N, 2, n_fft//2+1, W) -> mask same shape.  ``conv`` runs every
+    Conv2DBNActiv, with conv_bn_act's signature (oracle/precision_oracle.py emulates the product's arithmetic)."""
     with torch.no_grad():
         if not torch.is_tensor(x):
             x = torch.from_numpy(x)
@@ -153,14 +154,14 @@ def forward(sd, x, n_fft=2048, return_stages=False):
         x = x[:, :, :max_bin]
         bandw = x.shape[2] // 2
         l1_in, h1_in = x[:, :, :bandw], x[:, :, bandw:]
-        l1 = conv_bn_act(sd, 'stg1_low_band_net.1', basenet(sd, 'stg1_low_band_net.0', l1_in), pad=0)
-        h1 = basenet(sd, 'stg1_high_band_net', h1_in)
+        l1 = conv(sd, 'stg1_low_band_net.1', basenet(sd, 'stg1_low_band_net.0', l1_in, conv), pad=0)
+        h1 = basenet(sd, 'stg1_high_band_net', h1_in, conv)
         aux1 = torch.cat([l1, h1], dim=2)
-        l2 = conv_bn_act(sd, 'stg2_low_band_net.1',
-                         basenet(sd, 'stg2_low_band_net.0', torch.cat([l1_in, l1], dim=1)), pad=0)
-        h2 = basenet(sd, 'stg2_high_band_net', torch.cat([h1_in, h1], dim=1))
+        l2 = conv(sd, 'stg2_low_band_net.1',
+                  basenet(sd, 'stg2_low_band_net.0', torch.cat([l1_in, l1], dim=1), conv), pad=0)
+        h2 = basenet(sd, 'stg2_high_band_net', torch.cat([h1_in, h1], dim=1), conv)
         aux2 = torch.cat([l2, h2], dim=2)
-        f3 = basenet(sd, 'stg3_full_band_net', torch.cat([x, aux1, aux2], dim=1))
+        f3 = basenet(sd, 'stg3_full_band_net', torch.cat([x, aux1, aux2], dim=1), conv)
         logit = F.conv2d(f3, _t(sd, 'out.weight'))
         mask = torch.sigmoid(logit)
         mask = F.pad(mask, (0, 0, 0, output_bin - mask.shape[2]), mode='replicate')

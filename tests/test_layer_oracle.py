@@ -1,16 +1,17 @@
 """The per-layer gates of tests/test_gpu_layer_parity.py rehearsed on the CPU (oracle/layer_oracle.py).
 
 The small net (CascadedNet(512, 256, 16, 32), one 192-frame window) runs through the oracle with every convolution
-replaced by the CPU emulation of the product's arithmetic (tests/precision_budget.py: split-bf16 operands, three
-products, fp32 accumulation, split-bf16 output).  Each convolution's input and emulated output then go through the
-helper the GPU test uses: the three-product scheme must pass the gate, and dropping either correction product must
-fail it by 8x.  The LSTM branch's gates are rehearsed the same way on fp32 CPU arithmetic.
+replaced by the CPU emulation of the product's arithmetic (oracle/precision_oracle.py's default scheme: split-bf16
+operands, three products, fp32 accumulation, split-bf16 output).  Each convolution's input and emulated output then go
+through the helper the GPU test uses: the three-product scheme must pass the gate, and dropping either correction
+product must fail it by 8x.  The LSTM branch's gates are rehearsed the same way on fp32 CPU arithmetic.
 """
 import numpy as np
 import pytest
 import torch
 
 from oracle import layer_oracle as lo
+from oracle import precision_oracle as po
 
 N_FFT, HOP, NOUT, NOUT_LSTM, CROP = 512, 256, 16, 32, 192
 
@@ -18,7 +19,6 @@ N_FFT, HOP, NOUT, NOUT_LSTM, CROP = 512, 256, 16, 32, 192
 @pytest.fixture(scope='module')
 def captured():
     """(prefix, x, y, conv kwargs) of every convolution of one emulated forward, and the float64 state dict"""
-    import precision_budget as pb
     from lib import synth
     from oracle import net_oracle, stft_oracle
     sd = synth.to_torch_state_dict(synth.make_state_dict(N_FFT, NOUT, NOUT_LSTM))
@@ -26,18 +26,13 @@ def captured():
     x = torch.from_numpy(np.abs(X[None, :, :, :CROP]) / np.abs(X).max()).float()
     convs = []
 
-    def hook(sd_, p, x_, stride=1, pad=1, dil=1, act='relu'):
-        y = pb.conv_bn_act_emulated(sd_, p, x_, stride, pad, dil, act)
+    def conv(sd_, p, x_, stride=1, pad=1, dil=1, act='relu'):
+        y = po.Scheme().conv_bn_act(sd_, p, x_, stride, pad, dil, act)
         convs.append((p, x_, y, dict(stride=stride, pad=pad, dil=dil, act=act)))
         return y
 
-    exact = net_oracle.conv_bn_act
-    net_oracle.conv_bn_act = hook
-    try:
-        with torch.no_grad():
-            net_oracle.forward(sd, x, n_fft=N_FFT)
-    finally:
-        net_oracle.conv_bn_act = exact
+    with torch.no_grad():
+        net_oracle.forward(sd, x, n_fft=N_FFT, conv=conv)
     return convs, lo.state_dict64(sd, 'cpu')
 
 
@@ -80,7 +75,7 @@ def test_lstm_gates_on_cpu(captured):
             continue
         q = p[:-len('.conv')]
         sd32 = {k: (v.float() if v.is_floating_point() else v) for k, v in sd64.items()}
-        scale, shift = lo.fold_bn(sd64, q + '.conv.conv.1')
+        scale, shift = po.fold_bn(sd64, q + '.conv.conv.1')
         w = (net_oracle._t(sd64, q + '.conv.conv.0.weight')[0, :, 0, 0] * scale[0]).float()
         l0 = torch.einsum('nchw,c->nhw', x, w)
         a = F.relu(l0 + float(shift[0])).permute(0, 2, 1)
