@@ -189,6 +189,29 @@ VR_API int vr_flac_scan(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, int64
 VR_API int vr_flac_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int64_t* frames, int32_t n_frames,
                           int32_t channels, int64_t n_samples, float* out, int64_t* status, void* stream);
 
+/* FLAC encoding on the device (RFC 9639 streamable subset; lib/flac.py is the caller, oracle/flac_oracle.py decodes
+ * the result independently): fixed block size FLAC_ENCODE_BLOCK (the last block shorter), 16 bits per sample, one or
+ * two channels.  All buffers are DEVICE memory owned by the caller; neither call allocates.  ctx may be NULL, as for
+ * vr_flac_scan.  frames = ceil(n / FLAC_ENCODE_BLOCK); rate_code is the frame header's sample-rate code (1-11 from
+ * the table, 12-14 with rate_value written after the header as RFC 9639 section 9.1.2 gives).
+ *
+ * vr_flac_encode_analyse: one CTA per frame.  x: [channels][n] float32, quantised as clip(rint(x * 32767), -32768,
+ * 32767) in fp32 (NaN -> 0) into pcm: [n][channels] int16 (interleaved, as the STREAMINFO MD5 reads it).  Chooses
+ * every subframe's coding and the channel assignment by exact size and writes plan: frames rows of
+ * FLAC_ENCODE_PLAN_INTS int32, plan[f * FLAC_ENCODE_PLAN_INTS] = frame f's size in bytes (the rest is private to
+ * vr_flac_encode_pack).  The plan, and with it every byte, is the same on every run.
+ *
+ * vr_flac_encode_pack: one CTA per frame.  offsets: frames int64, the byte offset of each frame in out (the exclusive
+ * scan of the plan's sizes, plus the caller's header length); writes each frame, CRC-8 and CRC-16 included, to its
+ * span.  status: frames int32, 0 when the frame filled exactly the size the plan gave, else nonzero.        */
+#define FLAC_ENCODE_BLOCK 4096
+#define FLAC_ENCODE_PLAN_INTS 192
+VR_API int vr_flac_encode_analyse(vr_ctx* ctx, const float* x, int32_t channels, int64_t n, int32_t rate_code,
+                                  int16_t* pcm, int32_t* plan, void* stream);
+VR_API int vr_flac_encode_pack(vr_ctx* ctx, const int16_t* pcm, int32_t channels, int64_t n, const int32_t* plan,
+                               const int64_t* offsets, int32_t rate_code, int32_t rate_value, uint8_t* out,
+                               int32_t* status, void* stream);
+
 /* Multi-GPU mask exchange over NVLink peer memory (one process per GPU).  The owner (rank 0) allocates the
  * whole-track mask with vr_shared_alloc and publishes the 64-byte CUDA IPC handle; every other rank maps it
  * with vr_shared_open and passes the mapped pointer as `mask` to vr_separate_windows, so the mask epilogue

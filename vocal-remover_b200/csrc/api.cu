@@ -264,6 +264,22 @@ int vr_flac_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int6
                                             (cudaStream_t)stream));
 }
 
+int vr_flac_encode_analyse(vr_ctx* ctx, const float* x, int32_t channels, int64_t n, int32_t rate_code, int16_t* pcm,
+                           int32_t* plan, void* stream) {
+  if (ctx && ctx->eng) cudaSetDevice(ctx->eng->cfg().device);
+  return flac_result(ctx, "vr_flac_encode_analyse",
+                     vr::launch_flac_encode_analyse(x, channels, n, rate_code, pcm, plan, (cudaStream_t)stream));
+}
+
+int vr_flac_encode_pack(vr_ctx* ctx, const int16_t* pcm, int32_t channels, int64_t n, const int32_t* plan,
+                        const int64_t* offsets, int32_t rate_code, int32_t rate_value, uint8_t* out, int32_t* status,
+                        void* stream) {
+  if (ctx && ctx->eng) cudaSetDevice(ctx->eng->cfg().device);
+  return flac_result(ctx, "vr_flac_encode_pack",
+                     vr::launch_flac_encode_pack(pcm, channels, n, plan, offsets, rate_code, rate_value, out, status,
+                                                 (cudaStream_t)stream));
+}
+
 int vr_shared_alloc(vr_ctx* ctx, int64_t bytes, void** dev_ptr, unsigned char* handle64) {
   CHECK_CTX(ctx);
   if (!dev_ptr || !handle64 || bytes <= 0) return fail(ctx, "vr_shared_alloc: bad arguments");

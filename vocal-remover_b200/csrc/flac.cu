@@ -17,11 +17,14 @@
 // every write stays in the frame's own samples, and each frame leaves a status word (0, or code << 40 | bit offset in
 // the frame) for the host to turn into an error.
 #include "common.cuh"
+#include "flac_common.cuh"
 #include "kernels.h"
 
 namespace vr {
 
 namespace {
+
+using flac::crc8_byte;
 
 constexpr int kWarpsPerBlock = 4;
 constexpr int kMaxChannels = 8;
@@ -46,13 +49,6 @@ enum FlacError : int64_t {
 };
 
 __device__ __forceinline__ int64_t flac_status(int64_t code, int64_t bit) { return (code << 40) | (bit & 0xFFFFFFFFFFLL); }
-
-__device__ __forceinline__ uint32_t crc8_byte(uint32_t c, uint32_t b) {
-  c ^= b;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) c = (c & 0x80) ? ((c << 1) ^ 0x07) & 0xFF : (c << 1) & 0xFF;
-  return c;
-}
 
 // the frame header at byte i (d[i] == 0xFF and d[i+1] is 0xF8 / 0xF9 already); false if it is not one
 __device__ bool parse_frame_header(const uint8_t* __restrict__ d, int64_t n, int64_t i, int64_t rec[4]) {
@@ -328,11 +324,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) flac_decode_kernel(
   __shared__ SubMeta meta_s[kWarpsPerBlock][kMaxChannels];
   __shared__ int32_t coef_s[kWarpsPerBlock][kMaxChannels][kMaxLpcOrder];
   __shared__ int32_t hist_s[kWarpsPerBlock][kMaxChannels][kMaxLpcOrder];
-  for (int b = threadIdx.x; b < 256; b += blockDim.x) {
-    uint32_t c = (uint32_t)b << 8;
-    for (int k = 0; k < 8; ++k) c = (c & 0x8000) ? ((c << 1) ^ 0x8005) : (c << 1);
-    crc_tab[b] = (uint16_t)c;
-  }
+  flac::crc16_table(crc_tab);
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int f = blockIdx.x * kWarpsPerBlock + warp;
@@ -366,24 +358,9 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) flac_decode_kernel(
   e = __shfl_sync(0xffffffffu, e, 0);
   __syncwarp();   // lane 0's staged samples are visible to the other lanes
 
-  if (!err) {   // CRC-16 of [start, e): lane t takes one chunk of the message left-padded with zeros to 32 chunks
-    const int64_t L = e - start;
-    const int64_t chunk = (L + 31) / 32, pad = 32 * chunk - L;
-    uint32_t c = 0, col = lane < 16 ? 1u << lane : 0u;   // col: bit `lane` advanced over `chunk` zero bytes
-    for (int64_t v = lane * chunk; v < (lane + 1) * chunk; ++v) {
-      if (v >= pad) c = ((c << 8) & 0xFFFF) ^ crc_tab[(c >> 8) ^ __ldg(d + start + v - pad)];
-      col = ((col << 8) & 0xFFFF) ^ crc_tab[col >> 8];
-    }
-    uint32_t cols[16];
-#pragma unroll
-    for (int b = 0; b < 16; ++b) cols[b] = __shfl_sync(0xffffffffu, col, b);
-    uint32_t r = 0;
-    for (int t = 0; t < 32; ++t) {
-      uint32_t a = 0;
-#pragma unroll
-      for (int b = 0; b < 16; ++b) a ^= ((r >> b) & 1u) ? cols[b] : 0u;
-      r = a ^ __shfl_sync(0xffffffffu, c, t);
-    }
+  if (!err) {   // CRC-16 of [start, e)
+    const uint8_t* fr = d + start;
+    const uint32_t r = flac::warp_crc16(e - start, crc_tab, [&](int64_t v) { return (uint32_t)__ldg(fr + v); });
     const uint32_t want = ((uint32_t)__ldg(d + e) << 8) | __ldg(d + e + 1);
     if (r != want) err = flac_status(kCrc16, 8 * (e - start));
   }

@@ -116,4 +116,13 @@ cudaError_t launch_flac_scan(const uint8_t* data, int64_t n_bytes, int64_t begin
 cudaError_t launch_flac_decode(const uint8_t* data, int64_t n_bytes, const int64_t* frames, int n_frames, int channels,
                                int64_t n_samples, float* out, int64_t* status, cudaStream_t stream);
 
+// ---- FLAC frame encoding (flac_encode.cu), the encode behind --output_format flac (lib/flac.py) ----------------------
+// analyse: one CTA per 4096-sample frame of x [channels][n] -> pcm [n][channels] int16, plan [frames][192] int32 (the
+// frame's size in bytes first); pack: plan + each frame's byte offset -> the frames' bytes in out, status[frames]
+cudaError_t launch_flac_encode_analyse(const float* x, int channels, int64_t n, int rate_code, int16_t* pcm,
+                                       int32_t* plan, cudaStream_t stream);
+cudaError_t launch_flac_encode_pack(const int16_t* pcm, int channels, int64_t n, const int32_t* plan,
+                                    const int64_t* offsets, int rate_code, int rate_value, uint8_t* out,
+                                    int32_t* status, cudaStream_t stream);
+
 }  // namespace vr

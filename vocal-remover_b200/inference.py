@@ -15,6 +15,7 @@ import torch
 from lib import _native
 from lib import audio_io
 from lib import dataset
+from lib import flac
 from lib import nets
 from lib import spec_utils
 from lib import utils
@@ -196,6 +197,8 @@ def main():
     p.add_argument('--tta', '-t', action='store_true')
     p.add_argument('--postprocess', '-p', action='store_true')
     p.add_argument('--output_dir', '-o', type=str, default="")
+    # an extension of the reference CLI: lossless 16-bit FLAC stems, encoded on the GPU (lib/flac.py)
+    p.add_argument('--output_format', choices=['wav', 'flac'], default='wav')
     args = p.parse_args()
 
     # missing requirements fail before any heavy work (model load, audio decode, output directory)
@@ -251,12 +254,20 @@ def main():
         images = False
 
     print('stft of wave source, separation, inverse stft of instruments and vocals...', end=' ')
-    out = sp.separate_wave(X, tta=args.tta, images=images)
+    flac_out = args.output_format == 'flac'
+    # FLAC: the stems stay on the device for the encoder, and only the compressed bytes come back
+    out = sp.separate_wave(torch.from_numpy(np.ascontiguousarray(X)).to(device) if flac_out else X, tta=args.tta,
+                           images=images)
     wave_inst, wave_voc = out[:2]
     print('done')
     writer = audio_io.AsyncWriter()   # the two stems (and images) are encoded and written concurrently
-    writer.write('{}{}_Instruments.wav'.format(output_dir, basename), wave_inst.T, sr)
-    writer.write('{}{}_Vocals.wav'.format(output_dir, basename), wave_voc.T, sr)
+    if flac_out:
+        writer.run(flac.encode, wave_inst, sr, '{}{}_Instruments.flac'.format(output_dir, basename))
+        writer.run(flac.encode, wave_voc, sr, '{}{}_Vocals.flac'.format(output_dir, basename))
+        out = [t.cpu().numpy() if i >= 2 else t for i, t in enumerate(out)]
+    else:
+        writer.write('{}{}_Instruments.wav'.format(output_dir, basename), wave_inst.T, sr)
+        writer.write('{}{}_Vocals.wav'.format(output_dir, basename), wave_voc.T, sr)
     if images:
         writer.run(utils.imwrite, '{}{}_Instruments.jpg'.format(output_dir, basename), out[2])
         writer.run(utils.imwrite, '{}{}_Vocals.jpg'.format(output_dir, basename), out[3])

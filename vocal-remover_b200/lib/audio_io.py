@@ -2,7 +2,8 @@
 
 The reference uses ``librosa.load(path, sr=sr, mono=False, dtype=np.float32, res_type='kaiser_fast')`` and
 ``soundfile.write`` (inference.py:136-138,173,178).  FLAC input is decoded on the GPU when there is one (lib/flac.py,
-csrc/flac.cu); other decoding and all encoding stay on the host (soundfile when installed, else a stdlib ``wave``
+csrc/flac.cu) and FLAC output encoded on it (csrc/flac_encode.cu); other decoding and encoding stay on the host
+(soundfile when installed, else a stdlib ``wave``
 reader for 8/16/24/32-bit PCM WAV and writer for 16-bit); the sample-rate conversion of non-``sr`` input - the
 expensive part of ``librosa.load`` - runs on the GPU (``vr_resample``, csrc/resample.cu): resampy 0.4's algorithm with the
 ``kaiser_fast`` table taken from an installed resampy, or regenerated from its documented parameters otherwise
@@ -122,7 +123,22 @@ def load(path, sr, mono=False, dtype=np.float32, device=None):
 
 
 def write(path, data, sr):
-    """data: (L, channels) float array, like soundfile.write."""
+    """data: (L, channels) float array, like soundfile.write.  A ``.flac`` path is encoded on the GPU whenever a CUDA
+    device is visible (lib/flac.py, 16 bits), else by soundfile; with neither it raises before creating the file."""
+    if str(path).lower().endswith('.flac'):
+        import torch
+        if torch.cuda.is_available():
+            from . import flac
+            x = data if torch.is_tensor(data) else np.asarray(data, np.float32)
+            flac.encode(x[None] if x.ndim == 1 else x.T, sr, path)   # (channels, L)
+            return
+        try:
+            import soundfile as sf
+        except ImportError:
+            raise RuntimeError('%s: writing FLAC needs a CUDA device (lib/flac.py) or the soundfile module, and neither '
+                               'is available' % path) from None
+        sf.write(path, data, sr)
+        return
     try:
         import soundfile as sf
         sf.write(path, data, sr)

@@ -14,13 +14,29 @@ length), copies the bytes to the device once, and runs two kernels of csrc/flac.
 
 Malformed input raises ``ValueError`` naming the file, the frame and its byte offset.  The MD5 in STREAMINFO is not
 checked on this path (libsndfile does not check it either).
+
+FLAC output, ``encode(x, rate, path=None) -> bytes``: 16 bits per sample, one or two channels, fixed block size
+``BLOCK`` (the last block shorter), inside the streamable subset.  Two kernels of csrc/flac_encode.cu with a host step
+between them:
+
+1. ``vr_flac_encode_analyse`` quantises each frame to int16 and chooses every subframe's coding and the channel
+   assignment by exact size; it leaves the int16 samples and a plan with each frame's size in bytes.
+2. The host scans the frame sizes into byte offsets (numpy).
+3. ``vr_flac_encode_pack`` writes every frame to its span, CRCs included.
+
+The host puts ``fLaC`` and STREAMINFO in front; STREAMINFO's MD5 is computed with hashlib from the int16 samples.
 """
+import hashlib
 import os
 
 import numpy as np
 
 BPS_CODES = {1: 8, 2: 12, 4: 16, 5: 20, 6: 24}
 MAX_BLOCK = 65535
+BLOCK = 4096                 # FLAC_ENCODE_BLOCK (include/vr_b200.h)
+PLAN_INTS = 192              # FLAC_ENCODE_PLAN_INTS
+RATE_CODES = {88200: 1, 176400: 2, 192000: 3, 8000: 4, 16000: 5, 22050: 6, 24000: 7, 32000: 8, 44100: 9, 48000: 10,
+              96000: 11}
 
 # status codes of flac_decode_kernel (csrc/flac.cu)
 ERRORS = {
@@ -231,3 +247,105 @@ def decode(src, device=None):
                          % (name, k, int(frames[k, 0]), ERRORS.get(code, 'error %d' % code), bit))
     check_length(info, total, name)
     return out, info['rate'], info['bps']
+
+
+# ------------------------------------------------------------------------------------------------------------- encoder
+
+
+def rate_code(rate):
+    """(frame-header sample-rate code, value written after the header) of ``rate``; codes 12-14 for rates that are not
+    in the table, as the streamable subset requires."""
+    rate = int(rate)
+    if rate in RATE_CODES:
+        return RATE_CODES[rate], 0
+    if rate % 1000 == 0 and rate // 1000 <= 255:
+        return 12, rate // 1000
+    if 0 < rate <= 65535:
+        return 13, rate
+    if rate % 10 == 0 and rate // 10 <= 65535:
+        return 14, rate // 10
+    raise ValueError('FLAC output: a sample rate of %d Hz cannot be coded in a frame header' % rate)
+
+
+def stream_header(channels, total, rate, frame_sizes, md5, block=BLOCK):
+    """``fLaC`` and the one STREAMINFO block of a fixed-block-size 16-bit stream: min / max block size (the last block
+    excluded, unless it is the only one), min / max frame size, rate, channels, 16 bits, total samples, MD5."""
+    sizes = [block] * (len(frame_sizes) - 1) + [total - block * (len(frame_sizes) - 1)]
+    bmin = max(16, min(sizes[:-1] or sizes))
+    bmax = min(65535, max(16, max(sizes)))
+    fmin, fmax = int(min(frame_sizes)), int(max(frame_sizes))
+    si = bmin.to_bytes(2, 'big') + bmax.to_bytes(2, 'big') + fmin.to_bytes(3, 'big') + fmax.to_bytes(3, 'big')
+    si += ((int(rate) << 44) | ((channels - 1) << 41) | (15 << 36) | int(total)).to_bytes(8, 'big') + bytes(md5)
+    return b'fLaC' + bytes([0x80]) + len(si).to_bytes(3, 'big') + si
+
+
+class Frames(object):
+    """The frames of one encode: ``body`` (bytes), ``sizes`` (int64 per frame), ``pcm`` (the int16 samples the frames
+    code, (n, channels) on the device), ``channels``, ``total`` and ``rate``."""
+
+    def __init__(self, body, sizes, pcm, channels, total, rate):
+        self.body, self.sizes, self.pcm = body, sizes, pcm
+        self.channels, self.total, self.rate = channels, total, rate
+
+
+def encode_frames(x, rate, device=None):
+    """float (channels, n) -> Frames.  ``x``: a CUDA float32 tensor (stays on its device) or an array."""
+    import torch
+    from . import _native
+    if not torch.cuda.is_available():
+        raise RuntimeError('FLAC encoding runs on the GPU and no CUDA device is visible')
+    code, value = rate_code(rate)
+    if torch.is_tensor(x) and x.is_cuda:
+        dev = x.device
+    else:
+        dev = torch.device(device if device is not None else 'cuda:0')
+    if x.ndim != 2 or x.shape[0] not in (1, 2) or x.shape[1] < 1:
+        raise ValueError('FLAC output takes (channels, n) samples with one or two channels and n >= 1, not %s'
+                         % (tuple(x.shape),))
+    C, n = int(x.shape[0]), int(x.shape[1])
+    if n >= 1 << 36:
+        raise ValueError('FLAC output: %d samples per channel exceed STREAMINFO\'s 36 bits' % n)
+    lib = _native.load_library()
+
+    def check(rc, what):
+        if rc != 0:
+            raise _native.NativeError('%s failed: %s' % (what, lib.vr_last_error(None).decode()))
+
+    with torch.cuda.device(dev):
+        xd = x if torch.is_tensor(x) else torch.from_numpy(np.ascontiguousarray(x, np.float32))
+        xd = xd.to(dev, torch.float32).contiguous()
+        F = (n + BLOCK - 1) // BLOCK
+        pcm = torch.empty((n, C), dtype=torch.int16, device=dev)
+        plan = torch.empty((F, PLAN_INTS), dtype=torch.int32, device=dev)
+        stream = _native.stream_ptr()
+        check(lib.vr_flac_encode_analyse(None, _native.ptr(xd), C, n, code, _native.ptr(pcm), _native.ptr(plan),
+                                         stream), 'vr_flac_encode_analyse')
+        sizes = plan[:, 0].cpu().numpy().astype(np.int64)
+        offsets = np.zeros(F, np.int64)
+        np.cumsum(sizes[:-1], out=offsets[1:])
+        out = torch.empty(int(sizes.sum()), dtype=torch.uint8, device=dev)
+        status = torch.empty(F, dtype=torch.int32, device=dev)
+        d_off = torch.from_numpy(offsets).to(dev)
+        check(lib.vr_flac_encode_pack(None, _native.ptr(pcm), C, n, _native.ptr(plan), _native.ptr(d_off), code, value,
+                                      _native.ptr(out), _native.ptr(status), stream), 'vr_flac_encode_pack')
+        body = out.cpu().numpy().tobytes()
+        st = status.cpu().numpy()
+    bad = np.flatnonzero(st)
+    if bad.size:
+        raise RuntimeError('FLAC encode: frame %d did not fill the size its plan gave (status %d)'
+                           % (int(bad[0]), int(st[bad[0]])))
+    return Frames(body, sizes, pcm, C, n, int(rate))
+
+
+def encode(x, rate, path=None, md5=True):
+    """float (channels, n) -> the whole FLAC stream (bytes): ``fLaC``, STREAMINFO, the frames; also written to ``path``
+    when one is given.  ``x`` is a CUDA float32 tensor (it stays on the device; only the compressed bytes and the int16
+    samples for the MD5 are copied back) or an array; samples are quantised as clip(rint(x * 32767)), NaN -> 0.
+    ``md5=False`` leaves STREAMINFO's MD5 zero (unknown), which skips the copy of the samples and the hash."""
+    fr = encode_frames(x, rate)
+    digest = hashlib.md5(fr.pcm.cpu().numpy().astype('<i2', copy=False).tobytes()).digest() if md5 else bytes(16)
+    data = stream_header(fr.channels, fr.total, fr.rate, fr.sizes, digest) + fr.body
+    if path is not None:
+        with open(path, 'wb') as f:
+            f.write(data)
+    return data
