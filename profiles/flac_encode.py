@@ -3,11 +3,12 @@
 Inputs: ``synth.sine_mix(240)`` and the two stems of separating it with the seeded checkpoint (synth.make_state_dict).
 Reported per input: the analyse and pack kernel times (CUDA events, warm-up, median of --runs), one whole
 ``flac.encode`` call with and without the host MD5 (CUDA events around the call, which ends in copies to the host),
-bytes in (float32) and out, the ratio to a 16-bit WAV, and the separation of the same track for comparison.  With
+bytes in (float32) and out, the ratio to PCM of the same width, and the separation of the same track for comparison.
+--bits 24 measures the 24-bit instantiations of the kernels (and ``vr_pcm_pack``, which makes the MD5's bytes).  With
 --cli, also the wall time of ``inference.py`` with ``--output_format wav`` and ``flac``, alternating.  The card's name
 and power limit are read in the same run (read-only ``nvidia-smi --query-gpu``).
 
-Usage: python profiles/flac_encode.py [--runs 20] [--cli 2] [--out flac_encode.json]
+Usage: python profiles/flac_encode.py [--bits 16] [--runs 20] [--cli 2] [--out flac_encode.json]
 """
 import argparse
 import json
@@ -52,7 +53,7 @@ def _median_ms(fn, runs, warmup=3):
     return [float(np.median(times)), float(np.min(times)), float(np.max(times))]
 
 
-def _kernels(x, runs):
+def _kernels(x, runs, bits):
     """analyse and pack kernel times of one input, as lib/flac.encode_frames launches them"""
     import torch
     from lib import _native, flac
@@ -60,12 +61,13 @@ def _kernels(x, runs):
     C, n = x.shape
     F = (n + flac.BLOCK - 1) // flac.BLOCK
     code, value = flac.rate_code(44100)
-    pcm = torch.empty((n, C), dtype=torch.int16, device=x.device)
+    pcm = torch.empty((n, C), dtype=getattr(torch, flac.BITS[bits]), device=x.device)
     plan = torch.empty((F, flac.PLAN_INTS), dtype=torch.int32, device=x.device)
     st = _native.stream_ptr()
 
     def analyse():
-        assert lib.vr_flac_encode_analyse(None, _native.ptr(x), C, n, code, _native.ptr(pcm), _native.ptr(plan), st) == 0
+        assert lib.vr_flac_encode_analyse(None, _native.ptr(x), C, n, code, bits, _native.ptr(pcm), _native.ptr(plan),
+                                          st) == 0
     analyse_ms = _median_ms(analyse, runs)
     sizes = plan[:, 0].cpu().numpy().astype(np.int64)
     offsets = torch.from_numpy(np.concatenate([[0], np.cumsum(sizes)[:-1]])).to(x.device)
@@ -73,14 +75,18 @@ def _kernels(x, runs):
     status = torch.empty(F, dtype=torch.int32, device=x.device)
 
     def pack():
-        assert lib.vr_flac_encode_pack(None, _native.ptr(pcm), C, n, _native.ptr(plan), _native.ptr(offsets), code,
-                                       value, _native.ptr(out), _native.ptr(status), st) == 0
+        assert lib.vr_flac_encode_pack(None, _native.ptr(pcm), C, n, bits, _native.ptr(plan), _native.ptr(offsets),
+                                       code, value, _native.ptr(out), _native.ptr(status), st) == 0
     pack_ms = _median_ms(pack, runs)
     assert not status.cpu().numpy().any()
-    return F, analyse_ms, pack_ms
+    raw = torch.empty(n * C * (bits // 8), dtype=torch.uint8, device=x.device)
+
+    def pcm_pack():
+        assert lib.vr_pcm_pack(None, _native.ptr(x), C, n, bits, _native.ptr(raw), st) == 0
+    return F, analyse_ms, pack_ms, _median_ms(pcm_pack, runs)
 
 
-def _cli(runs):
+def _cli(runs, bits):
     """wall time of inference.py on a 4-minute 16-bit WAV, --output_format wav and flac alternating"""
     import torch
     from lib import synth
@@ -101,7 +107,8 @@ def _cli(runs):
                 out = os.path.join(tmp, '%s%d' % (fmt, i))
                 t0 = time.perf_counter()
                 r = subprocess.run([sys.executable, os.path.join(PKG, 'inference.py'), '-g', '0', '-P', ckpt, '-i', src,
-                                    '-o', out, '--output_format', fmt], capture_output=True, text=True, cwd=PKG)
+                                    '-o', out, '--output_format', fmt, '--output_bits', str(bits)],
+                                   capture_output=True, text=True, cwd=PKG)
                 walls[fmt].append(round(time.perf_counter() - t0, 2))
                 assert r.returncode == 0, r.stderr
                 sizes[fmt] = sum(os.path.getsize(os.path.join(out, f)) for f in os.listdir(out))
@@ -110,6 +117,7 @@ def _cli(runs):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument('--bits', type=int, choices=[16, 24], default=16, help='bits per encoded sample')
     ap.add_argument('--runs', type=int, default=20)
     ap.add_argument('--cli', type=int, default=0, help='CLI runs per format (0: skip)')
     ap.add_argument('--out', default=None)
@@ -126,24 +134,25 @@ def main():
     sp = inference.Separator(model, dev, 4, 256, False)
     separate_ms = _median_ms(lambda: sp.separate_wave(mix), max(3, args.runs // 4), warmup=2)
     inst, voc = sp.separate_wave(mix)
-    res = dict(_gpu_info(), torch_device=torch.cuda.get_device_name(0), separate_wave_4min_ms=separate_ms, inputs={})
+    res = dict(_gpu_info(), torch_device=torch.cuda.get_device_name(0), bits=args.bits,
+               separate_wave_4min_ms=separate_ms, inputs={})
     for name, x in (('sine_mix', mix), ('instruments', inst), ('vocals', voc)):
-        frames, analyse_ms, pack_ms = _kernels(x, args.runs)
-        call_ms = _median_ms(lambda: flac.encode(x, 44100), args.runs)
-        call_nomd5_ms = _median_ms(lambda: flac.encode(x, 44100, md5=False), args.runs)
-        data = flac.encode(x, 44100)
-        wav = 44 + x.numel() * 2
+        frames, analyse_ms, pack_ms, pcm_pack_ms = _kernels(x, args.runs, args.bits)
+        call_ms = _median_ms(lambda: flac.encode(x, 44100, bits=args.bits), args.runs)
+        call_nomd5_ms = _median_ms(lambda: flac.encode(x, 44100, md5=False, bits=args.bits), args.runs)
+        data = flac.encode(x, 44100, bits=args.bits)
+        wav = 44 + x.numel() * (args.bits // 8)
         res['inputs'][name] = dict(frames=frames, samples_per_channel=int(x.shape[1]), bytes_in_float32=x.numel() * 4,
-                                   bytes_out=len(data), wav16_bytes=wav, ratio_to_wav16=round(len(data) / wav, 4),
-                                   analyse_kernel_ms=analyse_ms, pack_kernel_ms=pack_ms, encode_call_ms=call_ms,
-                                   encode_call_no_md5_ms=call_nomd5_ms)
+                                   bytes_out=len(data), wav_bytes=wav, ratio_to_wav=round(len(data) / wav, 4),
+                                   analyse_kernel_ms=analyse_ms, pack_kernel_ms=pack_ms, pcm_pack_kernel_ms=pcm_pack_ms,
+                                   encode_call_ms=call_ms, encode_call_no_md5_ms=call_nomd5_ms)
     stems = res['inputs']
     res['both_stems_kernels_ms'] = round(sum(stems[s]['analyse_kernel_ms'][0] + stems[s]['pack_kernel_ms'][0]
                                              for s in ('instruments', 'vocals')), 3)
     res['timing_note'] = ('[median, min, max] over %d runs after 3 warm-up runs; separate_wave over %d runs'
                           % (args.runs, max(3, args.runs // 4)))
     if args.cli:
-        res.update(_cli(args.cli))
+        res.update(_cli(args.cli, args.bits))
     line = json.dumps(res)
     print(line)
     if args.out:

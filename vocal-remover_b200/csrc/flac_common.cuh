@@ -8,6 +8,7 @@ namespace vr {
 namespace flac {
 
 constexpr int kBpsCode16 = 4;   // sample-size code of 16 bits per sample
+constexpr int kBpsCode24 = 6;   // and of 24
 constexpr int kBlockCodeTable4096 = 12;   // block-size code 256 << (12 - 8) = 4096
 constexpr int kBlockCode8Bit = 6;         // block size - 1 in one byte after the coded number
 constexpr int kBlockCode16Bit = 7;        // block size - 1 in two bytes

@@ -1,10 +1,16 @@
 // FLAC encoding (RFC 9639) of float32 stems on the device: the encode behind `--output_format flac` (lib/flac.py drives
-// it; oracle/flac_oracle.py decodes the result independently).
+// it; oracle/flac_oracle.py decodes the result independently), and the PCM packer behind 24-bit WAV output.
 //
-// The stream has a fixed block size of 4096 (the last block is shorter), 16 bits per sample, one or two channels, and
-// stays inside the streamable subset: LPC order <= 12, coefficient precision 15 with shift 0..15, Rice partition order
-// <= 8, sample-rate and sample-size codes in every frame header.  Two kernels with a host step between them:
-//   flac_analyse_kernel  one CTA per frame.  Quantises the frame to int16 (clip(rint(x * 32767)), NaN -> 0) into the
+// The stream has a fixed block size of 4096 (the last block is shorter), 16 or 24 bits per sample, one or two channels,
+// and stays inside the streamable subset: LPC order <= 12, coefficient precision 15 with shift 0..15, Rice partition
+// order <= 8, sample-rate and sample-size codes in every frame header.  The sample width BITS is a template parameter
+// of both kernels: it sets the quantiser's scale, the element type of pcm (int16 / int32), the subframes' sample bits
+// (BITS, and BITS + 1 for the side channel S = L - R, which spans 25 bits at 24), the sample-size code and the size of
+// the pack kernel's bit buffer.  Everything downstream of the samples is width-blind: residuals are int32 (an LPC
+// residual outside it, or INT32_MIN, which RFC 9639 forbids, rules that predictor out; FIXED order 4 of 25-bit
+// samples reaches 29 bits), their zigzag is uint32, and sums of code lengths are 64-bit.
+// Two kernels with a host step between them:
+//   flac_analyse_kernel  one CTA per frame.  Quantises the frame (clip(rint(x * (2^(BITS-1) - 1))), NaN -> 0) into the
 //                        interleaved pcm buffer and shared memory, then codes every signal (L, R, M = (L+R)>>1,
 //                        S = L-R for stereo) as CONSTANT, VERBATIM, FIXED 0-4 or LPC 1-12 (Tukey(0.5)-windowed
 //                        autocorrelation, Levinson-Durbin in fp64) and prices each predictor exactly: bit-plane counts of
@@ -16,7 +22,11 @@
 //   flac_pack_kernel     one CTA per frame.  Recomputes the chosen residuals, places every code by a block prefix sum
 //                        of code lengths, ORs the codes into a shared bit buffer (the bits are disjoint, so the order of
 //                        the ORs does not matter), copies the frame to its byte span and appends CRC-8 / CRC-16.
+//   pcm_pack_kernel      the quantiser alone: x [channels][n] -> interleaved little-endian 2- or 3-byte PCM, what a WAV
+//                        file's data chunk and the STREAMINFO MD5 read.  One thread per 16 samples, 16-byte stores.
 // Every reduction is integer or in a fixed order and no float atomics are used: the bytes are the same on every run.
+#include <type_traits>
+
 #include "common.cuh"
 #include "flac_common.cuh"
 #include "kernels.h"
@@ -33,7 +43,9 @@ constexpr int kLpcPrecision = 15;
 constexpr int kPlanInts = 192;        // FLAC_ENCODE_PLAN_INTS
 constexpr int kSubBase = 8, kSubInts = 24, kParamBase = 64;
 constexpr int kTreeRows = (2 << kMaxPorder) - 1;   // partitions of all orders 0..8
-constexpr int kBufWords = (16 * 8 + 2 * (8 + 17 * kBlock) + 31) / 32 + 2;   // largest frame: two VERBATIM subframes
+// words of the largest frame: a 16-byte header and two VERBATIM subframes
+template <int BITS>
+constexpr int kBufWords = (16 * 8 + 2 * (8 + (BITS + 1) * kBlock) + 31) / 32 + 2;
 constexpr uint64_t kInf = ~0ull >> 2;
 
 enum Kind { kConstant = 0, kVerbatim = 1, kFixed = 2, kLpc = 3 };
@@ -58,10 +70,19 @@ __device__ __forceinline__ int header_bytes(int f, int bs, int rate_code) {
   return 4 + utf8_len(f) + bs_extra + flac::rate_code_bytes(rate_code) + 1;
 }
 
-__device__ __forceinline__ int16_t quantise(float v) {
+template <int BITS>
+struct Pcm {
+  static_assert(BITS == 16 || BITS == 24, "16 or 24 bits per sample");
+  using type = typename std::conditional<BITS == 16, int16_t, int32_t>::type;
+};
+
+// the integers of every writer: clip(rint(v * (2^(BITS-1) - 1))) with the product rounded once in fp32, NaN -> 0
+template <int BITS>
+__device__ __forceinline__ typename Pcm<BITS>::type quantise(float v) {
+  constexpr float kTop = (float)((1 << (BITS - 1)) - 1);
   if (v != v) return 0;
-  const float s = rintf(__fmul_rn(v, 32767.0f));
-  return (int16_t)fminf(fmaxf(s, -32768.0f), 32767.0f);
+  const float s = rintf(__fmul_rn(v, kTop));
+  return (typename Pcm<BITS>::type)fminf(fmaxf(s, -kTop - 1.0f), kTop);
 }
 
 // signal s of a frame from its two channels: 0 L (or mono), 1 R, 2 M = (L + R) >> 1, 3 S = L - R
@@ -74,7 +95,8 @@ __device__ __forceinline__ int32_t signal_at(int s, const int32_t* x0, const int
   }
 }
 
-// residual of sample j >= order; false when an LPC prediction leaves a residual outside int32
+// residual of sample j >= order; false when an LPC prediction leaves a residual outside int32 or equal to INT32_MIN
+// (not a legal residual, RFC 9639 section 9.2.7.3)
 __device__ __forceinline__ bool residual_at(const int32_t* __restrict__ sig, int j, int kind, int order,
                                             const int32_t* __restrict__ coef, int shift, int32_t& r) {
   if (kind == kFixed) {
@@ -92,7 +114,7 @@ __device__ __forceinline__ bool residual_at(const int32_t* __restrict__ sig, int
   for (int i = 0; i < order; ++i) sum += (int64_t)coef[i] * sig[j - 1 - i];
   const int64_t v = (int64_t)sig[j] - (sum >> shift);
   r = (int32_t)v;
-  return v == (int64_t)r;
+  return v == (int64_t)r && r != INT32_MIN;
 }
 
 __device__ __forceinline__ uint32_t zigzag(int32_t r) { return ((uint32_t)r << 1) ^ (uint32_t)(r >> 31); }
@@ -341,8 +363,10 @@ __device__ __forceinline__ void choose_subframe(AnalyseSmem& sm, int s, int bs, 
 
 }  // namespace
 
+template <int BITS>
 __global__ void __launch_bounds__(kThreads, 2) flac_analyse_kernel(const float* __restrict__ x, int C, int64_t n,
-                                                               int rate_code, int16_t* __restrict__ pcm,
+                                                               int rate_code,
+                                                               typename Pcm<BITS>::type* __restrict__ pcm,
                                                                int32_t* __restrict__ plan) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   AnalyseSmem& sm = *reinterpret_cast<AnalyseSmem*>(smem_raw);
@@ -351,13 +375,13 @@ __global__ void __launch_bounds__(kThreads, 2) flac_analyse_kernel(const float* 
   const int bs = (int)(n - start < kBlock ? n - start : kBlock);
   for (int c = 0; c < C; ++c)
     for (int j = threadIdx.x; j < bs; j += kThreads) {
-      const int16_t q = quantise(x[(int64_t)c * n + start + j]);
+      const typename Pcm<BITS>::type q = quantise<BITS>(x[(int64_t)c * n + start + j]);
       sm.x[c][j] = q;
       pcm[(start + j) * C + c] = q;
     }
   __syncthreads();
   const int nsig = C == 2 ? 4 : 1;
-  for (int s = 0; s < nsig; ++s) choose_subframe(sm, s, bs, 16 + (s == 3));
+  for (int s = 0; s < nsig; ++s) choose_subframe(sm, s, bs, BITS + (s == 3));
 
   // channel assignment by exact size: independent, left/side, side/right, mid/side
   __shared__ int sig_of[2], ch_code;
@@ -393,7 +417,7 @@ __global__ void __launch_bounds__(kThreads, 2) flac_analyse_kernel(const float* 
     }
     if (threadIdx.x == 0) {
       sub[0] = ch.kind; sub[1] = ch.order; sub[2] = ch.porder; sub[3] = ch.rice5;
-      sub[5] = 16 + (s == 3); sub[6] = (int32_t)ch.bits;
+      sub[5] = BITS + (s == 3); sub[6] = (int32_t)ch.bits;
     }
     total += ch.bits;
   }
@@ -408,10 +432,11 @@ __global__ void __launch_bounds__(kThreads, 2) flac_analyse_kernel(const float* 
 
 namespace {
 
+template <int BITS>
 struct PackSmem {
   int32_t x[2][kBlock];
   int32_t sig[kBlock];
-  uint32_t buf[kBufWords];
+  uint32_t buf[kBufWords<BITS>];
   uint32_t warp_tot[kThreads / 32];
   uint16_t crc_tab[256];
   int32_t row[kPlanInts];
@@ -439,13 +464,14 @@ struct FieldWriter {
 
 }  // namespace
 
-__global__ void __launch_bounds__(kThreads, 2) flac_pack_kernel(const int16_t* __restrict__ pcm, int C, int64_t n,
-                                                            const int32_t* __restrict__ plan,
+template <int BITS>
+__global__ void __launch_bounds__(kThreads, 2) flac_pack_kernel(const typename Pcm<BITS>::type* __restrict__ pcm, int C,
+                                                            int64_t n, const int32_t* __restrict__ plan,
                                                             const int64_t* __restrict__ offsets, int rate_code,
                                                             int rate_value, uint8_t* __restrict__ out,
                                                             int32_t* __restrict__ status) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  PackSmem& sm = *reinterpret_cast<PackSmem*>(smem_raw);
+  PackSmem<BITS>& sm = *reinterpret_cast<PackSmem<BITS>*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int f = blockIdx.x;
   const int64_t start = (int64_t)f * kBlock;
@@ -466,7 +492,7 @@ __global__ void __launch_bounds__(kThreads, 2) flac_pack_kernel(const int16_t* _
     h[k++] = 0xF8;
     const int bs_code = bs == kBlock ? flac::kBlockCodeTable4096 : (bs <= 256 ? flac::kBlockCode8Bit : flac::kBlockCode16Bit);
     h[k++] = (uint8_t)((bs_code << 4) | rate_code);
-    h[k++] = (uint8_t)((ch_code << 4) | (flac::kBpsCode16 << 1));
+    h[k++] = (uint8_t)((ch_code << 4) | ((BITS == 16 ? flac::kBpsCode16 : flac::kBpsCode24) << 1));
     const int nl = utf8_len(f);
     if (nl == 1) {
       h[k++] = (uint8_t)f;
@@ -597,34 +623,102 @@ __global__ void __launch_bounds__(kThreads, 2) flac_pack_kernel(const int16_t* _
   }
 }
 
-cudaError_t launch_flac_encode_analyse(const float* x, int channels, int64_t n, int rate_code, int16_t* pcm,
-                                       int32_t* plan, cudaStream_t stream) {
-  if (!x || !pcm || !plan || channels < 1 || channels > 2 || n < 1 || rate_code < 1 || rate_code > 14)
-    return cudaErrorInvalidValue;
-  const int64_t frames = (n + kBlock - 1) / kBlock;
-  if (frames > (1ll << 30)) return cudaErrorInvalidValue;
+namespace {
+
+// x [C][n] -> interleaved little-endian PCM of BITS / 8 bytes per sample.  A thread takes 16 consecutive interleaved
+// samples, which are BITS / 8 aligned 16-byte words of the output.
+template <int BITS>
+__global__ void __launch_bounds__(kThreads) pcm_pack_kernel(const float* __restrict__ x, int C, int64_t n,
+                                                            uint8_t* __restrict__ out) {
+  constexpr int kBytes = BITS / 8;
+  const int64_t total = n * C;
+  const int64_t i0 = 16 * ((int64_t)blockIdx.x * kThreads + threadIdx.x);
+  if (i0 >= total) return;
+  auto sample = [&](int64_t t) {   // interleaved index -> quantised sample
+    return (uint32_t)(int32_t)quantise<BITS>(C == 1 ? x[t] : x[(t & 1) * n + (t >> 1)]);
+  };
+  uint8_t* dst = out + i0 * kBytes;
+  if (total - i0 < 16) {   // the last, partial group: byte stores
+    for (int i = 0; i < (int)(total - i0); ++i) {
+      const uint32_t q = sample(i0 + i);
+      for (int b = 0; b < kBytes; ++b) dst[kBytes * i + b] = (uint8_t)(q >> (8 * b));
+    }
+    return;
+  }
+  uint32_t w[4 * kBytes];
+#pragma unroll
+  for (int k = 0; k < 4 * kBytes; ++k) w[k] = 0;
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const uint32_t q = sample(i0 + i);
+#pragma unroll
+    for (int b = 0; b < kBytes; ++b) w[(kBytes * i + b) >> 2] |= ((q >> (8 * b)) & 0xFFu) << (8 * ((kBytes * i + b) & 3));
+  }
+#pragma unroll
+  for (int k = 0; k < kBytes; ++k)
+    reinterpret_cast<uint4*>(dst)[k] = make_uint4(w[4 * k], w[4 * k + 1], w[4 * k + 2], w[4 * k + 3]);
+}
+
+template <int BITS>
+cudaError_t analyse(const float* x, int channels, int64_t n, int rate_code, void* pcm, int32_t* plan, int64_t frames,
+                    cudaStream_t stream) {
   const int smem = (int)sizeof(AnalyseSmem);
-  cudaError_t e = cudaFuncSetAttribute(flac_analyse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  cudaError_t e = cudaFuncSetAttribute(flac_analyse_kernel<BITS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (e != cudaSuccess) return e;
-  flac_analyse_kernel<<<(unsigned)frames, kThreads, smem, stream>>>(x, channels, n, rate_code, pcm, plan);
+  flac_analyse_kernel<BITS><<<(unsigned)frames, kThreads, smem, stream>>>(
+      x, channels, n, rate_code, static_cast<typename Pcm<BITS>::type*>(pcm), plan);
   return cudaGetLastError();
 }
 
-cudaError_t launch_flac_encode_pack(const int16_t* pcm, int channels, int64_t n, const int32_t* plan,
+template <int BITS>
+cudaError_t pack(const void* pcm, int channels, int64_t n, const int32_t* plan, const int64_t* offsets, int rate_code,
+                 int rate_value, uint8_t* out, int32_t* status, int64_t frames, cudaStream_t stream) {
+  const int smem = (int)sizeof(PackSmem<BITS>);
+  cudaError_t e = cudaFuncSetAttribute(flac_pack_kernel<BITS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e != cudaSuccess) return e;
+  flac_pack_kernel<BITS><<<(unsigned)frames, kThreads, smem, stream>>>(
+      static_cast<const typename Pcm<BITS>::type*>(pcm), channels, n, plan, offsets, rate_code, rate_value, out, status);
+  return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t launch_flac_encode_analyse(const float* x, int channels, int64_t n, int rate_code, int bits, void* pcm,
+                                       int32_t* plan, cudaStream_t stream) {
+  if (!x || !pcm || !plan || channels < 1 || channels > 2 || n < 1 || rate_code < 1 || rate_code > 14 ||
+      (bits != 16 && bits != 24))
+    return cudaErrorInvalidValue;
+  const int64_t frames = (n + kBlock - 1) / kBlock;
+  if (frames > (1ll << 30)) return cudaErrorInvalidValue;
+  return bits == 16 ? analyse<16>(x, channels, n, rate_code, pcm, plan, frames, stream)
+                    : analyse<24>(x, channels, n, rate_code, pcm, plan, frames, stream);
+}
+
+cudaError_t launch_flac_encode_pack(const void* pcm, int channels, int64_t n, int bits, const int32_t* plan,
                                     const int64_t* offsets, int rate_code, int rate_value, uint8_t* out,
                                     int32_t* status, cudaStream_t stream) {
   if (!pcm || !plan || !offsets || !out || !status || channels < 1 || channels > 2 || n < 1 || rate_code < 1 ||
-      rate_code > 14)
+      rate_code > 14 || (bits != 16 && bits != 24))
     return cudaErrorInvalidValue;
   const int64_t frames = (n + kBlock - 1) / kBlock;
   if (frames > (1ll << 30)) return cudaErrorInvalidValue;
   cudaError_t e = cudaMemsetAsync(status, 0, sizeof(int32_t) * frames, stream);
   if (e != cudaSuccess) return e;
-  const int smem = (int)sizeof(PackSmem);
-  e = cudaFuncSetAttribute(flac_pack_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  if (e != cudaSuccess) return e;
-  flac_pack_kernel<<<(unsigned)frames, kThreads, smem, stream>>>(pcm, channels, n, plan, offsets, rate_code, rate_value,
-                                                                 out, status);
+  return bits == 16 ? pack<16>(pcm, channels, n, plan, offsets, rate_code, rate_value, out, status, frames, stream)
+                    : pack<24>(pcm, channels, n, plan, offsets, rate_code, rate_value, out, status, frames, stream);
+}
+
+cudaError_t launch_pcm_pack(const float* x, int channels, int64_t n, int bits, uint8_t* out, cudaStream_t stream) {
+  if (!x || !out || channels < 1 || channels > 2 || n < 1 || (bits != 16 && bits != 24) ||
+      (reinterpret_cast<uintptr_t>(out) & 15))
+    return cudaErrorInvalidValue;
+  const int64_t groups = (n * channels + 15) / 16;
+  const int64_t blocks = (groups + kThreads - 1) / kThreads;
+  if (blocks > 0x7fffffffll) return cudaErrorInvalidValue;
+  if (bits == 16)
+    pcm_pack_kernel<16><<<(unsigned)blocks, kThreads, 0, stream>>>(x, channels, n, out);
+  else
+    pcm_pack_kernel<24><<<(unsigned)blocks, kThreads, 0, stream>>>(x, channels, n, out);
   return cudaGetLastError();
 }
 

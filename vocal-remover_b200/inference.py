@@ -183,7 +183,7 @@ DEFAULT_MODEL_PATH = os.path.join(MODEL_DIR, 'baseline.pth')
 JPEG_MAX_WIDTH = utils.JPEG_MAX_WIDTH
 
 
-def main():
+def build_parser():
     p = argparse.ArgumentParser()
     p.add_argument('--gpu', '-g', type=int, default=-1)
     p.add_argument('--pretrained_model', '-P', type=str, default=DEFAULT_MODEL_PATH)
@@ -197,9 +197,16 @@ def main():
     p.add_argument('--tta', '-t', action='store_true')
     p.add_argument('--postprocess', '-p', action='store_true')
     p.add_argument('--output_dir', '-o', type=str, default="")
-    # an extension of the reference CLI: lossless 16-bit FLAC stems, encoded on the GPU (lib/flac.py)
+    # an extension of the reference CLI: lossless FLAC stems, encoded on the GPU (lib/flac.py)
     p.add_argument('--output_format', choices=['wav', 'flac'], default='wav')
-    args = p.parse_args()
+    # an extension of the reference CLI too: bits per written sample of either format; 24 keeps the depth of a 24-bit
+    # input, which the float32 stems carry and 16-bit output throws away
+    p.add_argument('--output_bits', type=int, choices=[16, 24], default=16)
+    return p
+
+
+def main():
+    args = build_parser().parse_args()
 
     # missing requirements fail before any heavy work (model load, audio decode, output directory)
     if args.output_image:
@@ -255,19 +262,23 @@ def main():
 
     print('stft of wave source, separation, inverse stft of instruments and vocals...', end=' ')
     flac_out = args.output_format == 'flac'
-    # FLAC: the stems stay on the device for the encoder, and only the compressed bytes come back
-    out = sp.separate_wave(torch.from_numpy(np.ascontiguousarray(X)).to(device) if flac_out else X, tta=args.tta,
+    # FLAC and 24-bit WAV: the stems stay on the device for the encoder or the PCM packer, and only the file's bytes
+    # come back
+    on_device = flac_out or args.output_bits == 24
+    out = sp.separate_wave(torch.from_numpy(np.ascontiguousarray(X)).to(device) if on_device else X, tta=args.tta,
                            images=images)
     wave_inst, wave_voc = out[:2]
     print('done')
     writer = audio_io.AsyncWriter()   # the two stems (and images) are encoded and written concurrently
     if flac_out:
-        writer.run(flac.encode, wave_inst, sr, '{}{}_Instruments.flac'.format(output_dir, basename))
-        writer.run(flac.encode, wave_voc, sr, '{}{}_Vocals.flac'.format(output_dir, basename))
-        out = [t.cpu().numpy() if i >= 2 else t for i, t in enumerate(out)]
+        writer.run(flac.encode, wave_inst, sr, '{}{}_Instruments.flac'.format(output_dir, basename), True,
+                   args.output_bits)
+        writer.run(flac.encode, wave_voc, sr, '{}{}_Vocals.flac'.format(output_dir, basename), True, args.output_bits)
     else:
-        writer.write('{}{}_Instruments.wav'.format(output_dir, basename), wave_inst.T, sr)
-        writer.write('{}{}_Vocals.wav'.format(output_dir, basename), wave_voc.T, sr)
+        writer.write('{}{}_Instruments.wav'.format(output_dir, basename), wave_inst.T, sr, args.output_bits)
+        writer.write('{}{}_Vocals.wav'.format(output_dir, basename), wave_voc.T, sr, args.output_bits)
+    if on_device:
+        out = [t.cpu().numpy() if i >= 2 else t for i, t in enumerate(out)]
     if images:
         writer.run(utils.imwrite, '{}{}_Instruments.jpg'.format(output_dir, basename), out[2])
         writer.run(utils.imwrite, '{}{}_Vocals.jpg'.format(output_dir, basename), out[3])

@@ -4,7 +4,8 @@ The reference uses ``librosa.load(path, sr=sr, mono=False, dtype=np.float32, res
 ``soundfile.write`` (inference.py:136-138,173,178).  FLAC input is decoded on the GPU when there is one (lib/flac.py,
 csrc/flac.cu) and FLAC output encoded on it (csrc/flac_encode.cu); other decoding and encoding stay on the host
 (soundfile when installed, else a stdlib ``wave``
-reader for 8/16/24/32-bit PCM WAV and writer for 16-bit); the sample-rate conversion of non-``sr`` input - the
+reader for 8/16/24/32-bit PCM WAV and writer for 16-bit), except the samples of a 24-bit WAV, which are quantised and
+packed on the GPU like the FLAC encoder's (``vr_pcm_pack``); the sample-rate conversion of non-``sr`` input - the
 expensive part of ``librosa.load`` - runs on the GPU (``vr_resample``, csrc/resample.cu): resampy 0.4's algorithm with the
 ``kaiser_fast`` table taken from an installed resampy, or regenerated from its documented parameters otherwise
 (oracle/resample_oracle.py states what is and is not pinned).
@@ -122,22 +123,60 @@ def load(path, sr, mono=False, dtype=np.float32, device=None):
     return np.ascontiguousarray(x.astype(dtype)), rate
 
 
-def write(path, data, sr):
-    """data: (L, channels) float array, like soundfile.write.  A ``.flac`` path is encoded on the GPU whenever a CUDA
-    device is visible (lib/flac.py, 16 bits), else by soundfile; with neither it raises before creating the file."""
+def _write_wav24(path, data, sr):
+    """24-bit PCM WAV of (L, channels) or (L,) float samples, a CUDA tensor or an array: clip(rint(x * 8388607)) in fp32,
+    NaN -> 0.  With a CUDA device the samples are quantised and packed to 3 bytes there (lib/flac.pcm_bytes), soundfile
+    or not, so that the file holds the integers a 24-bit FLAC of the same data does."""
+    import torch
+    if torch.cuda.is_available():
+        from . import flac
+        x = data if torch.is_tensor(data) else np.asarray(data, np.float32)
+        channels = 1 if x.ndim == 1 else x.shape[1]
+        raw = flac.pcm_bytes(x[None] if x.ndim == 1 else x.T, 24)   # (channels, L)
+    else:
+        data = data.cpu().numpy() if torch.is_tensor(data) else np.asarray(data)
+        try:
+            import soundfile as sf
+            sf.write(path, data, sr, subtype='PCM_24')
+            return
+        except ImportError:
+            pass
+        v = np.rint(data.astype(np.float32) * np.float32(8388607.0))
+        q = np.clip(np.where(np.isnan(v), np.float32(0.0), v), -8388608, 8388607).astype('<i4')
+        channels = 1 if q.ndim == 1 else q.shape[1]
+        raw = np.ascontiguousarray(q).view(np.uint8).reshape(-1, 4)[:, :3].tobytes()
+    with open(path, 'wb') as fh, _wave.open(fh, 'wb') as f:
+        f.setnchannels(channels)
+        f.setsampwidth(3)
+        f.setframerate(sr)
+        f.writeframes(raw)
+
+
+def write(path, data, sr, bits=16):
+    """data: (L, channels) float array, like soundfile.write; ``bits``: 16 or 24 bits per written sample.  A ``.flac``
+    path is encoded on the GPU whenever a CUDA device is visible (lib/flac.py), else by soundfile; with neither it
+    raises before creating the file.  A 24-bit ``.wav`` is packed on the GPU when there is one (_write_wav24)."""
+    if bits not in (16, 24):
+        raise ValueError('%s: output samples are 16 or 24 bits wide, not %r' % (path, bits))
     if str(path).lower().endswith('.flac'):
         import torch
         if torch.cuda.is_available():
             from . import flac
             x = data if torch.is_tensor(data) else np.asarray(data, np.float32)
-            flac.encode(x[None] if x.ndim == 1 else x.T, sr, path)   # (channels, L)
+            flac.encode(x[None] if x.ndim == 1 else x.T, sr, path, bits=bits)   # (channels, L)
             return
         try:
             import soundfile as sf
         except ImportError:
             raise RuntimeError('%s: writing FLAC needs a CUDA device (lib/flac.py) or the soundfile module, and neither '
                                'is available' % path) from None
-        sf.write(path, data, sr)
+        if bits == 24:
+            sf.write(path, data, sr, subtype='PCM_24')
+        else:
+            sf.write(path, data, sr)
+        return
+    if bits == 24:
+        _write_wav24(path, data, sr)
         return
     try:
         import soundfile as sf
@@ -166,8 +205,8 @@ class AsyncWriter(object):
         self._threading = threading
         self._jobs = []
 
-    def write(self, path, data, sr):
-        self.run(write, path, data, sr)
+    def write(self, path, data, sr, bits=16):
+        self.run(write, path, data, sr, bits)
 
     def run(self, fn, *args):
         """Runs ``fn(*args)`` on a worker thread (e.g. lib.utils.imwrite of the --output_image JPGs)."""

@@ -15,16 +15,21 @@ length), copies the bytes to the device once, and runs two kernels of csrc/flac.
 Malformed input raises ``ValueError`` naming the file, the frame and its byte offset.  The MD5 in STREAMINFO is not
 checked on this path (libsndfile does not check it either).
 
-FLAC output, ``encode(x, rate, path=None) -> bytes``: 16 bits per sample, one or two channels, fixed block size
-``BLOCK`` (the last block shorter), inside the streamable subset.  Two kernels of csrc/flac_encode.cu with a host step
-between them:
+FLAC output, ``encode(x, rate, path=None, md5=True, bits=16) -> bytes``: 16 or 24 bits per sample, one or two channels,
+fixed block size ``BLOCK`` (the last block shorter), inside the streamable subset.  Two kernels of csrc/flac_encode.cu
+with a host step between them:
 
-1. ``vr_flac_encode_analyse`` quantises each frame to int16 and chooses every subframe's coding and the channel
-   assignment by exact size; it leaves the int16 samples and a plan with each frame's size in bytes.
+1. ``vr_flac_encode_analyse`` quantises each frame to ``bits``-wide integers and chooses every subframe's coding and
+   the channel assignment by exact size; it leaves the samples (int16, or int32 for 24 bits) and a plan with each
+   frame's size in bytes.
 2. The host scans the frame sizes into byte offsets (numpy).
 3. ``vr_flac_encode_pack`` writes every frame to its span, CRCs included.
 
-The host puts ``fLaC`` and STREAMINFO in front; STREAMINFO's MD5 is computed with hashlib from the int16 samples.
+The host puts ``fLaC`` and STREAMINFO in front; STREAMINFO's MD5 is computed with hashlib from the samples as
+interleaved little-endian ``bits / 8``-byte integers: the int16 samples as they are, the 24-bit ones packed to 3 bytes
+on the device by ``vr_pcm_pack`` (``pcm_bytes``), which is also what a 24-bit WAV file holds (lib/audio_io.write).
+
+The integers are ``clip(rint(x * (2^(bits-1) - 1)))`` with the product in fp32 and NaN -> 0, for every writer.
 """
 import hashlib
 import os
@@ -35,6 +40,7 @@ BPS_CODES = {1: 8, 2: 12, 4: 16, 5: 20, 6: 24}
 MAX_BLOCK = 65535
 BLOCK = 4096                 # FLAC_ENCODE_BLOCK (include/vr_b200.h)
 PLAN_INTS = 192              # FLAC_ENCODE_PLAN_INTS
+BITS = {16: 'int16', 24: 'int32'}   # output sample widths and the dtype of Frames.pcm for each
 RATE_CODES = {88200: 1, 176400: 2, 192000: 3, 8000: 4, 16000: 5, 22050: 6, 24000: 7, 32000: 8, 44100: 9, 48000: 10,
               96000: 11}
 
@@ -267,34 +273,38 @@ def rate_code(rate):
     raise ValueError('FLAC output: a sample rate of %d Hz cannot be coded in a frame header' % rate)
 
 
-def stream_header(channels, total, rate, frame_sizes, md5, block=BLOCK):
-    """``fLaC`` and the one STREAMINFO block of a fixed-block-size 16-bit stream: min / max block size (the last block
-    excluded, unless it is the only one), min / max frame size, rate, channels, 16 bits, total samples, MD5."""
+def _check_bits(bits):
+    if bits not in BITS:
+        raise ValueError('output samples are 16 or 24 bits wide, not %r' % (bits,))
+
+
+def stream_header(channels, total, rate, frame_sizes, md5, block=BLOCK, bits=16):
+    """``fLaC`` and the one STREAMINFO block of a fixed-block-size stream: min / max block size (the last block
+    excluded, unless it is the only one), min / max frame size, rate, channels, bits per sample, total samples, MD5."""
     sizes = [block] * (len(frame_sizes) - 1) + [total - block * (len(frame_sizes) - 1)]
     bmin = max(16, min(sizes[:-1] or sizes))
     bmax = min(65535, max(16, max(sizes)))
     fmin, fmax = int(min(frame_sizes)), int(max(frame_sizes))
     si = bmin.to_bytes(2, 'big') + bmax.to_bytes(2, 'big') + fmin.to_bytes(3, 'big') + fmax.to_bytes(3, 'big')
-    si += ((int(rate) << 44) | ((channels - 1) << 41) | (15 << 36) | int(total)).to_bytes(8, 'big') + bytes(md5)
+    si += ((int(rate) << 44) | ((channels - 1) << 41) | ((bits - 1) << 36) | int(total)).to_bytes(8, 'big') + bytes(md5)
     return b'fLaC' + bytes([0x80]) + len(si).to_bytes(3, 'big') + si
 
 
 class Frames(object):
-    """The frames of one encode: ``body`` (bytes), ``sizes`` (int64 per frame), ``pcm`` (the int16 samples the frames
-    code, (n, channels) on the device), ``channels``, ``total`` and ``rate``."""
+    """The frames of one encode: ``body`` (bytes), ``sizes`` (int64 per frame), ``pcm`` (the samples the frames code,
+    (n, channels) on the device: int16 for ``bits`` 16, int32 holding the 24-bit integers for 24), ``channels``,
+    ``total``, ``rate`` and ``bits``."""
 
-    def __init__(self, body, sizes, pcm, channels, total, rate):
+    def __init__(self, body, sizes, pcm, channels, total, rate, bits=16):
         self.body, self.sizes, self.pcm = body, sizes, pcm
-        self.channels, self.total, self.rate = channels, total, rate
+        self.channels, self.total, self.rate, self.bits = channels, total, rate, bits
 
 
-def encode_frames(x, rate, device=None):
-    """float (channels, n) -> Frames.  ``x``: a CUDA float32 tensor (stays on its device) or an array."""
+def _on_device(x, device=None):
+    """(channels, n) float samples, a CUDA tensor (kept where it is) or an array -> contiguous float32 CUDA tensor."""
     import torch
-    from . import _native
     if not torch.cuda.is_available():
         raise RuntimeError('FLAC encoding runs on the GPU and no CUDA device is visible')
-    code, value = rate_code(rate)
     if torch.is_tensor(x) and x.is_cuda:
         dev = x.device
     else:
@@ -302,49 +312,84 @@ def encode_frames(x, rate, device=None):
     if x.ndim != 2 or x.shape[0] not in (1, 2) or x.shape[1] < 1:
         raise ValueError('FLAC output takes (channels, n) samples with one or two channels and n >= 1, not %s'
                          % (tuple(x.shape),))
-    C, n = int(x.shape[0]), int(x.shape[1])
+    xd = x if torch.is_tensor(x) else torch.from_numpy(np.ascontiguousarray(x, np.float32))
+    return xd.to(dev, torch.float32).contiguous()
+
+
+def _check(lib, rc, what):
+    from . import _native
+    if rc != 0:
+        raise _native.NativeError('%s failed: %s' % (what, lib.vr_last_error(None).decode()))
+
+
+def pcm_bytes(x, bits, device=None):
+    """float (channels, n) -> numpy uint8 array: the samples quantised and interleaved as little-endian ``bits / 8``-byte
+    integers on the device (``vr_pcm_pack``); only those bytes are copied back."""
+    import torch
+    from . import _native
+    _check_bits(bits)
+    xd = _on_device(x, device)
+    lib = _native.load_library()
+    with torch.cuda.device(xd.device):
+        out = torch.empty(xd.numel() * (bits // 8), dtype=torch.uint8, device=xd.device)
+        _check(lib, lib.vr_pcm_pack(None, _native.ptr(xd), int(xd.shape[0]), int(xd.shape[1]), bits, _native.ptr(out),
+                                    _native.stream_ptr()), 'vr_pcm_pack')
+        return out.cpu().numpy()
+
+
+def encode_frames(x, rate, device=None, bits=16):
+    """float (channels, n) -> Frames.  ``x``: a CUDA float32 tensor (stays on its device) or an array."""
+    import torch
+    from . import _native
+    _check_bits(bits)
+    xd = _on_device(x, device)
+    dev = xd.device
+    code, value = rate_code(rate)
+    C, n = int(xd.shape[0]), int(xd.shape[1])
     if n >= 1 << 36:
         raise ValueError('FLAC output: %d samples per channel exceed STREAMINFO\'s 36 bits' % n)
     lib = _native.load_library()
-
-    def check(rc, what):
-        if rc != 0:
-            raise _native.NativeError('%s failed: %s' % (what, lib.vr_last_error(None).decode()))
-
     with torch.cuda.device(dev):
-        xd = x if torch.is_tensor(x) else torch.from_numpy(np.ascontiguousarray(x, np.float32))
-        xd = xd.to(dev, torch.float32).contiguous()
         F = (n + BLOCK - 1) // BLOCK
-        pcm = torch.empty((n, C), dtype=torch.int16, device=dev)
+        pcm = torch.empty((n, C), dtype=getattr(torch, BITS[bits]), device=dev)
         plan = torch.empty((F, PLAN_INTS), dtype=torch.int32, device=dev)
         stream = _native.stream_ptr()
-        check(lib.vr_flac_encode_analyse(None, _native.ptr(xd), C, n, code, _native.ptr(pcm), _native.ptr(plan),
-                                         stream), 'vr_flac_encode_analyse')
+        _check(lib, lib.vr_flac_encode_analyse(None, _native.ptr(xd), C, n, code, bits, _native.ptr(pcm),
+                                               _native.ptr(plan), stream), 'vr_flac_encode_analyse')
         sizes = plan[:, 0].cpu().numpy().astype(np.int64)
         offsets = np.zeros(F, np.int64)
         np.cumsum(sizes[:-1], out=offsets[1:])
         out = torch.empty(int(sizes.sum()), dtype=torch.uint8, device=dev)
         status = torch.empty(F, dtype=torch.int32, device=dev)
         d_off = torch.from_numpy(offsets).to(dev)
-        check(lib.vr_flac_encode_pack(None, _native.ptr(pcm), C, n, _native.ptr(plan), _native.ptr(d_off), code, value,
-                                      _native.ptr(out), _native.ptr(status), stream), 'vr_flac_encode_pack')
+        _check(lib, lib.vr_flac_encode_pack(None, _native.ptr(pcm), C, n, bits, _native.ptr(plan), _native.ptr(d_off),
+                                            code, value, _native.ptr(out), _native.ptr(status), stream),
+               'vr_flac_encode_pack')
         body = out.cpu().numpy().tobytes()
         st = status.cpu().numpy()
     bad = np.flatnonzero(st)
     if bad.size:
         raise RuntimeError('FLAC encode: frame %d did not fill the size its plan gave (status %d)'
                            % (int(bad[0]), int(st[bad[0]])))
-    return Frames(body, sizes, pcm, C, n, int(rate))
+    return Frames(body, sizes, pcm, C, n, int(rate), bits)
 
 
-def encode(x, rate, path=None, md5=True):
+def encode(x, rate, path=None, md5=True, bits=16):
     """float (channels, n) -> the whole FLAC stream (bytes): ``fLaC``, STREAMINFO, the frames; also written to ``path``
-    when one is given.  ``x`` is a CUDA float32 tensor (it stays on the device; only the compressed bytes and the int16
-    samples for the MD5 are copied back) or an array; samples are quantised as clip(rint(x * 32767)), NaN -> 0.
+    when one is given.  ``x`` is a CUDA float32 tensor (it stays on the device; only the compressed bytes and the
+    samples' bytes for the MD5 are copied back) or an array; samples are quantised as clip(rint(x * 32767)), or
+    clip(rint(x * 8388607)) for ``bits=24``, NaN -> 0.
     ``md5=False`` leaves STREAMINFO's MD5 zero (unknown), which skips the copy of the samples and the hash."""
-    fr = encode_frames(x, rate)
-    digest = hashlib.md5(fr.pcm.cpu().numpy().astype('<i2', copy=False).tobytes()).digest() if md5 else bytes(16)
-    data = stream_header(fr.channels, fr.total, fr.rate, fr.sizes, digest) + fr.body
+    _check_bits(bits)
+    x = _on_device(x)
+    fr = encode_frames(x, rate, bits=bits)
+    if not md5:
+        digest = bytes(16)
+    elif bits == 16:
+        digest = hashlib.md5(fr.pcm.cpu().numpy().astype('<i2', copy=False).tobytes()).digest()
+    else:
+        digest = hashlib.md5(pcm_bytes(x, bits)).digest()
+    data = stream_header(fr.channels, fr.total, fr.rate, fr.sizes, digest, bits=bits) + fr.body
     if path is not None:
         with open(path, 'wb') as f:
             f.write(data)
