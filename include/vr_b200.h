@@ -223,6 +223,33 @@ VR_API int vr_flac_encode_pack(vr_ctx* ctx, const void* pcm, int32_t channels, i
 VR_API int vr_pcm_pack(vr_ctx* ctx, const float* x, int32_t channels, int64_t n, int32_t bits, uint8_t* out,
                        void* stream);
 
+/* BSS Eval images with time-invariant distortion filters (lib/bsseval.py is the caller, oracle/bsseval_oracle.py the
+ * float64 restatement, DESIGN.md section 10 the contract): K sources of C channels, M = K * C <= BSS_EVAL_MAX_SIGNALS,
+ * filters of L <= BSS_EVAL_MAX_FILTER taps, N >= window samples.  refs / ests: DEVICE float32 [K][C][N] on the calling
+ * thread's current device (or the context's, when ctx is not NULL; ctx may be NULL, as for vr_resample).
+ *
+ * vr_bss_eval_workspace: the bytes of device workspace vr_bss_eval needs for these sizes, or -1 (message from
+ * vr_last_error(NULL)) for sizes it does not take.
+ *
+ * vr_bss_eval: frames = (N - window + hop) / hop windows, frame w = samples [w * hop, w * hop + window).  Writes to the
+ * HOST array frames_host [K][frames][8] the float64 sums over frame w and the C channels of source j of
+ *   s^2, (P_j - s)^2, (shat - s)^2, P_j^2, (P_all - P_j)^2, P_all^2, (shat - P_all)^2, shat^2
+ * with s / shat the reference / estimate and P_all / P_j the estimate's projections on the delayed references of all
+ * sources / of source j; the four ratios and the silence rule follow from these on the host.  corr_host (HOST, may be
+ * NULL) receives r[a][b](l) = sum_u s_a(u) y_b(u + l), [M][2M][L], y = the M references then the M estimates: G and d.
+ * The systems are G + eps I over all K*C*L unknowns and each source's block + eps I, eps = scale * max diag G with
+ * scale = 2^-40, raised by 2^8 per retry for a system whose Cholesky factorisation meets a non-positive pivot (G is only
+ * positive semidefinite), up to 2^-20; loading_host (HOST, may be NULL) receives the K + 1 scales used (all unknowns,
+ * then source 0, 1, ...).  phase_ms (HOST, may be NULL) receives the CUDA-event times of {correlations, assembly +
+ * Cholesky + solves, projections + frame sums, all}.  Synchronises the stream; the results are bit-identical from
+ * call to call.  NaN or Inf in refs or ests, or a system still not factored at 2^-20, is an error.            */
+#define BSS_EVAL_MAX_SIGNALS 8
+#define BSS_EVAL_MAX_FILTER 1024
+VR_API int64_t vr_bss_eval_workspace(int32_t K, int32_t C, int64_t N, int32_t L, int64_t window, int64_t hop);
+VR_API int vr_bss_eval(vr_ctx* ctx, const float* refs, const float* ests, int32_t K, int32_t C, int64_t N, int32_t L,
+                       int64_t window, int64_t hop, void* workspace, int64_t workspace_bytes, double* frames_host,
+                       double* corr_host, double* loading_host, double* phase_ms, void* stream);
+
 /* Multi-GPU mask exchange over NVLink peer memory (one process per GPU).  The owner (rank 0) allocates the
  * whole-track mask with vr_shared_alloc and publishes the 64-byte CUDA IPC handle; every other rank maps it
  * with vr_shared_open and passes the mapped pointer as `mask` to vr_separate_windows, so the mask epilogue

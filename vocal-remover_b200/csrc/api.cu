@@ -285,6 +285,27 @@ int vr_pcm_pack(vr_ctx* ctx, const float* x, int32_t channels, int64_t n, int32_
   return flac_result(ctx, "vr_pcm_pack", vr::launch_pcm_pack(x, channels, n, bits, out, (cudaStream_t)stream));
 }
 
+int64_t vr_bss_eval_workspace(int32_t K, int32_t C, int64_t N, int32_t L, int64_t window, int64_t hop) {
+  std::string err;
+  const int64_t bytes = vr::bss_eval_workspace(K, C, N, L, window, hop, err);
+  if (bytes < 0) g_create_err = err;
+  return bytes;
+}
+
+int vr_bss_eval(vr_ctx* ctx, const float* refs, const float* ests, int32_t K, int32_t C, int64_t N, int32_t L,
+                int64_t window, int64_t hop, void* workspace, int64_t workspace_bytes, double* frames_host,
+                double* corr_host, double* loading_host, double* phase_ms, void* stream) {
+  // ctx may be NULL, as for vr_resample
+  if (ctx && ctx->eng) cudaSetDevice(ctx->eng->cfg().device);
+  std::string err;
+  if (vr::bss_eval(refs, ests, K, C, N, L, window, hop, workspace, workspace_bytes, frames_host, corr_host,
+                   loading_host, phase_ms, (cudaStream_t)stream, err))
+    return 0;
+  if (ctx) return fail(ctx, err);
+  g_create_err = err;
+  return -1;
+}
+
 int vr_shared_alloc(vr_ctx* ctx, int64_t bytes, void** dev_ptr, unsigned char* handle64) {
   CHECK_CTX(ctx);
   if (!dev_ptr || !handle64 || bytes <= 0) return fail(ctx, "vr_shared_alloc: bad arguments");

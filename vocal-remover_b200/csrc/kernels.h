@@ -2,6 +2,9 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <string>
+
 #include "common.cuh"
 
 namespace vr {
@@ -126,5 +129,11 @@ cudaError_t launch_flac_encode_pack(const void* pcm, int channels, int64_t n, in
                                     const int64_t* offsets, int rate_code, int rate_value, uint8_t* out,
                                     int32_t* status, cudaStream_t stream);
 cudaError_t launch_pcm_pack(const float* x, int channels, int64_t n, int bits, uint8_t* out, cudaStream_t stream);
+
+// ---- BSS Eval (bsseval.cu): workspace bytes, or -1 with err set; the whole evaluation of one track, synchronous ------
+int64_t bss_eval_workspace(int K, int C, int64_t N, int L, int64_t window, int64_t hop, std::string& err);
+bool bss_eval(const float* refs, const float* ests, int K, int C, int64_t N, int L, int64_t window, int64_t hop,
+              void* workspace, int64_t workspace_bytes, double* frames_host, double* corr_host, double* loading_host,
+              double* phase_ms, cudaStream_t stream, std::string& err);
 
 }  // namespace vr
