@@ -250,6 +250,29 @@ VR_API int vr_bss_eval(vr_ctx* ctx, const float* refs, const float* ests, int32_
                        int64_t window, int64_t hop, void* workspace, int64_t workspace_bytes, double* frames_host,
                        double* corr_host, double* loading_host, double* phase_ms, void* stream);
 
+/* BSS Eval images with framewise distortion filters (BSS Eval v3, museval's mode 'v3'; DESIGN.md section 10,
+ * "Framewise filters (v3)"): the same frames, K, C, L, refs and ests as vr_bss_eval, but each frame w is scored as a
+ * signal of its own: the window samples from w * hop, zero outside them, with its own Gram matrix, loadings, filters
+ * and projections, on its own timeline of window + L - 1 samples.  Requires window >= L.
+ *
+ * vr_bss_eval_framewise_workspace: the bytes of device workspace for frames_per_batch frames at a time (clamped to
+ * [1, min(frames, 4096)]; about frames_per_batch * ((K*C*L)^2 + K (C*L)^2) * 8 bytes), or -1 (vr_last_error(NULL)).
+ *
+ * vr_bss_eval_framewise: frames_host [K][frames][8] receives the eight sums of vr_bss_eval, in the same order, over
+ * the window + L - 1 samples of each frame's timeline and the source's channels; corr_host (may be NULL) each frame's
+ * correlations [frames][M][2M][L] of its window samples; loading_host (may be NULL) each frame's K + 1 loading scales
+ * [frames][K + 1], NaN for a frame in which a reference source or an estimate is all zeros (its systems are the
+ * identity and are not factored); phase_ms as vr_bss_eval's, each phase summed over the batches.  Synchronises the
+ * stream; the results are bit-identical from call to call and for every frames_per_batch.  NaN or Inf in refs or
+ * ests, or a system still not factored at 2^-20, is an error.                                                      */
+VR_API int64_t vr_bss_eval_framewise_workspace(int32_t K, int32_t C, int64_t N, int32_t L, int64_t window,
+                                               int64_t hop, int32_t frames_per_batch);
+VR_API int vr_bss_eval_framewise(vr_ctx* ctx, const float* refs, const float* ests, int32_t K, int32_t C, int64_t N,
+                                 int32_t L, int64_t window, int64_t hop, int32_t frames_per_batch, void* workspace,
+                                 int64_t workspace_bytes, double* frames_host /* [K][nwin][8] */,
+                                 double* corr_host /* [nwin][M][2M][L] or NULL */,
+                                 double* loading_host /* [nwin][K+1] or NULL */, double* phase_ms, void* stream);
+
 /* Multi-GPU mask exchange over NVLink peer memory (one process per GPU).  The owner (rank 0) allocates the
  * whole-track mask with vr_shared_alloc and publishes the 64-byte CUDA IPC handle; every other rank maps it
  * with vr_shared_open and passes the mapped pointer as `mask` to vr_separate_windows, so the mask epilogue

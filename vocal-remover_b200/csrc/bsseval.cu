@@ -16,7 +16,15 @@
 //   bss_frames_kernel       the task sums of every frame, over the source's channels
 //
 // Every sum is float64 and reduced in a fixed order (no atomics), so two calls give identical bits.
+//
+// Framewise filters (BSS Eval v3, bss_eval_framewise, DESIGN.md section 10 "Framewise filters (v3)"): every frame is a
+// signal of its own, its window samples zero outside them.  The same kernels run on batches of F frames with a segment
+// index (grid z for the correlations, y for the systems, the task's frame for the projections): per-frame
+// correlations, F full and F * K block systems per Cholesky launch sequence, a pivot status and a loading per system,
+// and projections on each frame's timeline of window + L - 1 samples.  bss_live_kernel finds the silent frames, whose
+// systems are the identity and are not factored.
 #include <algorithm>
+#include <cmath>
 #include <string>
 #include <vector>
 
@@ -40,10 +48,12 @@ constexpr int CORR_NB = 4;                    // 16-sample blocks per lane per c
 constexpr int CORR_TC = 32 * BR * CORR_NB;    // samples per chunk (2048)
 constexpr int CORR_GROUPS = 64;               // CTAs along time per (a, b, lag tile): the partial sums kept
 
-// grid: x = lag tile + Lc / CORR_LT * (b + 2M * a), y = time group.  part[g][a][b][Lc].
+// grid: x = lag tile + Lc / CORR_LT * (b + 2M * a), y = time group, z = segment.  Segment z is the len samples from
+// z * seg_hop of each signal (N apart), zero outside them: the whole track (len = N, one segment) or one frame each.
+// part[z][g][a][b][Lc].
 __global__ void __launch_bounds__(CORR_THREADS, 2)
-bss_corr_kernel(const float* __restrict__ refs, const float* __restrict__ ests, int M, int64_t N, int Lc,
-                int64_t nchunks, double* __restrict__ part) {
+bss_corr_kernel(const float* __restrict__ refs, const float* __restrict__ ests, int M, int64_t N, int64_t len,
+                int64_t seg_hop, int Lc, int64_t nchunks, double* __restrict__ part) {
   __shared__ double s_a[spad(CORR_TC)];
   __shared__ double s_y[spad(CORR_TC + CORR_LT)];
   const int ntile = Lc / CORR_LT;
@@ -53,8 +63,9 @@ bss_corr_kernel(const float* __restrict__ refs, const float* __restrict__ ests, 
   const int b = bid % (2 * M);
   const int a = bid / (2 * M);
   const int g = blockIdx.y, groups = gridDim.y;
-  const float* sa = refs + (int64_t)a * N;
-  const float* yb = b < M ? refs + (int64_t)b * N : ests + (int64_t)(b - M) * N;
+  const int64_t base = blockIdx.z * seg_hop;
+  const float* sa = refs + (int64_t)a * N + base;
+  const float* yb = (b < M ? refs + (int64_t)b * N : ests + (int64_t)(b - M) * N) + base;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t c0 = nchunks * g / groups, c1 = nchunks * (g + 1) / groups;
 
@@ -67,11 +78,11 @@ bss_corr_kernel(const float* __restrict__ refs, const float* __restrict__ ests, 
     __syncthreads();
     for (int i = threadIdx.x; i < CORR_TC; i += CORR_THREADS) {
       const int64_t t = t0 + i;
-      s_a[spad(i)] = t < N ? (double)sa[t] : 0.0;
+      s_a[spad(i)] = t < len ? (double)sa[t] : 0.0;
     }
     for (int i = threadIdx.x; i < CORR_TC + CORR_LT; i += CORR_THREADS) {
       const int64_t t = ty0 + i;
-      s_y[spad(i)] = t < N ? (double)yb[t] : 0.0;
+      s_y[spad(i)] = t < len ? (double)yb[t] : 0.0;
     }
     __syncthreads();
 #pragma unroll 1
@@ -98,19 +109,33 @@ bss_corr_kernel(const float* __restrict__ refs, const float* __restrict__ ests, 
     acc[e] = v;
   }
   if (lane == 0) {
-    double* out = part + (((int64_t)g * M + a) * 2 * M + b) * Lc + lt * CORR_LT + warp * BR;
+    double* out = part + ((((int64_t)blockIdx.z * groups + g) * M + a) * 2 * M + b) * Lc + lt * CORR_LT + warp * BR;
 #pragma unroll
     for (int e = 0; e < BR; ++e) out[e] = acc[e];
   }
 }
 
-__global__ void bss_corr_reduce_kernel(const double* __restrict__ part, int groups, int64_t total,
+// out[z][k] = sum over g, in group order, of part[z][g][k], k < per (the values of one segment)
+__global__ void bss_corr_reduce_kernel(const double* __restrict__ part, int groups, int64_t per, int64_t total,
                                        double* __restrict__ out) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
+  const double* p = part + i / per * groups * per + i % per;
   double s = 0.0;
-  for (int g = 0; g < groups; ++g) s += part[(int64_t)g * total + i];
+  for (int g = 0; g < groups; ++g) s += p[(int64_t)g * per];
   out[i] = s;
+}
+
+// live[z][sig] = 1 if signal sig (the M references, then the M estimates) has a nonzero sample among the len from
+// z * seg_hop.  grid (segment, 2M)
+__global__ void bss_live_kernel(const float* __restrict__ refs, const float* __restrict__ ests, int M, int64_t N,
+                                int64_t len, int64_t seg_hop, int* __restrict__ live) {
+  const int sig = blockIdx.y;
+  const float* x = (sig < M ? refs + (int64_t)sig * N : ests + (int64_t)(sig - M) * N) + blockIdx.x * seg_hop;
+  bool any = false;
+  for (int64_t t = threadIdx.x; t < len; t += blockDim.x) any |= x[t] != 0.0f;
+  any = __syncthreads_or(any);
+  if (threadIdx.x == 0) live[(int64_t)blockIdx.x * 2 * M + sig] = any;
 }
 
 // ---- the linear systems ------------------------------------------------------------------------------------------
@@ -128,6 +153,11 @@ struct AssembleArgs {
   double* B;          // [np][M]
   double* Bb;         // [K][nbp][C]
   double scale[1 + BSS_EVAL_MAX_SIGNALS];   // eps = scale[s] * max diag G of system s (0: all unknowns, 1 + j: source j)
+  // frames (blockIdx.y = frame z of the batch, F = gridDim.y frames, every array above one per frame): the scale and
+  // the mode of system s of frame z at [z] (s = 0) and [F + z * K + s - 1]; mode 1 assembles the system, 2 assembles
+  // the identity with zero right-hand sides (a silent frame), 0 leaves it alone.  NULL: scale[] and mode 1.
+  const double* fscale;
+  const int* fmode;
 };
 
 // G[(a, t), (b, t')] = r[a][b](t - t') (r[b][a](t' - t) for negative lags), + eps on the diagonal; rows and columns
@@ -136,40 +166,57 @@ __global__ void bss_assemble_kernel(AssembleArgs p) {
   const int64_t n_g = (int64_t)p.np * p.np, n_gb = (int64_t)p.K * p.nbp * p.nbp;
   const int64_t n_b = (int64_t)p.np * p.M, n_bb = (int64_t)p.K * p.nbp * p.C;
   const int64_t total = n_g + n_gb + n_b + n_bb;
+  const int z = blockIdx.y, F = gridDim.y;
+  const double* R = p.R + (int64_t)z * p.M * 2 * p.M * p.Lc;
+  double* G = p.G + z * n_g;
+  double* Gb = p.Gb + z * n_gb;
+  double* B = p.B + z * n_b;
+  double* Bb = p.Bb + z * n_bb;
+  auto sys = [&](int s) { return s == 0 ? z : F + z * p.K + s - 1; };
+  auto mode = [&](int s) { return p.fmode ? p.fmode[sys(s)] : 1; };
+  auto scale = [&](int s) { return p.fscale ? p.fscale[sys(s)] : p.scale[s]; };
   double dmax = 0.0;
-  for (int a = 0; a < p.M; ++a) dmax = fmax(dmax, p.R[((int64_t)a * 2 * p.M + a) * p.Lc]);
-  const double eps = dmax * p.scale[0];
+  for (int a = 0; a < p.M; ++a) dmax = fmax(dmax, R[((int64_t)a * 2 * p.M + a) * p.Lc]);
+  const double eps = dmax * scale(0);
+  const int mode0 = mode(0);
   auto corr = [&](int a, int b, int t, int t2) {
     const int l = t - t2;
-    return l >= 0 ? p.R[((int64_t)a * 2 * p.M + b) * p.Lc + l] : p.R[((int64_t)b * 2 * p.M + a) * p.Lc - l];
+    return l >= 0 ? R[((int64_t)a * 2 * p.M + b) * p.Lc + l] : R[((int64_t)b * 2 * p.M + a) * p.Lc - l];
   };
   const int n = p.M * p.L, nb = p.C * p.L;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     if (i < n_g) {
+      if (mode0 == 0) continue;
       const int r = (int)(i / p.np), c = (int)(i % p.np);
       double v;
-      if (r >= n || c >= n) v = r == c ? 1.0 : 0.0;
+      if (r >= n || c >= n || mode0 == 2) v = r == c ? 1.0 : 0.0;
       else v = corr(r / p.L, c / p.L, r % p.L, c % p.L) + (r == c ? eps : 0.0);
-      p.G[i] = v;
+      G[i] = v;
     } else if (i < n_g + n_gb) {
       const int64_t k = i - n_g;
       const int j = (int)(k / ((int64_t)p.nbp * p.nbp));
+      const int mj = mode(1 + j);
+      if (mj == 0) continue;
       const int64_t q = k % ((int64_t)p.nbp * p.nbp);
       const int r = (int)(q / p.nbp), c = (int)(q % p.nbp);
       double v;
-      if (r >= nb || c >= nb) v = r == c ? 1.0 : 0.0;
-      else v = corr(j * p.C + r / p.L, j * p.C + c / p.L, r % p.L, c % p.L) + (r == c ? dmax * p.scale[1 + j] : 0.0);
-      p.Gb[k] = v;
+      if (r >= nb || c >= nb || mj == 2) v = r == c ? 1.0 : 0.0;
+      else v = corr(j * p.C + r / p.L, j * p.C + c / p.L, r % p.L, c % p.L) + (r == c ? dmax * scale(1 + j) : 0.0);
+      Gb[k] = v;
     } else if (i < n_g + n_gb + n_b) {
+      if (mode0 == 0) continue;
       const int64_t k = i - n_g - n_gb;
       const int r = (int)(k / p.M), e = (int)(k % p.M);
-      p.B[k] = r < n ? p.R[((int64_t)(r / p.L) * 2 * p.M + p.M + e) * p.Lc + r % p.L] : 0.0;
+      B[k] = r < n && mode0 == 1 ? R[((int64_t)(r / p.L) * 2 * p.M + p.M + e) * p.Lc + r % p.L] : 0.0;
     } else {
       const int64_t k = i - n_g - n_gb - n_b;
       const int j = (int)(k / ((int64_t)p.nbp * p.C));
+      const int mj = mode(1 + j);
+      if (mj == 0) continue;
       const int64_t q = k % ((int64_t)p.nbp * p.C);
       const int r = (int)(q / p.C), ci = (int)(q % p.C);
-      p.Bb[k] = r < nb ? p.R[((int64_t)(j * p.C + r / p.L) * 2 * p.M + p.M + j * p.C + ci) * p.Lc + r % p.L] : 0.0;
+      Bb[k] = r < nb && mj == 1 ? R[((int64_t)(j * p.C + r / p.L) * 2 * p.M + p.M + j * p.C + ci) * p.Lc + r % p.L]
+                                : 0.0;
     }
   }
 }
@@ -177,7 +224,9 @@ __global__ void bss_assemble_kernel(AssembleArgs p) {
 // Right-looking blocked Cholesky, lower triangle in place, of a batch of n x n row-major matrices (blockIdx.z or x
 // selects one, stride n * n).  Step k: factor diagonal tile k, solve the panel below it, update the trailing tiles.
 // status[z] receives 1 + the first row whose pivot is not positive (a NaN pivot included) and is left alone otherwise.
-__global__ void __launch_bounds__(256) chol_diag_kernel(double* A, int n, int k, int* status) {
+// todo (may be NULL: every matrix): only the matrices z with todo[z] == 1 are factored.
+__global__ void __launch_bounds__(256) chol_diag_kernel(double* A, int n, int k, int* status, const int* todo) {
+  if (todo && todo[blockIdx.x] != 1) return;
   __shared__ double t[NB][NB + 1];
   double* a = A + (int64_t)blockIdx.x * n * n;
   const int r0 = k * NB, tid = threadIdx.x;
@@ -202,7 +251,8 @@ __global__ void __launch_bounds__(256) chol_diag_kernel(double* A, int n, int k,
 }
 
 // tile row k + 1 + blockIdx.x of column k: X L_kk^T = A_ik, one thread per row
-__global__ void __launch_bounds__(NB) chol_panel_kernel(double* A, int n, int k) {
+__global__ void __launch_bounds__(NB) chol_panel_kernel(double* A, int n, int k, const int* todo) {
+  if (todo && todo[blockIdx.y] != 1) return;
   extern __shared__ double chol_smem[];   // two padded tiles (CHOL_TILES_SMEM bytes)
   double(*l)[NB + 1] = reinterpret_cast<double(*)[NB + 1]>(chol_smem);
   double(*x)[NB + 1] = l + NB;
@@ -223,9 +273,9 @@ __global__ void __launch_bounds__(NB) chol_panel_kernel(double* A, int n, int k)
 }
 
 // trailing tile (k + 1 + blockIdx.y, k + 1 + blockIdx.x) -= A_ik A_jk^T, lower tiles only; 4 x 4 outputs per thread
-__global__ void __launch_bounds__(256) chol_update_kernel(double* A, int n, int k) {
+__global__ void __launch_bounds__(256) chol_update_kernel(double* A, int n, int k, const int* todo) {
   const int ti = k + 1 + blockIdx.y, tj = k + 1 + blockIdx.x;
-  if (tj > ti) return;
+  if (tj > ti || (todo && todo[blockIdx.z] != 1)) return;
   extern __shared__ double chol_smem[];
   double(*sa)[NB + 1] = reinterpret_cast<double(*)[NB + 1]>(chol_smem);
   double(*sb)[NB + 1] = sa + NB;
@@ -259,16 +309,19 @@ struct SolveSys {
   const double* L;   // n x n, the factor in the lower triangle
   double* B;         // [n][nr]: right-hand sides in, solutions out
   int n, nr;         // nr <= 8
+  int64_t zl, zb;    // frames: the distance of frame z's L and B from frame z - 1's (elements)
 };
 struct SolveArgs {
   SolveSys s[9];
 };
 
-// L L^T x = b for one system per CTA: forward then backward substitution, tile by tile.  One warp solves each 64 x 64
-// triangle; all warps then update the rest of the right-hand sides.
+// L L^T x = b for one system per CTA (system blockIdx.x of frame blockIdx.y): forward then backward substitution,
+// tile by tile.  One warp solves each 64 x 64 triangle; all warps then update the rest of the right-hand sides.
 constexpr int SOLVE_THREADS = 512;
 __global__ void __launch_bounds__(SOLVE_THREADS) chol_solve_kernel(SolveArgs args) {
-  const SolveSys sys = args.s[blockIdx.x];
+  SolveSys sys = args.s[blockIdx.x];
+  sys.L += blockIdx.y * sys.zl;
+  sys.B += blockIdx.y * sys.zb;
   __shared__ double t[NB][NB + 1];
   __shared__ double xb[NB][8];
   const int n = sys.n, nr = sys.nr, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -336,11 +389,17 @@ __global__ void __launch_bounds__(SOLVE_THREADS) chol_solve_kernel(SolveArgs arg
   }
 }
 
-// the solutions as taps: ca[e][kc][Lp] from the full system, cs[e][c][Lp] from source j's (e = j * C + i), zero past L
+// the solutions as taps: ca[e][kc][Lp] from the full system, cs[e][c][Lp] from source j's (e = j * C + i), zero past L;
+// blockIdx.y: the frame (each array one per frame)
 __global__ void bss_coef_kernel(const double* __restrict__ X, const double* __restrict__ Xb, int K, int C, int L, int Lp,
-                                int nbp, double* __restrict__ ca, double* __restrict__ cs) {
+                                int np, int nbp, double* __restrict__ ca, double* __restrict__ cs) {
   const int M = K * C;
   const int64_t n_a = (int64_t)M * M * Lp, total = n_a + (int64_t)M * C * Lp;
+  const int z = blockIdx.y;
+  X += (int64_t)z * np * M;
+  Xb += (int64_t)z * K * nbp * C;
+  ca += z * n_a;
+  cs += z * (total - n_a);
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     if (i < n_a) {
       const int tau = (int)(i % Lp), kc = (int)(i / Lp % M), e = (int)(i / Lp / M);
@@ -378,15 +437,23 @@ __device__ __forceinline__ void fir_block(const double* __restrict__ pw, const d
 
 // grid: x = task, y = estimate channel e = j * C + i.  Thread b owns samples t = t_start + 16 b + [0, 16).
 // part[e][task][8] = sums over the task's samples of s^2, (P_j - s)^2, (shat - s)^2, P_j^2, (P_all - P_j)^2, P_all^2,
-// (shat - P_all)^2, shat^2, with s = s_e and shat = shat_e.
+// (shat - P_all)^2, shat^2, with s = s_e and shat = shat_e.  Task x belongs to segment z = x / tasks_per_seg, and
+// takes its range from tasks[x % tasks_per_seg] on the segment's timeline: the signals are the len samples from
+// z * seg_hop (N apart), zero outside them, and the coefficients are segment z's (one set per segment).
 __global__ void __launch_bounds__(PROJ_THREADS, 1)
-bss_project_kernel(const float* __restrict__ refs, const float* __restrict__ ests, int K, int C, int64_t N, int Lp,
-                   const double* __restrict__ coef_all, const double* __restrict__ coef_src,
-                   const int64_t* __restrict__ tasks, int ntask, double* __restrict__ part) {
+bss_project_kernel(const float* __restrict__ refs, const float* __restrict__ ests, int K, int C, int64_t N,
+                   int64_t len, int64_t seg_hop, int Lp, const double* __restrict__ coef_all,
+                   const double* __restrict__ coef_src, const int64_t* __restrict__ tasks, int tasks_per_seg, int ntask,
+                   double* __restrict__ part) {
   extern __shared__ double xs[];   // time t_start - Lp + p at spad(p), p < Lp + PROJ_TC
   __shared__ double red[PROJ_THREADS / 32][8];
   const int task = blockIdx.x, e = blockIdx.y, M = K * C, j = e / C;
-  const int64_t t_start = tasks[2 * task], t_end = tasks[2 * task + 1];
+  const int z = task / tasks_per_seg, tk = task % tasks_per_seg;
+  const int64_t t_start = tasks[2 * tk], t_end = tasks[2 * tk + 1];
+  refs += z * seg_hop;
+  ests += z * seg_hop;
+  coef_all += (int64_t)z * M * M * Lp;
+  coef_src += (int64_t)z * M * C * Lp;
   const int b = threadIdx.x;
   double pa[BR], pj[BR];
 #pragma unroll
@@ -396,7 +463,7 @@ bss_project_kernel(const float* __restrict__ refs, const float* __restrict__ est
     __syncthreads();
     for (int p = threadIdx.x; p < Lp + PROJ_TC; p += PROJ_THREADS) {
       const int64_t t = t_start - Lp + p;
-      xs[spad(p)] = (t >= 0 && t < N) ? (double)x[t] : 0.0;
+      xs[spad(p)] = (t >= 0 && t < len) ? (double)x[t] : 0.0;
     }
     __syncthreads();
     const double* ca = coef_all + ((int64_t)e * M + kc) * Lp;
@@ -420,7 +487,7 @@ bss_project_kernel(const float* __restrict__ refs, const float* __restrict__ est
   for (int r = 0; r < BR; ++r) {
     const int64_t t = t_start + (int64_t)BR * b + r;
     if (t < t_end) {
-      const double s = sr[t], y = se[t], Pj = pj[r], Pa = pa[r];
+      const double s = t < len ? sr[t] : 0.0f, y = t < len ? se[t] : 0.0f, Pj = pj[r], Pa = pa[r];
       q[0] = fma(s, s, q[0]);
       q[1] = fma(Pj - s, Pj - s, q[1]);
       q[2] = fma(y - s, y - s, q[2]);
@@ -483,7 +550,7 @@ struct Plan {
   size_t o_part, o_R, o_G, o_Gb, o_B, o_Bb, o_ca, o_cs, o_tasks, o_fr, o_ep, o_frames, o_status, bytes;
 };
 
-bool make_plan(int K, int C, int64_t N, int L, int64_t window, int64_t hop, Plan& p, std::string& err) {
+bool check_sizes(int K, int C, int64_t N, int L, int64_t window, int64_t hop, std::string& err) {
   if (K < 1 || C < 1 || K * C > BSS_EVAL_MAX_SIGNALS) {
     err = "bss_eval: K * C must be in [1, " + std::to_string(BSS_EVAL_MAX_SIGNALS) + "] (sources x channels), got K = " +
           std::to_string(K) + ", C = " + std::to_string(C);
@@ -502,6 +569,11 @@ bool make_plan(int K, int C, int64_t N, int L, int64_t window, int64_t hop, Plan
           std::to_string(window) + ")";
     return false;
   }
+  return true;
+}
+
+bool make_plan(int K, int C, int64_t N, int L, int64_t window, int64_t hop, Plan& p, std::string& err) {
+  if (!check_sizes(K, C, N, L, window, hop, err)) return false;
   p.K = K; p.C = C; p.M = K * C; p.L = L; p.N = N; p.window = window; p.hop = hop;
   p.Lc = (int)round_up(L, CORR_LT);
   p.Lp = (int)round_up(L, BR);
@@ -571,7 +643,7 @@ bool cuda_ok(cudaError_t e, const char* what, std::string& err) {
   return false;
 }
 
-bool cholesky(double* A, int n, int batch, int* status, cudaStream_t st, std::string& err) {
+bool cholesky(double* A, int n, int batch, int* status, const int* todo, cudaStream_t st, std::string& err) {
   const int T = n / NB;
   if (!cuda_ok(cudaFuncSetAttribute(chol_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CHOL_TILES_SMEM),
                "cudaFuncSetAttribute", err) ||
@@ -579,13 +651,85 @@ bool cholesky(double* A, int n, int batch, int* status, cudaStream_t st, std::st
                "cudaFuncSetAttribute", err))
     return false;
   for (int k = 0; k < T; ++k) {
-    chol_diag_kernel<<<batch, 256, 0, st>>>(A, n, k, status);
+    chol_diag_kernel<<<batch, 256, 0, st>>>(A, n, k, status, todo);
     if (k + 1 < T) {
-      chol_panel_kernel<<<dim3(T - k - 1, batch), NB, CHOL_TILES_SMEM, st>>>(A, n, k);
-      chol_update_kernel<<<dim3(T - k - 1, T - k - 1, batch), 256, CHOL_TILES_SMEM, st>>>(A, n, k);
+      chol_panel_kernel<<<dim3(T - k - 1, batch), NB, CHOL_TILES_SMEM, st>>>(A, n, k, todo);
+      chol_update_kernel<<<dim3(T - k - 1, T - k - 1, batch), 256, CHOL_TILES_SMEM, st>>>(A, n, k, todo);
     }
   }
   return cuda_ok(cudaGetLastError(), "cholesky", err);
+}
+
+// ---- framewise filters (BSS Eval v3): every frame its own signal of window samples, its own systems -----------------
+constexpr int64_t BSS_MAX_FRAMES_PER_BATCH = 4096;   // keeps K * F inside a grid's y and z limits
+
+struct FramePlan {
+  int K, C, M, L, Lc, Lp, np, nbp, groups, tpf;   // tpf: projection tasks per frame
+  int64_t N, window, hop, nwin, F, span, nchunks; // span = window + L - 1: a frame's projection timeline
+  std::vector<int64_t> tasks;     // [tpf][2] sample ranges of one frame's timeline
+  std::vector<int64_t> franges;   // [F][2] task range of frame z of a batch: [z * tpf, (z + 1) * tpf)
+  // workspace offsets (bytes); flags = status [F (1 + K)], live [F][2M], the non-finite input flag, mode [F (1 + K)]
+  size_t o_part, o_R, o_G, o_Gb, o_B, o_Bb, o_ca, o_cs, o_tasks, o_fr, o_ep, o_frames, o_flags, o_scale, bytes;
+};
+
+bool make_frame_plan(int K, int C, int64_t N, int L, int64_t window, int64_t hop, int64_t frames_per_batch,
+                     FramePlan& p, std::string& err) {
+  if (!check_sizes(K, C, N, L, window, hop, err)) return false;
+  if (window < L) {
+    err = "bss_eval: with framewise filters the window (" + std::to_string(window) +
+          " samples) must not be shorter than filters_len (" + std::to_string(L) + ")";
+    return false;
+  }
+  if (frames_per_batch < 1) {
+    err = "bss_eval: frames_per_batch must be positive, got " + std::to_string(frames_per_batch);
+    return false;
+  }
+  p.K = K; p.C = C; p.M = K * C; p.L = L; p.N = N; p.window = window; p.hop = hop;
+  p.Lc = (int)round_up(L, CORR_LT);
+  p.Lp = (int)round_up(L, BR);
+  p.np = (int)round_up(p.M * L, NB);
+  p.nbp = (int)round_up(C * L, NB);
+  p.nwin = (N - window + hop) / hop;
+  p.F = std::min(std::min(frames_per_batch, p.nwin), BSS_MAX_FRAMES_PER_BATCH);
+  p.span = window + L - 1;
+  p.nchunks = (window + CORR_TC - 1) / CORR_TC;
+  p.groups = (int)std::min<int64_t>(CORR_GROUPS, p.nchunks);
+  p.tasks.clear();
+  for (int64_t t = 0; t < p.span; t += PROJ_TC) {
+    p.tasks.push_back(t);
+    p.tasks.push_back(std::min(p.span, t + PROJ_TC));
+  }
+  p.tpf = (int)(p.tasks.size() / 2);
+  if (p.F * p.tpf > 0x7fffffff) p.F = 0x7fffffff / p.tpf;
+  p.franges.resize(2 * p.F);
+  for (int64_t z = 0; z < p.F; ++z) {
+    p.franges[2 * z] = z * p.tpf;
+    p.franges[2 * z + 1] = (z + 1) * p.tpf;
+  }
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    const size_t o = off;
+    off += (bytes + 255) / 256 * 256;
+    return o;
+  };
+  const int M = p.M;
+  const size_t F = (size_t)p.F, nsys = F * (1 + K);
+  p.o_part = take(sizeof(double) * F * p.groups * M * 2 * M * p.Lc);
+  p.o_R = take(sizeof(double) * F * M * 2 * M * p.Lc);
+  p.o_G = take(sizeof(double) * F * p.np * p.np);
+  p.o_Gb = take(sizeof(double) * F * K * p.nbp * p.nbp);
+  p.o_B = take(sizeof(double) * F * p.np * M);
+  p.o_Bb = take(sizeof(double) * F * K * p.nbp * C);
+  p.o_ca = take(sizeof(double) * F * M * M * p.Lp);
+  p.o_cs = take(sizeof(double) * F * M * C * p.Lp);
+  p.o_tasks = take(sizeof(int64_t) * p.tasks.size());
+  p.o_fr = take(sizeof(int64_t) * p.franges.size());
+  p.o_ep = take(sizeof(double) * M * F * p.tpf * 8);
+  p.o_frames = take(sizeof(double) * K * F * 8);
+  p.o_flags = take(sizeof(int) * (2 * nsys + F * 2 * M + 1));
+  p.o_scale = take(sizeof(double) * nsys);
+  p.bytes = off;
+  return true;
 }
 
 }  // namespace
@@ -648,22 +792,24 @@ bool bss_eval(const float* refs, const float* ests, int K, int C, int64_t N, int
   bss_finite_kernel<<<1024, 256, 0, st>>>(refs, ests, (int64_t)M * N, d_status + 1 + K);
 
   // correlations
-  bss_corr_kernel<<<dim3(p.Lc / CORR_LT * M * 2 * M, p.groups), CORR_THREADS, 0, st>>>(refs, ests, M, N, p.Lc,
+  bss_corr_kernel<<<dim3(p.Lc / CORR_LT * M * 2 * M, p.groups), CORR_THREADS, 0, st>>>(refs, ests, M, N, N, 0, p.Lc,
                                                                                       p.nchunks, part);
   const int64_t ncorr = (int64_t)M * 2 * M * p.Lc;
-  bss_corr_reduce_kernel<<<(unsigned)((ncorr + 255) / 256), 256, 0, st>>>(part, p.groups, ncorr, R);
+  bss_corr_reduce_kernel<<<(unsigned)((ncorr + 255) / 256), 256, 0, st>>>(part, p.groups, ncorr, ncorr, R);
   if (!cuda_ok(cudaGetLastError(), "correlation", err)) return false;
   if (phase_ms) cudaEventRecord(ev[1], st);
 
   // systems: G is only positive semidefinite, so a system whose factorisation fails is assembled and factored again
   // with its loading raised by BSS_LOADING_STEP, up to BSS_LOADING_LAST; the systems that succeeded come out the same
-  AssembleArgs aa{R, K, C, M, L, p.Lc, p.np, p.nbp, G, Gb, B, Bb, {}};
+  AssembleArgs aa{R, K, C, M, L, p.Lc, p.np, p.nbp, G, Gb, B, Bb, {}, nullptr, nullptr};
   for (int s = 0; s <= K; ++s) aa.scale[s] = BSS_LOADING_FIRST;
   std::vector<int> status(2 + K);
   for (;;) {
     bss_assemble_kernel<<<2048, 256, 0, st>>>(aa);
     if (!cuda_ok(cudaGetLastError(), "assemble", err)) return false;
-    if (!cholesky(G, p.np, 1, d_status, st, err) || !cholesky(Gb, p.nbp, K, d_status + 1, st, err)) return false;
+    if (!cholesky(G, p.np, 1, d_status, nullptr, st, err) ||
+        !cholesky(Gb, p.nbp, K, d_status + 1, nullptr, st, err))
+      return false;
     if (!cuda_ok(cudaMemcpyAsync(status.data(), d_status, sizeof(int) * (2 + K), cudaMemcpyDeviceToHost, st),
                  "copy status", err) ||
         !cuda_ok(cudaStreamSynchronize(st), "synchronize", err))
@@ -695,7 +841,7 @@ bool bss_eval(const float* refs, const float* ests, int K, int C, int64_t N, int
   for (int j = 0; j < K; ++j)
     sa.s[1 + j] = SolveSys{Gb + (int64_t)j * p.nbp * p.nbp, Bb + (int64_t)j * p.nbp * C, p.nbp, C};
   chol_solve_kernel<<<1 + K, SOLVE_THREADS, 0, st>>>(sa);
-  bss_coef_kernel<<<256, 256, 0, st>>>(B, Bb, K, C, L, p.Lp, p.nbp, ca, cs);
+  bss_coef_kernel<<<256, 256, 0, st>>>(B, Bb, K, C, L, p.Lp, p.np, p.nbp, ca, cs);
   if (!cuda_ok(cudaGetLastError(), "solve", err)) return false;
   if (phase_ms) cudaEventRecord(ev[2], st);
 
@@ -707,8 +853,8 @@ bool bss_eval(const float* refs, const float* ests, int K, int C, int64_t N, int
                "cudaFuncSetAttribute", err))
     return false;
   if (ntask > 0) {
-    bss_project_kernel<<<dim3(ntask, M), PROJ_THREADS, smem, st>>>(refs, ests, K, C, N, p.Lp, ca, cs, d_tasks, ntask,
-                                                                   ep);
+    bss_project_kernel<<<dim3(ntask, M), PROJ_THREADS, smem, st>>>(refs, ests, K, C, N, N, 0, p.Lp, ca, cs, d_tasks,
+                                                                   ntask, ntask, ep);
   }
   const int64_t nf = (int64_t)K * p.nwin * 8;
   bss_frames_kernel<<<(unsigned)((nf + 255) / 256), 256, 0, st>>>(ep, d_fr, K, C, p.nwin, ntask, d_frames);
@@ -730,6 +876,215 @@ bool bss_eval(const float* refs, const float* ests, int K, int C, int64_t N, int
       phase_ms[i] = ms;
     }
     cudaEventElapsedTime(&ms, ev[0], ev[3]);
+    phase_ms[3] = ms;
+  }
+  return true;
+}
+
+int64_t bss_eval_framewise_workspace(int K, int C, int64_t N, int L, int64_t window, int64_t hop,
+                                     int64_t frames_per_batch, std::string& err) {
+  FramePlan p;
+  if (!make_frame_plan(K, C, N, L, window, hop, frames_per_batch, p, err)) return -1;
+  return (int64_t)p.bytes;
+}
+
+// The frames in batches of F: each batch runs the stages of bss_eval with one segment per frame (its correlations,
+// systems, taps and timeline of window + L - 1 samples), so no frame's arithmetic depends on the others in its batch.
+bool bss_eval_framewise(const float* refs, const float* ests, int K, int C, int64_t N, int L, int64_t window,
+                        int64_t hop, int64_t frames_per_batch, void* workspace, int64_t workspace_bytes,
+                        double* frames_host, double* corr_host, double* loading_host, double* phase_ms,
+                        cudaStream_t st, std::string& err) {
+  FramePlan p;
+  if (!make_frame_plan(K, C, N, L, window, hop, frames_per_batch, p, err)) return false;
+  if (!refs || !ests || !workspace || !frames_host) {
+    err = "bss_eval: null pointer";
+    return false;
+  }
+  if (workspace_bytes < (int64_t)p.bytes) {
+    err = "bss_eval: workspace of " + std::to_string(workspace_bytes) + " bytes, " + std::to_string(p.bytes) +
+          " needed";
+    return false;
+  }
+  char* ws = (char*)workspace;
+  double* part = (double*)(ws + p.o_part);
+  double* R = (double*)(ws + p.o_R);
+  double* G = (double*)(ws + p.o_G);
+  double* Gb = (double*)(ws + p.o_Gb);
+  double* B = (double*)(ws + p.o_B);
+  double* Bb = (double*)(ws + p.o_Bb);
+  double* ca = (double*)(ws + p.o_ca);
+  double* cs = (double*)(ws + p.o_cs);
+  int64_t* d_tasks = (int64_t*)(ws + p.o_tasks);
+  int64_t* d_fr = (int64_t*)(ws + p.o_fr);
+  double* ep = (double*)(ws + p.o_ep);
+  double* d_frames = (double*)(ws + p.o_frames);
+  double* d_scale = (double*)(ws + p.o_scale);
+  const int M = p.M;
+  const int64_t F = p.F, nwin = p.nwin;
+  // flags: status [F (1 + K)], live [F][2M], the non-finite input flag, mode [F (1 + K)]
+  int* d_status = (int*)(ws + p.o_flags);
+  int* d_live = d_status + F * (1 + K);
+  int* d_bad = d_live + F * 2 * M;
+  int* d_mode = d_bad + 1;
+
+  cudaEvent_t ev[6] = {};   // start and end of the call, then the phase boundaries of the current batch
+  if (phase_ms)
+    for (auto& e : ev)
+      if (!cuda_ok(cudaEventCreate(&e), "cudaEventCreate", err)) return false;
+  struct Events {
+    cudaEvent_t* e;
+    ~Events() {
+      for (int i = 0; i < 6; ++i)
+        if (e[i]) cudaEventDestroy(e[i]);
+    }
+  } guard{ev};
+  double acc[3] = {};
+  if (phase_ms) cudaEventRecord(ev[0], st);
+
+  if (!cuda_ok(cudaMemcpyAsync(d_tasks, p.tasks.data(), sizeof(int64_t) * p.tasks.size(), cudaMemcpyHostToDevice, st),
+               "copy tasks", err) ||
+      !cuda_ok(cudaMemcpyAsync(d_fr, p.franges.data(), sizeof(int64_t) * p.franges.size(), cudaMemcpyHostToDevice, st),
+               "copy frame ranges", err) ||
+      !cuda_ok(cudaMemsetAsync(d_bad, 0, sizeof(int), st), "clear flags", err))
+    return false;
+  bss_finite_kernel<<<1024, 256, 0, st>>>(refs, ests, (int64_t)M * N, d_bad);
+  const size_t smem = sizeof(double) * spad(p.Lp + PROJ_TC);
+  if (!cuda_ok(cudaFuncSetAttribute(bss_project_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)(sizeof(double) * spad(BSS_EVAL_MAX_FILTER + PROJ_TC))),
+               "cudaFuncSetAttribute", err))
+    return false;
+
+  std::vector<double> scale(F * (1 + K));
+  std::vector<int> mode(F * (1 + K)), flags(F * (1 + K) + F * 2 * M + 1);
+  std::vector<char> silent(F);
+  for (int64_t w0 = 0; w0 < nwin; w0 += F) {
+    const int Fb = (int)std::min(F, nwin - w0), nsys = Fb * (1 + K);
+    const float* r0 = refs + w0 * hop;
+    const float* e0 = ests + w0 * hop;
+    auto sys = [&](int z, int s) { return s == 0 ? z : Fb + z * K + s - 1; };
+    if (phase_ms) cudaEventRecord(ev[2], st);
+
+    // correlations of each frame's window samples, and which of its signals are not all zero
+    bss_corr_kernel<<<dim3(p.Lc / CORR_LT * M * 2 * M, p.groups, Fb), CORR_THREADS, 0, st>>>(
+        r0, e0, M, N, window, hop, p.Lc, p.nchunks, part);
+    const int64_t per = (int64_t)M * 2 * M * p.Lc;
+    bss_corr_reduce_kernel<<<(unsigned)((Fb * per + 255) / 256), 256, 0, st>>>(part, p.groups, per, Fb * per, R);
+    bss_live_kernel<<<dim3(Fb, 2 * M), 256, 0, st>>>(r0, e0, M, N, window, hop, d_live);
+    if (phase_ms) cudaEventRecord(ev[3], st);
+    if (!cuda_ok(cudaGetLastError(), "correlation", err) ||
+        !cuda_ok(cudaMemcpyAsync(flags.data(), d_status, sizeof(int) * flags.size(), cudaMemcpyDeviceToHost, st),
+                 "copy flags", err) ||
+        !cuda_ok(cudaStreamSynchronize(st), "synchronize", err))
+      return false;
+    if (flags[F * (1 + K) + F * 2 * M]) {
+      err = "bss_eval: the references or the estimates hold NaN or Inf";
+      return false;
+    }
+
+    // the systems of every frame; a silent frame's are the identity and are not factored.  A system whose
+    // factorisation fails is assembled and factored again with its loading raised, the others are left alone.
+    for (int z = 0; z < Fb; ++z) {
+      const int* live = flags.data() + F * (1 + K) + (int64_t)z * 2 * M;
+      silent[z] = 0;
+      for (int j = 0; j < K; ++j) {
+        bool ref = false, est = false;
+        for (int c = 0; c < C; ++c) {
+          ref |= live[j * C + c] != 0;
+          est |= live[M + j * C + c] != 0;
+        }
+        silent[z] |= !ref || !est;
+      }
+      for (int s = 0; s <= K; ++s) {
+        scale[sys(z, s)] = BSS_LOADING_FIRST;
+        mode[sys(z, s)] = silent[z] ? 2 : 1;
+      }
+    }
+    AssembleArgs aa{R, K, C, M, L, p.Lc, p.np, p.nbp, G, Gb, B, Bb, {}, d_scale, d_mode};
+    for (;;) {
+      if (!cuda_ok(cudaMemcpyAsync(d_scale, scale.data(), sizeof(double) * nsys, cudaMemcpyHostToDevice, st),
+                   "copy loading", err) ||
+          !cuda_ok(cudaMemcpyAsync(d_mode, mode.data(), sizeof(int) * nsys, cudaMemcpyHostToDevice, st), "copy mode",
+                   err) ||
+          !cuda_ok(cudaMemsetAsync(d_status, 0, sizeof(int) * nsys, st), "clear status", err))
+        return false;
+      bss_assemble_kernel<<<dim3(std::max<int64_t>(1, 2048 / Fb), Fb), 256, 0, st>>>(aa);
+      if (!cuda_ok(cudaGetLastError(), "assemble", err)) return false;
+      if (!cholesky(G, p.np, Fb, d_status, d_mode, st, err) ||
+          !cholesky(Gb, p.nbp, Fb * K, d_status + Fb, d_mode + Fb, st, err))
+        return false;
+      if (!cuda_ok(cudaMemcpyAsync(flags.data(), d_status, sizeof(int) * nsys, cudaMemcpyDeviceToHost, st),
+                   "copy status", err) ||
+          !cuda_ok(cudaStreamSynchronize(st), "synchronize", err))
+        return false;
+      bool again = false;
+      for (int z = 0; z < Fb; ++z)
+        for (int s = 0; s <= K; ++s) {
+          const int q = sys(z, s);
+          if (mode[q] != 1 || !flags[q]) {
+            mode[q] = 0;
+            continue;
+          }
+          if (scale[q] * BSS_LOADING_STEP > BSS_LOADING_LAST) {
+            err = "bss_eval: in frame " + std::to_string(w0 + z) + ", " +
+                  (s == 0 ? std::string("the Gram matrix of all references")
+                          : "the Gram matrix of source " + std::to_string(s - 1) + "'s references") +
+                  " is not positive definite even with a diagonal loading of 2^-20 of its largest diagonal value "
+                  "(pivot " + std::to_string(flags[q]) + " of the Cholesky factorisation)";
+            return false;
+          }
+          scale[q] *= BSS_LOADING_STEP;
+          again = true;
+        }
+      if (!again) break;
+    }
+    if (loading_host)
+      for (int z = 0; z < Fb; ++z)
+        for (int s = 0; s <= K; ++s)
+          loading_host[(w0 + z) * (1 + K) + s] = silent[z] ? std::nan("") : scale[sys(z, s)];
+    SolveArgs sa{};
+    sa.s[0] = SolveSys{G, B, p.np, M, (int64_t)p.np * p.np, (int64_t)p.np * M};
+    for (int j = 0; j < K; ++j)
+      sa.s[1 + j] = SolveSys{Gb + (int64_t)j * p.nbp * p.nbp, Bb + (int64_t)j * p.nbp * C, p.nbp, C,
+                             (int64_t)K * p.nbp * p.nbp, (int64_t)K * p.nbp * C};
+    chol_solve_kernel<<<dim3(1 + K, Fb), SOLVE_THREADS, 0, st>>>(sa);
+    bss_coef_kernel<<<dim3(std::max<int64_t>(1, 256 / Fb), Fb), 256, 0, st>>>(B, Bb, K, C, L, p.Lp, p.np, p.nbp, ca,
+                                                                              cs);
+    if (!cuda_ok(cudaGetLastError(), "solve", err)) return false;
+    if (phase_ms) cudaEventRecord(ev[4], st);
+
+    // projections on each frame's timeline of window + L - 1 samples, and the frame sums
+    const int ntask = Fb * p.tpf;
+    bss_project_kernel<<<dim3(ntask, M), PROJ_THREADS, smem, st>>>(r0, e0, K, C, N, window, hop, p.Lp, ca, cs, d_tasks,
+                                                                   p.tpf, ntask, ep);
+    const int64_t nf = (int64_t)K * Fb * 8;
+    bss_frames_kernel<<<(unsigned)((nf + 255) / 256), 256, 0, st>>>(ep, d_fr, K, C, Fb, ntask, d_frames);
+    if (!cuda_ok(cudaGetLastError(), "projection", err)) return false;
+    if (phase_ms) cudaEventRecord(ev[5], st);
+
+    if (!cuda_ok(cudaMemcpy2DAsync(frames_host + w0 * 8, sizeof(double) * nwin * 8, d_frames, sizeof(double) * Fb * 8,
+                                   sizeof(double) * Fb * 8, K, cudaMemcpyDeviceToHost, st),
+                 "copy frames", err))
+      return false;
+    if (corr_host && !cuda_ok(cudaMemcpy2DAsync(corr_host + w0 * M * 2 * M * L, sizeof(double) * L, R,
+                                                sizeof(double) * p.Lc, sizeof(double) * L, (size_t)Fb * M * 2 * M,
+                                                cudaMemcpyDeviceToHost, st),
+                              "copy correlations", err))
+      return false;
+    if (!cuda_ok(cudaStreamSynchronize(st), "synchronize", err)) return false;
+    if (phase_ms) {
+      float ms;
+      for (int i = 0; i < 3; ++i) {
+        cudaEventElapsedTime(&ms, ev[2 + i], ev[3 + i]);
+        acc[i] += ms;
+      }
+    }
+  }
+  if (phase_ms) {
+    float ms;
+    cudaEventRecord(ev[1], st);
+    if (!cuda_ok(cudaEventSynchronize(ev[1]), "synchronize", err)) return false;
+    cudaEventElapsedTime(&ms, ev[0], ev[1]);
+    for (int i = 0; i < 3; ++i) phase_ms[i] = acc[i];
     phase_ms[3] = ms;
   }
   return true;

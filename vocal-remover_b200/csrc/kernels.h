@@ -135,5 +135,12 @@ int64_t bss_eval_workspace(int K, int C, int64_t N, int L, int64_t window, int64
 bool bss_eval(const float* refs, const float* ests, int K, int C, int64_t N, int L, int64_t window, int64_t hop,
               void* workspace, int64_t workspace_bytes, double* frames_host, double* corr_host, double* loading_host,
               double* phase_ms, cudaStream_t stream, std::string& err);
+// framewise filters (BSS Eval v3): every frame scored as a signal of its own, frames_per_batch frames per batch
+int64_t bss_eval_framewise_workspace(int K, int C, int64_t N, int L, int64_t window, int64_t hop,
+                                     int64_t frames_per_batch, std::string& err);
+bool bss_eval_framewise(const float* refs, const float* ests, int K, int C, int64_t N, int L, int64_t window,
+                        int64_t hop, int64_t frames_per_batch, void* workspace, int64_t workspace_bytes,
+                        double* frames_host, double* corr_host, double* loading_host, double* phase_ms,
+                        cudaStream_t stream, std::string& err);
 
 }  // namespace vr

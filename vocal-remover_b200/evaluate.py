@@ -6,7 +6,8 @@ per pair, both files are loaded and aligned as ``spec_utils.cache_or_load`` does
 ``y`` and the vocals ``X - y``, the estimates are ``Separator.separate_wave`` of the mixture (kept on the device), and
 ``lib/bsseval.bss_eval`` scores every ``--window`` second frame, hopping ``--hop`` seconds.  Each pair prints the median
 over its frames of the four ratios of both stems; the last line is the median over the pairs of those medians.
-``--json`` writes every frame's values as well.
+``--json`` writes every frame's values as well.  ``--framewise_filters`` scores with BSS Eval v3 instead (distortion
+filters solved for each frame on its own samples; ``--window`` of at least ``--filters_len`` samples).
 
 Split flags as validate.py (-g -s -r -H -f -d -S -v -V -P), separation flags as inference.py (-B -c -t -p).  Under
 ``torchrun --nproc-per-node N evaluate.py ...`` every rank scores the pairs ``dataset.shard_files(filelist, N, rank)``
@@ -40,9 +41,10 @@ def pair_waves(X_path, y_path, sr, device=None):
     return spec_utils.align_wave_head_and_tail(X, y, sr)
 
 
-def score_pair(separator, X, y, window, hop, filters_len, tta=False):
+def score_pair(separator, X, y, window, hop, filters_len, tta=False, framewise=False):
     """Frame metrics of one aligned pair: the estimates of ``separator`` against references (y, X - y), both cut to
-    the hop * (L // hop) samples separate_wave returns.  dict of (2, nwin) arrays, rows instruments, vocals."""
+    the hop * (L // hop) samples separate_wave returns.  dict of (2, nwin) arrays, rows instruments, vocals.
+    ``framewise``: BSS Eval v3 filters, solved per frame (bsseval.bss_eval)."""
     dev = separator._dev()
     with torch.cuda.device(dev):
         d_x = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float32)).to(dev)
@@ -51,7 +53,7 @@ def score_pair(separator, X, y, window, hop, filters_len, tta=False):
         n = inst.shape[1]
         refs = torch.stack([d_y[:, :n], (d_x - d_y)[:, :n]])
         ests = torch.stack([inst, voc])
-        return bsseval.bss_eval(refs, ests, window, hop, filters_len, device=dev)
+        return bsseval.bss_eval(refs, ests, window, hop, filters_len, device=dev, framewise=framewise)
 
 
 def dataset_medians(per_track):
@@ -109,6 +111,9 @@ def build_parser():
     p.add_argument('--hop', type=float, default=1.0, help='frame advance in seconds')
     p.add_argument('--filters_len', type=int, default=512, help='taps of the distortion filters')
     p.add_argument('--json', type=str, default=None, help='write every frame value to this file')
+    p.add_argument('--framewise_filters', action='store_true',
+                   help='BSS Eval v3: solve the distortion filters for each frame on its own samples (the SiSEC '
+                        'campaigns before 2018), instead of once per track')
     return p
 
 
@@ -152,6 +157,9 @@ def main():
         p.error('--window and --hop must be at least one sample')
     if not 1 <= args.filters_len <= bsseval.MAX_FILTER:
         p.error('--filters_len must be in [1, {}]'.format(bsseval.MAX_FILTER))
+    if args.framewise_filters and window < args.filters_len:
+        p.error('--framewise_filters needs a --window of at least --filters_len ({}) samples, got {}'.format(
+            args.filters_len, window))
     if args.json is not None and not os.path.isdir(os.path.dirname(os.path.abspath(args.json))):
         p.error('--json: no such directory: {}'.format(os.path.dirname(os.path.abspath(args.json))))
     filelist = select_pairs(p, args)
@@ -188,7 +196,8 @@ def main():
     for k, (X_path, y_path) in enumerate(dataset.shard_files(filelist, world, rank)):
         X, y = pair_waves(X_path, y_path, args.sr, index)
         try:
-            local_results.append(score_pair(sp, X, y, window, hop, args.filters_len, args.tta))
+            local_results.append(score_pair(sp, X, y, window, hop, args.filters_len, args.tta,
+                                            args.framewise_filters))
         except ValueError as e:
             raise ValueError('{}: {}'.format(validate.pair_name(X_path, y_path), e)) from e
         if world == 1:
@@ -200,9 +209,11 @@ def main():
                 report(i, r)
         print('median of {} pairs: {}'.format(len(results), format_values(dataset_medians(results))))
         if args.json is not None:
+            info = {'sr': args.sr, 'window': window, 'hop': hop, 'filters_len': args.filters_len}
+            if args.framewise_filters:
+                info['framewise_filters'] = True
             with open(args.json, 'w') as f:
-                json.dump(to_json(filelist, results, {'sr': args.sr, 'window': window, 'hop': hop,
-                                                      'filters_len': args.filters_len}), f)
+                json.dump(to_json(filelist, results, info), f)
     if world > 1:
         dist.destroy_process_group()
 

@@ -56,6 +56,9 @@ SIGNATURES = {
     'vr_bss_eval_workspace': (c_i64, [c_i32, c_i32, c_i64, c_i32, c_i64, c_i64]),
     'vr_bss_eval': (c_i32, [c_vp, c_fp, c_fp, c_i32, c_i32, c_i64, c_i32, c_i64, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp,
                             c_vp, c_vp]),
+    'vr_bss_eval_framewise_workspace': (c_i64, [c_i32, c_i32, c_i64, c_i32, c_i64, c_i64, c_i32]),
+    'vr_bss_eval_framewise': (c_i32, [c_vp, c_fp, c_fp, c_i32, c_i32, c_i64, c_i32, c_i64, c_i64, c_i32, c_vp, c_i64,
+                                      c_vp, c_vp, c_vp, c_vp, c_vp]),
     'vr_shared_alloc': (c_i32, [c_vp, c_i64, ctypes.POINTER(c_vp), ctypes.c_char_p]),
     'vr_shared_open': (c_i32, [c_vp, ctypes.c_char_p, ctypes.POINTER(c_vp)]),
     'vr_shared_close': (c_i32, [c_vp, c_vp, c_i32]),

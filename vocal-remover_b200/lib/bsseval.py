@@ -8,6 +8,10 @@ channel is projected on the ``filters_len`` delays of every reference channel (P
 
 over the frame and the source's channels.  A frame in which any reference source or any estimate is all zeros is NaN
 for every source.  ``track_medians`` gives the per-track value: the median over the frames that are not NaN.
+
+With ``framewise=True`` the metric is BSS Eval v3 instead (museval's mode 'v3', the SiSEC campaigns before 2018):
+every frame is scored as a signal of its own, with distortion filters solved on its samples alone and projections on
+its timeline of window + filters_len - 1 samples.
 """
 import numpy as np
 import torch
@@ -59,16 +63,51 @@ def _check_sizes(shape_s, shape_e, window, hop, filters_len):
         raise ValueError('the signals (%d samples) are shorter than one window (%d)' % (N, window))
 
 
-def frame_sums(references, estimates, window, hop, filters_len=512, device=None, correlations=False, timings=False):
+WORKSPACE_CAP = 4 << 30   # the framewise workspace budget: a quarter of the free device memory, at most this
+
+
+def framewise_batch(lib, K, C, N, window, hop, filters_len, budget):
+    """The largest number of frames per batch, at most the frame count, whose framewise workspace fits ``budget``
+    bytes; ValueError if even one frame does not."""
+    def need(f):
+        nbytes = lib.vr_bss_eval_framewise_workspace(K, C, N, filters_len, window, hop, f)
+        if nbytes < 0:
+            raise ValueError(lib.vr_last_error(None).decode())
+        return nbytes
+
+    lo, hi = 1, min(frame_count(N, window, hop), 4096)
+    if need(lo) > budget:
+        raise ValueError('one frame of framewise BSS Eval needs %d bytes of device workspace, over the budget of %d'
+                         % (need(lo), budget))
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        if need(mid) <= budget:
+            lo = mid
+        else:
+            hi = mid - 1
+    return lo
+
+
+def frame_sums(references, estimates, window, hop, filters_len=512, device=None, correlations=False, timings=False,
+               framewise=False, frames_per_batch=None):
     """The device evaluation without the ratios: a dict with 'sums', float64 (K, nwin, 8), the per-frame sums over the
     source's channels of s^2, (P_j - s)^2, (shat - s)^2, P_j^2, (P_all - P_j)^2, P_all^2, (shat - P_all)^2 and shat^2;
     'loading', the K + 1 diagonal loading scales the systems were solved with (all unknowns, then each source: eps =
     scale * max diag G, 2^-40 unless a factorisation needed more); with ``correlations`` also 'corr',
     (K*C, 2*K*C, filters_len) r[a][b](l) = sum_u s_a(u) y_b(u + l) with y the references then the estimates (G and d);
     with ``timings`` also 'phase_ms', the CUDA-event times of correlations,
-    solves, projections and the whole call."""
+    solves, projections and the whole call.
+
+    ``framewise``: BSS Eval v3, every frame scored as a signal of its own (DESIGN.md section 10, "Framewise filters
+    (v3)"), ``window >= filters_len``.  The sums are then over each frame's timeline of window + filters_len - 1
+    samples, 'loading' is (nwin, K + 1) with NaN rows for silent frames, 'corr' is (nwin, K*C, 2*K*C, filters_len) and
+    'frames_per_batch' the batch the frames were solved in: ``frames_per_batch``, or when None the largest that fits a
+    quarter of the device's free memory, at most WORKSPACE_CAP bytes.  The results do not depend on it."""
     window, hop, filters_len = int(window), int(hop), int(filters_len)
     _check_sizes(np.shape(references), np.shape(estimates), window, hop, filters_len)
+    if framewise and window < filters_len:
+        raise ValueError('with framewise filters the window (%d samples) must not be shorter than filters_len (%d)'
+                         % (window, filters_len))
     K, C, N = (int(v) for v in np.shape(references))
     if not torch.is_tensor(references) and not np.any(references):
         raise ValueError('every reference is zero: the ratios are undefined')
@@ -85,21 +124,43 @@ def frame_sums(references, estimates, window, hop, filters_len=512, device=None,
         for x, what in ((s, 'references'), (e, 'estimates')):
             if not bool(torch.isfinite(x).all()):
                 raise ValueError('the %s hold NaN or Inf' % what)
-        nbytes = lib.vr_bss_eval_workspace(K, C, N, filters_len, window, hop)
-        if nbytes < 0:
-            raise ValueError(lib.vr_last_error(None).decode())
-        ws = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
         nwin = frame_count(N, window, hop)
         sums = np.empty((K, nwin, 8), dtype=np.float64)
-        corr = np.empty((K * C, 2 * K * C, filters_len), dtype=np.float64) if correlations else None
         phase = np.empty(4, dtype=np.float64) if timings else None
-        loading = np.empty(K + 1, dtype=np.float64)
-        rc = lib.vr_bss_eval(None, _native.ptr(s), _native.ptr(e), K, C, N, filters_len, window, hop,
-                             _native.ptr(ws), int(nbytes), sums.ctypes.data, None if corr is None else corr.ctypes.data,
-                             loading.ctypes.data, None if phase is None else phase.ctypes.data, _native.stream_ptr())
-        if rc != 0:
-            raise _native.NativeError('vr_bss_eval failed: %s' % lib.vr_last_error(None).decode())
+        if framewise:
+            if frames_per_batch is None:
+                free, _ = torch.cuda.mem_get_info(dev)
+                frames_per_batch = framewise_batch(lib, K, C, N, window, hop, filters_len,
+                                                   min(free // 4, WORKSPACE_CAP))
+            frames_per_batch = int(frames_per_batch)
+            nbytes = lib.vr_bss_eval_framewise_workspace(K, C, N, filters_len, window, hop, frames_per_batch)
+            if nbytes < 0:
+                raise ValueError(lib.vr_last_error(None).decode())
+            ws = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
+            corr = np.empty((nwin, K * C, 2 * K * C, filters_len), dtype=np.float64) if correlations else None
+            loading = np.empty((nwin, K + 1), dtype=np.float64)
+            rc = lib.vr_bss_eval_framewise(None, _native.ptr(s), _native.ptr(e), K, C, N, filters_len, window, hop,
+                                           frames_per_batch, _native.ptr(ws), int(nbytes), sums.ctypes.data,
+                                           None if corr is None else corr.ctypes.data, loading.ctypes.data,
+                                           None if phase is None else phase.ctypes.data, _native.stream_ptr())
+            if rc != 0:
+                raise _native.NativeError('vr_bss_eval_framewise failed: %s' % lib.vr_last_error(None).decode())
+        else:
+            nbytes = lib.vr_bss_eval_workspace(K, C, N, filters_len, window, hop)
+            if nbytes < 0:
+                raise ValueError(lib.vr_last_error(None).decode())
+            ws = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
+            corr = np.empty((K * C, 2 * K * C, filters_len), dtype=np.float64) if correlations else None
+            loading = np.empty(K + 1, dtype=np.float64)
+            rc = lib.vr_bss_eval(None, _native.ptr(s), _native.ptr(e), K, C, N, filters_len, window, hop,
+                                 _native.ptr(ws), int(nbytes), sums.ctypes.data,
+                                 None if corr is None else corr.ctypes.data, loading.ctypes.data,
+                                 None if phase is None else phase.ctypes.data, _native.stream_ptr())
+            if rc != 0:
+                raise _native.NativeError('vr_bss_eval failed: %s' % lib.vr_last_error(None).decode())
     out = {'sums': sums, 'loading': loading}
+    if framewise:
+        out['frames_per_batch'] = frames_per_batch
     if correlations:
         out['corr'] = corr
     if timings:
@@ -122,14 +183,16 @@ def metrics(sums):
     return {m: out[m] for m in METRICS}
 
 
-def bss_eval(references, estimates, window, hop, filters_len=512, device=None):
+def bss_eval(references, estimates, window, hop, filters_len=512, device=None, framewise=False):
     """SDR, ISR, SIR and SAR of every frame of ``estimates`` against ``references``.
 
     references, estimates: (K, C, N) float32 numpy arrays or CUDA tensors (K sources of C channels, K * C <= 8).
     window, hop: frame length and advance in samples; filters_len: taps of the distortion filters (<= 1024).
+    framewise: BSS Eval v3 (museval's mode 'v3'), distortion filters solved for each frame on its own samples,
+    instead of one set per track (v4); needs window >= filters_len.
     Returns a dict of (K, nwin) float64 numpy arrays 'sdr', 'isr', 'sir', 'sar' (dB), nwin = frame_count(N, window,
     hop).  Raises ValueError for different shapes, N < window, all-zero references or NaN / Inf input."""
-    return metrics(frame_sums(references, estimates, window, hop, filters_len, device)['sums'])
+    return metrics(frame_sums(references, estimates, window, hop, filters_len, device, framewise=framewise)['sums'])
 
 
 def track_medians(result):
