@@ -158,6 +158,16 @@ VR_API int vr_spec_sub(vr_ctx* ctx, const void* a, const void* b, int64_t T, voi
 VR_API int vr_validation_loss(vr_ctx* ctx, const void* spec_x, const void* spec_y, int64_t T,
                               float* coef_out, double* window_sums, void* stream);
 
+/* --wiener_iterations (DESIGN.md §11): norbert 0.2's wiener(v, x, iterations, use_softmask=False) for two channels and
+ * two sources.  spec is the mixture, y_spec / v_spec the initial estimates (vr_apply_mask's outputs), all device
+ * complex64 [2][bins][T]; y_spec and v_spec are refined in place by `iterations` rounds of expectation-maximisation:
+ * per bin the spatial covariance R_j of each source over the whole track, then per (bin, frame)
+ * y_j = v_j R_j (sum_k v_k R_k + sqrt(eps) I)^-1 x, in fp64 on the mixture scaled by max(1, max|X| / 10), the estimates
+ * stored as complex64 between iterations.  iterations = 0 leaves them unchanged.  iterations < 0, T < 1 or a NULL
+ * pointer is an error.  The results are bit-identical from call to call.                                        */
+VR_API int vr_wiener(vr_ctx* ctx, const void* spec, void* y_spec, void* v_spec, int64_t T, int32_t iterations,
+                     void* stream);
+
 /* The sample-rate conversion inside librosa.load(path, sr=args.sr, res_type='kaiser_fast') (inference.py:136-138,
  * pseudo.py:47-50) = resampy.resample(y, orig_sr, sr, filter='kaiser_fast'): x [channels][n_in] -> y [channels][n_out],
  * n_out = (int64)(n_in * sample_ratio), sample_ratio = sr / orig_sr.  win / delta: DEVICE float64 arrays of nwin entries -

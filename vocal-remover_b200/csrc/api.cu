@@ -221,6 +221,12 @@ int vr_validation_loss(vr_ctx* ctx, const void* spec_x, const void* spec_y, int6
                                              (cudaStream_t)stream));
 }
 
+int vr_wiener(vr_ctx* ctx, const void* spec, void* y_spec, void* v_spec, int64_t T, int32_t iterations, void* stream) {
+  CHECK_CTX(ctx);
+  return done(ctx, ctx->eng->wiener((const float2*)spec, (float2*)y_spec, (float2*)v_spec, T, iterations,
+                                    (cudaStream_t)stream));
+}
+
 int vr_resample(vr_ctx* ctx, const float* x, int32_t channels, int64_t n_in, float* y, int64_t n_out, double sample_ratio,
                 const double* win, const double* delta, int32_t nwin, int32_t table_per_crossing, void* stream) {
   // ctx may be NULL (audio is usually loaded before a model context exists): the call then runs on the calling

@@ -811,6 +811,18 @@ bool Engine::validation_loss(const float2* spec_x, const float2* spec_y, int64_t
   });
 }
 
+bool Engine::wiener(const float2* spec, float2* y, float2* v, int64_t T, int iterations, cudaStream_t s) {
+  if (T < 1 || iterations < 0 || !spec || !y || !v) {
+    err = "wiener: needs spec, y_spec, v_spec, T >= 1 and iterations >= 0";
+    return false;
+  }
+  if (iterations == 0) return true;
+  if (!ck(ws_wiener_.ensure(wiener_scratch(bins())), "workspace wiener")) return false;
+  return timed("wiener", 1 + 3 * iterations, 1, bins(), (int)T, s, [&] {
+    return ck(launch_wiener(spec, y, v, bins(), T, iterations, ws_wiener_.get(), s), "wiener");
+  });
+}
+
 bool Engine::stft(const float* wave, int64_t L, float2* spec, int64_t T, float* absmax, cudaStream_t s) {
   if (!stft_range(wave, L, spec, T, 0, T, s)) return false;
   if (absmax) return normaliser(spec, T, 0, absmax, s);

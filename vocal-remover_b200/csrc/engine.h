@@ -209,6 +209,8 @@ class Engine {
   // validation loss of one (mixture, instruments) pair; see vr_validation_loss in include/vr_b200.h
   bool validation_loss(const float2* spec_x, const float2* spec_y, int64_t T, float* coef_out, double* window_sums,
                        cudaStream_t s);
+  // --wiener_iterations: EM refinement of the stems' spectrograms y / v in place; see vr_wiener in include/vr_b200.h
+  bool wiener(const float2* spec, float2* y, float2* v, int64_t T, int iterations, cudaStream_t s);
 
   // debug / tests: run one reference Conv2DBNActiv-shaped layer through a chosen kernel
   bool debug_conv(const float* x_nchw, int N, int Cin, int H, int W, const float* w, const float* bias, int Cout,
@@ -264,6 +266,7 @@ class Engine {
   unsigned int* ws_img_range_ = nullptr;   // [4] min / max keys of the spectrogram image pass (first use)
   GrowArray<unsigned char> ws_img_;   // two [bins][T][3] images (host-buffer entry)
   GrowArray<double> ws_val_;   // per-slice partial sums of the validation loss
+  GrowArray<double> ws_wiener_;   // per-slice moments, per-bin covariances and the scale of the Wiener filter
 
   // the high-band BaseNets of stages 1-2 run on their own stream next to the low-band chain (independent until
   // stage 3, lib/nets.py:88-99); disabled while per-kernel profiling is on so event timings stay per-kernel

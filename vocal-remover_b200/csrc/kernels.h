@@ -73,6 +73,13 @@ cudaError_t launch_validation_l1(const float2* spec_x, const float2* spec_y, con
                                  int roi, int n_windows, const float* coef, double* partial, double* window_sums,
                                  cudaStream_t stream);
 
+// ---- multichannel Wiener filter (wiener.cu), DESIGN.md §11 ------------------------------------------------------------
+// `iterations` EM refinements of the estimates y / v [2][bins][T] (complex64, in place) of the mixture spec [2][bins][T];
+// scratch: wiener_scratch(bins) doubles.  1 + 3 * iterations kernels.
+int64_t wiener_scratch(int bins);
+cudaError_t launch_wiener(const float2* spec, float2* y, float2* v, int bins, int64_t T, int iterations,
+                          double* scratch, cudaStream_t stream);
+
 // ---- LSTM branch (lstm.cu), reference lib/layers.py:108-133 ------------------------------------
 // 1x1 conv (C -> 1), pre-activation sums as an fp32 plane l0[n][bin][t] (dec2's epilogue accumulates the same sums
 // instead where its plan can: ConvFusion::dot_w in engine.h, TcConv::fuses_dot)

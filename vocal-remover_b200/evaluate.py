@@ -114,6 +114,9 @@ def build_parser():
     p.add_argument('--framewise_filters', action='store_true',
                    help='BSS Eval v3: solve the distortion filters for each frame on its own samples (the SiSEC '
                         'campaigns before 2018), instead of once per track')
+    p.add_argument('--wiener_iterations', type=inference.non_negative_int, default=0,
+                   help="score the stems refined by this many iterations of inference.py's multichannel Wiener filter "
+                        "(0: the masked stems; 1 is norbert's default)")
     return p
 
 
@@ -186,7 +189,8 @@ def main():
     spec_utils.set_device(index)
     if rank == 0:
         print('done')
-    sp = inference.Separator(model, device, args.batchsize, args.cropsize, args.postprocess)
+    sp = inference.Separator(model, device, args.batchsize, args.cropsize, args.postprocess,
+                             wiener_iterations=args.wiener_iterations)
 
     def report(i, result):
         X_path, y_path = filelist[i]
@@ -212,6 +216,8 @@ def main():
             info = {'sr': args.sr, 'window': window, 'hop': hop, 'filters_len': args.filters_len}
             if args.framewise_filters:
                 info['framewise_filters'] = True
+            if args.wiener_iterations > 0:
+                info['wiener_iterations'] = args.wiener_iterations
             with open(args.json, 'w') as f:
                 json.dump(to_json(filelist, results, info), f)
     if world > 1:

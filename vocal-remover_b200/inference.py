@@ -23,13 +23,18 @@ from lib import utils
 
 class Separator(object):
 
-    def __init__(self, model, device=None, batchsize=1, cropsize=256, postprocess=False):
+    def __init__(self, model, device=None, batchsize=1, cropsize=256, postprocess=False, wiener_iterations=0):
         self.model = model
         self.offset = model.offset
         self.device = device
         self.batchsize = batchsize
         self.cropsize = cropsize
         self.postprocess = postprocess
+        # an extension of the reference: > 0 refines both stems with that many iterations of a multichannel Wiener
+        # filter (vr_wiener, DESIGN.md §11) once the mask is final
+        if wiener_iterations < 0:
+            raise ValueError('wiener_iterations must be >= 0, got %d' % wiener_iterations)
+        self.wiener_iterations = int(wiener_iterations)
         if device is not None:
             model.to(device)
 
@@ -75,7 +80,15 @@ class Separator(object):
             v = torch.empty_like(d_spec)
             ctx.check(ctx.lib.vr_apply_mask(ctx.handle, _native.ptr(d_spec), _native.ptr(d_mask), d_spec.shape[2],
                                             _native.ptr(y), _native.ptr(v), _native.stream_ptr()), 'vr_apply_mask')
+            self._wiener(d_spec, y, v)
             return y.cpu().numpy(), v.cpu().numpy()
+
+    def _wiener(self, d_spec, y, v):
+        """--wiener_iterations: y / v refined in place (nothing to do for 0)."""
+        if self.wiener_iterations > 0:
+            ctx = self._ctx()
+            ctx.check(ctx.lib.vr_wiener(ctx.handle, _native.ptr(d_spec), _native.ptr(y), _native.ptr(v),
+                                        d_spec.shape[2], self.wiener_iterations, _native.stream_ptr()), 'vr_wiener')
 
     # ---- reference surface --------------------------------------------------------------------------
     def _separate(self, X_spec_pad, roi_size):
@@ -112,8 +125,8 @@ class Separator(object):
         as uint8 (bins, T, 3): (inst, voc, img_inst, img_voc); the stems are the same as with ``images=False``.
         """
         ctx = self._ctx()
-        if self.postprocess:
-            # staged on the device: STFT -> mask (+ postprocess) -> masked inverse STFT
+        if self.postprocess or self.wiener_iterations > 0:
+            # staged on the device: STFT -> mask (+ postprocess) [-> Wiener filter] -> inverse STFT
             return self._separate_wave_staged(wave, tta, images)
         dev = self._dev()
         hop = self.model.hop_length
@@ -164,16 +177,32 @@ class Separator(object):
             d_mask = self._mask_device(d_spec, tta)
             inst = torch.empty((2, hop * (T - 1)), dtype=torch.float32, device=dev)
             voc = torch.empty_like(inst)
-            ctx.check(ctx.lib.vr_apply_mask_istft(ctx.handle, _native.ptr(d_spec), _native.ptr(d_mask), T,
-                                                  _native.ptr(inst), _native.ptr(voc), _native.stream_ptr()),
-                      'vr_apply_mask_istft')
+            if self.wiener_iterations > 0:
+                # the filtered stems' spectrograms, then one inverse STFT (and image) per stem
+                y = torch.empty_like(d_spec)
+                v = torch.empty_like(d_spec)
+                ctx.check(ctx.lib.vr_apply_mask(ctx.handle, _native.ptr(d_spec), _native.ptr(d_mask), T,
+                                                _native.ptr(y), _native.ptr(v), _native.stream_ptr()), 'vr_apply_mask')
+                self._wiener(d_spec, y, v)
+                for spec, wave_out in ((y, inst), (v, voc)):
+                    ctx.check(ctx.lib.vr_istft(ctx.handle, _native.ptr(spec), T, _native.ptr(wave_out),
+                                               _native.stream_ptr()), 'vr_istft')
+            else:
+                ctx.check(ctx.lib.vr_apply_mask_istft(ctx.handle, _native.ptr(d_spec), _native.ptr(d_mask), T,
+                                                      _native.ptr(inst), _native.ptr(voc), _native.stream_ptr()),
+                          'vr_apply_mask_istft')
             out = [inst, voc]
             if images:
                 img_inst = torch.empty((n_fft // 2 + 1, T, 3), dtype=torch.uint8, device=dev)
                 img_voc = torch.empty_like(img_inst)
-                ctx.check(ctx.lib.vr_spec_image(ctx.handle, _native.ptr(d_spec), _native.ptr(d_mask), T,
-                                                _native.ptr(img_inst), _native.ptr(img_voc), _native.stream_ptr()),
-                          'vr_spec_image')
+                if self.wiener_iterations > 0:
+                    for spec, img in ((y, img_inst), (v, img_voc)):
+                        ctx.check(ctx.lib.vr_spec_image(ctx.handle, _native.ptr(spec), None, T, _native.ptr(img), None,
+                                                        _native.stream_ptr()), 'vr_spec_image')
+                else:
+                    ctx.check(ctx.lib.vr_spec_image(ctx.handle, _native.ptr(d_spec), _native.ptr(d_mask), T,
+                                                    _native.ptr(img_inst), _native.ptr(img_voc), _native.stream_ptr()),
+                              'vr_spec_image')
                 out += [img_inst, img_voc]
             return tuple(t.cpu().numpy() for t in out) if host else tuple(out)
 
@@ -202,7 +231,18 @@ def build_parser():
     # an extension of the reference CLI too: bits per written sample of either format; 24 keeps the depth of a 24-bit
     # input, which the float32 stems carry and 16-bit output throws away
     p.add_argument('--output_bits', type=int, choices=[16, 24], default=16)
+    # an extension as well: refine both stems with a multichannel Wiener filter (DESIGN.md §11) after the mask is final
+    p.add_argument('--wiener_iterations', type=non_negative_int, default=0,
+                   help="EM iterations of a multichannel Wiener filter applied to both stems (0: none; 1 is norbert's "
+                        "default)")
     return p
+
+
+def non_negative_int(text):
+    value = int(text)
+    if value < 0:
+        raise argparse.ArgumentTypeError('must be >= 0, got {}'.format(value))
+    return value
 
 
 def main():
@@ -242,7 +282,8 @@ def main():
         device=device,
         batchsize=args.batchsize,
         cropsize=args.cropsize,
-        postprocess=args.postprocess
+        postprocess=args.postprocess,
+        wiener_iterations=args.wiener_iterations
     )
 
     print('validating output directory...', end=' ')

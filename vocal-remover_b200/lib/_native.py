@@ -48,6 +48,7 @@ SIGNATURES = {
     'vr_vocal_image': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_vp, c_vp]),
     'vr_spec_sub': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_vp, c_vp]),
     'vr_validation_loss': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_fp, c_vp, c_vp]),
+    'vr_wiener': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp]),
     'vr_flac_scan': (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i32, c_vp, c_vp]),
     'vr_flac_decode': (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i32, c_i32, c_i64, c_fp, c_vp, c_vp]),
     'vr_flac_encode_analyse': (c_i32, [c_vp, c_fp, c_i32, c_i64, c_i32, c_i32, c_vp, c_vp, c_vp]),

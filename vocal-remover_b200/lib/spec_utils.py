@@ -154,6 +154,36 @@ def spectrogram_difference(a, b):
         return out if on_device else out.cpu().numpy()
 
 
+def wiener(X_spec, y_spec, v_spec, iterations=1):
+    """The two stems refined by a multichannel Wiener filter (expectation-maximisation, norbert 0.2's
+    ``wiener(v, x, iterations)`` for 2 channels and 2 sources; DESIGN.md §11), on the GPU (vr_wiener).
+
+    X_spec is the mixture, y_spec / v_spec the initial estimates (the masked spectrograms), each complex (2, bins, T).
+    Numpy arrays give numpy arrays, CUDA tensors new CUDA tensors; the inputs are not modified.  Returns
+    (y_spec, v_spec) as complex64; ``iterations = 0`` returns them unchanged.
+    """
+    if iterations < 0:
+        raise ValueError('wiener: iterations must be >= 0, got %d' % iterations)
+    on_device = torch.is_tensor(X_spec)
+    if torch.is_tensor(y_spec) != on_device or torch.is_tensor(v_spec) != on_device:
+        raise TypeError('wiener: X_spec, y_spec and v_spec must all be numpy arrays or all CUDA tensors')
+    if not on_device:
+        X_spec, y_spec, v_spec = np.asarray(X_spec), np.asarray(y_spec), np.asarray(v_spec)
+    if X_spec.ndim != 3 or X_spec.shape[0] != 2 or X_spec.shape[2] < 1 or \
+            not tuple(X_spec.shape) == tuple(y_spec.shape) == tuple(v_spec.shape):
+        raise ValueError('wiener: X_spec, y_spec and v_spec must all have shape (2, bins, T >= 1), got %s, %s and %s'
+                         % (tuple(X_spec.shape), tuple(y_spec.shape), tuple(v_spec.shape)))
+    bins, T = X_spec.shape[1], X_spec.shape[2]
+    ctx = _spectral_ctx(2 * (bins - 1), bins - 1)
+    dev = torch.device('cuda', ctx.device_index)
+    with torch.cuda.device(dev):
+        d_x = _to_device(X_spec, dev, 'wiener')
+        d_y, d_v = (_to_device(s, dev, 'wiener').clone() for s in (y_spec, v_spec))
+        ctx.check(ctx.lib.vr_wiener(ctx.handle, _native.ptr(d_x), _native.ptr(d_y), _native.ptr(d_v), T,
+                                    int(iterations), _native.stream_ptr()), 'vr_wiener')
+        return (d_y, d_v) if on_device else (d_y.cpu().numpy(), d_v.cpu().numpy())
+
+
 def artifact_weights(frame_min, thres=0.05, min_range=64, fade_size=32):
     """Per-frame fade weight of ``merge_artifacts`` from the per-frame minimum of the mask over (channel, bin).
 
