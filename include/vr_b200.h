@@ -148,6 +148,13 @@ VR_API int vr_vocal_image(vr_ctx* ctx, const void* spec_x, const void* spec_y, i
  * complex64 [2][bins][T] arrays a, b, out (IEEE fp32 subtraction, numpy's bits).                               */
 VR_API int vr_spec_sub(vr_ctx* ctx, const void* a, const void* b, int64_t T, void* out, void* stream);
 
+/* evaluate.py --oracle (DESIGN.md §12): the instruments mask of an ideal separation, from the mixture spec_x and the
+ * true instruments spec_y (device complex64 [2][bins][T]); the true vocals are V = spec_x - spec_y with vr_spec_sub's
+ * fp32 bits.  mask: device float32 [2][bins][T] in [0, 1].  kind: 0 iam, 1 ibm, 2 irm1, 3 irm2; anything else, T < 1
+ * or a NULL pointer is an error.  Needs no weights.  Bit-identical from call to call.                           */
+VR_API int vr_oracle_mask(vr_ctx* ctx, const void* spec_x, const void* spec_y, int64_t T, int32_t kind, float* mask,
+                          void* stream);
+
 /* train.py:108-134 validate_epoch over lib/dataset.py:220-248 make_validation_set, one track pair:
  * window_sums[j], j < ceil(T/roi), = sum over (2, bins, roi) of |mask*|X|/coef - |y|/coef| for patch j,
  * coef = max(max|X|, max|y|) written to *coef_out (device float, may be NULL).

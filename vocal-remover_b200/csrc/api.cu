@@ -214,6 +214,13 @@ int vr_spec_sub(vr_ctx* ctx, const void* a, const void* b, int64_t T, void* out,
   return done(ctx, ctx->eng->spec_sub((const float2*)a, (const float2*)b, T, (float2*)out, (cudaStream_t)stream));
 }
 
+int vr_oracle_mask(vr_ctx* ctx, const void* spec_x, const void* spec_y, int64_t T, int32_t kind, float* mask,
+                   void* stream) {
+  CHECK_CTX(ctx);
+  return done(ctx, ctx->eng->oracle_mask((const float2*)spec_x, (const float2*)spec_y, T, kind, mask,
+                                         (cudaStream_t)stream));
+}
+
 int vr_validation_loss(vr_ctx* ctx, const void* spec_x, const void* spec_y, int64_t T, float* coef_out,
                        double* window_sums, void* stream) {
   CHECK_NET(ctx);

@@ -641,6 +641,57 @@ cudaError_t launch_spec_sub(const float2* a, const float2* b, int64_t n, float2*
 }
 
 // ------------------------------------------------------------------------------------------------
+// Oracle masks (evaluate.py --oracle, DESIGN.md §12): the instruments mask of an ideal separation from the mixture X and
+// the true instruments Y, with the true vocals V = X - Y in spec_sub_kernel's fp32 bits.  Powers, square roots and the
+// quotient are fp64 with every operation IEEE-rounded and nothing contracted, then rounded once to fp32, so a float64
+// numpy restatement (tests/oracle_masks.py) gives the same bits.
+__device__ __forceinline__ double oracle_power(float re, float im) {
+  const double r = re, i = im;
+  return __dadd_rn(__dmul_rn(r, r), __dmul_rn(i, i));
+}
+
+template <int KIND>   // 0 iam, 1 ibm, 2 irm1, 3 irm2
+__global__ void oracle_mask_kernel(const float2* __restrict__ spec_x, const float2* __restrict__ spec_y, int64_t n,
+                                   float* __restrict__ mask) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float2 x = spec_x[i], y = spec_y[i];
+  const double pY = oracle_power(y.x, y.y);
+  double m;
+  if (KIND == 0) {
+    // clip(|Y| / |X|, 0, 1); X = 0 gives 1
+    const double pX = oracle_power(x.x, x.y);
+    m = pY >= pX ? 1.0 : __ddiv_rn(__dsqrt_rn(pY), __dsqrt_rn(pX));
+  } else {
+    const double pV = oracle_power(__fsub_rn(x.x, y.x), __fsub_rn(x.y, y.y));
+    if (KIND == 1) {
+      m = pY >= pV ? 1.0 : 0.0;
+    } else if (KIND == 2) {
+      const double a = __dsqrt_rn(pY), s = __dadd_rn(a, __dsqrt_rn(pV));
+      m = s == 0.0 ? 0.5 : __ddiv_rn(a, s);
+    } else {
+      const double s = __dadd_rn(pY, pV);
+      m = s == 0.0 ? 0.5 : __ddiv_rn(pY, s);
+    }
+  }
+  mask[i] = __double2float_rn(m);
+}
+
+cudaError_t launch_oracle_mask(const float2* spec_x, const float2* spec_y, int64_t n, int kind, float* mask,
+                               cudaStream_t stream) {
+  if (n == 0) return cudaSuccess;
+  const unsigned grid = (unsigned)((n + 255) / 256);
+  switch (kind) {
+    case 0: oracle_mask_kernel<0><<<grid, 256, 0, stream>>>(spec_x, spec_y, n, mask); break;
+    case 1: oracle_mask_kernel<1><<<grid, 256, 0, stream>>>(spec_x, spec_y, n, mask); break;
+    case 2: oracle_mask_kernel<2><<<grid, 256, 0, stream>>>(spec_x, spec_y, n, mask); break;
+    case 3: oracle_mask_kernel<3><<<grid, 256, 0, stream>>>(spec_x, spec_y, n, mask); break;
+    default: return cudaErrorInvalidValue;
+  }
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------
 // Validation loss (reference train.py:108-134 over lib/dataset.py:220-248): per window j, the sum over (channel, bin,
 // roi frames t in [j*roi, (j+1)*roi)) of |m*|X|*inv - |y|*inv|, inv = 1/coef, zero for t >= T.  The terms are fp32
 // with the pack kernel's hypotf-and-reciprocal arithmetic and accumulate in fp64.  Every window is cut into

@@ -772,6 +772,16 @@ bool Engine::spec_sub(const float2* a, const float2* b, int64_t T, float2* out, 
   });
 }
 
+bool Engine::oracle_mask(const float2* spec_x, const float2* spec_y, int64_t T, int kind, float* mask, cudaStream_t s) {
+  if (T < 1 || kind < 0 || kind > 3 || !spec_x || !spec_y || !mask) {
+    err = "oracle_mask: needs spec_x, spec_y, mask, T >= 1 and kind 0 (iam), 1 (ibm), 2 (irm1) or 3 (irm2)";
+    return false;
+  }
+  return timed("oracle_mask", 1, 1, bins(), (int)T, s, [&] {
+    return ck(launch_oracle_mask(spec_x, spec_y, (int64_t)2 * bins() * T, kind, mask, s), "oracle_mask");
+  });
+}
+
 // train.py:108-134 validate_epoch over lib/dataset.py:220-248 make_validation_set, one pair: coef = max(max|X|, max|y|),
 // ceil(T / roi) windows of X / coef padded by make_padding (left = offset) through the net, then the L1 sums of the
 // kept mask frames.  Only the mask workspace is needed (no inverse STFT, so not ensure_ws's frame workspace).

@@ -205,6 +205,8 @@ class Engine {
   // dataset tools: image of the vocal residual of a track pair, and out = a - b; see include/vr_b200.h
   bool vocal_image(const float2* spec_x, const float2* spec_y, int64_t T, unsigned char* img, cudaStream_t s);
   bool spec_sub(const float2* a, const float2* b, int64_t T, float2* out, cudaStream_t s);
+  // evaluate.py --oracle: the ideal instruments mask of a (mixture, instruments) pair; see vr_oracle_mask
+  bool oracle_mask(const float2* spec_x, const float2* spec_y, int64_t T, int kind, float* mask, cudaStream_t s);
   bool normaliser(const float2* spec, int64_t T, int mode, float* out, cudaStream_t s);
   // validation loss of one (mixture, instruments) pair; see vr_validation_loss in include/vr_b200.h
   bool validation_loss(const float2* spec_x, const float2* spec_y, int64_t T, float* coef_out, double* window_sums,

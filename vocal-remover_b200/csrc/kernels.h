@@ -65,6 +65,10 @@ cudaError_t launch_vocal_image(const float2* spec_x, const float2* spec_y, int64
                                unsigned char* img, cudaStream_t stream);
 // out[i] = a[i] - b[i] over n complex elements
 cudaError_t launch_spec_sub(const float2* a, const float2* b, int64_t n, float2* out, cudaStream_t stream);
+// oracle masks (evaluate.py --oracle, DESIGN.md §12): mask[i] in [0, 1] of the mixture spec_x and the true instruments
+// spec_y over n complex elements; kind 0 iam, 1 ibm, 2 irm1, 3 irm2
+cudaError_t launch_oracle_mask(const float2* spec_x, const float2* spec_y, int64_t n, int kind, float* mask,
+                               cudaStream_t stream);
 // validation loss (reference train.py:108-134): window_sums[j] = sum over (channel, bin, frames [j*roi, (j+1)*roi) of
 // the track) of |mask * |X| / coef - |y| / coef|, spec_x / spec_y [2][bins][T], mask [2][bins][n_windows * roi],
 // *coef on the device; partial: validation_l1_scratch(n_windows) doubles of scratch

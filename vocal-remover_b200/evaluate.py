@@ -9,6 +9,10 @@ over its frames of the four ratios of both stems; the last line is the median ov
 ``--json`` writes every frame's values as well.  ``--framewise_filters`` scores with BSS Eval v3 instead (distortion
 filters solved for each frame on its own samples; ``--window`` of at least ``--filters_len`` samples).
 
+``--oracle KIND`` (instead of ``-P``) scores an oracle separation computed from the true stems at the STFT of ``-f`` /
+``-H`` (DESIGN.md §12): the ideal amplitude, binary or ratio masks (iam, ibm, irm1, irm2) applied as Separator applies
+the net's mask, or the oracle multichannel Wiener filter (mwf).  No checkpoint is read and no net context is made.
+
 Split flags as validate.py (-g -s -r -H -f -d -S -v -V -P), separation flags as inference.py (-B -c -t -p).  Under
 ``torchrun --nproc-per-node N evaluate.py ...`` every rank scores the pairs ``dataset.shard_files(filelist, N, rank)``
 and rank 0 prints them in file order; each pair is scored on one GPU, so the numbers do not depend on N.
@@ -47,13 +51,32 @@ def score_pair(separator, X, y, window, hop, filters_len, tta=False, framewise=F
     ``framewise``: BSS Eval v3 filters, solved per frame (bsseval.bss_eval)."""
     dev = separator._dev()
     with torch.cuda.device(dev):
-        d_x = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float32)).to(dev)
-        d_y = torch.from_numpy(np.ascontiguousarray(y, dtype=np.float32)).to(dev)
+        d_x, d_y = _device_pair(X, y, dev)
         inst, voc = separator.separate_wave(d_x, tta)
-        n = inst.shape[1]
-        refs = torch.stack([d_y[:, :n], (d_x - d_y)[:, :n]])
-        ests = torch.stack([inst, voc])
-        return bsseval.bss_eval(refs, ests, window, hop, filters_len, device=dev, framewise=framewise)
+        return score_stems(d_x, d_y, inst, voc, window, hop, filters_len, framewise, dev)
+
+
+def score_oracle_pair(kind, X, y, n_fft, hop_length, window, hop, filters_len, framewise=False, wiener_iterations=0):
+    """Frame metrics of one aligned pair for the oracle ``kind`` (spec_utils.ORACLES) at the STFT (n_fft, hop_length):
+    score_pair with the stems of spec_utils.oracle_separate_wave, on spec_utils' device."""
+    dev = spec_utils.current_device()
+    with torch.cuda.device(dev):
+        d_x, d_y = _device_pair(X, y, dev)
+        inst, voc = spec_utils.oracle_separate_wave(d_x, d_y, kind, n_fft, hop_length, wiener_iterations)
+        return score_stems(d_x, d_y, inst, voc, window, hop, filters_len, framewise, dev)
+
+
+def _device_pair(X, y, dev):
+    return (torch.from_numpy(np.ascontiguousarray(w, dtype=np.float32)).to(dev) for w in (X, y))
+
+
+def score_stems(d_x, d_y, inst, voc, window, hop, filters_len, framewise, dev):
+    """Frame metrics of the estimates (inst, voc) of the device pair (d_x, d_y) against the references (y, X - y), both
+    cut to the estimates' length.  dict of (2, nwin) arrays, rows instruments, vocals."""
+    n = inst.shape[1]
+    refs = torch.stack([d_y[:, :n], (d_x - d_y)[:, :n]])
+    ests = torch.stack([inst, voc])
+    return bsseval.bss_eval(refs, ests, window, hop, filters_len, device=dev, framewise=framewise)
 
 
 def dataset_medians(per_track):
@@ -101,7 +124,12 @@ def build_parser():
     p.add_argument('--split_mode', '-S', type=str, choices=['random', 'subdirs'], default='random')
     p.add_argument('--val_rate', '-v', type=float, default=0.2)
     p.add_argument('--val_filelist', '-V', type=str, default=None)
-    p.add_argument('--pretrained_model', '-P', type=str, required=True)
+    source = p.add_mutually_exclusive_group(required=True)
+    source.add_argument('--pretrained_model', '-P', type=str)
+    source.add_argument('--oracle', choices=spec_utils.ORACLES,
+                        help='score an oracle separation computed from the true stems instead of a checkpoint: the '
+                             'ideal amplitude mask (iam, the best mask the net can output), binary mask (ibm), ratio '
+                             'masks (irm1, irm2) or multichannel Wiener filter (mwf)')
     p.add_argument('--batchsize', '-B', type=int, default=4)
     p.add_argument('--cropsize', '-c', type=int, default=256)
     p.add_argument('--tta', '-t', action='store_true')
@@ -149,7 +177,14 @@ def main():
     args = p.parse_args()
 
     # argument and dataset errors come before the model is loaded
-    if not os.path.isfile(args.pretrained_model):
+    if args.oracle is not None:
+        # an oracle has no net: the flags that configure one are errors
+        for flag, name in ((args.tta, '--tta/-t'), (args.postprocess, '--postprocess/-p')):
+            if flag:
+                p.error('{} configures the net and cannot be used with --oracle'.format(name))
+        if args.oracle == 'mwf' and args.wiener_iterations > 0:
+            p.error('--oracle mwf is one Wiener filter iteration from the true stems: --wiener_iterations must be 0')
+    elif not os.path.isfile(args.pretrained_model):
         p.error('--pretrained_model: no such file: {}'.format(args.pretrained_model))
     if args.batchsize < 1:
         p.error('--batchsize must be at least 1')
@@ -179,18 +214,29 @@ def main():
         import torch.distributed as dist
         dist.init_process_group('gloo')   # only the per-frame values are exchanged, on the host
 
-    if rank == 0:
-        print('loading model...', end=' ')
     device = torch.device('cuda:{}'.format(index))
     torch.cuda.set_device(device)
-    model = nets.CascadedNet(args.n_fft, args.hop_length, 32, 128)
-    model.load_state_dict(torch.load(args.pretrained_model, map_location='cpu'))
-    model.to(device)
-    spec_utils.set_device(index)
-    if rank == 0:
-        print('done')
-    sp = inference.Separator(model, device, args.batchsize, args.cropsize, args.postprocess,
-                             wiener_iterations=args.wiener_iterations)
+    if args.oracle is not None:
+        # no checkpoint and no net context: the spectral context of (-f, -H) computes the oracle stems
+        spec_utils.set_device(index)
+
+        def score(X, y):
+            return score_oracle_pair(args.oracle, X, y, args.n_fft, args.hop_length, window, hop, args.filters_len,
+                                     args.framewise_filters, args.wiener_iterations)
+    else:
+        if rank == 0:
+            print('loading model...', end=' ')
+        model = nets.CascadedNet(args.n_fft, args.hop_length, 32, 128)
+        model.load_state_dict(torch.load(args.pretrained_model, map_location='cpu'))
+        model.to(device)
+        spec_utils.set_device(index)
+        if rank == 0:
+            print('done')
+        sp = inference.Separator(model, device, args.batchsize, args.cropsize, args.postprocess,
+                                 wiener_iterations=args.wiener_iterations)
+
+        def score(X, y):
+            return score_pair(sp, X, y, window, hop, args.filters_len, args.tta, args.framewise_filters)
 
     def report(i, result):
         X_path, y_path = filelist[i]
@@ -200,8 +246,7 @@ def main():
     for k, (X_path, y_path) in enumerate(dataset.shard_files(filelist, world, rank)):
         X, y = pair_waves(X_path, y_path, args.sr, index)
         try:
-            local_results.append(score_pair(sp, X, y, window, hop, args.filters_len, args.tta,
-                                            args.framewise_filters))
+            local_results.append(score(X, y))
         except ValueError as e:
             raise ValueError('{}: {}'.format(validate.pair_name(X_path, y_path), e)) from e
         if world == 1:
@@ -214,6 +259,8 @@ def main():
         print('median of {} pairs: {}'.format(len(results), format_values(dataset_medians(results))))
         if args.json is not None:
             info = {'sr': args.sr, 'window': window, 'hop': hop, 'filters_len': args.filters_len}
+            if args.oracle is not None:
+                info['oracle'] = args.oracle
             if args.framewise_filters:
                 info['framewise_filters'] = True
             if args.wiener_iterations > 0:

@@ -47,6 +47,7 @@ SIGNATURES = {
     'vr_spec_image': (c_i32, [c_vp, c_vp, c_fp, c_i64, c_vp, c_vp, c_vp]),
     'vr_vocal_image': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_vp, c_vp]),
     'vr_spec_sub': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_vp, c_vp]),
+    'vr_oracle_mask': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_i32, c_vp, c_vp]),
     'vr_validation_loss': (c_i32, [c_vp, c_vp, c_vp, c_i64, c_fp, c_vp, c_vp]),
     'vr_wiener': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp]),
     'vr_flac_scan': (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i32, c_vp, c_vp]),

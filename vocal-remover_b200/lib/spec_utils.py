@@ -184,6 +184,146 @@ def wiener(X_spec, y_spec, v_spec, iterations=1):
         return (d_y, d_v) if on_device else (d_y.cpu().numpy(), d_v.cpu().numpy())
 
 
+# evaluate.py --oracle (DESIGN.md §12): the masks vr_oracle_mask computes, by kind number, then the oracle MWF
+MASK_ORACLES = ('iam', 'ibm', 'irm1', 'irm2')
+ORACLES = MASK_ORACLES + ('mwf',)
+
+
+def current_device():
+    """The CUDA device of the module-level spectral functions (set_device)."""
+    return torch.device('cuda', _DEVICE_INDEX)
+
+
+def oracle_mask(X_spec, y_spec, kind):
+    """The instruments mask of an ideal separation (DESIGN.md §12), on the GPU (vr_oracle_mask): float32 (2, bins, T)
+    in [0, 1] from the mixture X_spec and the true instruments y_spec, each complex (2, bins, T); the vocals' mask is
+    ``1 - mask``.  ``kind`` is one of MASK_ORACLES: 'iam' clip(|Y| / |X|, 0, 1), 'ibm' the dominant source, 'irm1'
+    |Y| / (|Y| + |V|), 'irm2' |Y|^2 / (|Y|^2 + |V|^2), with V = X - Y.  Numpy arrays give a numpy array, CUDA tensors a
+    CUDA tensor; the inputs are not modified."""
+    if kind not in MASK_ORACLES:
+        raise ValueError('oracle_mask: kind must be one of %s, got %r' % (', '.join(MASK_ORACLES), kind))
+    on_device = torch.is_tensor(X_spec)
+    if torch.is_tensor(y_spec) != on_device:
+        raise TypeError('oracle_mask: X_spec and y_spec must both be numpy arrays or both CUDA tensors')
+    if not on_device:
+        X_spec, y_spec = np.asarray(X_spec), np.asarray(y_spec)
+    if X_spec.ndim != 3 or X_spec.shape[0] != 2 or X_spec.shape[2] < 1 or tuple(X_spec.shape) != tuple(y_spec.shape):
+        raise ValueError('oracle_mask: X_spec and y_spec must both have shape (2, bins, T >= 1), got %s and %s'
+                         % (tuple(X_spec.shape), tuple(y_spec.shape)))
+    bins, T = X_spec.shape[1], X_spec.shape[2]
+    ctx = _spectral_ctx(2 * (bins - 1), bins - 1)
+    dev = torch.device('cuda', ctx.device_index)
+    with torch.cuda.device(dev):
+        d_x, d_y = (_to_device(s, dev, 'oracle_mask') for s in (X_spec, y_spec))
+        mask = torch.empty((2, bins, T), dtype=torch.float32, device=dev)
+        ctx.check(ctx.lib.vr_oracle_mask(ctx.handle, _native.ptr(d_x), _native.ptr(d_y), T, MASK_ORACLES.index(kind),
+                                         _native.ptr(mask), _native.stream_ptr()), 'vr_oracle_mask')
+        return mask if on_device else mask.cpu().numpy()
+
+
+def _check_oracle(kind, wiener_iterations):
+    if kind not in ORACLES:
+        raise ValueError('oracle: kind must be one of %s, got %r' % (', '.join(ORACLES), kind))
+    if wiener_iterations < 0:
+        raise ValueError('oracle: wiener_iterations must be >= 0, got %d' % wiener_iterations)
+    if kind == 'mwf' and wiener_iterations > 0:
+        raise ValueError('oracle: mwf is one Wiener iteration from the true stems; wiener_iterations must be 0')
+
+
+def oracle_spectrograms(X_spec, y_spec, kind, wiener_iterations=0):
+    """The oracle estimates (y_spec, v_spec) of the mixture X_spec given the true instruments y_spec (DESIGN.md §12):
+    a mask oracle applies ``oracle_mask`` as the Separator applies the net's mask (vr_apply_mask), refined by
+    ``wiener_iterations`` of the Wiener filter; 'mwf' is one Wiener iteration (vr_wiener) started from the true stems
+    y_spec and X_spec - y_spec.  Numpy arrays give numpy arrays, CUDA tensors CUDA tensors; the inputs are not
+    modified."""
+    _check_oracle(kind, wiener_iterations)
+    on_device = torch.is_tensor(X_spec)
+    if torch.is_tensor(y_spec) != on_device:
+        raise TypeError('oracle_spectrograms: X_spec and y_spec must both be numpy arrays or both CUDA tensors')
+    if not on_device:
+        X_spec, y_spec = np.asarray(X_spec), np.asarray(y_spec)
+    if X_spec.ndim != 3 or X_spec.shape[0] != 2 or X_spec.shape[2] < 1 or tuple(X_spec.shape) != tuple(y_spec.shape):
+        raise ValueError('oracle_spectrograms: X_spec and y_spec must both have shape (2, bins, T >= 1), got %s and %s'
+                         % (tuple(X_spec.shape), tuple(y_spec.shape)))
+    bins = X_spec.shape[1]
+    ctx = _spectral_ctx(2 * (bins - 1), bins - 1)
+    dev = torch.device('cuda', ctx.device_index)
+    with torch.cuda.device(dev):
+        d_x, d_y = (_to_device(s, dev, 'oracle_spectrograms') for s in (X_spec, y_spec))
+        y, v = _oracle_specs(ctx, d_x, d_y, kind, wiener_iterations)
+        return (y, v) if on_device else (y.cpu().numpy(), v.cpu().numpy())
+
+
+def _oracle_specs(ctx, d_x, d_y, kind, wiener_iterations):
+    """oracle_spectrograms on device complex64 tensors, into new tensors."""
+    T = d_x.shape[2]
+    y, v = torch.empty_like(d_x), torch.empty_like(d_x)
+    if kind == 'mwf':
+        y.copy_(d_y)
+        ctx.check(ctx.lib.vr_spec_sub(ctx.handle, _native.ptr(d_x), _native.ptr(d_y), T, _native.ptr(v),
+                                      _native.stream_ptr()), 'vr_spec_sub')
+        iterations = 1
+    else:
+        mask = torch.empty(d_x.shape, dtype=torch.float32, device=d_x.device)
+        ctx.check(ctx.lib.vr_oracle_mask(ctx.handle, _native.ptr(d_x), _native.ptr(d_y), T, MASK_ORACLES.index(kind),
+                                         _native.ptr(mask), _native.stream_ptr()), 'vr_oracle_mask')
+        ctx.check(ctx.lib.vr_apply_mask(ctx.handle, _native.ptr(d_x), _native.ptr(mask), T, _native.ptr(y),
+                                        _native.ptr(v), _native.stream_ptr()), 'vr_apply_mask')
+        iterations = wiener_iterations
+    if iterations > 0:
+        ctx.check(ctx.lib.vr_wiener(ctx.handle, _native.ptr(d_x), _native.ptr(y), _native.ptr(v), T, iterations,
+                                    _native.stream_ptr()), 'vr_wiener')
+    return y, v
+
+
+def oracle_separate_wave(X, y, kind, n_fft=2048, hop_length=1024, wiener_iterations=0):
+    """The oracle stems (instruments, vocals), float32 (2, hop * (L // hop)) each, of the mixture wave X given the
+    true instruments wave y, both float32 (2, L), at the STFT (n_fft, hop_length) - what ``Separator.separate_wave``
+    returns with the net's mask replaced by the oracle's (DESIGN.md §12).  A mask oracle without the Wiener filter runs
+    the Separator's masked inverse STFT (vr_apply_mask_istft); otherwise both estimates of ``oracle_spectrograms`` are
+    inverted (vr_istft).  CUDA tensors give CUDA tensors, numpy arrays numpy arrays."""
+    _check_oracle(kind, wiener_iterations)
+    on_device = torch.is_tensor(X)
+    if torch.is_tensor(y) != on_device:
+        raise TypeError('oracle_separate_wave: X and y must both be numpy arrays or both CUDA tensors')
+    if tuple(X.shape) != tuple(y.shape) or len(X.shape) != 2 or X.shape[0] != 2 or X.shape[1] < 1:
+        raise ValueError('oracle_separate_wave: X and y must both have shape (2, L >= 1), got %s and %s'
+                         % (tuple(X.shape), tuple(y.shape)))
+    ctx = _spectral_ctx(n_fft, hop_length)
+    dev = torch.device('cuda', ctx.device_index)
+    with torch.cuda.device(dev):
+        waves = []
+        for w in (X, y):
+            if on_device:
+                if w.device != dev:
+                    raise ValueError('oracle_separate_wave: wave is on %s, the spectral functions use %s'
+                                     % (w.device, dev))
+                waves.append(w.contiguous().float())
+            else:
+                waves.append(torch.from_numpy(np.ascontiguousarray(np.asarray(w, dtype=np.float32))).to(dev))
+        L = waves[0].shape[1]
+        T = 1 + L // hop_length
+        d_x, d_y = (torch.empty((2, n_fft // 2 + 1, T), dtype=torch.complex64, device=dev) for _ in range(2))
+        for w, spec in zip(waves, (d_x, d_y)):
+            ctx.check(ctx.lib.vr_stft(ctx.handle, _native.ptr(w), L, _native.ptr(spec), T, None,
+                                      _native.stream_ptr()), 'vr_stft')
+        inst = torch.empty((2, hop_length * (T - 1)), dtype=torch.float32, device=dev)
+        voc = torch.empty_like(inst)
+        if kind in MASK_ORACLES and wiener_iterations == 0:
+            mask = torch.empty((2, n_fft // 2 + 1, T), dtype=torch.float32, device=dev)
+            ctx.check(ctx.lib.vr_oracle_mask(ctx.handle, _native.ptr(d_x), _native.ptr(d_y), T,
+                                             MASK_ORACLES.index(kind), _native.ptr(mask), _native.stream_ptr()),
+                      'vr_oracle_mask')
+            ctx.check(ctx.lib.vr_apply_mask_istft(ctx.handle, _native.ptr(d_x), _native.ptr(mask), T,
+                                                  _native.ptr(inst), _native.ptr(voc), _native.stream_ptr()),
+                      'vr_apply_mask_istft')
+        else:
+            for spec, wave_out in zip(_oracle_specs(ctx, d_x, d_y, kind, wiener_iterations), (inst, voc)):
+                ctx.check(ctx.lib.vr_istft(ctx.handle, _native.ptr(spec), T, _native.ptr(wave_out),
+                                           _native.stream_ptr()), 'vr_istft')
+        return (inst, voc) if on_device else (inst.cpu().numpy(), voc.cpu().numpy())
+
+
 def artifact_weights(frame_min, thres=0.05, min_range=64, fade_size=32):
     """Per-frame fade weight of ``merge_artifacts`` from the per-frame minimum of the mask over (channel, bin).
 
