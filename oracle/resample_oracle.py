@@ -47,17 +47,24 @@ def prepare(sr_orig, sr_new, filt=None):
     return interp_win, interp_delta, num_table, min(1.0, sample_ratio), sample_ratio
 
 
-def resample(x, sr_orig, sr_new, filt=None):
-    """x: (..., n) float array -> (..., int(n * sr_new / sr_orig)), same dtype (vectorised over the output instants)."""
+def resample(x, sr_orig, sr_new, filt=None, out_range=None, time_dtype=np.float64):
+    """x: (..., n) float array -> (..., int(n * sr_new / sr_orig)), same dtype (vectorised over the output instants).
+
+    out_range=(t0, t1) computes only the output samples [t0, t1) of that result, with the same arithmetic: a window of
+    a long signal costs memory in proportion to the window, not to the signal.  time_dtype is the type the output
+    instants are rounded to: resampy's float64, or float32 to see what a single-precision time register computes."""
     x = np.asarray(x)
     interp_win, interp_delta, num_table, scale, ratio = prepare(sr_orig, sr_new, filt)
     n_in = x.shape[-1]
     n_out = int(n_in * ratio)
     if n_out < 1:
         raise ValueError('Input signal length=%d is too small to resample from %s->%s' % (n_in, sr_orig, sr_new))
+    t0, t1 = (0, n_out) if out_range is None else (int(out_range[0]), int(out_range[1]))
+    if not 0 <= t0 <= t1 <= n_out:
+        raise ValueError('out_range [%d, %d) is outside the %d output samples' % (t0, t1, n_out))
     xf = x.reshape(-1, n_in).astype(np.float64)
-    y = np.zeros((xf.shape[0], n_out), np.float64)
-    t_out = np.arange(n_out) * (1.0 / ratio)
+    y = np.zeros((xf.shape[0], t1 - t0), np.float64)
+    t_out = (np.arange(t0, t1) * (1.0 / ratio)).astype(time_dtype).astype(np.float64)
     n = t_out.astype(np.int64)
     nwin = interp_win.shape[0]
     index_step = int(scale * num_table)
@@ -76,7 +83,7 @@ def resample(x, sr_orig, sr_new, filt=None):
             w = np.where(live, interp_win[idx] + eta * interp_delta[idx], 0.0)
             src = np.where(live, (n - i) if wing == 0 else (n + i + 1), 0)
             y += w[None, :] * xf[:, src]
-    return y.reshape(x.shape[:-1] + (n_out,)).astype(x.dtype)
+    return y.reshape(x.shape[:-1] + (t1 - t0,)).astype(x.dtype)
 
 
 def resample_literal(x, sr_orig, sr_new, filt=None):

@@ -34,6 +34,10 @@ CONFIGS = {
     'D1024': (DEFAULT, 0, 1024, 1, (0,)),
     'E': ((512, 256, 16, 32), 0, 192, 2, (0, 1)),    # generic kernel, staged decoders, LSTM HID 16 / 8
     'F': ((2048, 1024, 64, 128), 0, 256, 2, (0, 1)),  # dec1 with two N tiles: mask_out_kernel runs
+    'G1024': ((1024, 256, 32, 128), 0, 256, 2, (0, 1)),    # band height 256
+    'G4096': ((4096, 1024, 32, 128), 0, 256, 2, (0, 1)),   # band height 1024
+    'H144': (DEFAULT, 0, 144, 2, (0, 1)),   # the smallest cropsize: maps 144/72/36/18/9 wide tile for no wgmma kernel
+    'H320': (DEFAULT, 0, 320, 2, (0, 1)),   # maps 320/160/80/40/20 wide: no tiling either, no crop-mask fusion
 }
 OFFSET = 64
 DILATIONS = ((4, 2), (8, 4), (12, 6))   # lib/nets.py:10
@@ -42,6 +46,34 @@ FAMILY_MAX = {}                          # kernel family -> (largest ratio to it
 
 def _round_up(a, b):
     return (a + b - 1) // b * b
+
+
+def _on_tensor_cores(w, H, W, stride):
+    """whether the layer of weights w (Cout, Cin, k, k), stride `stride` and H x W output maps runs on a tensor-core
+    kernel.  Mirrors every TC_NONE exit of tc_choose (conv_tc.cu), which must be kept in step with it: a kernel size
+    other than 1 or 3, a stride other than 1 or 2, fewer than 4 output channels, maps that tile_geom does not split
+    into 128-pixel tiles, a tile taller or wider than 256 input pixels, and more output-channel tiles than the 256
+    bias floats every tensor-core kernel stages.  Any other layer runs on the CUDA-core kernel."""
+    cout, k = w.shape[0], w.shape[-1]
+    if k not in (1, 3) or stride not in (1, 2) or cout < 4:
+        return False
+    # tile_geom
+    if W >= 128:
+        if W % 128:
+            return False
+        Wt, Ht = 128, 1
+    else:
+        if 128 % W:
+            return False
+        Wt, Ht = W, min(128 // W, H)
+        if H % Ht or (128 // W) % Ht:
+            return False
+    if Wt * stride > 256 or Ht * stride > 256:
+        return False
+    # n_tiling of the generic and halo kernels (the row kernel's tiles fit exactly when these do)
+    cout16 = _round_up(cout, 16)
+    n_tiles = -(-cout16 // 128)
+    return n_tiles * _round_up(-(-cout16 // n_tiles), 16) <= 256
 
 
 class Checks:
@@ -68,7 +100,7 @@ class Checks:
             self.failed.append('%s: not exact' % name)
 
     def family(self, w, y, stride, dil):
-        if self.conv_mode == 1:
+        if self.conv_mode == 1 or not _on_tensor_cores(w, y.shape[-2], y.shape[-1], stride):
             return 'cuda-core'
         k, W = w.shape[-1], y.shape[-1]
         if k == 3 and stride == 1 and dil == 1:

@@ -64,33 +64,53 @@ def test_istft_matches_oracle_and_roundtrip(wave10):
 
 
 def test_frame_ranges_match_the_whole_track_calls(wave10):
-    """The shard-sized entry points of the multi-GPU path (vr_stft_range, vr_apply_mask_istft_range) on ONE GPU: frame
-    ranges with odd starts and lengths that are not multiples of the four frames a CTA of the n_fft = 2048 kernels
-    transforms must reproduce the whole-track calls exactly (the same kernels, other alignment / tail branches)."""
+    """The shard-sized entry points of the multi-GPU path (vr_stft_range, vr_normaliser_range,
+    vr_apply_mask_istft_range) on ONE GPU: frame ranges with odd starts and lengths that are not multiples of the four
+    frames a CTA of the n_fft = 2048 kernels transforms, the last one ending at the track's end, must reproduce the
+    whole-track calls exactly (the same kernels, other alignment / tail branches).  Every n_fft at hop n_fft / 2 (the
+    radix-2 kernels and the n_fft = 2048 ones), and n_fft = 2048 at hop 512, where each output sample reads four
+    frames and a range's first and last frames lie outside its own hops."""
     from lib import _native, spec_utils
-    ctx = spec_utils._spectral_ctx(2048, 1024)
     dev = _dev()
     L = wave10.shape[1]
-    T = 1 + L // 1024
     d_wave = torch.from_numpy(wave10).to(dev)
     st = _native.stream_ptr()
-    full = torch.empty((2, 1025, T), dtype=torch.complex64, device=dev)
-    ctx.check(ctx.lib.vr_stft(ctx.handle, _native.ptr(d_wave), L, _native.ptr(full), T, None, st), 'vr_stft')
-    part = torch.zeros_like(full)
-    for a, b in ((0, 3), (3, 10), (10, 11), (11, T - 5), (T - 5, T)):
-        ctx.check(ctx.lib.vr_stft_range(ctx.handle, _native.ptr(d_wave), L, _native.ptr(part), T, a, b, st), 'vr_stft_range')
-    assert torch.equal(torch.view_as_real(part), torch.view_as_real(full))
-    mask = torch.rand((2, 1025, T), device=dev)
-    Lo = 1024 * (T - 1)
-    ia, va = torch.empty((2, Lo), device=dev), torch.empty((2, Lo), device=dev)
-    ctx.check(ctx.lib.vr_apply_mask_istft(ctx.handle, _native.ptr(full), _native.ptr(mask), T, _native.ptr(ia),
-                                          _native.ptr(va), st), 'vr_apply_mask_istft')
-    ib, vb = torch.zeros_like(ia), torch.zeros_like(va)
-    for k0, k1 in ((0, 1), (1, 6), (6, 7), (7, T - 4), (T - 4, T - 1)):
-        ctx.check(ctx.lib.vr_apply_mask_istft_range(ctx.handle, _native.ptr(full), _native.ptr(mask), T, k0, k1,
-                                                    _native.ptr(ib), _native.ptr(vb), st), 'vr_apply_mask_istft_range')
-    torch.cuda.synchronize()
-    assert torch.equal(ia, ib) and torch.equal(va, vb)
+    g = torch.Generator(device=dev).manual_seed(5)
+    for n_fft, hop in [(n, n // 2) for n in (64, 128, 256, 512, 1024, 2048, 4096)] + [(2048, 512)]:
+        ctx = spec_utils._spectral_ctx(n_fft, hop)
+        T = 1 + L // hop
+        bins = n_fft // 2 + 1
+        full = torch.empty((2, bins, T), dtype=torch.complex64, device=dev)
+        ctx.check(ctx.lib.vr_stft(ctx.handle, _native.ptr(d_wave), L, _native.ptr(full), T, None, st), 'vr_stft')
+        part = torch.zeros_like(full)
+        ranges = ((0, 3), (3, 10), (10, 11), (11, T - 5), (T - 5, T))
+        for a, b in ranges:
+            ctx.check(ctx.lib.vr_stft_range(ctx.handle, _native.ptr(d_wave), L, _native.ptr(part), T, a, b, st),
+                      'vr_stft_range')
+        norm = torch.empty(1, device=dev)
+        ctx.check(ctx.lib.vr_normaliser(ctx.handle, _native.ptr(full), T, 0, _native.ptr(norm), st), 'vr_normaliser')
+        norms = torch.empty(len(ranges), device=dev)
+        for i, (a, b) in enumerate(ranges):
+            ctx.check(ctx.lib.vr_normaliser_range(ctx.handle, _native.ptr(full), T, a, b, _native.ptr(norms[i:]), st),
+                      'vr_normaliser_range')
+        mask = torch.rand((2, bins, T), device=dev, generator=g)
+        Lo = hop * (T - 1)
+        ia, va = torch.empty((2, Lo), device=dev), torch.empty((2, Lo), device=dev)
+        ctx.check(ctx.lib.vr_apply_mask_istft(ctx.handle, _native.ptr(full), _native.ptr(mask), T, _native.ptr(ia),
+                                              _native.ptr(va), st), 'vr_apply_mask_istft')
+        ib, vb = torch.zeros_like(ia), torch.zeros_like(va)
+        for k0, k1 in ((0, 1), (1, 6), (6, 7), (7, T - 4), (T - 4, T - 1)):
+            ctx.check(ctx.lib.vr_apply_mask_istft_range(ctx.handle, _native.ptr(full), _native.ptr(mask), T, k0, k1,
+                                                        _native.ptr(ib), _native.ptr(vb), st),
+                      'vr_apply_mask_istft_range')
+        torch.cuda.synchronize()
+        diff = max((part - full).abs().max().item(), (norms.max() - norm[0]).abs().item(),
+                   (ia - ib).abs().max().item(), (va - vb).abs().max().item())
+        record_parity('frame_ranges_nfft%d_hop%d_vs_whole_track' % (n_fft, hop), diff, 0.0)
+        assert torch.equal(torch.view_as_real(part), torch.view_as_real(full)), (n_fft, hop)
+        # the whole-track normaliser is the largest of the ranges' (hypotf in both kernels, no rounding in a max)
+        assert torch.equal(norms.max(), norm[0]), (n_fft, hop)
+        assert torch.equal(ia, ib) and torch.equal(va, vb), (n_fft, hop)
 
 
 def test_stft_ragged_and_small_fft():
@@ -345,6 +365,41 @@ def test_edge_lengths_vs_oracle(default_model, n_frames):
     inst, voc = sp.separate_wave(wave)
     assert inst.shape == (2, 1024 * (n_frames - 1))
     assert np.abs(inst + voc - wave[:, :inst.shape[1]]).max() < 1e-4
+
+
+@pytest.mark.parametrize('n_fft,hop,cropsize', [(1024, 256, 256), (4096, 1024, 256), (2048, 512, 144),
+                                                (2048, 512, 320)])
+def test_other_geometries_vs_oracle(n_fft, hop, cropsize):
+    """Band heights 256 and 1024, and the cropsizes whose maps tile for no tensor-core kernel (144, the smallest legal
+    one, keeps a 16-frame roi): the mask of a three-window track against the oracle, and separate_wave at a hop other
+    than n_fft / 2, whose stems must add up to the input.  The oracle's mask one frame late must miss the mask gate by
+    a wide factor, so the windows' placement is what the gate sees."""
+    import inference
+    from lib import nets, synth
+    from oracle import separator_oracle, stft_oracle
+    sd = synth.make_state_dict(n_fft, 32, 128)
+    model = nets.CascadedNet(n_fft, hop, 32, 128)
+    model.load_state_dict(synth.to_torch_state_dict(sd))
+    model.to(_dev())
+    roi = cropsize - 2 * 64
+    n_frames = 2 * roi + 5
+    L = hop * (n_frames - 1) + 100
+    wave = synth.sine_mix(L / 44100.0 + 0.01, seed=n_fft + cropsize)[:, :L]
+    X = stft_oracle.wave_to_spectrogram(wave, hop, n_fft)
+    assert X.shape == (2, n_fft // 2 + 1, n_frames)
+    ref = separator_oracle.separate_mask(synth.to_torch_state_dict(sd), X, n_fft=n_fft, cropsize=cropsize)
+    sp = inference.Separator(model, _dev(), 2, cropsize, False)
+    got = sp._mask_device(torch.from_numpy(X).cuda(), False).cpu().numpy()
+    assert got.shape == ref.shape
+    err = float(np.abs(got - ref).max())
+    record_parity('mask_nfft%d_crop%d_vs_oracle' % (n_fft, cropsize), err, MASK_TOL)
+    assert err < MASK_TOL
+    assert np.abs(ref[..., 1:] - ref[..., :-1]).max() > 10 * MASK_TOL
+    inst, voc = sp.separate_wave(wave)
+    assert inst.shape == voc.shape == (2, hop * (n_frames - 1))
+    recon = float(np.abs(inst + voc - wave[:, :inst.shape[1]]).max())
+    record_parity('stems_sum_nfft%d_hop%d_crop%d_vs_input' % (n_fft, hop, cropsize), recon, 1e-4)
+    assert recon < 1e-4
 
 
 def test_full_size_track_properties(default_model):

@@ -46,6 +46,39 @@ def test_small_fft_and_ragged_lengths():
         assert np.abs(w - x[:len(w)]).max() < 1e-5
 
 
+def test_istft_of_non_hermitian_spectra_matches_torch():
+    """Spectra whose DC and Nyquist rows have imaginary parts (no real signal has them): the oracle drops those parts
+    as a c2r transform does (np.fft.irfft, librosa.istft), which torch.istft / torch.fft.irfft confirm.  At hop = n_fft
+    torch.istft refuses the spectrum (the window-sum-square is zero at every frame's first sample), so there the frames
+    are inverted with torch.fft.irfft, windowed, and divided by the window square where it exceeds float32's tiny."""
+    rng = np.random.default_rng(5)
+    for n_fft, hop, T in ((64, 16, 40), (64, 64, 9), (4096, 1024, 9), (4096, 4096, 5)):
+        bins = n_fft // 2 + 1
+        S = (rng.standard_normal((bins, T)) + 1j * rng.standard_normal((bins, T))).astype(np.complex64)
+        S[[0, -1]] += 8j   # large imaginary DC and Nyquist
+        w = stft_oracle.istft(S, hop)
+        assert w.shape == (hop * (T - 1),)
+        win = torch.hann_window(n_fft, periodic=True, dtype=torch.float64)
+        St = torch.from_numpy(S).to(torch.complex128)
+        if hop < n_fft:
+            ref = torch.istft(St, n_fft, hop, window=win, center=True).numpy()
+        else:
+            frames = torch.fft.irfft(St, n_fft, dim=0) * win[:, None]
+            wsq = win * win
+            frames = torch.where((wsq > np.finfo(np.float32).tiny)[:, None], frames / wsq[:, None], frames)
+            ref = frames.T.reshape(-1)[n_fft // 2:n_fft // 2 + hop * (T - 1)].numpy()
+        assert ref.shape == w.shape
+        # relative to each sample's own size: at hop = n_fft the division by the window square scales samples by 1e7
+        err = np.abs(w - ref) / np.maximum(np.abs(ref), 1.0)
+        assert err.max() < 1e-6, (n_fft, hop, err.max())
+        # the gate resolves perturbations of the size of those imaginary parts: the Hermitian extension's complex
+        # inverse, real plus imaginary part (not what any c2r transform computes; its real part alone is the irfft)
+        full = np.concatenate([S, np.conj(S[-2:0:-1])]).astype(np.complex128)
+        z = np.fft.ifft(full, axis=0)
+        perturbed = stft_oracle.istft(np.fft.rfft(z.real + z.imag, axis=0), hop)
+        assert (np.abs(perturbed - ref) / np.maximum(np.abs(ref), 1.0)).max() > 1e-3
+
+
 def test_golden_spectrogram(golden_default):
     g = golden_default
     x = synth.sine_mix(10.0)

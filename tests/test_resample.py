@@ -45,6 +45,22 @@ def test_oracle_contract_and_scipy_anchor():
         ro.resample(np.zeros(10), 0, 8000)
 
 
+@pytest.mark.parametrize('rates', [(48000, 44100), (44100, 48000)])
+def test_oracle_output_range_matches_the_full_call(rates):
+    """out_range computes the same samples as the full call, to the bit, for windows at both ends (where the taps are
+    clipped by the signal) and inside; and it refuses a range outside the output."""
+    a, b = rates
+    x = np.stack([_tones(a, 0.1), _tones(a, 0.1, (1000.0, 3000.0, 7000.0))]).astype(np.float64)
+    full = ro.resample(x, a, b)
+    n_out = full.shape[-1]
+    for t0, t1 in ((0, 37), (0, 1), (1000, 1777), (n_out - 41, n_out), (n_out, n_out), (0, n_out)):
+        part = ro.resample(x, a, b, out_range=(t0, t1))
+        assert part.shape == (2, t1 - t0) and np.array_equal(part, full[:, t0:t1]), (t0, t1)
+    for bad in ((-1, 5), (5, 4), (0, n_out + 1)):
+        with pytest.raises(ValueError):
+            ro.resample(x, a, b, out_range=bad)
+
+
 def test_host_table_matches_oracle_table():
     sys.path.insert(0, os.path.join(ROOT, 'vocal-remover_b200'))
     from lib import audio_io
@@ -67,6 +83,33 @@ def test_gpu_resample_vs_oracle(rates):
     err = float(np.abs(y - ref).max())
     record_parity('resample_%d_%d' % (a, b), err, 2e-6)
     assert err < 2e-6      # fp64 accumulation on both sides, fp32 output
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('rates', [(48000, 44100), (44100, 48000)])
+def test_gpu_resample_four_minutes_vs_oracle(rates):
+    """A 4-minute stereo track, the length real input has: the output instant t / ratio reaches ~1.1e7 there, where a
+    float32 time register would keep no fraction at all.  Windows at the start, the middle and the end are compared
+    with the oracle over the same output range; the oracle with its output instants rounded to float32 must miss the
+    gate by a wide factor, so the windows see where the fractional table index comes from."""
+    from conftest import record_parity
+    from lib import audio_io
+    a, b = rates
+    seconds = 240.0
+    x = np.stack([_tones(a, seconds), _tones(a, seconds, (1000.0, 3000.0, 7000.0))])
+    y = audio_io.resample(x, a, b)
+    n_out = int(x.shape[1] * (float(b) / a))
+    assert y.shape == (2, n_out) and y.dtype == np.float32
+    x64 = x.astype(np.float64)
+    width = 4096
+    for where, t0 in (('start', 0), ('middle', n_out // 2 - width // 2 + 7), ('end', n_out - width)):
+        ref = ro.resample(x64, a, b, out_range=(t0, t0 + width))
+        err = float(np.abs(y[:, t0:t0 + width] - ref).max())
+        record_parity('resample_4min_%d_%d_%s' % (a, b, where), err, 2e-6)
+        assert err < 2e-6, (where, err)
+        # float32 instants miss by ~20x the gate at the start (t < 5000) and by ~4e4x from the middle on
+        wrong = ro.resample(x64, a, b, out_range=(t0, t0 + width), time_dtype=np.float32)
+        assert np.abs(wrong - ref).max() > (10 if where == 'start' else 1000) * 2e-6, where
 
 
 @pytest.mark.gpu
