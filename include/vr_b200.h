@@ -258,8 +258,13 @@ VR_API int vr_pcm_pack(vr_ctx* ctx, const float* x, int32_t channels, int64_t n,
  * scale = 2^-40, raised by 2^8 per retry for a system whose Cholesky factorisation meets a non-positive pivot (G is only
  * positive semidefinite), up to 2^-20; loading_host (HOST, may be NULL) receives the K + 1 scales used (all unknowns,
  * then source 0, 1, ...).  phase_ms (HOST, may be NULL) receives the CUDA-event times of {correlations, assembly +
- * Cholesky + solves, projections + frame sums, all}.  Synchronises the stream; the results are bit-identical from
- * call to call.  NaN or Inf in refs or ests, or a system still not factored at 2^-20, is an error.            */
+ * Cholesky + solves, projections + frame sums, all}; "all" runs from the start of the call to the end of its last
+ * projections, and alone includes the input check and the upload of the task list.  Synchronises the stream; the
+ * results are bit-identical from call to call.  NaN or Inf in refs or ests, or a system still not factored at 2^-20,
+ * is an error.
+ *
+ * Both calls run one host driver (csrc/bsseval.cu): this one scores the whole track as a single segment, the
+ * framewise one below scores each frame as a segment of its own, in batches.                                     */
 #define BSS_EVAL_MAX_SIGNALS 8
 #define BSS_EVAL_MAX_FILTER 1024
 VR_API int64_t vr_bss_eval_workspace(int32_t K, int32_t C, int64_t N, int32_t L, int64_t window, int64_t hop);
@@ -279,7 +284,7 @@ VR_API int vr_bss_eval(vr_ctx* ctx, const float* refs, const float* ests, int32_
  * the window + L - 1 samples of each frame's timeline and the source's channels; corr_host (may be NULL) each frame's
  * correlations [frames][M][2M][L] of its window samples; loading_host (may be NULL) each frame's K + 1 loading scales
  * [frames][K + 1], NaN for a frame in which a reference source or an estimate is all zeros (its systems are the
- * identity and are not factored); phase_ms as vr_bss_eval's, each phase summed over the batches.  Synchronises the
+ * identity and are not factored); phase_ms as vr_bss_eval's, the first three summed over the batches.  Synchronises the
  * stream; the results are bit-identical from call to call and for every frames_per_batch.  NaN or Inf in refs or
  * ests, or a system still not factored at 2^-20, is an error.                                                      */
 VR_API int64_t vr_bss_eval_framewise_workspace(int32_t K, int32_t C, int64_t N, int32_t L, int64_t window,

@@ -17,19 +17,28 @@ struct vr_ctx {
 
 static std::string g_create_err;
 
+// The calls that need no model (resampling, FLAC and PCM, BSS Eval) take a ctx that may be NULL: audio is usually
+// loaded, and stems scored, before a model context exists.  Such a call then runs on the calling thread's current
+// device, and its error message is read with vr_last_error(NULL).
 static int fail(vr_ctx* c, const std::string& m) {
-  if (c) c->err = m;
+  (c ? c->err : g_create_err) = m;
   return -1;
+}
+static void use_device(const vr_ctx* c) {
+  if (c && c->eng) cudaSetDevice(c->eng->cfg().device);
 }
 static int done(vr_ctx* c, bool ok) {
   if (ok) return 0;
   c->err = c->eng->err;
   return -1;
 }
+static int cuda_result(vr_ctx* c, const char* what, cudaError_t e) {
+  return e == cudaSuccess ? 0 : fail(c, std::string(what) + ": " + cudaGetErrorString(e));
+}
 // Every entry point that takes a context runs on the context's device ...
 #define CHECK_CTX(c)                  \
   if (!(c) || !(c)->eng) return -2;   \
-  cudaSetDevice((c)->eng->cfg().device);
+  use_device(c);
 // ... and one that runs the net needs its weights finalized.
 #define CHECK_NET(c) \
   CHECK_CTX(c)       \
@@ -236,110 +245,93 @@ int vr_wiener(vr_ctx* ctx, const void* spec, void* y_spec, void* v_spec, int64_t
 
 int vr_resample(vr_ctx* ctx, const float* x, int32_t channels, int64_t n_in, float* y, int64_t n_out, double sample_ratio,
                 const double* win, const double* delta, int32_t nwin, int32_t table_per_crossing, void* stream) {
-  // ctx may be NULL (audio is usually loaded before a model context exists): the call then runs on the calling
-  // thread's current device and its error message is read with vr_last_error(NULL)
-  auto bad = [&](const std::string& m) {
-    if (ctx) return fail(ctx, m);
-    g_create_err = m;
-    return -1;
-  };
-  if (!x || !y || !win || !delta) return bad("vr_resample: null pointer");
+  if (!x || !y || !win || !delta) return fail(ctx, "vr_resample: null pointer");
   if (n_out != (int64_t)((double)n_in * sample_ratio))
-    return bad("vr_resample: n_out must be int(n_in * sample_ratio) (resampy.core.resample)");
-  if (ctx && ctx->eng) cudaSetDevice(ctx->eng->cfg().device);
-  cudaError_t e = vr::launch_resample_sinc(x, channels, n_in, y, n_out, sample_ratio, win, delta, nwin, table_per_crossing,
-                                           (cudaStream_t)stream);
-  if (e != cudaSuccess) return bad(std::string("vr_resample: ") + cudaGetErrorString(e));
-  return 0;
-}
-
-// ctx may be NULL for the FLAC and PCM calls, as for vr_resample
-static int flac_result(vr_ctx* ctx, const char* what, cudaError_t e) {
-  if (e == cudaSuccess) return 0;
-  const std::string m = std::string(what) + ": " + cudaGetErrorString(e);
-  if (ctx) return fail(ctx, m);
-  g_create_err = m;
-  return -1;
+    return fail(ctx, "vr_resample: n_out must be int(n_in * sample_ratio) (resampy.core.resample)");
+  use_device(ctx);
+  return cuda_result(ctx, "vr_resample",
+                     vr::launch_resample_sinc(x, channels, n_in, y, n_out, sample_ratio, win, delta, nwin,
+                                              table_per_crossing, (cudaStream_t)stream));
 }
 
 int vr_flac_scan(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, int64_t begin, int64_t* cands, int32_t max_cands,
                  int32_t* count, void* stream) {
-  if (ctx && ctx->eng) cudaSetDevice(ctx->eng->cfg().device);
-  return flac_result(ctx, "vr_flac_scan",
+  use_device(ctx);
+  return cuda_result(ctx, "vr_flac_scan",
                      vr::launch_flac_scan(data, n_bytes, begin, cands, max_cands, count, (cudaStream_t)stream));
 }
 
 int vr_flac_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int64_t* frames, int32_t n_frames,
                    int32_t channels, int64_t n_samples, float* out, int64_t* status, void* stream) {
-  if (ctx && ctx->eng) cudaSetDevice(ctx->eng->cfg().device);
-  return flac_result(ctx, "vr_flac_decode",
+  use_device(ctx);
+  return cuda_result(ctx, "vr_flac_decode",
                      vr::launch_flac_decode(data, n_bytes, frames, n_frames, channels, n_samples, out, status,
                                             (cudaStream_t)stream));
 }
 
 int vr_flac_encode_analyse(vr_ctx* ctx, const float* x, int32_t channels, int64_t n, int32_t rate_code, int32_t bits,
                            void* pcm, int32_t* plan, void* stream) {
-  if (ctx && ctx->eng) cudaSetDevice(ctx->eng->cfg().device);
-  return flac_result(ctx, "vr_flac_encode_analyse",
+  use_device(ctx);
+  return cuda_result(ctx, "vr_flac_encode_analyse",
                      vr::launch_flac_encode_analyse(x, channels, n, rate_code, bits, pcm, plan, (cudaStream_t)stream));
 }
 
 int vr_flac_encode_pack(vr_ctx* ctx, const void* pcm, int32_t channels, int64_t n, int32_t bits, const int32_t* plan,
                         const int64_t* offsets, int32_t rate_code, int32_t rate_value, uint8_t* out, int32_t* status,
                         void* stream) {
-  if (ctx && ctx->eng) cudaSetDevice(ctx->eng->cfg().device);
-  return flac_result(ctx, "vr_flac_encode_pack",
+  use_device(ctx);
+  return cuda_result(ctx, "vr_flac_encode_pack",
                      vr::launch_flac_encode_pack(pcm, channels, n, bits, plan, offsets, rate_code, rate_value, out,
                                                  status, (cudaStream_t)stream));
 }
 
 int vr_pcm_pack(vr_ctx* ctx, const float* x, int32_t channels, int64_t n, int32_t bits, uint8_t* out, void* stream) {
-  if (ctx && ctx->eng) cudaSetDevice(ctx->eng->cfg().device);
-  return flac_result(ctx, "vr_pcm_pack", vr::launch_pcm_pack(x, channels, n, bits, out, (cudaStream_t)stream));
+  use_device(ctx);
+  return cuda_result(ctx, "vr_pcm_pack", vr::launch_pcm_pack(x, channels, n, bits, out, (cudaStream_t)stream));
+}
+
+static int64_t bss_workspace(bool framewise, int32_t K, int32_t C, int64_t N, int32_t L, int64_t window, int64_t hop,
+                             int32_t frames_per_batch) {
+  std::string err;
+  const int64_t bytes = vr::bss_eval_workspace(framewise, K, C, N, L, window, hop, frames_per_batch, err);
+  if (bytes < 0) fail(nullptr, err);
+  return bytes;
+}
+
+static int bss_run(vr_ctx* ctx, bool framewise, const float* refs, const float* ests, int32_t K, int32_t C, int64_t N,
+                   int32_t L, int64_t window, int64_t hop, int32_t frames_per_batch, void* workspace,
+                   int64_t workspace_bytes, double* frames_host, double* corr_host, double* loading_host,
+                   double* phase_ms, void* stream) {
+  use_device(ctx);
+  std::string err;
+  return vr::bss_eval(framewise, refs, ests, K, C, N, L, window, hop, frames_per_batch, workspace, workspace_bytes,
+                      frames_host, corr_host, loading_host, phase_ms, (cudaStream_t)stream, err)
+             ? 0
+             : fail(ctx, err);
 }
 
 int64_t vr_bss_eval_workspace(int32_t K, int32_t C, int64_t N, int32_t L, int64_t window, int64_t hop) {
-  std::string err;
-  const int64_t bytes = vr::bss_eval_workspace(K, C, N, L, window, hop, err);
-  if (bytes < 0) g_create_err = err;
-  return bytes;
+  return bss_workspace(false, K, C, N, L, window, hop, 1);
 }
 
 int vr_bss_eval(vr_ctx* ctx, const float* refs, const float* ests, int32_t K, int32_t C, int64_t N, int32_t L,
                 int64_t window, int64_t hop, void* workspace, int64_t workspace_bytes, double* frames_host,
                 double* corr_host, double* loading_host, double* phase_ms, void* stream) {
-  // ctx may be NULL, as for vr_resample
-  if (ctx && ctx->eng) cudaSetDevice(ctx->eng->cfg().device);
-  std::string err;
-  if (vr::bss_eval(refs, ests, K, C, N, L, window, hop, workspace, workspace_bytes, frames_host, corr_host,
-                   loading_host, phase_ms, (cudaStream_t)stream, err))
-    return 0;
-  if (ctx) return fail(ctx, err);
-  g_create_err = err;
-  return -1;
+  return bss_run(ctx, false, refs, ests, K, C, N, L, window, hop, 1, workspace, workspace_bytes, frames_host,
+                 corr_host, loading_host, phase_ms, stream);
 }
 
 int64_t vr_bss_eval_framewise_workspace(int32_t K, int32_t C, int64_t N, int32_t L, int64_t window, int64_t hop,
                                         int32_t frames_per_batch) {
-  std::string err;
-  const int64_t bytes = vr::bss_eval_framewise_workspace(K, C, N, L, window, hop, frames_per_batch, err);
-  if (bytes < 0) g_create_err = err;
-  return bytes;
+  return bss_workspace(true, K, C, N, L, window, hop, frames_per_batch);
 }
 
 int vr_bss_eval_framewise(vr_ctx* ctx, const float* refs, const float* ests, int32_t K, int32_t C, int64_t N,
                           int32_t L, int64_t window, int64_t hop, int32_t frames_per_batch, void* workspace,
                           int64_t workspace_bytes, double* frames_host, double* corr_host, double* loading_host,
                           double* phase_ms, void* stream) {
-  // ctx may be NULL, as for vr_bss_eval
-  if (ctx && ctx->eng) cudaSetDevice(ctx->eng->cfg().device);
-  std::string err;
-  if (vr::bss_eval_framewise(refs, ests, K, C, N, L, window, hop, frames_per_batch, workspace, workspace_bytes,
-                             frames_host, corr_host, loading_host, phase_ms, (cudaStream_t)stream, err))
-    return 0;
-  if (ctx) return fail(ctx, err);
-  g_create_err = err;
-  return -1;
+  return bss_run(ctx, true, refs, ests, K, C, N, L, window, hop, frames_per_batch, workspace, workspace_bytes,
+                 frames_host, corr_host, loading_host, phase_ms, stream);
 }
 
 int vr_shared_alloc(vr_ctx* ctx, int64_t bytes, void** dev_ptr, unsigned char* handle64) {

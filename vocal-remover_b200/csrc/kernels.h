@@ -142,16 +142,12 @@ cudaError_t launch_flac_encode_pack(const void* pcm, int channels, int64_t n, in
 cudaError_t launch_pcm_pack(const float* x, int channels, int64_t n, int bits, uint8_t* out, cudaStream_t stream);
 
 // ---- BSS Eval (bsseval.cu): workspace bytes, or -1 with err set; the whole evaluation of one track, synchronous ------
-int64_t bss_eval_workspace(int K, int C, int64_t N, int L, int64_t window, int64_t hop, std::string& err);
-bool bss_eval(const float* refs, const float* ests, int K, int C, int64_t N, int L, int64_t window, int64_t hop,
-              void* workspace, int64_t workspace_bytes, double* frames_host, double* corr_host, double* loading_host,
-              double* phase_ms, cudaStream_t stream, std::string& err);
-// framewise filters (BSS Eval v3): every frame scored as a signal of its own, frames_per_batch frames per batch
-int64_t bss_eval_framewise_workspace(int K, int C, int64_t N, int L, int64_t window, int64_t hop,
-                                     int64_t frames_per_batch, std::string& err);
-bool bss_eval_framewise(const float* refs, const float* ests, int K, int C, int64_t N, int L, int64_t window,
-                        int64_t hop, int64_t frames_per_batch, void* workspace, int64_t workspace_bytes,
-                        double* frames_host, double* corr_host, double* loading_host, double* phase_ms,
-                        cudaStream_t stream, std::string& err);
+// framewise: BSS Eval v3, every frame scored as a signal of its own, frames_per_batch frames per batch; otherwise one
+// set of filters for the whole track (v4), and frames_per_batch is not read
+int64_t bss_eval_workspace(bool framewise, int K, int C, int64_t N, int L, int64_t window, int64_t hop,
+                           int64_t frames_per_batch, std::string& err);
+bool bss_eval(bool framewise, const float* refs, const float* ests, int K, int C, int64_t N, int L, int64_t window,
+              int64_t hop, int64_t frames_per_batch, void* workspace, int64_t workspace_bytes, double* frames_host,
+              double* corr_host, double* loading_host, double* phase_ms, cudaStream_t stream, std::string& err);
 
 }  // namespace vr

@@ -133,31 +133,21 @@ def frame_sums(references, estimates, window, hop, filters_len=512, device=None,
                 frames_per_batch = framewise_batch(lib, K, C, N, window, hop, filters_len,
                                                    min(free // 4, WORKSPACE_CAP))
             frames_per_batch = int(frames_per_batch)
-            nbytes = lib.vr_bss_eval_framewise_workspace(K, C, N, filters_len, window, hop, frames_per_batch)
-            if nbytes < 0:
-                raise ValueError(lib.vr_last_error(None).decode())
-            ws = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
-            corr = np.empty((nwin, K * C, 2 * K * C, filters_len), dtype=np.float64) if correlations else None
-            loading = np.empty((nwin, K + 1), dtype=np.float64)
-            rc = lib.vr_bss_eval_framewise(None, _native.ptr(s), _native.ptr(e), K, C, N, filters_len, window, hop,
-                                           frames_per_batch, _native.ptr(ws), int(nbytes), sums.ctypes.data,
-                                           None if corr is None else corr.ctypes.data, loading.ctypes.data,
-                                           None if phase is None else phase.ctypes.data, _native.stream_ptr())
-            if rc != 0:
-                raise _native.NativeError('vr_bss_eval_framewise failed: %s' % lib.vr_last_error(None).decode())
+            name, batch, per_frame = 'vr_bss_eval_framewise', (frames_per_batch,), (nwin,)
         else:
-            nbytes = lib.vr_bss_eval_workspace(K, C, N, filters_len, window, hop)
-            if nbytes < 0:
-                raise ValueError(lib.vr_last_error(None).decode())
-            ws = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
-            corr = np.empty((K * C, 2 * K * C, filters_len), dtype=np.float64) if correlations else None
-            loading = np.empty(K + 1, dtype=np.float64)
-            rc = lib.vr_bss_eval(None, _native.ptr(s), _native.ptr(e), K, C, N, filters_len, window, hop,
-                                 _native.ptr(ws), int(nbytes), sums.ctypes.data,
-                                 None if corr is None else corr.ctypes.data, loading.ctypes.data,
-                                 None if phase is None else phase.ctypes.data, _native.stream_ptr())
-            if rc != 0:
-                raise _native.NativeError('vr_bss_eval failed: %s' % lib.vr_last_error(None).decode())
+            name, batch, per_frame = 'vr_bss_eval', (), ()
+        nbytes = getattr(lib, name + '_workspace')(K, C, N, filters_len, window, hop, *batch)
+        if nbytes < 0:
+            raise ValueError(lib.vr_last_error(None).decode())
+        ws = torch.empty(int(nbytes), dtype=torch.uint8, device=dev)
+        corr = np.empty(per_frame + (K * C, 2 * K * C, filters_len), dtype=np.float64) if correlations else None
+        loading = np.empty(per_frame + (K + 1,), dtype=np.float64)
+        rc = getattr(lib, name)(None, _native.ptr(s), _native.ptr(e), K, C, N, filters_len, window, hop, *batch,
+                                _native.ptr(ws), int(nbytes), sums.ctypes.data,
+                                None if corr is None else corr.ctypes.data, loading.ctypes.data,
+                                None if phase is None else phase.ctypes.data, _native.stream_ptr())
+        if rc != 0:
+            raise _native.NativeError('%s failed: %s' % (name, lib.vr_last_error(None).decode()))
     out = {'sums': sums, 'loading': loading}
     if framewise:
         out['frames_per_batch'] = frames_per_batch
