@@ -206,6 +206,32 @@ VR_API int vr_flac_scan(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, int64
 VR_API int vr_flac_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int64_t* frames, int32_t n_frames,
                           int32_t channels, int64_t n_samples, float* out, int64_t* status, void* stream);
 
+/* MPEG-1 Audio Layer III decoding on the device (ISO/IEC 11172-3, 32 / 44.1 / 48 kHz; lib/mp3.py is the caller,
+ * oracle/mp3_oracle.py restates the standard).  All buffers are DEVICE memory owned by the caller; no call allocates.
+ * ctx may be NULL, as for vr_flac_scan.
+ *
+ * vr_mp3_scan: every 11-bit frame sync at a byte offset in [begin, end - 4] of data.  Writes min(count, max_cands)
+ * rows of 2 int64, in no particular order: (offset, the 4 header bytes as a big-endian word); *count (one int32) is
+ * set to the number found.  Header fields are not judged: the host chains the frames and rejects what it does not take.
+ *
+ * vr_mp3_workspace: bytes of the workspace vr_mp3_decode needs for n_frames frames of channels (1 or 2) channels
+ * holding md_bytes bytes of main data in all (-1 for invalid arguments).
+ *
+ * vr_mp3_decode: frames: n_frames rows of 2 int64 (offset, header word) of consecutive MPEG-1 Layer III frames of one
+ * rate (rate_index 0 / 1 / 2 = 44.1 / 48 / 32 kHz) and one channel mode; md_off: n_frames + 1 int64, the exclusive
+ * scan of the frames' main-data byte counts (frame length less header, CRC and side info), md_off[n_frames] =
+ * md_bytes.  out: [channels][1152 * n_frames] float32, the synthesis output at full scale 1, not clipped, with zero
+ * filterbank state before the first frame.  status: one int64 per frame, 0 or code << 40 | bit offset (codes:
+ * lib/mp3.py); code 1 (main data begins before the first frame) is not an error: that frame decodes as an all-zero
+ * spectrum and the synthesis carries on through it.  Malformed bytes never fault: they give a status and zeros. */
+VR_API int64_t vr_mp3_workspace(int64_t n_frames, int32_t channels, int64_t md_bytes);
+VR_API int vr_mp3_scan(vr_ctx* ctx, const uint8_t* data, int64_t begin, int64_t end, int64_t* cands, int32_t max_cands,
+                       int32_t* count, void* stream);
+VR_API int vr_mp3_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int64_t* frames,
+                         const int64_t* md_off, int32_t n_frames, int32_t channels, int32_t rate_index,
+                         int64_t md_bytes, void* workspace, int64_t workspace_bytes, float* out, int64_t* status,
+                         void* stream);
+
 /* FLAC encoding on the device (RFC 9639 streamable subset; lib/flac.py is the caller, oracle/flac_oracle.py decodes
  * the result independently): fixed block size FLAC_ENCODE_BLOCK (the last block shorter), bits = 16 or 24 bits per
  * sample (anything else is an error), one or two channels.  All buffers are DEVICE memory owned by the caller; no call

@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(HERE, 'build')
 LIB = os.path.join(HERE, 'libvr_b200.so')
-SOURCES = ['api.cu', 'engine.cu', 'conv_simt.cu', 'conv_tc.cu', 'conv_tc_rows.cu', 'conv_tc_halo.cu', 'elementwise.cu', 'lstm.cu', 'fft.cu', 'resample.cu', 'flac.cu', 'flac_encode.cu', 'bsseval.cu', 'wiener.cu']
+SOURCES = ['api.cu', 'engine.cu', 'conv_simt.cu', 'conv_tc.cu', 'conv_tc_rows.cu', 'conv_tc_halo.cu', 'elementwise.cu', 'lstm.cu', 'fft.cu', 'resample.cu', 'flac.cu', 'flac_encode.cu', 'mp3.cu', 'bsseval.cu', 'wiener.cu']
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
          '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden', '--expt-relaxed-constexpr']

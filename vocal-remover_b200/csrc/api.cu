@@ -269,6 +269,26 @@ int vr_flac_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int6
                                             (cudaStream_t)stream));
 }
 
+int64_t vr_mp3_workspace(int64_t n_frames, int32_t channels, int64_t md_bytes) {
+  return vr::mp3_workspace_bytes(n_frames, channels, md_bytes);
+}
+
+int vr_mp3_scan(vr_ctx* ctx, const uint8_t* data, int64_t begin, int64_t end, int64_t* cands, int32_t max_cands,
+                int32_t* count, void* stream) {
+  use_device(ctx);
+  return cuda_result(ctx, "vr_mp3_scan", vr::launch_mp3_scan(data, begin, end, cands, max_cands, count,
+                                                             (cudaStream_t)stream));
+}
+
+int vr_mp3_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int64_t* frames, const int64_t* md_off,
+                  int32_t n_frames, int32_t channels, int32_t rate_index, int64_t md_bytes, void* workspace,
+                  int64_t workspace_bytes, float* out, int64_t* status, void* stream) {
+  use_device(ctx);
+  return cuda_result(ctx, "vr_mp3_decode",
+                     vr::launch_mp3_decode(data, n_bytes, frames, md_off, n_frames, channels, rate_index, md_bytes,
+                                           workspace, workspace_bytes, out, status, (cudaStream_t)stream));
+}
+
 int vr_flac_encode_analyse(vr_ctx* ctx, const float* x, int32_t channels, int64_t n, int32_t rate_code, int32_t bits,
                            void* pcm, int32_t* plan, void* stream) {
   use_device(ctx);

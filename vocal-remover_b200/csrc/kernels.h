@@ -130,6 +130,18 @@ cudaError_t launch_flac_scan(const uint8_t* data, int64_t n_bytes, int64_t begin
 cudaError_t launch_flac_decode(const uint8_t* data, int64_t n_bytes, const int64_t* frames, int n_frames, int channels,
                                int64_t n_samples, float* out, int64_t* status, cudaStream_t stream);
 
+// ---- MPEG-1 Layer III decoding (mp3.cu), the decode in front of the path for .mp3 input (lib/mp3.py) ---------------
+// scan: every 11-bit sync at byte offsets [begin, end - 4] -> cands[*count][2] = (offset, the 4 header bytes
+// big-endian); decode: frames[n_frames][2] = (offset, header word) of the chained frames, md_off[n_frames + 1] = the
+// exclusive scan of their main-data byte counts (md_bytes = md_off[n_frames]) -> out [channels][1152 * n_frames],
+// status[n_frames]; the workspace (mp3_workspace_bytes) holds the reservoir buffer and every intermediate
+int64_t mp3_workspace_bytes(int64_t n_frames, int channels, int64_t md_bytes);
+cudaError_t launch_mp3_scan(const uint8_t* data, int64_t begin, int64_t end, int64_t* cands, int max_cands, int* count,
+                            cudaStream_t stream);
+cudaError_t launch_mp3_decode(const uint8_t* data, int64_t n_bytes, const int64_t* frames, const int64_t* md_off,
+                              int n_frames, int channels, int rate_index, int64_t md_bytes, void* workspace,
+                              int64_t workspace_bytes, float* out, int64_t* status, cudaStream_t stream);
+
 // ---- FLAC frame encoding (flac_encode.cu), the encode behind --output_format flac (lib/flac.py) ----------------------
 // analyse: one CTA per 4096-sample frame of x [channels][n] -> pcm [n][channels] (int16 for bits = 16, int32 for 24),
 // plan [frames][192] int32 (the frame's size in bytes first); pack: plan + each frame's byte offset -> the frames' bytes

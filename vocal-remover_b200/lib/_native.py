@@ -52,6 +52,10 @@ SIGNATURES = {
     'vr_wiener': (c_i32, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_vp]),
     'vr_flac_scan': (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i32, c_vp, c_vp]),
     'vr_flac_decode': (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i32, c_i32, c_i64, c_fp, c_vp, c_vp]),
+    'vr_mp3_workspace': (c_i64, [c_i64, c_i32, c_i64]),
+    'vr_mp3_scan': (c_i32, [c_vp, c_vp, c_i64, c_i64, c_vp, c_i32, c_vp, c_vp]),
+    'vr_mp3_decode': (c_i32, [c_vp, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_i32, c_i64, c_vp, c_i64, c_fp, c_vp,
+                              c_vp]),
     'vr_flac_encode_analyse': (c_i32, [c_vp, c_fp, c_i32, c_i64, c_i32, c_i32, c_vp, c_vp, c_vp]),
     'vr_flac_encode_pack': (c_i32, [c_vp, c_vp, c_i32, c_i64, c_i32, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp]),
     'vr_pcm_pack': (c_i32, [c_vp, c_fp, c_i32, c_i64, c_i32, c_vp, c_vp]),

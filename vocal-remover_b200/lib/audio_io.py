@@ -1,9 +1,9 @@
 """Audio file I/O either side of the hot path (SURVEY 8(f) rank 2).
 
 The reference uses ``librosa.load(path, sr=sr, mono=False, dtype=np.float32, res_type='kaiser_fast')`` and
-``soundfile.write`` (inference.py:136-138,173,178).  FLAC input is decoded on the GPU when there is one (lib/flac.py,
-csrc/flac.cu) and FLAC output encoded on it (csrc/flac_encode.cu); other decoding and encoding stay on the host
-(soundfile when installed, else a stdlib ``wave``
+``soundfile.write`` (inference.py:136-138,173,178).  FLAC and MP3 input are decoded on the GPU when there is one
+(lib/flac.py, csrc/flac.cu; lib/mp3.py, csrc/mp3.cu) and FLAC output encoded on it (csrc/flac_encode.cu); other
+decoding and encoding stay on the host (soundfile when installed, else a stdlib ``wave``
 reader for 8/16/24/32-bit PCM WAV and writer for 16-bit), except the samples of a 24-bit WAV, which are quantised and
 packed on the GPU like the FLAC encoder's (``vr_pcm_pack``); the sample-rate conversion of non-``sr`` input - the
 expensive part of ``librosa.load`` - runs on the GPU (``vr_resample``, csrc/resample.cu): resampy 0.4's algorithm with the
@@ -76,14 +76,16 @@ def resample(y, orig_sr, target_sr, device=None, filt=None):
 
 
 def _decode(path, device=None):
-    """(channels, n) float32 at the file's own rate.  FLAC (recognised by content) is decoded on the GPU whenever a
-    CUDA device is visible (lib/flac.py); otherwise soundfile reads it if it is installed."""
-    from . import flac
+    """(channels, n) float32 at the file's own rate.  FLAC and MPEG-1 Layer III (recognised by content, FLAC first) are
+    decoded on the GPU whenever a CUDA device is visible (lib/flac.py, lib/mp3.py); otherwise soundfile reads them if
+    it is installed."""
+    from . import flac, mp3
     is_flac = flac.sniff(path)
-    if is_flac:
+    is_mp3 = not is_flac and mp3.sniff(path)
+    if is_flac or is_mp3:
         import torch
         if torch.cuda.is_available():
-            x, rate, _ = flac.decode(path, device)
+            x, rate, _ = (flac if is_flac else mp3).decode(path, device)
             return x.cpu().numpy(), rate
     try:
         import soundfile as sf
@@ -93,6 +95,9 @@ def _decode(path, device=None):
         pass
     if is_flac:
         raise RuntimeError('%s is a FLAC file: decoding it needs a CUDA device (lib/flac.py) or the soundfile module, '
+                           'and neither is available' % path)
+    if is_mp3:
+        raise RuntimeError('%s is an MP3 file: decoding it needs a CUDA device (lib/mp3.py) or the soundfile module, '
                            'and neither is available' % path)
     with _wave.open(path, 'rb') as f:
         nch, width, rate, nframes = f.getnchannels(), f.getsampwidth(), f.getframerate(), f.getnframes()
