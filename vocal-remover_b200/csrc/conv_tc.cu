@@ -12,9 +12,11 @@
 //     (bf16 x bf16 -> fp32 in registers).  Three passes per k-step, hi*hi + lo*hi + hi*lo, give a ~2^-16
 //     relative product error - the precision the 1e-3 mask gate needs (single-pass bf16/fp16 measurably
 //     fails it, DESIGN.md).
-//   * Warp-specialised persistent kernel: warp 8 is the TMA producer; the consumer warpgroups release a stage
-//     as soon as the wgmma group that read it has completed, then run the epilogue (bias -> ReLU/LeakyReLU ->
-//     split to bf16 hi/lo -> channel slice of the destination NHWC buffer, which is how concats are written in
+//   * The paired variants (PAIR_M / PAIR_N, DESIGN 5.3) run four consumer warpgroups that share one operand box
+//     per stage: two m-tiles share the weights, or both N tiles of a layer share the activations.
+//   * Warp-specialised persistent kernel: the warp after the consumers is the TMA producer; the consumer
+//     warpgroups release a stage as soon as the wgmma group that read it has completed, then run the epilogue
+//     (bias -> ReLU/LeakyReLU -> split to bf16 hi/lo -> 16-byte stores of 8 channels where the layout allows -> slice of the destination NHWC buffer, which is how concats are written in
 //     place) from registers while the producer already fills the ring for the next tile.
 #include <cuda.h>
 #include <stdio.h>
@@ -29,8 +31,11 @@
 namespace vr {
 
 static constexpr int kMaxStages = 8;
-static constexpr int kConsumerWarps = 8;                 // two warpgroups
-static constexpr int kThreads = 32 * kConsumerWarps + 32;   // + the TMA producer warp
+// two consumer warpgroups, or four in the paired variants (PAIR_M / PAIR_N), + the TMA producer warp
+__host__ __device__ constexpr int consumer_warps(int mode) { return mode == PAIR_NONE ? 8 : 16; }
+__host__ __device__ constexpr int tc_threads(int mode) { return 32 * consumer_warps(mode) + 32; }
+// channels of K per pipeline stage: 32 in the paired variants, so that at BN = 128 a stage is 48 KB and four fit
+__host__ __device__ constexpr int stage_k(int mode) { return mode == PAIR_NONE ? 64 : 32; }
 static constexpr int kStaticSmem = 2048;   // shared memory not given to the dynamic part: barriers and staged bias
 
 struct TcParams {
@@ -42,22 +47,41 @@ struct TcParams {
   int64_t osn, osh;
   int osw;
   const float* bias;
+  int vec16;   // the output planes and strides allow 16-byte stores of 8 channels
 };
 
+// bias + activation + split into bf16 hi / lo of the channel pair (c, c + 1) a thread holds: epilogue_pair's arithmetic
+__device__ __forceinline__ void act_split2(float v0, float v1, const float* bias_s, int c, float slope, uint32_t& hi,
+                                           uint32_t& lo) {
+  const float t0 = v0 + bias_s[c], t1 = v1 + bias_s[c + 1];
+  const float y0 = fmaxf(t0, 0.f) + slope * fminf(t0, 0.f);
+  const float y1 = fmaxf(t1, 0.f) + slope * fminf(t1, 0.f);
+  hi = f2_to_bf2(y0, y1);
+  const float2 hf = bf2_to_f2(hi);
+  lo = f2_to_bf2(y0 - hf.x, y1 - hf.y);
+}
+
 // ------------------------------------------------------------------------------------------------
-// KB: channels per operand sub-tile (64 / 32 / 16 = SWIZZLE_128B / 64B / 32B); a pipeline stage holds 64 / KB sub-tiles.
-// BN: output channels per tile (the wgmma N), a multiple of 16 up to 128.
-template <int KB, int BN>
-__global__ void __launch_bounds__(kThreads, 1)
+// KB: channels per operand sub-tile (64 / 32 / 16 = SWIZZLE_128B / 64B / 32B); a pipeline stage holds stage_k / KB
+// sub-tiles.  BN: output channels per tile (the wgmma N), a multiple of 16 up to 128.
+// MODE (TcPair): PAIR_NONE, a CTA unit is one 128-pixel x BN tile for two consumer warpgroups.  PAIR_M, a unit is the
+// m-tiles 2q and 2q + 1 of one N tile for four warpgroups (0-1 and 2-3), which share each B box.  PAIR_N, a unit is one
+// m-tile with both N tiles of a two-tile layer (warpgroups 0-1 and 2-3), which share each A box.  Every warpgroup
+// owns one 64-pixel x BN accumulator block and receives its products in the same order in all three.
+template <int KB, int BN, int MODE>
+__global__ void __launch_bounds__(tc_threads(MODE), 1)
     conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcParams p) {
-  constexpr int SUBS = 64 / KB;
+  constexpr int kConsumerWarps = consumer_warps(MODE);
+  constexpr int SUBS = stage_k(MODE) / KB;
+  constexpr int NA = MODE == PAIR_M ? 2 : 1;     // A boxes per sub-tile (m-tiles of a unit)
+  constexpr int NB = MODE == PAIR_N ? 2 : 1;     // B boxes per sub-tile (N tiles of a unit)
   constexpr int kSteps = KB / 16;
   constexpr uint32_t kAPlane = 128 * KB * 2;     // one plane of an A sub-tile (128 pixels x KB channels)
   constexpr uint32_t kASub = 2 * kAPlane;        // hi + lo
   constexpr uint32_t kBPlane = BN * KB * 2;
   constexpr uint32_t kBSub = 2 * kBPlane;
-  constexpr uint32_t kStageBytes = SUBS * (kASub + kBSub);
-  constexpr uint32_t kBRegion = SUBS * kASub;    // B sub-tiles follow the A sub-tiles inside a stage
+  constexpr uint32_t kStageBytes = SUBS * (NA * kASub + NB * kBSub);
+  constexpr uint32_t kBRegion = SUBS * NA * kASub;   // B sub-tiles follow the A sub-tiles inside a stage
   constexpr uint32_t kLayout = KB == 64 ? 1u : KB == 32 ? 2u : 3u;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_full[kMaxStages];
@@ -67,7 +91,9 @@ __global__ void __launch_bounds__(kThreads, 1)
   const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);   // provably warp-uniform: keeps wgmma unserialised
   const int lane = threadIdx.x & 31;
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const int total_tiles = p.m_tiles * p.n_tiles;
+  // units: m groups of NA m-tiles (the last one short when m_tiles is odd) x N groups of NB N tiles
+  const int n_units = p.n_tiles / NB;
+  const int total_units = (p.m_tiles + NA - 1) / NA * n_units;
   const int num_iters = (p.total_sub + SUBS - 1) / SUBS;
 
   if (warp == kConsumerWarps && lane == 0) {
@@ -83,27 +109,38 @@ __global__ void __launch_bounds__(kThreads, 1)
     // ===================== TMA producer (one elected lane runs the whole loop nest) =====================
     if (elect_one_sync()) {
       MbarRing ring(smem_u32(&bar_full[0]), smem_u32(&bar_empty[0]), 0, p.stages);
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int nt = tile % p.n_tiles;
-        const int mt = tile / p.n_tiles;
-        const int w0 = (mt % p.tiles_w) * p.Wt;
-        const int h0 = ((mt / p.tiles_w) % p.tiles_h) * p.Ht;
-        const int n0 = (mt / (p.tiles_w * p.tiles_h)) * p.Nt;
-        const int wbase = w0 * p.stride - p.pad_w, hbase = h0 * p.stride - p.pad_h;
-        const int nrow = nt * BN;
+      for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x) {
+        const int nt0 = unit % n_units * NB;
+        const int mt0 = unit / n_units * NA;
+        // the m-tiles of the unit that exist: a PAIR_M unit past the last m-tile loads (and its warpgroups store) nothing
+        const int na = min(NA, p.m_tiles - mt0);
+        int wbase[NA], hbase[NA], n0[NA];
+#pragma unroll
+        for (int a = 0; a < NA; ++a) {
+          const int mt = mt0 + a;
+          wbase[a] = (mt % p.tiles_w) * p.Wt * p.stride - p.pad_w;
+          hbase[a] = ((mt / p.tiles_w) % p.tiles_h) * p.Ht * p.stride - p.pad_h;
+          n0[a] = (mt / (p.tiles_w * p.tiles_h)) * p.Nt;
+        }
         int cc = 0, kw = 0, kh = 0, sub = 0;   // (tap, channel chunk) of the next sub-tile, advanced without divisions
         for (int it = 0; it < num_iters; ++it) {
           ring.wait_empty();
           const int nsub = min(SUBS, p.total_sub - sub);
           const uint32_t full = ring.full();
           const uint32_t sbase = smem_base + (uint32_t)ring.slot * kStageBytes;
-          mbar_expect_tx(full, (uint32_t)nsub * (kASub + kBSub));
+          mbar_expect_tx(full, (uint32_t)nsub * ((uint32_t)na * kASub + NB * kBSub));
 #pragma unroll
           for (int j = 0; j < SUBS; ++j) {
             if (j < nsub) {
-              tma_load_5d(sbase + (uint32_t)j * kASub, &tmA, cc * KB, wbase + kw * p.dil_w, hbase + kh * p.dil_h, n0, 0, full);
-              tma_load_3d(sbase + kBRegion + (uint32_t)j * kBSub, &tmB, (kh * p.KW + kw) * p.CinPadTC + cc * KB, nrow, 0,
-                          full);
+#pragma unroll
+              for (int a = 0; a < NA; ++a)
+                if (a < na)
+                  tma_load_5d(sbase + (uint32_t)(j * NA + a) * kASub, &tmA, cc * KB, wbase[a] + kw * p.dil_w,
+                              hbase[a] + kh * p.dil_h, n0[a], 0, full);
+#pragma unroll
+              for (int b = 0; b < NB; ++b)
+                tma_load_3d(sbase + kBRegion + (uint32_t)(j * NB + b) * kBSub, &tmB,
+                            (kh * p.KW + kw) * p.CinPadTC + cc * KB, (nt0 + b) * BN, 0, full);
               ++sub;
               if (++cc == p.cchunks) {
                 cc = 0;
@@ -121,12 +158,25 @@ __global__ void __launch_bounds__(kThreads, 1)
     __syncwarp();
   } else {
     // ===================== consumer warpgroups: wgmma into registers, then the epilogue =====================
-    const int wg = warp >> 2;   // pixels [64 wg, 64 wg + 64) of the tile
+    const int half = (warp >> 2) & 1;   // pixels [64 half, 64 half + 64) of its m-tile
+    const int pair = warp >> 3;         // which m-tile (PAIR_M) or N tile (PAIR_N) of the unit
+    const int a_sel = MODE == PAIR_M ? pair : 0, b_sel = MODE == PAIR_N ? pair : 0;
     const float slope = act_slope(p.act);
     const uint32_t dhi = desc_hi(8 * KB * 2, kLayout);
     MbarRing ring(smem_u32(&bar_full[0]), smem_u32(&bar_empty[0]), 0, p.stages);
     float acc[BN / 2];
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    for (int unit = blockIdx.x; unit < total_units; unit += gridDim.x) {
+      const int nt = unit % n_units * NB + b_sel;
+      const int mt = unit / n_units * NA + a_sel;
+      if (mt >= p.m_tiles) {
+        // the missing second m-tile of a PAIR_M unit: release every stage unread, store nothing
+        for (int it = 0; it < num_iters; ++it) {
+          ring.wait_full();
+          warp_arrive(ring.empty(), lane);
+          ring.advance();
+        }
+        continue;
+      }
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       HeldSlot held;
@@ -138,9 +188,9 @@ __global__ void __launch_bounds__(kThreads, 1)
 #pragma unroll
         for (int j = 0; j < SUBS; ++j) {
           if (j < nsub) {
-            const uint32_t a_hi = sdesc + ((j * kASub + (uint32_t)wg * (kAPlane / 2)) >> 4);
+            const uint32_t a_hi = sdesc + (((j * NA + a_sel) * kASub + (uint32_t)half * (kAPlane / 2)) >> 4);
             const uint32_t a_lo = a_hi + (kAPlane >> 4);
-            const uint32_t b_hi = sdesc + ((kBRegion + j * kBSub) >> 4);
+            const uint32_t b_hi = sdesc + ((kBRegion + (j * NB + b_sel) * kBSub) >> 4);
             const uint32_t b_lo = b_hi + (kBPlane >> 4);
 #pragma unroll
             for (int k = 0; k < kSteps; ++k)
@@ -156,32 +206,79 @@ __global__ void __launch_bounds__(kThreads, 1)
       wg_wait<0>();
       held.release_last(ring, lane);
 
-      const int nt = tile % p.n_tiles;
-      const int mt = tile / p.n_tiles;
       const int w0 = (mt % p.tiles_w) * p.Wt;
       const int h0 = ((mt / p.tiles_w) % p.tiles_h) * p.Ht;
       const int n0 = (mt / (p.tiles_w * p.tiles_h)) * p.Nt;
-      const int c_lane = nt * BN + 2 * (lane & 3);
+      const int q = lane & 3;
+      const int c_lane = nt * BN + 2 * q;
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
-        const int row = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
+        const int row = 64 * half + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
         const int dw = row % p.Wt;
         const int dh = (row / p.Wt) % p.Ht;
         const int n = n0 + row / (p.Wt * p.Ht);
-        if (n >= p.N) continue;
         const int64_t obase = (int64_t)n * p.osn + (int64_t)(h0 + dh) * p.osh + (int64_t)(w0 + dw) * p.osw;
+        // 16-byte stores where a warpgroup has registers to spare for the transpose (without them, the BN = 128 paired
+        // variants spill)
+        if constexpr (BN % 32 == 0 && (MODE == PAIR_NONE || BN <= 64)) {
+          const bool keep = n < p.N;
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j)
-          epilogue_pair(acc[4 * j + 2 * hr], acc[4 * j + 2 * hr + 1], bias_s, c_lane + 8 * j, p.Cout, slope,
-                        p.out_hi + obase, p.out_lo + obase);
+          for (int jb = 0; jb < BN / 8; jb += 4) {
+            if (p.vec16 && nt * BN + 8 * (jb + 4) <= p.Cout) {
+              // 32 channels of the pixel in one 16-byte store per plane and lane: the quad transposes its four
+              // 8-channel groups so that lane q holds group jb + q (every lane shuffles; rows past the batch store
+              // nothing)
+              uint32_t hi[4], lo[4], oh[4], ol[4];
+#pragma unroll
+              for (int g = 0; g < 4; ++g)
+                act_split2(acc[4 * (jb + g) + 2 * hr], acc[4 * (jb + g) + 2 * hr + 1], bias_s, c_lane + 8 * (jb + g),
+                           slope, hi[g], lo[g]);
+#pragma unroll
+              for (int s = 0; s < 4; ++s) {
+                const int gs = (q + s) & 3, src = (q - s) & 3;   // send group gs, receive group q from lane src
+                const uint32_t sh = gs == 0 ? hi[0] : gs == 1 ? hi[1] : gs == 2 ? hi[2] : hi[3];
+                const uint32_t sl = gs == 0 ? lo[0] : gs == 1 ? lo[1] : gs == 2 ? lo[2] : lo[3];
+                const uint32_t rh = __shfl_sync(0xffffffffu, sh, (lane & ~3) | src);
+                const uint32_t rl = __shfl_sync(0xffffffffu, sl, (lane & ~3) | src);
+#pragma unroll
+                for (int g = 0; g < 4; ++g)
+                  if (src == g) {
+                    oh[g] = rh;
+                    ol[g] = rl;
+                  }
+              }
+              if (keep) {
+                const int c = nt * BN + 8 * (jb + q);
+                *reinterpret_cast<uint4*>(p.out_hi + obase + c) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
+                *reinterpret_cast<uint4*>(p.out_lo + obase + c) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
+              }
+            } else if (keep) {
+#pragma unroll
+              for (int j = jb; j < jb + 4; ++j)
+                epilogue_pair(acc[4 * j + 2 * hr], acc[4 * j + 2 * hr + 1], bias_s, c_lane + 8 * j, p.Cout, slope,
+                              p.out_hi + obase, p.out_lo + obase);
+            }
+          }
+        } else {
+          if (n >= p.N) continue;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j)
+            epilogue_pair(acc[4 * j + 2 * hr], acc[4 * j + 2 * hr + 1], bias_s, c_lane + 8 * j, p.Cout, slope,
+                          p.out_hi + obase, p.out_lo + obase);
+        }
       }
     }
   }
 }
 
-// every (KB, BN) instantiation the host can launch
-#define VR_TC_FOR_BN(X, KB) X(KB, 16) X(KB, 32) X(KB, 48) X(KB, 64) X(KB, 80) X(KB, 96) X(KB, 112) X(KB, 128)
-#define VR_TC_FOR_ALL(X) VR_TC_FOR_BN(X, 64) VR_TC_FOR_BN(X, 32) VR_TC_FOR_BN(X, 16)
+// every (KB, BN, MODE) instantiation the host can launch.  The paired variants take KB = min(KB, 32) (pair_KB), and
+// PAIR_N the BN of two N tiles (129 to 256 output channels) at KB = 32.
+#define VR_TC_FOR_BN(X, KB, M) \
+  X(KB, 16, M) X(KB, 32, M) X(KB, 48, M) X(KB, 64, M) X(KB, 80, M) X(KB, 96, M) X(KB, 112, M) X(KB, 128, M)
+#define VR_TC_FOR_ALL(X)                                                                                   \
+  VR_TC_FOR_BN(X, 64, PAIR_NONE) VR_TC_FOR_BN(X, 32, PAIR_NONE) VR_TC_FOR_BN(X, 16, PAIR_NONE)             \
+  VR_TC_FOR_BN(X, 32, PAIR_M) VR_TC_FOR_BN(X, 16, PAIR_M)                                                  \
+  X(32, 80, PAIR_N) X(32, 96, PAIR_N) X(32, 112, PAIR_N) X(32, 128, PAIR_N)
 
 
 // ------------------------------------------------------------------------------------------------
@@ -199,8 +296,8 @@ const TcDevice& tc_device() {
     if (cudaDeviceGetAttribute(&d.max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&d.num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
       return none;
-#define VR_TC_SET_SMEM(KB, BN) \
-  cudaFuncSetAttribute(conv_tc_kernel<KB, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem - kStaticSmem);
+#define VR_TC_SET_SMEM(KB, BN, M) \
+  cudaFuncSetAttribute(conv_tc_kernel<KB, BN, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, d.max_smem - kStaticSmem);
     VR_TC_FOR_ALL(VR_TC_SET_SMEM)
 #undef VR_TC_SET_SMEM
     tc_rows_set_attributes(d.max_smem);
@@ -333,14 +430,15 @@ static unsigned long long weight_group_mask(const ConvLayer& L, const float* wp,
   return m;
 }
 
-// TMA map of the packed weights [2][rows][K]: boxes of KB channels x box_rows rows, both planes
-static bool encode_weight_map(TcConv& tc, int rows, int K, int box_rows, std::string& err, const std::string& name) {
+// TMA map of the packed weights [2][rows][K]: boxes of kb channels x box_rows rows, both planes
+static bool encode_weight_map(const TcConv& tc, CUtensorMap* map, int kb, int rows, int K, int box_rows,
+                              std::string& err, const std::string& name) {
   cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)rows, 2};
   cuuint64_t strides[2] = {(cuuint64_t)K * 2, (cuuint64_t)rows * K * 2};
-  cuuint32_t box[3] = {(cuuint32_t)tc.KB, (cuuint32_t)box_rows, 2};
+  cuuint32_t box[3] = {(cuuint32_t)kb, (cuuint32_t)box_rows, 2};
   cuuint32_t es[3] = {1, 1, 1};
-  CUresult r = tc_encode_fn()(&tc.map_b, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, tc.w_planes.get(), dims, strides, box, es,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(tc.KB), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+  CUresult r = tc_encode_fn()(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, tc.w_planes.get(), dims, strides, box, es,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(kb), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     err = "cuTensorMapEncodeTiled(weights) failed for " + name + " code " + std::to_string((int)r);
@@ -350,8 +448,9 @@ static bool encode_weight_map(TcConv& tc, int rows, int K, int box_rows, std::st
 }
 
 const CUtensorMap* tc_activation_map(TcConv& tc, const ActView& v, int bw, int bh, int bn, int es, std::string& err,
-                                     const std::string& name) {
-  const ViewKey key = std::make_tuple((const void*)v.hi, (const void*)v.lo, v.N, v.H, v.W, v.C, bw, bh, bn);
+                                     const std::string& name, int kb) {
+  if (kb == 0) kb = tc.KB;
+  const ViewKey key = std::make_tuple((const void*)v.hi, (const void*)v.lo, v.N, v.H, v.W, v.C, bw, bh, bn, kb);
   auto it = tc.map_a.find(key);
   if (it != tc.map_a.end()) return &it->second;
   // TMA reads 16-byte aligned rows; the lo plane is the box's outermost dimension
@@ -362,11 +461,11 @@ const CUtensorMap* tc_activation_map(TcConv& tc, const ActView& v, int bw, int b
   }
   cuuint64_t dims[5] = {(cuuint64_t)v.C, (cuuint64_t)v.W, (cuuint64_t)v.H, (cuuint64_t)v.N, 2};
   cuuint64_t strides[4] = {(cuuint64_t)v.sw * 2, (cuuint64_t)v.sh * 2, (cuuint64_t)v.sn * 2, (cuuint64_t)plane};
-  cuuint32_t box[5] = {(cuuint32_t)tc.KB, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bn, 2};
+  cuuint32_t box[5] = {(cuuint32_t)kb, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bn, 2};
   cuuint32_t estr[5] = {1, (cuuint32_t)es, (cuuint32_t)es, 1, 1};
   CUtensorMap m;
   CUresult r = tc_encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)v.hi, dims, strides, box, estr,
-                              CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(tc.KB), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_for(kb), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     err = "cuTensorMapEncodeTiled(activations) failed for " + name + " code " + std::to_string((int)r);
@@ -417,10 +516,33 @@ bool tc_prepare(ConvLayer& L, const float* w, const float* b, int H, int W, bool
   }
   if (!upload(tc->w_planes.get(), planes.data(), planes.size() * 2, err) ||
       !upload(tc->bias.get(), bias.data(), bias.size() * 4, err) ||
-      !encode_weight_map(*tc, brows, K, kind == TC_ROWS ? 3 * BN : BN, err, L.name))
+      !encode_weight_map(*tc, &tc->map_b, tc->KB, brows, K, kind == TC_ROWS ? 3 * BN : BN, err, L.name))
     return false;
+  if (kind == TC_GENERIC) {
+    // the paired variants stage 32 channels of K: a KB = 64 layer runs them in 32-channel boxes.  The k-steps, and so
+    // every accumulator's sum order, are the same in either box width.
+    tc->pair_KB = tc->KB < 32 ? tc->KB : 32;
+    tc->pair = tc->n_tiles == 2 && tc->pair_KB == 32 ? PAIR_N : PAIR_M;
+    if (!encode_weight_map(*tc, &tc->map_b_pair, tc->pair_KB, brows, K, BN, err, L.name)) return false;
+  }
   L.tc = tc;
   return true;
+}
+
+// The pairing of one generic-kernel launch.  Only layers with at most 32 channels per chunk and per N tile pair
+// automatically: on an H100 at 700 W (profiles/generic_conv.py, DESIGN 5.3) those ran 10-30 % faster paired, while the
+// wider layers ran from 6 % faster to 24 % slower, the KB = 64 ones (moved to 32-channel boxes) slowest.  A paired unit does the work of two tiles and takes about 1.9x as long
+// as one (the halo kernel's 256-pixel tiles measured the same), so pair only where that does not lose to the last wave
+// of the persistent grid: 1.9 x the paired waves <= the unpaired waves.  vr_debug_set(8, 1 / 2 / 3) pins none /
+// PAIR_M / PAIR_N where the layer allows it.
+static TcPair launch_pairing(const TcConv& tc, int m_tiles, int num_sms) {
+  if (g_debug.pair == 1) return PAIR_NONE;
+  if (g_debug.pair == 2) return PAIR_M;
+  if (g_debug.pair == 3) return tc.pair == PAIR_N ? PAIR_N : PAIR_NONE;
+  if (tc.KB > 32 || tc.BN > 32) return PAIR_NONE;
+  const int units = tc.pair == PAIR_N ? m_tiles : ceil_div(m_tiles, 2) * tc.n_tiles;
+  const int waves1 = ceil_div(m_tiles * tc.n_tiles, num_sms), waves2 = ceil_div(units, num_sms);
+  return 19 * waves2 <= 10 * waves1 ? tc.pair : PAIR_NONE;
 }
 
 cudaError_t tc_launch(const ConvLayer& L, const ActView& in, const ActView& out, cudaStream_t s, std::string& err,
@@ -436,10 +558,12 @@ cudaError_t tc_launch(const ConvLayer& L, const ActView& in, const ActView& out,
     return cudaErrorInvalidValue;
   }
   if (tc.kind == TC_HALO) return tc_halo_launch(L, tc, in, out, s, err);
+  const TcDevice& dv = tc_device();
+  if (!dv.ok) {
+    err = "tc_launch: cannot query the current device";
+    return cudaErrorInvalidValue;
+  }
   const TileGeom g = tile_geom(out.H, out.W);
-  const CUtensorMap* map_a = tc_activation_map(tc, in, g.Wt * L.stride, g.Ht * L.stride, g.Nt, L.stride, err, L.name);
-  if (!map_a) return cudaErrorInvalidValue;
-  const int SUBS = 64 / tc.KB;
   TcParams p;
   p.N = out.N; p.Ho = out.H; p.Wo = out.W;
   p.Wt = g.Wt; p.Ht = g.Ht; p.Nt = g.Nt;
@@ -449,14 +573,15 @@ cudaError_t tc_launch(const ConvLayer& L, const ActView& in, const ActView& out,
   p.stride = L.stride; p.dil_h = L.dil_h; p.dil_w = L.dil_w;
   p.pad_h = L.dil_h * (L.k / 2); p.pad_w = L.dil_w * (L.k / 2);
   p.KW = L.k;
-  p.cchunks = tc.chunks; p.total_sub = L.k * L.k * tc.chunks;
   p.CinPadTC = tc.CinPad; p.Cout = L.Cout; p.act = L.act;
-  const int stage_bytes = SUBS * (2 * 128 * tc.KB * 2 + 2 * tc.BN * tc.KB * 2);
-  const TcDevice& dv = tc_device();
-  if (!dv.ok) {
-    err = "tc_launch: cannot query the current device";
-    return cudaErrorInvalidValue;
-  }
+  const TcPair mode = launch_pairing(tc, p.m_tiles, dv.num_sms);
+  const int KB = mode == PAIR_NONE ? tc.KB : tc.pair_KB;
+  p.cchunks = tc.CinPad / KB; p.total_sub = L.k * L.k * p.cchunks;
+  const CUtensorMap* map_a = tc_activation_map(tc, in, g.Wt * L.stride, g.Ht * L.stride, g.Nt, L.stride, err, L.name, KB);
+  if (!map_a) return cudaErrorInvalidValue;
+  const CUtensorMap& map_b = mode == PAIR_NONE ? tc.map_b : tc.map_b_pair;
+  const int na = mode == PAIR_M ? 2 : 1, nb = mode == PAIR_N ? 2 : 1;
+  const int stage_bytes = stage_k(mode) / KB * (na * 2 * 128 * KB * 2 + nb * 2 * tc.BN * KB * 2);
   const int dyn = dv.max_smem - kStaticSmem;
   p.stages = (dyn - 1024) / stage_bytes;
   if (p.stages > kMaxStages) p.stages = kMaxStages;
@@ -466,13 +591,15 @@ cudaError_t tc_launch(const ConvLayer& L, const ActView& in, const ActView& out,
   }
   p.out_hi = out.hi; p.out_lo = out.lo;
   p.osn = out.sn; p.osh = out.sh; p.osw = out.sw;
+  p.vec16 = ((reinterpret_cast<uintptr_t>(out.hi) | reinterpret_cast<uintptr_t>(out.lo)) & 15) == 0 && out.sn % 8 == 0 &&
+            out.sh % 8 == 0 && out.sw % 8 == 0;
   p.bias = tc.bias.get();
-  const int total_tiles = p.m_tiles * p.n_tiles;
-  const int grid = total_tiles < dv.num_sms ? total_tiles : dv.num_sms;
-#define VR_TC_LAUNCH(KB_, BN_)                                                       \
-  if (tc.KB == KB_ && tc.BN == BN_) {                                                \
-    conv_tc_kernel<KB_, BN_><<<grid, kThreads, dyn, s>>>(*map_a, tc.map_b, p);       \
-    return cudaGetLastError();                                                       \
+  const int total_units = ceil_div(p.m_tiles, na) * (p.n_tiles / nb);
+  const int grid = total_units < dv.num_sms ? total_units : dv.num_sms;
+#define VR_TC_LAUNCH(KB_, BN_, M_)                                                          \
+  if (KB == KB_ && tc.BN == BN_ && mode == M_) {                                            \
+    conv_tc_kernel<KB_, BN_, M_><<<grid, tc_threads(M_), dyn, s>>>(*map_a, map_b, p);       \
+    return cudaGetLastError();                                                              \
   }
   VR_TC_FOR_ALL(VR_TC_LAUNCH)
 #undef VR_TC_LAUNCH

@@ -19,8 +19,12 @@ enum TcKind {
   TC_HALO,      // halo tile: 3x3, stride 1, dilation 1, W in {16, 32, 64} (conv_tc_halo.cu)
 };
 
-// activation view (hi, lo, N, H, W, C) and TMA box (W, H, N extents)
-typedef std::tuple<const void*, const void*, int, int, int, int, int, int, int> ViewKey;
+// How the generic kernel's four-warpgroup variants pair work in one CTA (conv_tc.cu, DESIGN §5.3):
+// PAIR_M: two adjacent 128-pixel m-tiles share each weight box; PAIR_N: both N tiles of a layer share each activation box.
+enum TcPair { PAIR_NONE = 0, PAIR_M = 1, PAIR_N = 2 };
+
+// activation view (hi, lo, N, H, W, C), TMA box (W, H, N extents) and channels per box
+typedef std::tuple<const void*, const void*, int, int, int, int, int, int, int, int> ViewKey;
 
 struct TcConv {
   TcKind kind = TC_NONE;
@@ -34,6 +38,12 @@ struct TcConv {
   DevPtr<float> bias;   // [n_tiles*BN]
   CUtensorMap map_b;
   std::map<ViewKey, CUtensorMap> map_a;
+  // generic kernel only: the pairing a launch considers (PAIR_N where n_tiles == 2 and KB >= 32, else PAIR_M; whether
+  // it pays depends on the batch, so tc_launch decides), and the weights in the paired variants' boxes of pair_KB
+  // channels.  PAIR_M is legal for every generic layer.
+  TcPair pair = PAIR_NONE;
+  int pair_KB = 0;
+  CUtensorMap map_b_pair;
   // What a launch of this plan can fuse (ConvFusion); the launchers reject anything else.
   // the row kernel can produce the leading up_C channels of its input as the x2 upsample of a half-resolution tensor
   bool fuses_upsample(int up_C) const { return kind == TC_ROWS && up_C % 32 == 0 && up_C <= CinPad; }
@@ -50,10 +60,10 @@ struct TcConv {
 };
 
 TcKind tc_choose(const ConvLayer& L, int H, int W, bool rows_wide);
-// tensor map of an activation view: both split-bf16 planes in one box of {tc.KB, bw, bh, bn, 2} elements, element
-// stride es along W and H; cached in the plan.  nullptr (err set) if TMA cannot read the view.
+// tensor map of an activation view: both split-bf16 planes in one box of {kb, bw, bh, bn, 2} elements (kb = 0:
+// tc.KB), element stride es along W and H; cached in the plan.  nullptr (err set) if TMA cannot read the view.
 const CUtensorMap* tc_activation_map(TcConv& tc, const ActView& v, int bw, int bh, int bn, int es, std::string& err,
-                                     const std::string& name);
+                                     const std::string& name, int kb = 0);
 
 // conv_tc_rows.cu
 cudaError_t tc_rows_launch(const ConvLayer& L, TcConv& tc, const ActView& in, const ActView& out, cudaStream_t s,
@@ -86,6 +96,8 @@ struct TcDebug {
   int kskip = 1;       // key 6 = 1 (default): the row and halo kernels skip channel groups whose weights are all zero
   int crop_mask = 1;   // key 7 = 1 (default): stage 3's dec1 computes only the kept frames and applies the output layer
                        // in its epilogue where it can; 0: it computes every frame into f3_, then mask_out_kernel runs
+  int pair = 0;        // key 8: generic kernel pairing, 0 = automatic, 1 = never (two warpgroups), 2 / 3 = PAIR_M /
+                       // PAIR_N in every launch where the layer allows it
 };
 extern TcDebug g_debug;
 
