@@ -376,8 +376,10 @@ VR_API int vr_debug_tensor(vr_ctx* ctx, const char* name, int32_t n0, int32_t n,
  * one, key 3 = 2 / 3 makes the halo-tile kernel use MB = 1 / 2, key 6 = 1 (default) skips channel groups whose weights
  * are all zero, key 7 = 1 (default) lets stage 3's last convolution compute only the frames the mask keeps and write
  * the mask itself (0: every frame, then a separate output-layer kernel), key 8 chooses the generic kernel's pairing
- * (0 = automatic per launch, 1 = never, 2 / 3 = two m-tiles / both N tiles per CTA wherever the layer allows it).
- * Returns -1 for any other key.                                                                                      */
+ * (0 = automatic per launch, 1 = never, 2 / 3 = two m-tiles / both N tiles per CTA wherever the layer allows it),
+ * key 9 chooses the epilogue stores of the three tensor-core kernels (0 = 16-byte stores of 8 channels wherever the
+ * output allows them, 1 = 4-byte stores of channel pairs everywhere; both write the same values).
+ * Returns -1 for any other key.                                                                                    */
 VR_API int vr_debug_set(int32_t key, int32_t value);
 /* timeline of CTA 0 of the last row-kernel launch made with vr_debug_set(0, 1): 3 roles x 2048 events x 3 clock64 stamps
  * (unused / TMA producer / interpolation warp 0), copied to HOST memory; returns the number of values or -1 */

@@ -443,7 +443,7 @@ int vr_debug_tensor(vr_ctx* ctx, const char* name, int32_t n0, int32_t n, float*
 int vr_debug_set(int32_t key, int32_t value) {
   int* knob = key == 0 ? &vr::g_debug.trace : key == 2 ? &vr::g_debug.rows_wide : key == 3 ? &vr::g_debug.halo
             : key == 6 ? &vr::g_debug.kskip : key == 7 ? &vr::g_debug.crop_mask
-            : key == 8 ? &vr::g_debug.pair : nullptr;
+            : key == 8 ? &vr::g_debug.pair : key == 9 ? &vr::g_debug.pair_stores : nullptr;
   if (!knob) return -1;
   *knob = value;
   return 0;

@@ -47,19 +47,8 @@ struct TcParams {
   int64_t osn, osh;
   int osw;
   const float* bias;
-  int vec16;   // the output planes and strides allow 16-byte stores of 8 channels
+  int vec16;   // 16-byte stores of 8 channels (tc_vec16)
 };
-
-// bias + activation + split into bf16 hi / lo of the channel pair (c, c + 1) a thread holds: epilogue_pair's arithmetic
-__device__ __forceinline__ void act_split2(float v0, float v1, const float* bias_s, int c, float slope, uint32_t& hi,
-                                           uint32_t& lo) {
-  const float t0 = v0 + bias_s[c], t1 = v1 + bias_s[c + 1];
-  const float y0 = fmaxf(t0, 0.f) + slope * fminf(t0, 0.f);
-  const float y1 = fmaxf(t1, 0.f) + slope * fminf(t1, 0.f);
-  hi = f2_to_bf2(y0, y1);
-  const float2 hf = bf2_to_f2(hi);
-  lo = f2_to_bf2(y0 - hf.x, y1 - hf.y);
-}
 
 // ------------------------------------------------------------------------------------------------
 // KB: channels per operand sub-tile (64 / 32 / 16 = SWIZZLE_128B / 64B / 32B); a pipeline stage holds stage_k / KB
@@ -209,64 +198,20 @@ __global__ void __launch_bounds__(tc_threads(MODE), 1)
       const int w0 = (mt % p.tiles_w) * p.Wt;
       const int h0 = ((mt / p.tiles_w) % p.tiles_h) * p.Ht;
       const int n0 = (mt / (p.tiles_w * p.tiles_h)) * p.Nt;
-      const int q = lane & 3;
-      const int c_lane = nt * BN + 2 * q;
+      // 16-byte stores where a warpgroup has registers to spare for the transpose (without them, the BN >= 80 paired
+      // variants spill); rows past the batch store nothing
+      constexpr bool kVec16 = MODE == PAIR_NONE || BN <= 64;
+      EpiDest d{p.out_hi, p.out_lo, {0, 0}, {false, false}, nt * BN, p.Cout, kVec16 && p.vec16};
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
         const int row = 64 * half + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
         const int dw = row % p.Wt;
         const int dh = (row / p.Wt) % p.Ht;
         const int n = n0 + row / (p.Wt * p.Ht);
-        const int64_t obase = (int64_t)n * p.osn + (int64_t)(h0 + dh) * p.osh + (int64_t)(w0 + dw) * p.osw;
-        // 16-byte stores where a warpgroup has registers to spare for the transpose (without them, the BN = 128 paired
-        // variants spill)
-        if constexpr (BN % 32 == 0 && (MODE == PAIR_NONE || BN <= 64)) {
-          const bool keep = n < p.N;
-#pragma unroll
-          for (int jb = 0; jb < BN / 8; jb += 4) {
-            if (p.vec16 && nt * BN + 8 * (jb + 4) <= p.Cout) {
-              // 32 channels of the pixel in one 16-byte store per plane and lane: the quad transposes its four
-              // 8-channel groups so that lane q holds group jb + q (every lane shuffles; rows past the batch store
-              // nothing)
-              uint32_t hi[4], lo[4], oh[4], ol[4];
-#pragma unroll
-              for (int g = 0; g < 4; ++g)
-                act_split2(acc[4 * (jb + g) + 2 * hr], acc[4 * (jb + g) + 2 * hr + 1], bias_s, c_lane + 8 * (jb + g),
-                           slope, hi[g], lo[g]);
-#pragma unroll
-              for (int s = 0; s < 4; ++s) {
-                const int gs = (q + s) & 3, src = (q - s) & 3;   // send group gs, receive group q from lane src
-                const uint32_t sh = gs == 0 ? hi[0] : gs == 1 ? hi[1] : gs == 2 ? hi[2] : hi[3];
-                const uint32_t sl = gs == 0 ? lo[0] : gs == 1 ? lo[1] : gs == 2 ? lo[2] : lo[3];
-                const uint32_t rh = __shfl_sync(0xffffffffu, sh, (lane & ~3) | src);
-                const uint32_t rl = __shfl_sync(0xffffffffu, sl, (lane & ~3) | src);
-#pragma unroll
-                for (int g = 0; g < 4; ++g)
-                  if (src == g) {
-                    oh[g] = rh;
-                    ol[g] = rl;
-                  }
-              }
-              if (keep) {
-                const int c = nt * BN + 8 * (jb + q);
-                *reinterpret_cast<uint4*>(p.out_hi + obase + c) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
-                *reinterpret_cast<uint4*>(p.out_lo + obase + c) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
-              }
-            } else if (keep) {
-#pragma unroll
-              for (int j = jb; j < jb + 4; ++j)
-                epilogue_pair(acc[4 * j + 2 * hr], acc[4 * j + 2 * hr + 1], bias_s, c_lane + 8 * j, p.Cout, slope,
-                              p.out_hi + obase, p.out_lo + obase);
-            }
-          }
-        } else {
-          if (n >= p.N) continue;
-#pragma unroll
-          for (int j = 0; j < BN / 8; ++j)
-            epilogue_pair(acc[4 * j + 2 * hr], acc[4 * j + 2 * hr + 1], bias_s, c_lane + 8 * j, p.Cout, slope,
-                          p.out_hi + obase, p.out_lo + obase);
-        }
+        d.obase[hr] = (int64_t)n * p.osn + (int64_t)(h0 + dh) * p.osh + (int64_t)(w0 + dw) * p.osw;
+        d.keep[hr] = n < p.N;
       }
+      epilogue_store<BN>(acc, bias_s, slope, lane, d);
     }
   }
 }
@@ -535,6 +480,12 @@ bool tc_prepare(ConvLayer& L, const float* w, const float* b, int H, int W, bool
 // as one (the halo kernel's 256-pixel tiles measured the same), so pair only where that does not lose to the last wave
 // of the persistent grid: 1.9 x the paired waves <= the unpaired waves.  vr_debug_set(8, 1 / 2 / 3) pins none /
 // PAIR_M / PAIR_N where the layer allows it.
+bool tc_vec16(const ActView& out) {
+  return g_debug.pair_stores != 1 &&
+         ((reinterpret_cast<uintptr_t>(out.hi) | reinterpret_cast<uintptr_t>(out.lo)) & 15) == 0 && out.sn % 8 == 0 &&
+         out.sh % 8 == 0 && out.sw % 8 == 0;
+}
+
 static TcPair launch_pairing(const TcConv& tc, int m_tiles, int num_sms) {
   if (g_debug.pair == 1) return PAIR_NONE;
   if (g_debug.pair == 2) return PAIR_M;
@@ -591,8 +542,7 @@ cudaError_t tc_launch(const ConvLayer& L, const ActView& in, const ActView& out,
   }
   p.out_hi = out.hi; p.out_lo = out.lo;
   p.osn = out.sn; p.osh = out.sh; p.osw = out.sw;
-  p.vec16 = ((reinterpret_cast<uintptr_t>(out.hi) | reinterpret_cast<uintptr_t>(out.lo)) & 15) == 0 && out.sn % 8 == 0 &&
-            out.sh % 8 == 0 && out.sw % 8 == 0;
+  p.vec16 = tc_vec16(out);
   p.bias = tc.bias.get();
   const int total_units = ceil_div(p.m_tiles, na) * (p.n_tiles / nb);
   const int grid = total_units < dv.num_sms ? total_units : dv.num_sms;

@@ -58,6 +58,7 @@ struct HaloParams {
   bf16* out_lo;
   int64_t osn, osh;
   int osw;
+  int vec16;   // 16-byte stores of 8 channels (tc_vec16)
   const float* bias;
 };
 
@@ -201,20 +202,21 @@ __global__ void __launch_bounds__(kThreads, 1)
       const int mt = tile / p.n_tiles;
       const int h0 = (mt % p.tiles_h) * p.Ht;
       const int n = mt / p.tiles_h;
-      const int c_lane = nt * BN + 2 * (lane & 3);
+      // 16-byte stores except at MB = 2, BN = 128, whose 128 accumulators leave too few registers for the transposes
+      // (they spill, DESIGN 5.7): that variant stores each pixel with 8-byte stores
+      constexpr bool kVec16 = !(MB == 2 && BN == 128);
 #pragma unroll
       for (int b = 0; b < MB; ++b) {
+        EpiDest d{p.out_hi, p.out_lo, {0, 0}, {true, true}, nt * BN, p.Cout, p.vec16 != 0};
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
           const int px = 64 * (MB * wg + b) + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
-          const int64_t obase =
-              (int64_t)n * p.osn + (int64_t)(h0 + (px >> p.lw)) * p.osh + (int64_t)(px & (p.W - 1)) * p.osw;
-          const float* v = acc + b * (BN / 2) + 2 * hr;
-#pragma unroll
-          for (int j = 0; j < BN / 8; ++j)
-            epilogue_pair(v[4 * j], v[4 * j + 1], bias_s, c_lane + 8 * j, p.Cout, slope, p.out_hi + obase,
-                          p.out_lo + obase);
+          d.obase[hr] = (int64_t)n * p.osn + (int64_t)(h0 + (px >> p.lw)) * p.osh + (int64_t)(px & (p.W - 1)) * p.osw;
+          if constexpr (!kVec16)
+            epilogue_pixel8<BN>(acc + b * (BN / 2) + 2 * hr, bias_s, nt * BN, p.Cout, slope, lane,
+                                p.out_hi + d.obase[hr], p.out_lo + d.obase[hr], d.vec16);
         }
+        if constexpr (kVec16) epilogue_store<BN>(acc + b * (BN / 2), bias_s, slope, lane, d);
       }
     }
   }
@@ -265,6 +267,7 @@ cudaError_t tc_halo_launch(const ConvLayer& L, TcConv& tc, const ActView& in, co
   p.kmask = g_debug.kskip == 1 ? tc.kmask : ~0ull;
   p.out_hi = out.hi; p.out_lo = out.lo;
   p.osn = out.sn; p.osh = out.sh; p.osw = out.sw;
+  p.vec16 = tc_vec16(out);
   p.bias = tc.bias.get();
   // the halo tile, both planes
   const CUtensorMap* map_a = tc_activation_map(tc, in, p.Wb, p.Ht + 2, 1, 1, err, L.name);

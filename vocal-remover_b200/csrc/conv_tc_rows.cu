@@ -91,6 +91,7 @@ struct RowsParams {
   bf16* out_lo;
   int64_t osn, osh;
   int osw;
+  int vec16;   // 16-byte stores of 8 channels (tc_vec16)
   const float* bias;
   // fused bilinear x2 producer for the first up_chunks chunks (0: everything comes from the TMA map)
   int up_chunks, xH, xW;
@@ -325,31 +326,48 @@ __global__ void __launch_bounds__(rows_threads(UP), 1)
       const RowsTile tl = rows_tile<R>(p, tile);
       const int w0 = tl.w0, h0 = tl.h0, n = tl.n;
       const int c_lane = tl.nt * BN + 2 * (lane & 3);
+      // this thread's share of the fused single-channel 1x1 convolution on pixel px of output row orow
+      auto dot = [&](const float* v, int orow, int px) {
+        float d = 0.f;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) d += dot_pair(v[4 * j], v[4 * j + 1], bias_s, dot_s, c_lane + 8 * j, slope);
+        d += __shfl_xor_sync(0xffffffffu, d, 1);
+        d += __shfl_xor_sync(0xffffffffu, d, 2);
+        if ((lane & 3) == 0) atomicAdd(p.dot_out + ((int64_t)n * p.H + (h0 + orow)) * p.W + (w0 + px), d);
+      };
+      const int px0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // pixel of fragment row m; row m + 8 is px0 + 8
 #pragma unroll
       for (int orow = 0; orow < R; ++orow) {
+        if constexpr (UP) {
+          // With the fused upsample the consumers hold 128 registers, next to the interpolation warps, and the
+          // transposes of the 16-byte stores spill there (DESIGN 5.2): these variants store each pixel with 8-byte stores,
+          // except at BN = 16, whose decoders (dec1 of stages 1 and 2) measured slower with them than with channel pairs.
+          constexpr bool kPixel8 = BN > 16;
 #pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-          const int px = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * hr;
-          const float* v = acc + orow * (BN / 2) + 2 * hr;
-          if constexpr (kMaskable) {
-            if (p.mask.out) {
-              mask_pixel<BN>(p, v, bias_s, dot_s, slope, lane, n, h0 + orow, w0 + px);
-              continue;
+          for (int hr = 0; hr < 2; ++hr) {
+            const int px = px0 + 8 * hr;
+            const float* v = acc + orow * (BN / 2) + 2 * hr;
+            if constexpr (kMaskable) {
+              if (p.mask.out) {
+                mask_pixel<BN>(p, v, bias_s, dot_s, slope, lane, n, h0 + orow, w0 + px);
+                continue;
+              }
             }
+            if (p.dot_out) dot(v, orow, px);
+            const int64_t obase = (int64_t)n * p.osn + (int64_t)(h0 + orow) * p.osh + (int64_t)(w0 + px) * p.osw;
+            epilogue_pixel8<BN>(v, bias_s, tl.nt * BN, p.Cout, slope, lane, p.out_hi + obase, p.out_lo + obase,
+                                kPixel8 && p.vec16 != 0);
           }
+        } else {
+          const float* v = acc + orow * (BN / 2);
           if (p.dot_out) {
-            float d = 0.f;
-#pragma unroll
-            for (int j = 0; j < BN / 8; ++j) d += dot_pair(v[4 * j], v[4 * j + 1], bias_s, dot_s, c_lane + 8 * j, slope);
-            d += __shfl_xor_sync(0xffffffffu, d, 1);
-            d += __shfl_xor_sync(0xffffffffu, d, 2);
-            if ((lane & 3) == 0) atomicAdd(p.dot_out + ((int64_t)n * p.H + (h0 + orow)) * p.W + (w0 + px), d);
+            dot(v, orow, px0);
+            dot(v + 2, orow, px0 + 8);
           }
-          const int64_t obase = (int64_t)n * p.osn + (int64_t)(h0 + orow) * p.osh + (int64_t)(w0 + px) * p.osw;
-#pragma unroll
-          for (int j = 0; j < BN / 8; ++j)
-            epilogue_pair(v[4 * j], v[4 * j + 1], bias_s, c_lane + 8 * j, p.Cout, slope, p.out_hi + obase,
-                          p.out_lo + obase);
+          const int64_t obase = (int64_t)n * p.osn + (int64_t)(h0 + orow) * p.osh + (int64_t)(w0 + px0) * p.osw;
+          const EpiDest d{p.out_hi, p.out_lo, {obase, obase + 8 * (int64_t)p.osw}, {true, true}, tl.nt * BN, p.Cout,
+                          p.vec16 != 0};
+          epilogue_store<BN>(v, bias_s, slope, lane, d);
         }
       }
     }
@@ -616,6 +634,7 @@ cudaError_t tc_rows_launch(const ConvLayer& L, TcConv& tc, const ActView& in, co
   p.chunks = tc.chunks; p.CinPadR = tc.CinPad; p.Cout = L.Cout; p.act = L.act;
   p.out_hi = out.hi; p.out_lo = out.lo;
   p.osn = out.sn; p.osh = out.sh; p.osw = out.sw;
+  p.vec16 = tc_vec16(out);
   p.bias = tc.bias.get();
   p.up_chunks = 0; p.xH = p.xW = 0;
   p.x_hi = p.x_lo = nullptr; p.xsn = p.xsh = 0; p.xsw = 0;

@@ -375,6 +375,136 @@ __device__ __forceinline__ void epilogue_pair(float v0, float v1, const float* b
   }
 }
 
+// bias + activation + split into bf16 hi / lo of the channel pair (c, c + 1) a thread holds: epilogue_pair's arithmetic
+__device__ __forceinline__ void act_split2(float v0, float v1, const float* bias_s, int c, float slope, uint32_t& hi,
+                                           uint32_t& lo) {
+  const float t0 = v0 + bias_s[c], t1 = v1 + bias_s[c + 1];
+  const float y0 = fmaxf(t0, 0.f) + slope * fminf(t0, 0.f);
+  const float y1 = fmaxf(t1, 0.f) + slope * fminf(t1, 0.f);
+  hi = f2_to_bf2(y0, y1);
+  const float2 hf = bf2_to_f2(hi);
+  lo = f2_to_bf2(y0 - hf.x, y1 - hf.y);
+}
+
+// The destination of one thread's two pixels of a 64-pixel accumulator block: the fragment rows m and m + 8 (pixel
+// halves hr = 0 / 1) at element offsets obase[hr] of the output planes, stored where keep[hr]; channel c0 + c of the
+// block is channel c of the pixel's slice, and those at or past Cout do not exist.  vec16: the planes are 16-byte
+// aligned and the strides multiples of 8 channels.
+struct EpiDest {
+  bf16* out_hi;
+  bf16* out_lo;
+  int64_t obase[2];
+  bool keep[2];
+  int c0, Cout;
+  bool vec16;
+};
+
+// One set of four (pixel half, 8-channel group) slots of the block: SPLIT = false, groups j0 .. j0 + 3 of pixel half hr;
+// SPLIT = true, groups j0 and j0 + 1 of both halves.  With 16-byte stores every lane of the quad that shares the pixels
+// computes its channel pair of each slot, the quad transposes them with four shuffles (every lane takes part) so that
+// lane q holds the 8 consecutive channels of slot q, and lane q stores them with one 16-byte store per plane if its
+// group lies below Cout.  A set with a group that straddles Cout, or a launch without vec16, takes epilogue_pair.
+template <bool SPLIT>
+__device__ __forceinline__ void epilogue_set(const float* v, const float* bias_s, float slope, int lane,
+                                             const EpiDest& d, int hr, int j0) {
+  const int q = lane & 3;
+  bool straddle = false;   // warp-uniform, as the shuffles need
+#pragma unroll
+  for (int s = 0; s < 4; ++s) {
+    const int c = d.c0 + 8 * (SPLIT ? j0 + (s & 1) : j0 + s);
+    straddle |= c < d.Cout && c + 8 > d.Cout;
+  }
+  if (d.vec16 && !straddle) {
+    uint32_t hi[4], lo[4], oh[4], ol[4];
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const int j = SPLIT ? j0 + (s & 1) : j0 + s, h = SPLIT ? s >> 1 : hr;
+      act_split2(v[4 * j + 2 * h], v[4 * j + 2 * h + 1], bias_s, d.c0 + 8 * j + 2 * q, slope, hi[s], lo[s]);
+    }
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const int gs = (q + s) & 3, src = (q - s) & 3;   // send slot gs, receive slot q from lane src
+      const uint32_t sh = gs == 0 ? hi[0] : gs == 1 ? hi[1] : gs == 2 ? hi[2] : hi[3];
+      const uint32_t sl = gs == 0 ? lo[0] : gs == 1 ? lo[1] : gs == 2 ? lo[2] : lo[3];
+      const uint32_t rh = __shfl_sync(0xffffffffu, sh, (lane & ~3) | src);
+      const uint32_t rl = __shfl_sync(0xffffffffu, sl, (lane & ~3) | src);
+#pragma unroll
+      for (int g = 0; g < 4; ++g)
+        if (src == g) {
+          oh[g] = rh;
+          ol[g] = rl;
+        }
+    }
+    const int h = SPLIT ? q >> 1 : hr;
+    const int c = d.c0 + 8 * (SPLIT ? j0 + (q & 1) : j0 + q);
+    if ((h ? d.keep[1] : d.keep[0]) && c + 8 <= d.Cout) {
+      const int64_t o = (h ? d.obase[1] : d.obase[0]) + c;
+      *reinterpret_cast<uint4*>(d.out_hi + o) = make_uint4(oh[0], oh[1], oh[2], oh[3]);
+      *reinterpret_cast<uint4*>(d.out_lo + o) = make_uint4(ol[0], ol[1], ol[2], ol[3]);
+    }
+  } else {
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const int j = SPLIT ? j0 + (s & 1) : j0 + s, h = SPLIT ? s >> 1 : hr;
+      if (h ? d.keep[1] : d.keep[0]) {
+        const int64_t o = h ? d.obase[1] : d.obase[0];
+        epilogue_pair(v[4 * j + 2 * h], v[4 * j + 2 * h + 1], bias_s, d.c0 + 8 * j + 2 * (lane & 3), d.Cout, slope,
+                      d.out_hi + o, d.out_lo + o);
+      }
+    }
+  }
+}
+
+// The store of one pixel with 8-byte stores, for the variants that have no registers to spare for epilogue_store's
+// transposes.  v: this lane's accumulators of the pixel (channels c0 + 8 j + 2 (lane % 4) + {0, 1} in v[4 j], v[4 j + 1]),
+// out_hi / out_lo: the pixel's channel 0.  For each pair of groups j, j + 1 the lanes q and q ^ 1 swap one channel pair
+// (one shuffle per plane): an even lane then holds channels 2 q .. 2 q + 3 of group j, an odd lane channels
+// 2 (q - 1) .. 2 q + 1 of group j + 1, and each writes its four with one 8-byte store per plane.  The quad so writes the
+// 16 channels of both groups, 32 bytes per plane, in one instruction instead of four half-sector ones.  The store rules
+// and the values are those of epilogue_store: a lane stores only where its group lies below Cout, and a pair with a
+// group straddling Cout, or a launch without vec16, takes epilogue_pair.
+template <int BN>
+__device__ __forceinline__ void epilogue_pixel8(const float* v, const float* bias_s, int c0, int Cout, float slope,
+                                                int lane, bf16* out_hi, bf16* out_lo, bool vec16) {
+  const int q = lane & 3;
+  const bool odd = q & 1;
+#pragma unroll
+  for (int j = 0; j < BN / 8; j += 2) {
+    const int cj = c0 + 8 * j;
+    const bool straddle = (cj < Cout && cj + 8 > Cout) || (cj + 8 < Cout && cj + 16 > Cout);   // warp-uniform
+    if (vec16 && !straddle) {
+      uint32_t h0, l0, h1, l1;
+      act_split2(v[4 * j], v[4 * j + 1], bias_s, cj + 2 * q, slope, h0, l0);
+      act_split2(v[4 * j + 4], v[4 * j + 5], bias_s, cj + 8 + 2 * q, slope, h1, l1);
+      // an even lane keeps group j and sends group j + 1, an odd lane the reverse
+      const uint32_t rh = __shfl_xor_sync(0xffffffffu, odd ? h0 : h1, 1);
+      const uint32_t rl = __shfl_xor_sync(0xffffffffu, odd ? l0 : l1, 1);
+      const int g = odd ? cj + 8 : cj;   // first channel of the lane's group
+      if (g + 8 <= Cout) {
+        const int c = odd ? g + 2 * (q - 1) : g + 2 * q;
+        *reinterpret_cast<uint2*>(out_hi + c) = odd ? make_uint2(rh, h1) : make_uint2(h0, rh);
+        *reinterpret_cast<uint2*>(out_lo + c) = odd ? make_uint2(rl, l1) : make_uint2(l0, rl);
+      }
+    } else {
+      epilogue_pair(v[4 * j], v[4 * j + 1], bias_s, cj + 2 * q, Cout, slope, out_hi, out_lo);
+      epilogue_pair(v[4 * j + 4], v[4 * j + 5], bias_s, cj + 8 + 2 * q, Cout, slope, out_hi, out_lo);
+    }
+  }
+}
+
+// The epilogue of one thread's share of a 64 x BN accumulator block v[BN / 2] (the Wgmma fragment): bias, activation
+// and split-bf16 store of both its pixels.  The slot sets are four groups of one pixel half where BN % 32 == 0; where
+// BN % 32 == 16 the last two groups of both halves form one more set.  The three wgmma kernels store through it.
+template <int BN>
+__device__ __forceinline__ void epilogue_store(const float* v, const float* bias_s, float slope, int lane,
+                                               const EpiDest& d) {
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+    for (int j0 = 0; j0 + 4 <= BN / 8; j0 += 4) epilogue_set<false>(v, bias_s, slope, lane, d, hr, j0);
+  if constexpr (BN % 32 == 16) epilogue_set<true>(v, bias_s, slope, lane, d, 0, BN / 8 - 2);
+}
+
 // 8-channel groups of chunk cc that carry any non-zero weight (4 bits per 32-channel chunk)
 __device__ __forceinline__ uint32_t chunk_groups(unsigned long long kmask, int cc) {
   const int sh = cc * 4;

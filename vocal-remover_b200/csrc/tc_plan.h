@@ -98,7 +98,13 @@ struct TcDebug {
                        // in its epilogue where it can; 0: it computes every frame into f3_, then mask_out_kernel runs
   int pair = 0;        // key 8: generic kernel pairing, 0 = automatic, 1 = never (two warpgroups), 2 / 3 = PAIR_M /
                        // PAIR_N in every launch where the layer allows it
+  int pair_stores = 0;   // key 9: 0 = 16-byte epilogue stores wherever the launch allows them, 1 = epilogue_pair's
+                         // 4-byte channel-pair stores in every launch
 };
 extern TcDebug g_debug;
+
+// The epilogue of a launch into `out` may store 8 channels with one 16-byte store per plane (epilogue_store,
+// tc_common.cuh): both planes are 16-byte aligned, every stride is a multiple of 8 channels, and key 9 is not 1.
+bool tc_vec16(const ActView& out);
 
 }  // namespace vr
