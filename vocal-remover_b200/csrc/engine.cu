@@ -872,8 +872,12 @@ bool Engine::istft(const float2* spec, const float* mask, int64_t T, float* wave
   return istft_range(spec, mask, T, 0, T - 1, wave_a, wave_b, s);
 }
 
+// Frames past its own index that output hop k reads: its last sample, hop*k + hop - 1, lies at hop*k + hop - 1 + NF/2
+// in the centre-padded signal, and the last window reaching that is frame k + ceil(NF / (2*hop)).
+int64_t Engine::istft_lookahead() const { return (cfg_.n_fft / 2 + cfg_.hop - 1) / cfg_.hop; }
+
 // Output hops [k0, k1) (samples [hop*k0, hop*k1)) of wave [2][hop*(T-1)]; reads frames of spec / mask that overlap
-// them (k0 - n_fft/hop/2 + 1 .. k1 + n_fft/hop/2 - 1 clipped to the track; k0..k1 for hop = n_fft/2).
+// them (k0 + 1 - istft_lookahead() .. k1 - 1 + istft_lookahead() clipped to the track; k0..k1 for hop = n_fft/2).
 // wave_a / wave_b may point into another GPU's memory (peer-mapped).
 bool Engine::istft_range(const float2* spec, const float* mask, int64_t T, int64_t k0, int64_t k1, float* wave_a,
                          float* wave_b, cudaStream_t s) {
@@ -883,10 +887,10 @@ bool Engine::istft_range(const float2* spec, const float* mask, int64_t T, int64
   }
   if (k1 == k0) return true;
   const int NF = cfg_.n_fft, hop = cfg_.hop;
-  // first / last frame touching samples [hop*k0, hop*k1): u = s + NF/2, frames ceil((u-NF+1)/hop) .. floor(u/hop)
+  // first frame touching samples [hop*k0, hop*k1): u = s + NF/2, frames ceil((u-NF+1)/hop) .. floor(u/hop)
   int64_t f0 = ((int64_t)hop * k0 + NF / 2 - NF + hop) / hop;
   if ((int64_t)hop * k0 + NF / 2 - NF + 1 <= 0) f0 = 0;
-  int64_t f1 = ((int64_t)hop * k1 - 1 + NF / 2) / hop;
+  int64_t f1 = k1 - 1 + istft_lookahead();
   if (f1 > T - 1) f1 = T - 1;
   const int64_t nfr = f1 - f0 + 1;
   if (!ck(ws_frames_.ensure((int64_t)4 * nfr * NF), "workspace frames")) return false;
@@ -930,8 +934,9 @@ bool Engine::separate_wave_host(const float* wave, int64_t L, int tta, float* in
   int64_t k_done = 0;
   bool ok = true;
   auto flush = [&](int64_t f) -> bool {
-    // output hop k needs mask frames k and k+1
-    int64_t k1 = f >= T ? T - 1 : f - 1;
+    // mask frames [0, f) are final: output hop k is finished once k + istft_lookahead() < f (k + 1 < f for
+    // hop = n_fft/2); frames from f on may still hold the previous track's mask, or only the first pass of --tta
+    int64_t k1 = f >= T ? T - 1 : f - istft_lookahead();
     if (k1 <= k_done) return true;
     if (!istft_range(spec, mask, T, k_done, k1, d_inst, d_voc, s)) return false;
     if (!ck(cudaEventRecord(ev_span_, s), "span event") || !ck(cudaStreamWaitEvent(s_copy_, ev_span_, 0), "span wait"))

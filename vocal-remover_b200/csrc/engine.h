@@ -185,6 +185,8 @@ class Engine {
   bool normaliser_range(const float2* spec, int64_t T, int64_t t0, int64_t t1, float* out, cudaStream_t s);
   bool istft_range(const float2* spec, const float* mask, int64_t T, int64_t k0, int64_t k1, float* wave_a,
                    float* wave_b, cudaStream_t s);
+  // frames past its own index that output hop k of the inverse STFT reads: ceil(n_fft / (2*hop))
+  int64_t istft_lookahead() const;
   bool predict_mask(const float* mag, int N, float* mask_out, int offset, cudaStream_t s);
   // windows [first, first+count) of the padded spectrogram -> mask frames; see include/vr_b200.h
   bool separate_windows(const float2* spec, int64_t T, const float* norm, int pad_l, int first, int count,
