@@ -232,6 +232,23 @@ VR_API int vr_mp3_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, cons
                          int64_t md_bytes, void* workspace, int64_t workspace_bytes, float* out, int64_t* status,
                          void* stream);
 
+/* MPEG-4 AAC-LC decoding on the device (ISO/IEC 14496-3 subpart 4, the twelve sampling-frequency indices, 1 or 2
+ * channels, 1024-sample frames; lib/aac.py is the caller and walks the MP4 container, oracle/aac_oracle.py restates
+ * the standard).  All buffers are DEVICE memory owned by the caller; no call allocates.
+ *
+ * vr_aac_workspace: bytes of the workspace vr_aac_decode needs for n_packets packets of channels (1 or 2) channels
+ * (-1 for invalid arguments).
+ *
+ * vr_aac_decode: table: n_packets rows of 2 int64 (byte offset in data, byte size) of consecutive raw_data_blocks of
+ * one track (rate_index 0..11, the AudioSpecificConfig's samplingFrequencyIndex).  out: [channels][1024 * n_packets]
+ * float32 at full scale 1, not clipped, with zero filterbank state before the first packet and no edit-list trim.
+ * status: one int64 per packet, 0 or code << 40 | bit offset in the packet (codes: lib/aac.py).  Malformed bytes never
+ * fault: they give a status and a finite output. */
+VR_API int64_t vr_aac_workspace(int64_t n_packets, int32_t channels);
+VR_API int vr_aac_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int64_t* table, int32_t n_packets,
+                         int32_t channels, int32_t rate_index, void* workspace, int64_t workspace_bytes, float* out,
+                         int64_t* status, void* stream);
+
 /* FLAC encoding on the device (RFC 9639 streamable subset; lib/flac.py is the caller, oracle/flac_oracle.py decodes
  * the result independently): fixed block size FLAC_ENCODE_BLOCK (the last block shorter), bits = 16 or 24 bits per
  * sample (anything else is an error), one or two channels.  All buffers are DEVICE memory owned by the caller; no call

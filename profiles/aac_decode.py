@@ -1,0 +1,159 @@
+"""Times the GPU AAC-LC decoder (csrc/aac.cu through lib/aac.py) on 4-minute stereo 44.1 kHz M4A files at 128 and
+256 kbit/s and on a 40-minute one at 128 kbit/s, and ``separate_wave`` on the 4-minute track in the same run.
+
+Each file is a 10-second ``synth.sine_mix`` encoded by the oracle (oracle/aac_oracle.py) with its packets repeated, in
+a plain MP4 (moov first, one chunk): a valid file whose decode cost is that of a real one of the same length and
+bitrate (the oracle encoder is too slow for 40 minutes).  Reported per file, as medians over --runs calls after
+warm-up: bytes and packets; each kernel's time (torch.profiler) and their sum; the H2D and D2H copies per call; one
+whole ``aac.decode`` call (CUDA events around it, and host wall time); the host container walk (``aac.parse`` timed on
+its own).  ``separate_wave`` runs the default CLI settings with a synthetic checkpoint (the cost does not depend on
+the weights).  The card's name and power limit are read in the same run (read-only ``nvidia-smi --query-gpu``).
+
+Usage: python profiles/aac_decode.py [--runs 20] [--out aac_decode.json]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+for p in (ROOT, os.path.join(ROOT, 'vocal-remover_b200')):
+    if p not in sys.path:
+        sys.path.insert(0, p)
+
+
+def _gpu_info():
+    try:
+        r = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
+                           capture_output=True, text=True, timeout=30)
+        name, power, clock = [s.strip() for s in r.stdout.splitlines()[0].split(',')]
+        return dict(gpu=name, power_limit=power, max_sm_clock=clock)
+    except Exception as e:
+        return dict(gpu=None, nvidia_smi_error=str(e))
+
+
+def _stream(kbps, seconds):
+    from lib import synth
+    from oracle import aac_oracle as ao
+    packets, asc = ao.encode(synth.sine_mix(10.0).astype(np.float64), 44100, kbps, seed=kbps)
+    return ao.mp4(packets * int(np.ceil(seconds / 10.0)), asc, 44100, 2)[0]
+
+
+def _host_parse_ms(data, runs):
+    from lib import aac
+    times = []
+    for _ in range(runs):
+        t0 = time.perf_counter()
+        aac.parse(data)
+        times.append(1e3 * (time.perf_counter() - t0))
+    return float(np.median(times))
+
+
+KERNELS = ('parse', 'spectral', 'filterbank', 'overlap')
+
+
+def _measure(data, runs):
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    from lib import aac
+    for _ in range(3):
+        aac.decode(data)
+    torch.cuda.synchronize()
+    call_ms, wall_ms = [], []
+    for _ in range(runs):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        w0 = time.perf_counter()
+        a.record()
+        aac.decode(data)
+        b.record()
+        b.synchronize()
+        wall_ms.append(1e3 * (time.perf_counter() - w0))
+        call_ms.append(a.elapsed_time(b))
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(runs):
+            aac.decode(data)
+        torch.cuda.synchronize()
+    per = {}   # key -> [(start, ms)] in launch order
+    for ev in prof.events():
+        if ev.device_type.name != 'CUDA':
+            continue
+        name = ev.name
+        key = next((k for k in KERNELS if 'aac_%s_kernel' % k in name), None)
+        if key is None:
+            key = 'memcpy HtoD' if 'HtoD' in name else ('memcpy DtoH' if 'DtoH' in name else None)
+        if key is None:
+            continue
+        ms = (ev.device_time_total if hasattr(ev, 'device_time_total') else ev.cuda_time_total) / 1e3
+        per.setdefault(key, []).append((ev.time_range.start, ms))
+    # every kernel runs once per call: the median over the calls; the copies run several times per call: their sum
+    # per call (in launch order), then the median
+    device = {}
+    for k, v in per.items():
+        ms = np.asarray([m for _, m in sorted(v)])
+        if len(ms) % runs == 0:
+            device[k] = float(np.median(ms.reshape(runs, -1).sum(axis=1)))
+    kernel_sum = sum(v for k, v in device.items() if k in KERNELS)
+    return dict(bytes=len(data), ms_per_call_median=float(np.median(call_ms)),
+                wall_ms_median=float(np.median(wall_ms)), host_parse_ms_median=_host_parse_ms(data, runs),
+                device_ms_per_call_median=device, decode_kernels_ms=kernel_sum)
+
+
+def _separate_ms(x, runs):
+    """Median CUDA-event time of Separator.separate_wave on x (channels, n) with the CLI's default settings."""
+    import torch
+    sys.path.insert(0, os.path.join(ROOT, 'vocal-remover_b200'))
+    import inference
+    from lib import nets, spec_utils, synth
+    args = inference.build_parser().parse_args(['-P', 'unused', '-i', 'unused'])
+    device = torch.device('cuda:0')
+    model = nets.CascadedNet(args.n_fft, args.hop_length, 32, 128)
+    model.load_state_dict(synth.to_torch_state_dict(synth.make_state_dict()))
+    model.to(device)
+    spec_utils.set_device(0)
+    sp = inference.Separator(model=model, device=device, batchsize=args.batchsize, cropsize=args.cropsize,
+                             postprocess=args.postprocess, wiener_iterations=args.wiener_iterations)
+    sp.separate_wave(x)
+    times = []
+    for _ in range(runs):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        a.record()
+        sp.separate_wave(x)
+        b.record()
+        b.synchronize()
+        times.append(a.elapsed_time(b))
+    return float(np.median(times))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--runs', type=int, default=20)
+    ap.add_argument('--out', default=None)
+    args = ap.parse_args()
+    import torch
+    from lib import aac
+    assert torch.cuda.is_available(), 'profiles/aac_decode.py measures on the GPU'
+    res = dict(_gpu_info(), torch_device=torch.cuda.get_device_name(0), runs=args.runs)
+    for label, kbps, seconds in (('4 min 128 kbit/s', 128, 240), ('4 min 256 kbit/s', 256, 240),
+                                 ('40 min 128 kbit/s', 128, 2400)):
+        data = _stream(kbps, seconds)
+        y, _, info = aac.decode(data)
+        r = _measure(data, args.runs)
+        r['packets'] = info['frames']
+        if label == '4 min 128 kbit/s':
+            r['separate_wave_ms_median'] = _separate_ms(y.cpu().numpy(), max(3, args.runs // 4))
+        res[label] = r
+        print(label, json.dumps(r), flush=True)
+    if args.out:
+        with open(args.out, 'w') as f:
+            json.dump(res, f, indent=1)
+    print(json.dumps(dict((k, v) for k, v in res.items() if not isinstance(v, dict))))
+
+
+if __name__ == '__main__':
+    main()

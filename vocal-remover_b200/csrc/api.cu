@@ -289,6 +289,17 @@ int vr_mp3_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int64
                                            workspace, workspace_bytes, out, status, (cudaStream_t)stream));
 }
 
+int64_t vr_aac_workspace(int64_t n_packets, int32_t channels) { return vr::aac_workspace_bytes(n_packets, channels); }
+
+int vr_aac_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int64_t* table, int32_t n_packets,
+                  int32_t channels, int32_t rate_index, void* workspace, int64_t workspace_bytes, float* out,
+                  int64_t* status, void* stream) {
+  use_device(ctx);
+  return cuda_result(ctx, "vr_aac_decode",
+                     vr::launch_aac_decode(data, n_bytes, table, n_packets, channels, rate_index, workspace,
+                                           workspace_bytes, out, status, (cudaStream_t)stream));
+}
+
 int vr_flac_encode_analyse(vr_ctx* ctx, const float* x, int32_t channels, int64_t n, int32_t rate_code, int32_t bits,
                            void* pcm, int32_t* plan, void* stream) {
   use_device(ctx);

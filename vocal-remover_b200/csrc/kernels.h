@@ -130,6 +130,14 @@ cudaError_t launch_flac_scan(const uint8_t* data, int64_t n_bytes, int64_t begin
 cudaError_t launch_flac_decode(const uint8_t* data, int64_t n_bytes, const int64_t* frames, int n_frames, int channels,
                                int64_t n_samples, float* out, int64_t* status, cudaStream_t stream);
 
+// ---- MPEG-4 AAC-LC decoding (aac.cu), the decode in front of the path for .m4a / .mp4 input (lib/aac.py) -----------
+// table[n_packets][2] = (byte offset, byte size) of each raw_data_block in data -> out [channels][1024 * n_packets]
+// (no trim), status[n_packets]; the workspace (aac_workspace_bytes) holds the descriptors, quantised values and spectra
+int64_t aac_workspace_bytes(int64_t n_packets, int channels);
+cudaError_t launch_aac_decode(const uint8_t* data, int64_t n_bytes, const int64_t* table, int n_packets, int channels,
+                              int rate_index, void* workspace, int64_t workspace_bytes, float* out, int64_t* status,
+                              cudaStream_t stream);
+
 // ---- MPEG-1 Layer III decoding (mp3.cu), the decode in front of the path for .mp3 input (lib/mp3.py) ---------------
 // scan: every 11-bit sync at byte offsets [begin, end - 4] -> cands[*count][2] = (offset, the 4 header bytes
 // big-endian); decode: frames[n_frames][2] = (offset, header word) of the chained frames, md_off[n_frames + 1] = the

@@ -2,7 +2,8 @@
 
 The reference uses ``librosa.load(path, sr=sr, mono=False, dtype=np.float32, res_type='kaiser_fast')`` and
 ``soundfile.write`` (inference.py:136-138,173,178).  FLAC and MP3 input are decoded on the GPU when there is one
-(lib/flac.py, csrc/flac.cu; lib/mp3.py, csrc/mp3.cu) and FLAC output encoded on it (csrc/flac_encode.cu); other
+(lib/flac.py, csrc/flac.cu; lib/mp3.py, csrc/mp3.cu), M4A / MP4 (AAC-LC) input always is (lib/aac.py, csrc/aac.cu),
+and FLAC output encoded on it (csrc/flac_encode.cu); other
 decoding and encoding stay on the host (soundfile when installed, else a stdlib ``wave``
 reader for 8/16/24/32-bit PCM WAV and writer for 16-bit), except the samples of a 24-bit WAV, which are quantised and
 packed on the GPU like the FLAC encoder's (``vr_pcm_pack``); the sample-rate conversion of non-``sr`` input - the
@@ -76,12 +77,20 @@ def resample(y, orig_sr, target_sr, device=None, filt=None):
 
 
 def _decode(path, device=None):
-    """(channels, n) float32 at the file's own rate.  FLAC and MPEG-1 Layer III (recognised by content, FLAC first) are
-    decoded on the GPU whenever a CUDA device is visible (lib/flac.py, lib/mp3.py); otherwise soundfile reads them if
-    it is installed."""
-    from . import flac, mp3
+    """(channels, n) float32 at the file's own rate.  FLAC, MPEG-1 Layer III and MP4 (recognised by content, in that
+    order) are decoded on the GPU whenever a CUDA device is visible (lib/flac.py, lib/mp3.py, lib/aac.py); otherwise
+    soundfile reads FLAC and MP3 if it is installed.  libsndfile has no MP4 reader, so an M4A without a CUDA device
+    raises RuntimeError."""
+    from . import aac, flac, mp3
     is_flac = flac.sniff(path)
     is_mp3 = not is_flac and mp3.sniff(path)
+    if not is_flac and not is_mp3 and aac.sniff(path):
+        import torch
+        if not torch.cuda.is_available():
+            raise RuntimeError('%s is an MP4 / M4A file: decoding it needs a CUDA device (lib/aac.py; soundfile has no '
+                               'MP4 reader), and none is visible' % path)
+        x, rate, _ = aac.decode(path, device)
+        return x.cpu().numpy(), rate
     if is_flac or is_mp3:
         import torch
         if torch.cuda.is_available():
