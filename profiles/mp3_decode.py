@@ -45,8 +45,8 @@ def _stream(kbps, seconds):
 def _host_chain_ms(data, runs):
     """Median time of lib.mp3.build_chain (the host chain walk) on the stream's sync candidates in byte order, as
     vr_mp3_scan and the device sort hand them over (found here with numpy)."""
-    from lib import flac, mp3
-    start = flac._id3_size(data)
+    from lib import codec, mp3
+    start = codec.id3v2_size(data)
     end = mp3.audio_end(data, start)
     d = np.frombuffer(data, np.uint8)
     i = np.flatnonzero((d[:-1] == 0xFF) & ((d[1:] & 0xE0) == 0xE0))

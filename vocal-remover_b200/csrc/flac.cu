@@ -16,6 +16,7 @@
 // Malformed input is data: every read is bounded by the frame's span (bits past it read as zero and fail the frame),
 // every write stays in the frame's own samples, and each frame leaves a status word (0, or code << 40 | bit offset in
 // the frame) for the host to turn into an error.
+#include "bitstream.cuh"
 #include "common.cuh"
 #include "flac_common.cuh"
 #include "kernels.h"
@@ -47,8 +48,6 @@ enum FlacError : int64_t {
   kFrameShape = 13,     // channel assignment, bit depth or sample span the stream does not have
   kWastedBits = 14,     // wasted bits leave no sample bits
 };
-
-__device__ __forceinline__ int64_t flac_status(int64_t code, int64_t bit) { return (code << 40) | (bit & 0xFFFFFFFFFFLL); }
 
 // the frame header at byte i (d[i] == 0xFF and d[i+1] is 0xF8 / 0xF9 already); false if it is not one
 __device__ bool parse_frame_header(const uint8_t* __restrict__ d, int64_t n, int64_t i, int64_t rec[4]) {
@@ -180,12 +179,12 @@ __device__ __forceinline__ bool is_side(int ch_code, int c) {
 // residual of one subframe into dst[order, bs); returns 0 or a status
 __device__ int64_t read_residual(BitReader& br, int64_t frame_bit0, int32_t* __restrict__ dst, int bs, int order) {
   const uint32_t method = br.read(2);
-  if (method > 1) return flac_status(kResidualMethod, br.pos() - frame_bit0);
+  if (method > 1) return frame_status(kResidualMethod, br.pos() - frame_bit0);
   const int pbits = method ? 5 : 4;
   const uint32_t escape = method ? 31u : 15u;
   const int porder = (int)br.read(4);
   const int psize = bs >> porder;
-  if ((psize << porder) != bs || psize < order) return flac_status(kPartitionOrder, br.pos() - frame_bit0);
+  if ((psize << porder) != bs || psize < order) return frame_status(kPartitionOrder, br.pos() - frame_bit0);
   int j = order;
   for (int p = 0; p < (1 << porder); ++p) {
     const int stop = (p + 1) * psize;
@@ -196,12 +195,12 @@ __device__ int64_t read_residual(BitReader& br, int64_t frame_bit0, int32_t* __r
     } else {
       for (; j < stop; ++j) {
         const uint64_t q = br.unary();
-        if (q >> (32 - k)) return flac_status(kRiceOverflow, br.pos() - frame_bit0);
+        if (q >> (32 - k)) return frame_status(kRiceOverflow, br.pos() - frame_bit0);
         const uint32_t u = ((uint32_t)q << k) | br.read((int)k);
         dst[j] = (int32_t)(u >> 1) ^ -(int32_t)(u & 1);
       }
     }
-    if (br.pos() > 8 * br.end) return flac_status(kOverrun, br.pos() - frame_bit0);
+    if (br.pos() > 8 * br.end) return frame_status(kOverrun, br.pos() - frame_bit0);
   }
   return 0;
 }
@@ -213,12 +212,12 @@ __device__ int64_t parse_subframes(BitReader& br, int64_t frame_bit0, int32_t* _
   for (int c = 0; c < C; ++c) {
     int32_t* dst = stage + (int64_t)c * n;
     const int sub_bps = bps + (is_side(ch_code, c) ? 1 : 0);
-    if (br.read(1)) return flac_status(kPadBit, br.pos() - 1 - frame_bit0);
+    if (br.read(1)) return frame_status(kPadBit, br.pos() - 1 - frame_bit0);
     const int type = (int)br.read(6);
     int wasted = 0;
     if (br.read(1)) {
       const uint64_t w = br.unary() + 1;
-      if (w >= (uint64_t)sub_bps) return flac_status(kWastedBits, br.pos() - frame_bit0);
+      if (w >= (uint64_t)sub_bps) return frame_status(kWastedBits, br.pos() - frame_bit0);
       wasted = (int)w;
     }
     const int eb = sub_bps - wasted;
@@ -232,21 +231,21 @@ __device__ int64_t parse_subframes(BitReader& br, int64_t frame_bit0, int32_t* _
     } else if ((type >= 8 && type <= 12) || type >= 32) {
       m.kind = type >= 32 ? 3 : 2;
       m.order = type >= 32 ? type - 31 : type - 8;
-      if (m.order > bs) return flac_status(kOrderTooLarge, br.pos() - frame_bit0);
+      if (m.order > bs) return frame_status(kOrderTooLarge, br.pos() - frame_bit0);
       for (int j = 0; j < m.order; ++j) dst[j] = br.read_signed(eb);
       if (m.kind == 3) {
         const int prec = (int)br.read(4) + 1;
-        if (prec == 16) return flac_status(kLpcPrecision, br.pos() - 4 - frame_bit0);
+        if (prec == 16) return frame_status(kLpcPrecision, br.pos() - 4 - frame_bit0);
         m.shift = br.read_signed(5);
-        if (m.shift < 0) return flac_status(kLpcShift, br.pos() - 5 - frame_bit0);
+        if (m.shift < 0) return frame_status(kLpcShift, br.pos() - 5 - frame_bit0);
         for (int j = 0; j < m.order; ++j) coef[c][j] = br.read_signed(prec);
       }
       const int64_t e = read_residual(br, frame_bit0, dst, bs, m.order);
       if (e) return e;
     } else {
-      return flac_status(kReservedType, br.pos() - 6 - frame_bit0);
+      return frame_status(kReservedType, br.pos() - 6 - frame_bit0);
     }
-    if (br.pos() > 8 * br.end) return flac_status(kOverrun, br.pos() - frame_bit0);
+    if (br.pos() > 8 * br.end) return frame_status(kOverrun, br.pos() - frame_bit0);
     meta[c] = m;
   }
   return 0;
@@ -273,7 +272,7 @@ __device__ int64_t restore_channel(int32_t* __restrict__ dst, int bs, const SubM
           case 4: s += 4 * s1 - 6 * s2 + 4 * s3 - s4; break;
           default: break;
         }
-        if (s < lo || s > hi) return flac_status(kSampleRange, j);
+        if (s < lo || s > hi) return frame_status(kSampleRange, j);
       }
       s4 = s3; s3 = s2; s2 = s1; s1 = s;
       dst[j] = (int32_t)s;
@@ -284,7 +283,7 @@ __device__ int64_t restore_channel(int32_t* __restrict__ dst, int bs, const SubM
       int64_t sum = 0;
       for (int k = 0; k < m.order; ++k) sum += (int64_t)coef[k] * hist[(j - 1 - k) & (kMaxLpcOrder - 1)];
       const int64_t s = (int64_t)dst[j] + (sum >> m.shift);
-      if (s < lo || s > hi) return flac_status(kSampleRange, j);
+      if (s < lo || s > hi) return frame_status(kSampleRange, j);
       hist[j & (kMaxLpcOrder - 1)] = (int32_t)s;
       dst[j] = (int32_t)s;
     }
@@ -302,19 +301,10 @@ __global__ void __launch_bounds__(256) flac_scan_kernel(const uint8_t* __restric
   int64_t rec[4];
   bool found = false;
   if (i + 1 < n && d[i] == 0xFF && (d[i + 1] & 0xFE) == 0xF8) found = parse_frame_header(d, n, i, rec);
-  const unsigned mask = __ballot_sync(0xffffffffu, found);
-  if (!mask) return;
-  const int lane = threadIdx.x & 31, leader = __ffs(mask) - 1;
-  int base = 0;
-  if (lane == leader) base = atomicAdd(count, __popc(mask));
-  base = __shfl_sync(0xffffffffu, base, leader);
-  if (found) {
-    const int slot = base + __popc(mask & ((1u << lane) - 1));
-    if (slot < max_cands) {
+  const int slot = warp_append(found, count, max_cands);
+  if (slot < 0) return;
 #pragma unroll
-      for (int k = 0; k < 4; ++k) cands[(int64_t)slot * 4 + k] = rec[k];
-    }
-  }
+  for (int k = 0; k < 4; ++k) cands[(int64_t)slot * 4 + k] = rec[k];
 }
 
 __global__ void __launch_bounds__(kWarpsPerBlock * 32) flac_decode_kernel(
@@ -341,7 +331,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) flac_decode_kernel(
   int64_t err = 0;
   if (nch != C || C > kMaxChannels || bs < 1 || off < 0 || off + bs > n || bps < 4 || bps > 24 || start < 0 ||
       start + hlen >= end)
-    err = flac_status(kFrameShape, 0);
+    err = frame_status(kFrameShape, 0);
   int64_t e = 0;   // the byte after the subframes (where the CRC-16 sits)
   if (!err && lane == 0) {
     BitReader br(d, start + hlen, end);
@@ -349,9 +339,9 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) flac_decode_kernel(
     err = parse_subframes(br, bit0, stage, n, C, ch_code, bs, bps, meta_s[warp], coef_s[warp]);
     if (!err) {
       const int pad = (int)((8 - (br.pos() & 7)) & 7);
-      if (br.read(pad)) err = flac_status(kPadBit, br.pos() - bit0);
+      if (br.read(pad)) err = frame_status(kPadBit, br.pos() - bit0);
       e = br.pos() >> 3;
-      if (!err && e + 2 != end) err = flac_status(kFrameEnd, 8 * e - bit0);
+      if (!err && e + 2 != end) err = frame_status(kFrameEnd, 8 * e - bit0);
     }
   }
   err = __shfl_sync(0xffffffffu, err, 0);
@@ -362,7 +352,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32) flac_decode_kernel(
     const uint8_t* fr = d + start;
     const uint32_t r = flac::warp_crc16(e - start, crc_tab, [&](int64_t v) { return (uint32_t)__ldg(fr + v); });
     const uint32_t want = ((uint32_t)__ldg(d + e) << 8) | __ldg(d + e + 1);
-    if (r != want) err = flac_status(kCrc16, 8 * (e - start));
+    if (r != want) err = frame_status(kCrc16, 8 * (e - start));
   }
 
   if (!err) {

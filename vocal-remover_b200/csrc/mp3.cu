@@ -21,6 +21,7 @@
 //   mp3_window_kernel     one thread per output sample: the 512-tap window D over the 16 V vectors up to its slot.
 #include <math.h>
 
+#include "bitstream.cuh"
 #include "common.cuh"
 #include "kernels.h"
 
@@ -189,37 +190,10 @@ enum Mp3Status : int64_t {
   kGranuleEnd = 5,      // scale factors or big values run past the granule's part2_3_length
 };
 
-__device__ __forceinline__ int64_t mp3_status(int64_t code, int64_t bit) { return (code << 40) | (bit & 0xFFFFFFFFFFLL); }
-
 struct Granule {
   int64_t start;   // bit offset of the part2_3 data in the reservoir buffer
   int32_t p23, big, gain, sfc, ws, bt, mixed, ts[3], sbg[3], r0, r1, pre, sfs, c1, scfsi, skip;
 };
-
-// MSB-first reads at any bit offset of [0, 8 * n) of d; bytes past n read as zero
-struct Bits {
-  const uint8_t* __restrict__ d;
-  int64_t n, pos;
-  __device__ __forceinline__ uint32_t peek32() const {
-    const int64_t b = pos >> 3;
-    uint64_t w = 0;
-#pragma unroll
-    for (int k = 0; k < 5; ++k) w = (w << 8) | (b + k < n ? (uint64_t)__ldg(d + b + k) : 0ull);
-    return (uint32_t)(w >> (8 - (pos & 7)));
-  }
-  __device__ __forceinline__ uint32_t read(int k) {   // 0 <= k <= 24
-    if (k == 0) return 0;
-    const uint32_t v = peek32() >> (32 - k);
-    pos += k;
-    return v;
-  }
-};
-
-__device__ __forceinline__ float exp2_quarter(int q4) {   // 2^(q4 / 4), exactly rounded for the four fractions
-  const int r = q4 & 3;
-  const float frac = r == 0 ? 1.0f : r == 1 ? 1.18920711500272f : r == 2 ? 1.41421356237310f : 1.68179283050743f;
-  return ldexpf(frac, q4 >> 2);
-}
 
 }  // namespace
 
@@ -228,20 +202,11 @@ __global__ void __launch_bounds__(256) mp3_scan_kernel(const uint8_t* __restrict
                                                        int* __restrict__ count) {
   const int64_t i = begin + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const bool found = i + 4 <= end && d[i] == 0xFF && (d[i + 1] & 0xE0) == 0xE0;
-  const unsigned mask = __ballot_sync(0xffffffffu, found);
-  if (!mask) return;
-  const int lane = threadIdx.x & 31, leader = __ffs(mask) - 1;
-  int base = 0;
-  if (lane == leader) base = atomicAdd(count, __popc(mask));
-  base = __shfl_sync(0xffffffffu, base, leader);
-  if (found) {
-    const int slot = base + __popc(mask & ((1u << lane) - 1));
-    if (slot < max_cands) {
-      cands[2 * (int64_t)slot] = i;
-      cands[2 * (int64_t)slot + 1] = (int64_t)(((uint32_t)d[i] << 24) | ((uint32_t)d[i + 1] << 16) |
-                                               ((uint32_t)d[i + 2] << 8) | d[i + 3]);
-    }
-  }
+  const int slot = warp_append(found, count, max_cands);
+  if (slot < 0) return;
+  cands[2 * (int64_t)slot] = i;
+  cands[2 * (int64_t)slot + 1] = (int64_t)(((uint32_t)d[i] << 24) | ((uint32_t)d[i + 1] << 16) |
+                                           ((uint32_t)d[i + 2] << 8) | d[i + 3]);
 }
 
 // one thread per frame: header and side info -> the frame's granule-channel descriptors and its status
@@ -254,7 +219,7 @@ __global__ void __launch_bounds__(128) mp3_side_info_kernel(const uint8_t* __res
   const int64_t off = frames[2 * f];
   const uint32_t h = (uint32_t)frames[2 * f + 1];
   const bool crc = ((h >> 16) & 1) == 0;
-  Bits br{d, n_bytes, 8 * (off + 4 + (crc ? 2 : 0))};
+  PeekBits br{d, n_bytes, 8 * (off + 4 + (crc ? 2 : 0))};
   const int mdb = (int)br.read(9);
   br.read(C == 1 ? 5 : 3);
   const int scfsi0 = (int)br.read(4), scfsi1 = C == 2 ? (int)br.read(4) : 0;
@@ -279,7 +244,7 @@ __global__ void __launch_bounds__(128) mp3_side_info_kernel(const uint8_t* __res
         g.sbg[1] = (int)br.read(3);
         g.sbg[2] = (int)br.read(3);
         g.r0 = g.r1 = 0;
-        if (g.bt == 0 && !err) err = mp3_status(kReservedBlock, br.pos - 8 * off - 3);
+        if (g.bt == 0 && !err) err = frame_status(kReservedBlock, br.pos - 8 * off - 3);
       } else {
         g.bt = g.mixed = 0;
         g.ts[0] = (int)br.read(5);
@@ -293,15 +258,15 @@ __global__ void __launch_bounds__(128) mp3_side_info_kernel(const uint8_t* __res
       g.sfs = (int)br.read(1);
       g.c1 = (int)br.read(1);
       g.scfsi = gr == 1 ? (ch ? scfsi1 : scfsi0) : 0;
-      if (g.big > 288 && !err) err = mp3_status(kBigValues, 0);
+      if (g.big > 288 && !err) err = frame_status(kBigValues, 0);
       g.start = bit;
       bit += g.p23;
       g.skip = 0;
       gran[(int64_t)(2 * f + gr) * C + ch] = g;
     }
   }
-  if (!err && begin < 0) err = mp3_status(kZeroed, 0);
-  if (!err && bit > 8 * md_off[f + 1]) err = mp3_status(kMainData, bit - 8 * md_off[f + 1]);
+  if (!err && begin < 0) err = frame_status(kZeroed, 0);
+  if (!err && bit > 8 * md_off[f + 1]) err = frame_status(kMainData, bit - 8 * md_off[f + 1]);
   if (err) {
     for (int k = 0; k < 2 * C; ++k) gran[(int64_t)2 * f * C + k].skip = 1;
   }
@@ -329,20 +294,8 @@ __global__ void __launch_bounds__(128, 1) mp3_huffman_kernel(const uint8_t* __re
                                                           const Granule* __restrict__ gran, int n_gc, int C, int sr,
                                                           const float* __restrict__ pow43, float* __restrict__ xr,
                                                           uint8_t* __restrict__ sf_out, int64_t* __restrict__ gstatus) {
-  __shared__ uint32_t codes[kHuffEntries];
-  __shared__ uint8_t syms[kHuffEntries], lens[kHuffEntries];
-  for (int i = threadIdx.x; i < kHuffEntries; i += blockDim.x) {
-    syms[i] = kHuffSymbols[i];
-    lens[i] = kHuffLengths[i];
-  }
-  if (threadIdx.x < 15) {   // each table's codes: the previous code plus one at its own length, left-aligned
-    uint32_t code = 0;
-    for (int i = kTableStart[threadIdx.x]; i < kTableStart[threadIdx.x + 1]; ++i) {
-      codes[i] = code;
-      code += 1u << (32 - kHuffLengths[i]);
-    }
-  }
-  __syncthreads();
+  __shared__ HuffBooks<uint8_t, kHuffEntries> bk;
+  bk.build(kHuffSymbols, kHuffLengths, kTableStart, 15);
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= n_gc) return;
   const Granule g = gran[q];
@@ -353,8 +306,7 @@ __global__ void __launch_bounds__(128, 1) mp3_huffman_kernel(const uint8_t* __re
   int k = 0;
   const bool shortb = g.ws && g.bt == 2;
   if (!g.skip) {
-    Bits br{md, md_bytes, g.start};
-    const int64_t end = g.start + g.p23;
+    PeekBits br{md, md_bytes, g.start, g.start + g.p23};
     const int s1 = kSlen[g.sfc][0], s2 = kSlen[g.sfc][1];
     if (shortb) {
       if (g.mixed)
@@ -376,11 +328,11 @@ __global__ void __launch_bounds__(128, 1) mp3_huffman_kernel(const uint8_t* __re
         if (g.scfsi & (8 >> grp)) {
           if (g0_short) {
             for (int b = first; b < last; ++b) {
-              Bits b0r{md, md_bytes, g0->start + (int64_t)b * a0};
+              PeekBits b0r{md, md_bytes, g0->start + (int64_t)b * a0};
               sf[b] = g0_mixed && b < 8 ? (uint8_t)b0r.read(a0) : 0;
             }
           } else {
-            Bits b0r{md, md_bytes, p0};
+            PeekBits b0r{md, md_bytes, p0};
             for (int b = first; b < last; ++b) sf[b] = (uint8_t)b0r.read(s0);
           }
         } else {
@@ -389,7 +341,7 @@ __global__ void __launch_bounds__(128, 1) mp3_huffman_kernel(const uint8_t* __re
         p0 += (int64_t)(last - first) * s0;
       }
     }
-    if (br.pos > end) err = mp3_status(kGranuleEnd, br.pos - g.start);
+    if (br.over()) err = frame_status(kGranuleEnd, br.pos - g.start);
     // region boundaries in lines
     const int big = 2 * g.big;
     int r1, r2;
@@ -418,17 +370,10 @@ __global__ void __launch_bounds__(128, 1) mp3_huffman_kernel(const uint8_t* __re
         continue;
       }
       const int lb = kLinbits[ts];
-      const int lo = kTableStart[t], n = kTableStart[t + 1] - lo;
+      const int first = kTableStart[t], last = kTableStart[t + 1];
       for (; k < stop; k += 2) {
-        const uint32_t w = br.peek32();
-        int a = 0, span = n;   // the last entry whose left-aligned code is <= w
-        while (span > 1) {
-          const int half = span >> 1;
-          if (codes[lo + a + half] <= w) a += half;
-          span -= half;
-        }
-        br.pos += lens[lo + a];
-        int vx = syms[lo + a] >> 4, vy = syms[lo + a] & 15;
+        const int sym = bk.sym[bk.decode(br, first, last)];
+        int vx = sym >> 4, vy = sym & 15;
         if (lb && vx == 15) vx += (int)br.read(lb);
         if (vx && br.read(1)) vx = -vx;
         if (lb && vy == 15) vy += (int)br.read(lb);
@@ -436,9 +381,9 @@ __global__ void __launch_bounds__(128, 1) mp3_huffman_kernel(const uint8_t* __re
         x[k] = (float)vx;
         x[k + 1] = (float)vy;
       }
-      if (br.pos > end) err = mp3_status(kGranuleEnd, br.pos - g.start);
+      if (br.over()) err = frame_status(kGranuleEnd, br.pos - g.start);
     }
-    while (!err && k <= 572 && br.pos < end) {
+    while (!err && k <= 572 && br.pos < br.end) {
       int v;
       if (g.c1) {
         v = 15 - (int)br.read(4);
@@ -455,7 +400,7 @@ __global__ void __launch_bounds__(128, 1) mp3_huffman_kernel(const uint8_t* __re
         const int bit = (v >> (3 - j)) & 1;
         qv[j] = bit ? (br.read(1) ? -1.0f : 1.0f) : 0.0f;
       }
-      if (br.pos > end) break;   // a quadruple that crosses the granule's end is dropped
+      if (br.over()) break;   // a quadruple that crosses the granule's end is dropped
 #pragma unroll
       for (int j = 0; j < 4; ++j) x[k + j] = qv[j];
       k += 4;
@@ -732,26 +677,19 @@ struct Mp3Workspace {
   int64_t bytes;
 };
 
-int64_t align256(int64_t v) { return (v + 255) & ~(int64_t)255; }
-
 Mp3Workspace carve(uint8_t* base, int64_t n_frames, int C, int64_t md_bytes) {
   Mp3Workspace w{};
+  Carver c{base};
   const int64_t gc = 2 * n_frames * C;
-  int64_t o = 0;
-  auto take = [&](int64_t n) {
-    const int64_t at = o;
-    o += align256(n);
-    return base ? base + at : nullptr;
-  };
-  w.md = take(md_bytes + 8);
-  w.gran = reinterpret_cast<Granule*>(take(gc * (int64_t)sizeof(Granule)));
-  w.fstatus = reinterpret_cast<int64_t*>(take(n_frames * 8));
-  w.gstatus = reinterpret_cast<int64_t*>(take(gc * 8));
-  w.sf = take(gc * kSfBytes);
-  w.xr = reinterpret_cast<float*>(take(gc * 576 * 4));
-  w.V = reinterpret_cast<float*>(take((int64_t)C * n_frames * 36 * 64 * 4));
-  w.pow43 = reinterpret_cast<float*>(take(kPow43 * 4));
-  w.bytes = o;
+  w.md = c.take(md_bytes + 8);
+  w.gran = c.take<Granule>(gc * (int64_t)sizeof(Granule));
+  w.fstatus = c.take<int64_t>(n_frames * 8);
+  w.gstatus = c.take<int64_t>(gc * 8);
+  w.sf = c.take(gc * kSfBytes);
+  w.xr = c.take<float>(gc * 576 * 4);
+  w.V = c.take<float>((int64_t)C * n_frames * 36 * 64 * 4);
+  w.pow43 = c.take<float>(kPow43 * 4);
+  w.bytes = c.bytes;
   return w;
 }
 

@@ -111,6 +111,12 @@ class NativeError(RuntimeError):
     pass
 
 
+def check(lib, rc, what):
+    """Raises NativeError('<what> failed: <message>') when a call made without a context returned nonzero."""
+    if rc != 0:
+        raise NativeError('%s failed: %s' % (what, lib.vr_last_error(None).decode()))
+
+
 class Context(object):
     """One vr_ctx: a CascadedNet bound to one GPU, a cropsize and a maximum window batch."""
 
@@ -119,9 +125,7 @@ class Context(object):
         self.cfg = VrConfig(int(device_index), int(n_fft), int(hop_length), int(nout), int(nout_lstm),
                             int(cropsize), int(max_batch), int(conv_mode))
         h = c_vp()
-        rc = self.lib.vr_create(ctypes.byref(self.cfg), ctypes.byref(h))
-        if rc != 0:
-            raise NativeError('vr_create failed: %s' % self.lib.vr_last_error(None).decode())
+        check(self.lib, self.lib.vr_create(ctypes.byref(self.cfg), ctypes.byref(h)), 'vr_create')
         self.handle = h
         self.device_index = int(device_index)
 

@@ -18,7 +18,7 @@ import struct
 
 import numpy as np
 
-from .flac import _name, _read
+from . import codec
 
 FRAME = 1024
 RATES = (96000, 88200, 64000, 48000, 44100, 32000, 24000, 22050, 16000, 12000, 11025, 8000)
@@ -300,8 +300,8 @@ def parse(src, name=None):
     """The container of an .m4a / .mp4 file (path or bytes) -> dict(rate_index, rate, channels, offsets, sizes
     (int64 arrays, one entry per packet), media_time, segment (kept samples, None: to the end), edit (bool),
     fragmented, asc).  ValueError for anything out of scope."""
-    name = name or _name(src)
-    data = _read(src)
+    src_name, data = codec.source(src)
+    name = name or src_name
     top = _boxes(data, 0, len(data), name)
     tops = {}
     for typ, a, b, o in top:
@@ -409,20 +409,11 @@ def decode(src, device=None):
     decoded), priming (samples the edit drops at the start), kept (samples returned), fragmented."""
     import torch
     from . import _native
-    name = _name(src)
-    data = _read(src)
+    name, data = codec.source(src)
     t = parse(data, name)
-    if not torch.cuda.is_available():
-        raise RuntimeError('%s: M4A decoding runs on the GPU and no CUDA device is visible' % name)
-    dev = torch.device(device if device is not None else 'cuda:0')
+    dev = codec.cuda_device(name, 'M4A', device)
     lib = _native.load_library()
-
-    def check(rc, what):
-        if rc != 0:
-            raise _native.NativeError('%s failed: %s' % (what, lib.vr_last_error(None).decode()))
-
     F, C, sfi = len(t['offsets']), t['channels'], t['rate_index']
-    table = np.stack([t['offsets'], t['sizes']], axis=1).astype(np.int64)   # in the file, for the error messages
     packed, dev_table = gather(data, t['offsets'], t['sizes'])
     with torch.cuda.device(dev):
         d_data = torch.from_numpy(packed).to(dev)
@@ -431,18 +422,11 @@ def decode(src, device=None):
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
         out = torch.empty((C, F * FRAME), dtype=torch.float32, device=dev)
         status = torch.empty(F, dtype=torch.int64, device=dev)
-        check(lib.vr_aac_decode(None, _native.ptr(d_data), len(packed), _native.ptr(d_table), F, C, sfi,
-                                _native.ptr(ws), ws_bytes, _native.ptr(out), _native.ptr(status),
-                                _native.stream_ptr()), 'vr_aac_decode')
+        _native.check(lib, lib.vr_aac_decode(None, _native.ptr(d_data), len(packed), _native.ptr(d_table), F, C, sfi,
+                                             _native.ptr(ws), ws_bytes, _native.ptr(out), _native.ptr(status),
+                                             _native.stream_ptr()), 'vr_aac_decode')
         st = status.cpu().numpy()
-    codes = st >> 40
-    bad = np.flatnonzero(codes != 0)
-    if bad.size:
-        k = int(bad[0])
-        raise ValueError('%s: packet %d (byte %d): %s (bit %d)' % (name, k, int(table[k, 0]),
-                                                                  ERRORS.get(int(codes[k]), 'error %d' % codes[k]),
-                                                                  int(st[k]) & ((1 << 40) - 1)))
+    codec.raise_first_bad(st, t['offsets'], ERRORS, name, 'packet')
     a, b = trim_range(F * FRAME, t)
     info = dict(frames=F, priming=a, kept=b - a, fragmented=t['fragmented'])
-    y = out if (a, b) == (0, F * FRAME) else out[:, a:b].contiguous()
-    return y, t['rate'], info
+    return codec.trim(out, a, b), t['rate'], info

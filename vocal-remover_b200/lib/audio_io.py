@@ -67,10 +67,9 @@ def resample(y, orig_sr, target_sr, device=None, filt=None):
         d_win = torch.from_numpy(half).to(dev)
         d_delta = torch.from_numpy(delta).to(dev)
         out = torch.empty((x.shape[0], n_out), dtype=torch.float32, device=dev)
-        rc = lib.vr_resample(None, _native.ptr(x), x.shape[0], n_in, _native.ptr(out), n_out, ratio, _native.ptr(d_win),
-                             _native.ptr(d_delta), int(half.shape[0]), per_crossing, _native.stream_ptr())
-        if rc != 0:
-            raise _native.NativeError('vr_resample failed: %s' % lib.vr_last_error(None).decode())
+        _native.check(lib, lib.vr_resample(None, _native.ptr(x), x.shape[0], n_in, _native.ptr(out), n_out, ratio,
+                                           _native.ptr(d_win), _native.ptr(d_delta), int(half.shape[0]), per_crossing,
+                                           _native.stream_ptr()), 'vr_resample')
         torch.cuda.current_stream().synchronize()   # d_win / d_delta go out of scope
     out = out[0] if squeeze else out.reshape(tuple(y.shape[:-1]) + (n_out,))
     return out if is_tensor else out.cpu().numpy().astype(np.asarray(y).dtype if np.asarray(y).dtype.kind == 'f' else np.float32)
@@ -82,32 +81,29 @@ def _decode(path, device=None):
     soundfile reads FLAC and MP3 if it is installed.  libsndfile has no MP4 reader, so an M4A without a CUDA device
     raises RuntimeError."""
     from . import aac, flac, mp3
-    is_flac = flac.sniff(path)
-    is_mp3 = not is_flac and mp3.sniff(path)
-    if not is_flac and not is_mp3 and aac.sniff(path):
+    # (sniff, decode, what the file is, the decoder's source, soundfile reads it) in detection order
+    formats = ((flac.sniff, flac.decode, 'a FLAC file', 'lib/flac.py', True),
+               (mp3.sniff, mp3.decode, 'an MP3 file', 'lib/mp3.py', True),
+               (aac.sniff, aac.decode, 'an MP4 / M4A file', 'lib/aac.py', False))
+    fmt = next((f for f in formats if f[0](path)), None)
+    if fmt is not None:
         import torch
-        if not torch.cuda.is_available():
-            raise RuntimeError('%s is an MP4 / M4A file: decoding it needs a CUDA device (lib/aac.py; soundfile has no '
-                               'MP4 reader), and none is visible' % path)
-        x, rate, _ = aac.decode(path, device)
-        return x.cpu().numpy(), rate
-    if is_flac or is_mp3:
-        import torch
+        _, decode, what, source, soundfile_reads = fmt
         if torch.cuda.is_available():
-            x, rate, _ = (flac if is_flac else mp3).decode(path, device)
+            x, rate, _ = decode(path, device)
             return x.cpu().numpy(), rate
+        if not soundfile_reads:
+            raise RuntimeError('%s is %s: decoding it needs a CUDA device (%s; soundfile has no MP4 reader), and none '
+                               'is visible' % (path, what, source))
     try:
         import soundfile as sf
         data, rate = sf.read(path, dtype='float32', always_2d=True)
         return np.ascontiguousarray(data.T), rate
     except ImportError:
         pass
-    if is_flac:
-        raise RuntimeError('%s is a FLAC file: decoding it needs a CUDA device (lib/flac.py) or the soundfile module, '
-                           'and neither is available' % path)
-    if is_mp3:
-        raise RuntimeError('%s is an MP3 file: decoding it needs a CUDA device (lib/mp3.py) or the soundfile module, '
-                           'and neither is available' % path)
+    if fmt is not None:
+        raise RuntimeError('%s is %s: decoding it needs a CUDA device (%s) or the soundfile module, and neither is '
+                           'available' % (path, what, source))
     with _wave.open(path, 'rb') as f:
         nch, width, rate, nframes = f.getnchannels(), f.getsampwidth(), f.getframerate(), f.getnframes()
         raw = f.readframes(nframes)

@@ -146,8 +146,7 @@ def frame_sums(references, estimates, window, hop, filters_len=512, device=None,
                                 _native.ptr(ws), int(nbytes), sums.ctypes.data,
                                 None if corr is None else corr.ctypes.data, loading.ctypes.data,
                                 None if phase is None else phase.ctypes.data, _native.stream_ptr())
-        if rc != 0:
-            raise _native.NativeError('%s failed: %s' % (name, lib.vr_last_error(None).decode()))
+        _native.check(lib, rc, name)
     out = {'sums': sums, 'loading': loading}
     if framewise:
         out['frames_per_batch'] = frames_per_batch

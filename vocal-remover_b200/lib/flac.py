@@ -32,9 +32,11 @@ on the device by ``vr_pcm_pack`` (``pcm_bytes``), which is also what a 24-bit WA
 The integers are ``clip(rint(x * (2^(bits-1) - 1)))`` with the product in fp32 and NaN -> 0, for every writer.
 """
 import hashlib
-import os
 
 import numpy as np
+
+from . import codec
+from .codec import id3v2_size as _id3_size   # the name tests/test_mp3.py takes it by
 
 BPS_CODES = {1: 8, 2: 12, 4: 16, 5: 20, 6: 24}
 MAX_BLOCK = 65535
@@ -62,25 +64,6 @@ ERRORS = {
     13: 'frame shape the stream does not have',
     14: 'wasted bits leave no sample bits',
 }
-
-
-def _name(src):
-    return src if isinstance(src, (str, os.PathLike)) else '<%d bytes>' % len(src)
-
-
-def _read(src):
-    if isinstance(src, (bytes, bytearray, memoryview)):
-        return bytes(src)
-    with open(src, 'rb') as f:
-        return f.read()
-
-
-def _id3_size(head):
-    """Bytes taken by an ID3v2 tag at the start of ``head`` (0 if there is none)."""
-    if len(head) < 10 or head[:3] != b'ID3':
-        return 0
-    return 10 + ((head[6] & 0x7F) << 21 | (head[7] & 0x7F) << 14 | (head[8] & 0x7F) << 7 | (head[9] & 0x7F)) + \
-        (10 if head[5] & 0x10 else 0)
 
 
 def sniff(path):
@@ -211,46 +194,25 @@ def decode(src, device=None):
     """FLAC file path or bytes -> (CUDA float32 tensor (channels, n), sample rate, bits per sample)."""
     import torch
     from . import _native
-    name = _name(src)
-    data = _read(src)
+    name, data = codec.source(src)
     start, info = parse_metadata(data, name)
     end = audio_end(data, start)
-    if not torch.cuda.is_available():
-        raise RuntimeError('%s: FLAC decoding runs on the GPU and no CUDA device is visible' % name)
-    dev = torch.device(device if device is not None else 'cuda:0')
+    dev = codec.cuda_device(name, 'FLAC', device)
     lib = _native.load_library()
-
-    def check(rc, what):
-        if rc != 0:
-            raise _native.NativeError('%s failed: %s' % (what, lib.vr_last_error(None).decode()))
-
     with torch.cuda.device(dev):
         d_data = torch.frombuffer(bytearray(data[:end]), dtype=torch.uint8).to(dev) if end else \
             torch.zeros(1, dtype=torch.uint8, device=dev)
-        count = torch.zeros(1, dtype=torch.int32, device=dev)
-        cap = 256 + end // 256      # a retry with the exact count covers streams of very short frames
-        while True:
-            cands = torch.empty((cap, 4), dtype=torch.int64, device=dev)
-            check(lib.vr_flac_scan(None, _native.ptr(d_data), end, start, _native.ptr(cands), cap, _native.ptr(count),
-                                   _native.stream_ptr()), 'vr_flac_scan')
-            found = int(count.item())
-            if found <= cap:
-                break
-            cap = found
-        frames, total = build_chain(cands[:found].cpu().numpy(), start, end, info, name)
+        # a retry with the exact count covers streams of very short frames
+        cands = codec.scan(lib, 'vr_flac_scan', d_data, end, start, 4, 256 + end // 256)
+        frames, total = build_chain(cands.cpu().numpy(), start, end, info, name)
         out = torch.empty((info['channels'], total), dtype=torch.float32, device=dev)
         status = torch.empty(frames.shape[0], dtype=torch.int64, device=dev)
         d_frames = torch.from_numpy(frames).to(dev)
-        check(lib.vr_flac_decode(None, _native.ptr(d_data), end, _native.ptr(d_frames), frames.shape[0],
-                                 info['channels'], total, _native.ptr(out), _native.ptr(status), _native.stream_ptr()),
-              'vr_flac_decode')
+        _native.check(lib, lib.vr_flac_decode(None, _native.ptr(d_data), end, _native.ptr(d_frames), frames.shape[0],
+                                              info['channels'], total, _native.ptr(out), _native.ptr(status),
+                                              _native.stream_ptr()), 'vr_flac_decode')
         st = status.cpu().numpy()
-    bad = np.flatnonzero(st)
-    if bad.size:
-        k = int(bad[0])
-        code, bit = int(st[k]) >> 40, int(st[k]) & ((1 << 40) - 1)
-        raise ValueError('%s: frame %d (byte %d): %s (bit %d of the frame)'
-                         % (name, k, int(frames[k, 0]), ERRORS.get(code, 'error %d' % code), bit))
+    codec.raise_first_bad(st, frames[:, 0], ERRORS, name, 'frame', bit_note=' of the frame')
     check_length(info, total, name)
     return out, info['rate'], info['bps']
 
@@ -316,12 +278,6 @@ def _on_device(x, device=None):
     return xd.to(dev, torch.float32).contiguous()
 
 
-def _check(lib, rc, what):
-    from . import _native
-    if rc != 0:
-        raise _native.NativeError('%s failed: %s' % (what, lib.vr_last_error(None).decode()))
-
-
 def pcm_bytes(x, bits, device=None):
     """float (channels, n) -> numpy uint8 array: the samples quantised and interleaved as little-endian ``bits / 8``-byte
     integers on the device (``vr_pcm_pack``); only those bytes are copied back."""
@@ -332,8 +288,8 @@ def pcm_bytes(x, bits, device=None):
     lib = _native.load_library()
     with torch.cuda.device(xd.device):
         out = torch.empty(xd.numel() * (bits // 8), dtype=torch.uint8, device=xd.device)
-        _check(lib, lib.vr_pcm_pack(None, _native.ptr(xd), int(xd.shape[0]), int(xd.shape[1]), bits, _native.ptr(out),
-                                    _native.stream_ptr()), 'vr_pcm_pack')
+        _native.check(lib, lib.vr_pcm_pack(None, _native.ptr(xd), int(xd.shape[0]), int(xd.shape[1]), bits,
+                                           _native.ptr(out), _native.stream_ptr()), 'vr_pcm_pack')
         return out.cpu().numpy()
 
 
@@ -354,17 +310,17 @@ def encode_frames(x, rate, device=None, bits=16):
         pcm = torch.empty((n, C), dtype=getattr(torch, BITS[bits]), device=dev)
         plan = torch.empty((F, PLAN_INTS), dtype=torch.int32, device=dev)
         stream = _native.stream_ptr()
-        _check(lib, lib.vr_flac_encode_analyse(None, _native.ptr(xd), C, n, code, bits, _native.ptr(pcm),
-                                               _native.ptr(plan), stream), 'vr_flac_encode_analyse')
+        _native.check(lib, lib.vr_flac_encode_analyse(None, _native.ptr(xd), C, n, code, bits, _native.ptr(pcm),
+                                                      _native.ptr(plan), stream), 'vr_flac_encode_analyse')
         sizes = plan[:, 0].cpu().numpy().astype(np.int64)
         offsets = np.zeros(F, np.int64)
         np.cumsum(sizes[:-1], out=offsets[1:])
         out = torch.empty(int(sizes.sum()), dtype=torch.uint8, device=dev)
         status = torch.empty(F, dtype=torch.int32, device=dev)
         d_off = torch.from_numpy(offsets).to(dev)
-        _check(lib, lib.vr_flac_encode_pack(None, _native.ptr(pcm), C, n, bits, _native.ptr(plan), _native.ptr(d_off),
-                                            code, value, _native.ptr(out), _native.ptr(status), stream),
-               'vr_flac_encode_pack')
+        _native.check(lib, lib.vr_flac_encode_pack(None, _native.ptr(pcm), C, n, bits, _native.ptr(plan),
+                                                   _native.ptr(d_off), code, value, _native.ptr(out),
+                                                   _native.ptr(status), stream), 'vr_flac_encode_pack')
         body = out.cpu().numpy().tobytes()
         st = status.cpu().numpy()
     bad = np.flatnonzero(st)

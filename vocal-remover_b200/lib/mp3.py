@@ -22,7 +22,7 @@ offset.  The output is float32 at full scale 1, not clipped, at the file's own r
 """
 import numpy as np
 
-from .flac import _id3_size, _name, _read
+from . import codec
 
 BITRATES = (0, 32, 40, 48, 56, 64, 80, 96, 112, 128, 160, 192, 224, 256, 320)   # kbit/s, MPEG-1 Layer III
 RATES = (44100, 48000, 32000)
@@ -186,7 +186,7 @@ def sniff(path):
     try:
         with open(path, 'rb') as f:
             head = f.read(10)
-            skip = _id3_size(head)
+            skip = codec.id3v2_size(head)
             f.seek(skip)
             b = f.read(4)
             if len(b) < 4 or b[0] != 0xFF or (b[1] & 0xE0) != 0xE0:   # the 11-bit sync
@@ -211,33 +211,15 @@ def decode(src, device=None):
     data began before the stream), xing, lame."""
     import torch
     from . import _native
-    name = _name(src)
-    data = _read(src)
-    start = _id3_size(data)
+    name, data = codec.source(src)
+    start = codec.id3v2_size(data)
     end = audio_end(data, start)
-    if not torch.cuda.is_available():
-        raise RuntimeError('%s: MP3 decoding runs on the GPU and no CUDA device is visible' % name)
-    dev = torch.device(device if device is not None else 'cuda:0')
+    dev = codec.cuda_device(name, 'MP3', device)
     lib = _native.load_library()
-
-    def check(rc, what):
-        if rc != 0:
-            raise _native.NativeError('%s failed: %s' % (what, lib.vr_last_error(None).decode()))
-
     with torch.cuda.device(dev):
         d_data = torch.frombuffer(bytearray(data[:end]), dtype=torch.uint8).to(dev) if end else \
             torch.zeros(1, dtype=torch.uint8, device=dev)
-        count = torch.zeros(1, dtype=torch.int32, device=dev)
-        cap = 256 + end // 128
-        while True:
-            cands = torch.empty((cap, 2), dtype=torch.int64, device=dev)
-            check(lib.vr_mp3_scan(None, _native.ptr(d_data), start, end, _native.ptr(cands), cap, _native.ptr(count),
-                                  _native.stream_ptr()), 'vr_mp3_scan')
-            found = int(count.item())
-            if found <= cap:
-                break
-            cap = found
-        rows = cands[:found]
+        rows = codec.scan(lib, 'vr_mp3_scan', d_data, start, end, 2, 256 + end // 128)
         h_cands = rows[torch.argsort(rows[:, 0])].cpu().numpy()   # in byte order (the scan appends unordered)
         frames, dropped = build_chain(h_cands, start, end, name)
         x = xing_info(data, int(frames[0, 0]), int(frames[0, 1]))
@@ -256,19 +238,13 @@ def decode(src, device=None):
         status = torch.empty(F, dtype=torch.int64, device=dev)
         d_frames = torch.from_numpy(np.ascontiguousarray(frames)).to(dev)
         d_md_off = torch.from_numpy(md_off).to(dev)
-        check(lib.vr_mp3_decode(None, _native.ptr(d_data), end, _native.ptr(d_frames), _native.ptr(d_md_off), F, C,
-                                sr, md_bytes, _native.ptr(ws), ws_bytes, _native.ptr(out), _native.ptr(status),
-                                _native.stream_ptr()), 'vr_mp3_decode')
+        _native.check(lib, lib.vr_mp3_decode(None, _native.ptr(d_data), end, _native.ptr(d_frames),
+                                             _native.ptr(d_md_off), F, C, sr, md_bytes, _native.ptr(ws), ws_bytes,
+                                             _native.ptr(out), _native.ptr(status), _native.stream_ptr()),
+                      'vr_mp3_decode')
         st = status.cpu().numpy()
-    codes = st >> 40
-    bad = np.flatnonzero((codes != 0) & (codes != ZEROED))
-    if bad.size:
-        k = int(bad[0])
-        raise ValueError('%s: frame %d (byte %d): %s (bit %d)' % (name, k + first, int(frames[k, 0]),
-                                                                  ERRORS.get(int(codes[k]), 'error %d' % codes[k]),
-                                                                  int(st[k]) & ((1 << 40) - 1)))
+    codec.raise_first_bad(st, frames[:, 0], ERRORS, name, 'frame', allowed=(ZEROED,), first=first)
     a, b = trim_range(F * FRAME, x)
     info = dict(frames=F, delay=x['delay'] if x else 0, padding=x['padding'] if x else 0, dropped=dropped,
-                zeroed=int((codes == ZEROED).sum()), xing=x is not None, lame=bool(x and x['lame']))
-    y = out if (a, b) == (0, F * FRAME) else out[:, a:b].contiguous()
-    return y, RATES[sr], info
+                zeroed=int(((st >> 40) == ZEROED).sum()), xing=x is not None, lame=bool(x and x['lame']))
+    return codec.trim(out, a, b), RATES[sr], info
