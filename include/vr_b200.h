@@ -249,6 +249,27 @@ VR_API int vr_aac_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, cons
                          int32_t channels, int32_t rate_index, void* workspace, int64_t workspace_bytes, float* out,
                          int64_t* status, void* stream);
 
+/* Vorbis I decoding on the device (1 or 2 channels, block sizes 64..8192, floor 1, residues 0-2; lib/vorbis.py is
+ * the caller, reads the Ogg pages and flattens the setup header; oracle/vorbis_oracle.py restates the specification).
+ * All buffers are DEVICE memory owned by the caller; no call allocates.
+ *
+ * vr_vorbis_workspace: bytes of the workspace vr_vorbis_decode needs for n_packets packets of channels (1 or 2)
+ * channels whose spectrum slots take slot_floats floats in all (the sum over packets of channels * blocksize / 2; -1
+ * for invalid arguments).
+ *
+ * vr_vorbis_decode: table: n_packets rows of 5 int64: byte offset in data, byte size, end of the packet's output range
+ * (the samples from the centre of the first block to the centre of this one), offset of its spectrum slot in floats,
+ * block flag | previous window flag << 1 | next window flag << 2 | mapping << 8.  setup: setup_words int32 in
+ * lib/vorbis.py's layout, holding n_codes codewords in all.  out: [channels][n_out] float32 at full scale 1, not
+ * clipped, no granule trim; n_out is the last row's output end.  status: one int64 per packet, 0 or code << 40 | bit
+ * offset in the packet (codes: lib/vorbis.py).  Malformed bytes never fault: they give a status and a finite
+ * output. */
+VR_API int64_t vr_vorbis_workspace(int64_t n_packets, int32_t channels, int64_t slot_floats);
+VR_API int vr_vorbis_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int64_t* table,
+                            int32_t n_packets, const int32_t* setup, int32_t setup_words, int32_t channels,
+                            int32_t n_codes, int64_t slot_floats, void* workspace, int64_t workspace_bytes, float* out,
+                            int64_t n_out, int64_t* status, void* stream);
+
 /* FLAC encoding on the device (RFC 9639 streamable subset; lib/flac.py is the caller, oracle/flac_oracle.py decodes
  * the result independently): fixed block size FLAC_ENCODE_BLOCK (the last block shorter), bits = 16 or 24 bits per
  * sample (anything else is an error), one or two channels.  All buffers are DEVICE memory owned by the caller; no call

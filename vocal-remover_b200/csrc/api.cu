@@ -300,6 +300,21 @@ int vr_aac_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int64
                                            workspace_bytes, out, status, (cudaStream_t)stream));
 }
 
+int64_t vr_vorbis_workspace(int64_t n_packets, int32_t channels, int64_t slot_floats) {
+  return vr::vorbis_workspace_bytes(n_packets, channels, slot_floats);
+}
+
+int vr_vorbis_decode(vr_ctx* ctx, const uint8_t* data, int64_t n_bytes, const int64_t* table, int32_t n_packets,
+                     const int32_t* setup, int32_t setup_words, int32_t channels, int32_t n_codes, int64_t slot_floats,
+                     void* workspace, int64_t workspace_bytes, float* out, int64_t n_out, int64_t* status,
+                     void* stream) {
+  use_device(ctx);
+  return cuda_result(ctx, "vr_vorbis_decode",
+                     vr::launch_vorbis_decode(data, n_bytes, table, n_packets, setup, setup_words, channels, n_codes,
+                                              slot_floats, workspace, workspace_bytes, out, n_out, status,
+                                              (cudaStream_t)stream));
+}
+
 int vr_flac_encode_analyse(vr_ctx* ctx, const float* x, int32_t channels, int64_t n, int32_t rate_code, int32_t bits,
                            void* pcm, int32_t* plan, void* stream) {
   use_device(ctx);

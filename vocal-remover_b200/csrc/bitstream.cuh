@@ -1,6 +1,6 @@
-// Bitstream pieces the input decoders (flac.cu, mp3.cu, aac.cu) share: the per-frame status word, an MSB-first reader
-// at absolute bit offsets, 2^(q/4), canonical Huffman books in shared memory, the warp-aggregated append of sync
-// candidates and the carving of one device workspace.
+// Bitstream pieces the input decoders (flac.cu, mp3.cu, aac.cu, vorbis.cu) share: the per-frame status word, MSB-first
+// and LSB-first readers at absolute bit offsets, 2^(q/4), canonical Huffman books in shared memory, the warp-aggregated
+// append of sync candidates and the carving of one device workspace.
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>
@@ -30,6 +30,27 @@ struct PeekBits {
     const uint32_t v = peek32() >> (32 - k);
     pos += k;
     return v;
+  }
+  __device__ __forceinline__ bool over() const { return pos > end; }
+};
+
+// LSB-first reads (Vorbis packs bits from the least significant end of each byte) at any bit offset of [0, 8 * n) of
+// d; bytes past n read as zero, and a read past ``end`` (the packet's last bit + 1) is caught by over()
+struct LsbBits {
+  const uint8_t* __restrict__ d;
+  int64_t n, pos, end;
+  __device__ __forceinline__ uint32_t peek32() const {
+    const int64_t b = pos >> 3;
+    uint64_t w = 0;
+#pragma unroll
+    for (int k = 4; k >= 0; --k) w = (w << 8) | (b + k < n ? (uint64_t)__ldg(d + b + k) : 0ull);
+    return (uint32_t)(w >> (pos & 7));
+  }
+  __device__ __forceinline__ uint32_t read(int k) {   // 0 <= k <= 32
+    if (k == 0) return 0;
+    const uint32_t v = peek32();
+    pos += k;
+    return k == 32 ? v : v & ((1u << k) - 1u);
   }
   __device__ __forceinline__ bool over() const { return pos > end; }
 };

@@ -138,6 +138,15 @@ cudaError_t launch_aac_decode(const uint8_t* data, int64_t n_bytes, const int64_
                               int rate_index, void* workspace, int64_t workspace_bytes, float* out, int64_t* status,
                               cudaStream_t stream);
 
+// ---- Vorbis I decoding (vorbis.cu), the decode in front of the path for .ogg input (lib/vorbis.py) ----------------
+// table[n_packets][5] (vr_b200.h) and the flattened setup -> out [channels][n_out] (no trim), status[n_packets]; the
+// workspace (vorbis_workspace_bytes) holds the floor points, the residue classes and the spectrum slots
+int64_t vorbis_workspace_bytes(int64_t n_packets, int channels, int64_t slot_floats);
+cudaError_t launch_vorbis_decode(const uint8_t* data, int64_t n_bytes, const int64_t* table, int n_packets,
+                                 const int* setup, int setup_words, int channels, int n_codes, int64_t slot_floats,
+                                 void* workspace, int64_t workspace_bytes, float* out, int64_t n_out, int64_t* status,
+                                 cudaStream_t stream);
+
 // ---- MPEG-1 Layer III decoding (mp3.cu), the decode in front of the path for .mp3 input (lib/mp3.py) ---------------
 // scan: every 11-bit sync at byte offsets [begin, end - 4] -> cands[*count][2] = (offset, the 4 header bytes
 // big-endian); decode: frames[n_frames][2] = (offset, header word) of the chained frames, md_off[n_frames + 1] = the

@@ -58,6 +58,9 @@ SIGNATURES = {
                               c_vp]),
     'vr_aac_workspace': (c_i64, [c_i64, c_i32]),
     'vr_aac_decode': (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i32, c_i32, c_i32, c_vp, c_i64, c_fp, c_vp, c_vp]),
+    'vr_vorbis_workspace': (c_i64, [c_i64, c_i32, c_i64]),
+    'vr_vorbis_decode': (c_i32, [c_vp, c_vp, c_i64, c_vp, c_i32, c_vp, c_i32, c_i32, c_i32, c_i64, c_vp, c_i64, c_fp,
+                                 c_i64, c_vp, c_vp]),
     'vr_flac_encode_analyse': (c_i32, [c_vp, c_fp, c_i32, c_i64, c_i32, c_i32, c_vp, c_vp, c_vp]),
     'vr_flac_encode_pack': (c_i32, [c_vp, c_vp, c_i32, c_i64, c_i32, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp]),
     'vr_pcm_pack': (c_i32, [c_vp, c_fp, c_i32, c_i64, c_i32, c_vp, c_vp]),

@@ -2,8 +2,8 @@
 
 The reference uses ``librosa.load(path, sr=sr, mono=False, dtype=np.float32, res_type='kaiser_fast')`` and
 ``soundfile.write`` (inference.py:136-138,173,178).  FLAC and MP3 input are decoded on the GPU when there is one
-(lib/flac.py, csrc/flac.cu; lib/mp3.py, csrc/mp3.cu), M4A / MP4 (AAC-LC) input always is (lib/aac.py, csrc/aac.cu),
-and FLAC output encoded on it (csrc/flac_encode.cu); other
+(lib/flac.py, csrc/flac.cu; lib/mp3.py, csrc/mp3.cu; lib/vorbis.py, csrc/vorbis.cu for Ogg Vorbis), M4A / MP4
+(AAC-LC) input always is (lib/aac.py, csrc/aac.cu), and FLAC output encoded on it (csrc/flac_encode.cu); other
 decoding and encoding stay on the host (soundfile when installed, else a stdlib ``wave``
 reader for 8/16/24/32-bit PCM WAV and writer for 16-bit), except the samples of a 24-bit WAV, which are quantised and
 packed on the GPU like the FLAC encoder's (``vr_pcm_pack``); the sample-rate conversion of non-``sr`` input - the
@@ -76,15 +76,17 @@ def resample(y, orig_sr, target_sr, device=None, filt=None):
 
 
 def _decode(path, device=None):
-    """(channels, n) float32 at the file's own rate.  FLAC, MPEG-1 Layer III and MP4 (recognised by content, in that
-    order) are decoded on the GPU whenever a CUDA device is visible (lib/flac.py, lib/mp3.py, lib/aac.py); otherwise
-    soundfile reads FLAC and MP3 if it is installed.  libsndfile has no MP4 reader, so an M4A without a CUDA device
-    raises RuntimeError."""
-    from . import aac, flac, mp3
+    """(channels, n) float32 at the file's own rate.  FLAC, MPEG-1 Layer III, MP4 and Ogg Vorbis (recognised by
+    content, in that order) are decoded on the GPU whenever a CUDA device is visible (lib/flac.py, lib/mp3.py,
+    lib/aac.py, lib/vorbis.py); otherwise soundfile reads FLAC, MP3 and Ogg Vorbis if it is installed.  libsndfile has
+    no MP4 reader, so an M4A without a CUDA device raises RuntimeError.  An Ogg file carrying another codec (Opus, FLAC,
+    Speex) is not claimed and goes to soundfile."""
+    from . import aac, flac, mp3, vorbis
     # (sniff, decode, what the file is, the decoder's source, soundfile reads it) in detection order
     formats = ((flac.sniff, flac.decode, 'a FLAC file', 'lib/flac.py', True),
                (mp3.sniff, mp3.decode, 'an MP3 file', 'lib/mp3.py', True),
-               (aac.sniff, aac.decode, 'an MP4 / M4A file', 'lib/aac.py', False))
+               (aac.sniff, aac.decode, 'an MP4 / M4A file', 'lib/aac.py', False),
+               (vorbis.sniff, vorbis.decode, 'an Ogg Vorbis file', 'lib/vorbis.py', True))
     fmt = next((f for f in formats if f[0](path)), None)
     if fmt is not None:
         import torch
