@@ -419,6 +419,11 @@ VR_API int vr_debug_tensor(vr_ctx* ctx, const char* name, int32_t n0, int32_t n,
  * output allows them, 1 = 4-byte stores of channel pairs everywhere; both write the same values).
  * Returns -1 for any other key.                                                                                    */
 VR_API int vr_debug_set(int32_t key, int32_t value);
+/* The last convolution launch of this process (any context), as its launcher decided it: out8 = {kind (0 CUDA-core,
+ * 1 generic, 2 row-streaming, 3 halo-tile tensor-core kernel), KB (channels per chunk), BN (output channels per tile),
+ * n_tiles, pairing (0 none, 1 PAIR_M, 2 PAIR_N), MB (halo kernel), UP (row kernel with fused upsample), 16-byte
+ * epilogue stores (0/1)}; fields the kernel does not have are 0.  Returns -1 if out8 is NULL.                        */
+VR_API int vr_debug_last_conv(int32_t* out8);
 /* timeline of CTA 0 of the last row-kernel launch made with vr_debug_set(0, 1): 3 roles x 2048 events x 3 clock64 stamps
  * (unused / TMA producer / interpolation warp 0), copied to HOST memory; returns the number of values or -1 */
 VR_API int64_t vr_debug_trace(uint64_t* host_out, int64_t capacity);

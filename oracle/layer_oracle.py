@@ -33,11 +33,17 @@ LSTM_H_GATE = 1e-5            # absolute, h in (-1, 1): fp32 gates with accurate
 PACK_GATE = 2.0 ** -16        # |X| / norm: hypotf, a reciprocal and a product in fp32, stored split-bf16 (2^-18)
 
 
+def nonvacuous_factor_fan_in(fan_in):
+    """How far above CONV_GATE both two-product emulations of a convolution summing ``fan_in`` products per output
+    (Cin * kh * kw) must land.  A dropped correction product errs by at most 2^-9 = 8 * CONV_GATE per product, so a
+    layer summing fewer than 16 products per output (the 1x1 bridge over 8 channels of the nout = 16 net: 6.9x on the
+    CPU emulation) can only be held to 4x."""
+    return NONVACUOUS if fan_in >= 16 else NONVACUOUS / 2
+
+
 def nonvacuous_factor(sd, p):
-    """How far above CONV_GATE both two-product emulations of Conv2DBNActiv ``p`` must land.  A dropped correction
-    product errs by at most 2^-9 = 8 * CONV_GATE per product, so a layer summing fewer than 16 products per output
-    (the 1x1 bridge over 8 channels of the nout = 16 net: 6.9x on the CPU emulation) can only be held to 4x."""
-    return NONVACUOUS if net_oracle._t(sd, p + '.conv.0.weight')[0].numel() >= 16 else NONVACUOUS / 2
+    """nonvacuous_factor_fan_in of Conv2DBNActiv ``p``"""
+    return nonvacuous_factor_fan_in(net_oracle._t(sd, p + '.conv.0.weight')[0].numel())
 
 
 def state_dict64(sd, device):
@@ -56,17 +62,29 @@ def max_ratio(err, den):
     return float(r.max()) if r.numel() else 0.0
 
 
-def conv_ratios(sd, p, x, y, stride=1, pad=1, dil=1, act='relu'):
-    """Conv2DBNActiv ``p`` on the GPU's input x against its output y (both float64, NCHW; y may be None):
-    (r of y, r of the no_wlo emulation, r of the no_xlo emulation, ref, den) with den the metric's denominator."""
-    ref = net_oracle.conv_bn_act(sd, p, x, stride=stride, pad=pad, dil=dil, act=act)
-    w, b = folded_conv(sd, p)
+def conv_ratios_of(x, w, b, y, stride=1, pad=1, dil=1, act='relu', ref=None):
+    """The convolution gate of act(conv2d(x, w) + b) on the GPU's input x against its output y (x, w, b, y float64,
+    NCHW; y may be None; act 'relu', 'leaky' or None for none): (r of y, r of the no_wlo emulation, r of the no_xlo
+    emulation, ref, den) with den the metric's denominator.  ref: the float64 reference when the caller has it."""
+    def act_of(v):
+        return v if act is None else activation(v, act)
+
     kw = dict(stride=stride, padding=pad, dilation=dil)
+    if ref is None:
+        ref = act_of(F.conv2d(x, w, b, **kw))
     den = F.conv2d(x * x, w * w, None, **kw).sqrt() + 2.0 ** -4 * ref.abs()
-    no_wlo = activation(F.conv2d(x, bf16(w), b, **kw), act)
-    no_xlo = activation(F.conv2d(bf16(x), w, b, **kw), act)
+    no_wlo = act_of(F.conv2d(x, bf16(w), b, **kw))
+    no_xlo = act_of(F.conv2d(bf16(x), w, b, **kw))
     r = None if y is None else max_ratio(y - ref, den)
     return r, max_ratio(no_wlo - ref, den), max_ratio(no_xlo - ref, den), ref, den
+
+
+def conv_ratios(sd, p, x, y, stride=1, pad=1, dil=1, act='relu'):
+    """Conv2DBNActiv ``p`` on the GPU's input x against its output y (both float64, NCHW; y may be None):
+    conv_ratios_of with the BatchNorm-folded weights, against the unfolded layer of the oracle."""
+    ref = net_oracle.conv_bn_act(sd, p, x, stride=stride, pad=pad, dil=dil, act=act)
+    w, b = folded_conv(sd, p)
+    return conv_ratios_of(x, w, b, y, stride=stride, pad=pad, dil=dil, act=act, ref=ref)
 
 
 def mask_ratio(m, z, ez):

@@ -475,6 +475,14 @@ int vr_debug_set(int32_t key, int32_t value) {
   return 0;
 }
 
+int vr_debug_last_conv(int32_t* out8) {
+  if (!out8) return -1;
+  const vr::TcLastConv& c = vr::g_last_conv;
+  const int32_t v[8] = {c.kind, c.KB, c.BN, c.n_tiles, c.pair, c.MB, c.up, c.vec16};
+  memcpy(out8, v, sizeof(v));
+  return 0;
+}
+
 int64_t vr_debug_trace(uint64_t* host_out, int64_t capacity) {
   return vr::tc_rows_read_trace((unsigned long long*)host_out, (long long)capacity);
 }

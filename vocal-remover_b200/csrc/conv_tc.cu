@@ -36,6 +36,9 @@ __host__ __device__ constexpr int consumer_warps(int mode) { return mode == PAIR
 __host__ __device__ constexpr int tc_threads(int mode) { return 32 * consumer_warps(mode) + 32; }
 // channels of K per pipeline stage: 32 in the paired variants, so that at BN = 128 a stage is 48 KB and four fit
 __host__ __device__ constexpr int stage_k(int mode) { return mode == PAIR_NONE ? 64 : 32; }
+// 16-byte stores where a warpgroup has registers to spare for the transpose (without them, the BN >= 80 paired
+// variants spill)
+__host__ __device__ constexpr bool generic_vec16(int mode, int bn) { return mode == PAIR_NONE || bn <= 64; }
 static constexpr int kStaticSmem = 2048;   // shared memory not given to the dynamic part: barriers and staged bias
 
 struct TcParams {
@@ -198,9 +201,8 @@ __global__ void __launch_bounds__(tc_threads(MODE), 1)
       const int w0 = (mt % p.tiles_w) * p.Wt;
       const int h0 = ((mt / p.tiles_w) % p.tiles_h) * p.Ht;
       const int n0 = (mt / (p.tiles_w * p.tiles_h)) * p.Nt;
-      // 16-byte stores where a warpgroup has registers to spare for the transpose (without them, the BN >= 80 paired
-      // variants spill); rows past the batch store nothing
-      constexpr bool kVec16 = MODE == PAIR_NONE || BN <= 64;
+      // 16-byte stores where the variant allows them (generic_vec16); rows past the batch store nothing
+      constexpr bool kVec16 = generic_vec16(MODE, BN);
       EpiDest d{p.out_hi, p.out_lo, {0, 0}, {false, false}, nt * BN, p.Cout, kVec16 && p.vec16};
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
@@ -229,6 +231,7 @@ __global__ void __launch_bounds__(tc_threads(MODE), 1)
 // ------------------------------------------------------------------------------------------------
 // host side
 TcDebug g_debug;
+TcLastConv g_last_conv;
 
 static constexpr int kMaxDevices = 64;
 const TcDevice& tc_device() {
@@ -546,8 +549,10 @@ cudaError_t tc_launch(const ConvLayer& L, const ActView& in, const ActView& out,
   p.bias = tc.bias.get();
   const int total_units = ceil_div(p.m_tiles, na) * (p.n_tiles / nb);
   const int grid = total_units < dv.num_sms ? total_units : dv.num_sms;
+  const TcLastConv launched{TC_GENERIC, KB, tc.BN, tc.n_tiles, mode, 0, 0, generic_vec16(mode, tc.BN) && p.vec16};
 #define VR_TC_LAUNCH(KB_, BN_, M_)                                                          \
   if (KB == KB_ && tc.BN == BN_ && mode == M_) {                                            \
+    g_last_conv = launched;                                                                 \
     conv_tc_kernel<KB_, BN_, M_><<<grid, tc_threads(M_), dyn, s>>>(*map_a, map_b, p);       \
     return cudaGetLastError();                                                              \
   }

@@ -286,8 +286,10 @@ cudaError_t tc_halo_launch(const ConvLayer& L, TcConv& tc, const ActView& in, co
     return cudaErrorInvalidValue;
   }
   const int grid = p.total_tiles < dv.num_sms ? p.total_tiles : dv.num_sms;   // persistent: one CTA per SM
+  const TcLastConv launched{TC_HALO, (int)kKB, tc.BN, tc.n_tiles, PAIR_NONE, MB, 0, p.vec16};
 #define VR_HALO_LAUNCH(BN_, MB_)                                                        \
   if (tc.BN == BN_ && MB == MB_) {                                                      \
+    g_last_conv = launched;                                                             \
     conv_tc_halo_kernel<BN_, MB_><<<grid, kThreads, dyn, s>>>(*map_a, tc.map_b, p);     \
     return cudaGetLastError();                                                          \
   }

@@ -676,8 +676,10 @@ cudaError_t tc_rows_launch(const ConvLayer& L, TcConv& tc, const ActView& in, co
   const int dyn = p.n_aslots * (int)kASlot + b_bytes + 1024;
   const int grid = p.total_tiles < dv.num_sms ? p.total_tiles : dv.num_sms;   // persistent: one CTA per SM
   const int threads = rows_threads(up);
+  const TcLastConv launched{TC_ROWS, (int)kKB, tc.BN, tc.n_tiles, PAIR_NONE, 0, up ? 1 : 0, p.vec16};
 #define VR_ROWS_LAUNCH(BN_, UP_)                                                              \
   if (tc.BN == BN_ && up == UP_) {                                                            \
+    g_last_conv = launched;                                                                   \
     conv_tc_rows_kernel<BN_, UP_><<<grid, threads, dyn, s>>>(*map_a, tc.map_b, *map_l, p);    \
     return cudaGetLastError();                                                                \
   }

@@ -513,6 +513,7 @@ bool Engine::run_conv(const ConvLayer& L, const ActView& in, const ActView& out,
     p.pad_h = L.dil_h * (L.k / 2); p.pad_w = L.dil_w * (L.k / 2);
     p.act = L.act;
     p.in.C = L.CinPad;
+    g_last_conv = TcLastConv{};
     ok = ck(launch_conv_simt(p, s), L.name.c_str());
   }
   prof_end(pi, s);

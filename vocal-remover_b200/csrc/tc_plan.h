@@ -103,6 +103,14 @@ struct TcDebug {
 };
 extern TcDebug g_debug;
 
+// The last convolution launch of this process, as the launchers decided it (vr_debug_last_conv): kind (TcKind), KB,
+// BN, n_tiles, pairing (TcPair, generic kernel), MB (halo kernel), fused upsample (row kernel) and whether the epilogue
+// stores 8 channels with 16-byte stores.  Fields a kernel does not have are 0.
+struct TcLastConv {
+  int kind = TC_NONE, KB = 0, BN = 0, n_tiles = 0, pair = PAIR_NONE, MB = 0, up = 0, vec16 = 0;
+};
+extern TcLastConv g_last_conv;
+
 // The epilogue of a launch into `out` may store 8 channels with one 16-byte store per plane (epilogue_store,
 // tc_common.cuh): both planes are 16-byte aligned, every stride is a multiple of 8 channels, and key 9 is not 1.
 bool tc_vec16(const ActView& out);

@@ -83,6 +83,7 @@ SIGNATURES = {
                                  c_fp, c_vp]),
     'vr_debug_tensor': (c_i32, [c_vp, ctypes.c_char_p, c_i32, c_i32, c_fp, ctypes.POINTER(c_i64), c_vp]),
     'vr_debug_set': (c_i32, [c_i32, c_i32]),
+    'vr_debug_last_conv': (c_i32, [ctypes.POINTER(c_i32)]),
     'vr_debug_trace': (c_i64, [c_vp, c_i64]),
 }
 
